@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """Benchmark of the SipMask inference hot path (BASELINE.json metric: images/sec @ 800x1333, bs=1/GPU).
 
-    python bench.py --gpus N --steps K --warmup W                      # this repo's sm_100a path, workload A (config 2)
+    python bench.py --gpus N --steps K --warmup W                      # this repo's sm_90a path, workload A (config 2)
     python bench.py --workload A101 | B                                 # R101 (config 3) | 544x544 bs=32 (config 4)
     python bench.py --impl reference --gpus N --steps K --warmup W      # the reference's CPU forward (oracle port)
+    python bench.py --dump-outputs DIR                                  # + what the last timed step returned, as DIR/*.npy
 
 One "step" = one pass of the whole hot path (image -> backbone/FPN -> head -> decode/NMS -> mask assembly ->
 bit-packed masks) over one synthetic image per GPU (workload B: one 32-image batch per GPU).  Prints ONE JSON line (rank 0).
@@ -70,22 +71,32 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))), 'measured'
     except Exception:
-        return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0), 'fallback'
+        # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense FP16 / BF16 tensor TFLOP/s
+        return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0), 'data sheet'
 
 
-def ncu_traffic():
-    """Per-launch DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum) of the roofline kernels, read from the committed
-    ncu --set full summary of this round (profiles/r02_ncu_traffic.json; bench.py itself never runs under a profiler)."""
-    try:
-        return json.load(open(os.path.join(ROOT, 'profiles', 'r02_ncu_traffic.json')))
-    except Exception:
-        return {}
+# mask_bits words written by --dump-outputs: all of them up to this count (float64 holds int32 exactly), else a fixed
+# seeded sample of this many (32 MB)
+DUMP_MASK_WORDS = 4 * 1024 * 1024
+
+
+def dump_outputs(out_dir, res):
+    """res: the engine result dict ({det_bboxes, det_labels, count, mask_bits, idxs_keep[, track_feats]}) -> out_dir/<name>.npy,
+    float32 for floating-point arrays, float64 for integer ones (exact)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in sorted(res.items()):
+        a = t.detach().cpu().numpy()
+        if name == 'mask_bits' and a.size > DUMP_MASK_WORDS:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, DUMP_MASK_WORDS, replace=False))
+            a, name = a.reshape(-1)[idx], 'mask_bits_sample'
+        np.save(os.path.join(out_dir, name + '.npy'), a.astype(np.float32 if a.dtype.kind == 'f' else np.float64))
 
 
 def host_threads():
     """Threads the CPU arm may really use: CPU affinity capped by the cgroup CPU quota (os.cpu_count() is the machine's
-    core count, 128 on the B200 hosts, of which a container usually owns a fraction - r1's CPU numbers moved 66x between
-    boxes because 128 threads were started on a few cores)."""
+    core count, of which a container usually owns a fraction: starting one thread per core on a few cores makes the CPU
+    numbers meaningless)."""
     aff = len(os.sched_getaffinity(0)) if hasattr(os, 'sched_getaffinity') else (os.cpu_count() or 1)
     quota = None
     try:
@@ -105,7 +116,7 @@ def host_threads():
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md 'clocks line')."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index, self.proc, self.lines = index, None, []
@@ -306,7 +317,11 @@ def run_ours(args):
         from sipmask_b200.tracker import Tracker
         tracker = Tracker()
 
+    capture = dict(on=False, res=None)          # --dump-outputs: the result the last timed step hands to its caller
+
     def consume(out):
+        if capture['on']:
+            capture['res'] = {k: v.clone() for k, v in out.items()}
         for b in range(B):
             log.append(out['det_bboxes'][b], out['det_labels'][b], out['count'][b:b + 1],
                        out['track_feats'][b] if vis else None)
@@ -350,7 +365,7 @@ def run_ours(args):
         runner.flush(consume)                  # the timed region ends when the last result is on the host
         finish_records()
 
-    def timed(fn, steps, sample_clocks=False, finish=None):
+    def timed(fn, steps, sample_clocks=False, finish=None, mark_last=False):
         """K steps between barrier+synchronize, CUDA events, max over ranks.  nvidia-smi samples clocks every 100 ms;
         a short timed region would get no sample, so ROLL untimed steps of the same load run before and after it and
         the sampler stays on throughout (clocks.window says so)."""
@@ -383,10 +398,12 @@ def run_ours(args):
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        for _ in range(steps):
+        for i in range(steps):
+            capture['on'] = mark_last and i == steps - 1
             fn()
         if finish is not None:
             finish()                                # joins the images in flight / downloads and issues the end-of-run gather
+        capture['on'] = False
         e1.record()
         torch.cuda.synchronize()
         if world > 1:
@@ -409,7 +426,9 @@ def run_ours(args):
         step()
     step_finish()
     torch.cuda.synchronize()
-    total_ms, clocks = timed(step, args.steps, sample_clocks=True, finish=step_finish)
+    total_ms, clocks = timed(step, args.steps, sample_clocks=True, finish=step_finish, mark_last=bool(args.dump_outputs))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, capture['res'])
     ms_per_step = total_ms / args.steps
     value = world * ips * 1000.0 / ms_per_step
     for _ in range(3):
@@ -431,7 +450,7 @@ def run_ours(args):
                                         'timed region)' % (world, nfl),
                             detections_per_image=ndet, cuda_graph=True, forwards_in_flight=nfl, batch_per_forward=B,
                             images_per_step_per_gpu=ips,
-                            l2='no flush: one step streams >= 1.3 GB of activations/masks through a 126 MB L2, so nothing but '
+                            l2='no flush: one step streams >= 1.3 GB of activations/masks through a 50 MB L2, so nothing but '
                                'weights can survive from the previous step'),
                 clocks=clocks, e2e=dict(value=e2e_value, unit='images/s', h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h,
                                         ms_per_step=e2e_ms / args.steps,
@@ -442,7 +461,6 @@ def run_ours(args):
 
     if rank == 0:
         pk, pk_kind = peaks()
-        traffic = ncu_traffic()
         # ---- roofline of the dominant kernel (conv_gemm_kernel): the conv launches of one step of EVERY engine in flight,
         # captured per engine (same stream schedule as in the step) and replayed concurrently on the pool's streams
         graphs = []
@@ -476,12 +494,9 @@ def run_ours(args):
         torch.cuda.synchronize()
         conv_ms = e0.elapsed_time(e1) / (reps * nfl)                      # per forward
         tf = eng.conv_flops / (conv_ms * 1e-3) / 1e12
-        peak_tf = float(pk.get('bf16_tflops_sustained', pk.get('bf16_tflops', 1400.0)))
-        tr = traffic.get('conv_gemm_kernel', {})
+        peak_tf = float(pk.get('bf16_tflops_sustained', pk.get('bf16_tflops', 989.0)))
         line['roofline'] = dict(bound='tensor', kernel='conv_gemm_kernel (%d launches/step)' % len(eng.conv_plans),
                                 achieved=tf, peak=peak_tf, unit='TFLOP/s', frac=tf / peak_tf,
-                                traffic=tr.get('dram_bytes_per_step') * nfl if tr.get('dram_bytes_per_step') else None,
-                                traffic_source=tr.get('source'),
                                 peak_source=pk_kind + ' bf16_tflops_sustained', algorithmic_gflop_per_step=eng.conv_flops * nfl / 1e9,
                                 ms_per_step=conv_ms * nfl, share_of_step=conv_ms * nfl / ms_per_step,
                                 ms_per_forward=conv_ms,
@@ -506,7 +521,7 @@ def run_ours(args):
                                   note='one forward in flight (latency-optimal planner settings), same GPU, N=1 rank only')
             del e1s
         if args.workload == 'A':
-            mask_rooflines(line, eng, pk, pk_kind, traffic, H, IMG_W)
+            mask_rooflines(line, eng, pk, pk_kind, H, IMG_W)
             line['e2e_dropin'] = dropin_timing(eng, sd, cfg, H, IMG_W)
             if not args.no_library_baseline:
                 line['library_gpu_baseline'] = library_baseline(wl, img_host, dev)
@@ -526,7 +541,7 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
-def mask_rooflines(line, eng, pk, pk_kind, traffic, H, IMG_W):
+def mask_rooflines(line, eng, pk, pk_kind, H, IMG_W):
     """Mask assembly (BASELINE metric part 2): HBM GB/s at N = max_per_img detections with 32-512 px boxes, L2 flushed
     between launches.  Each number is the whole ABI call (zero-fill memset node + kernel)."""
     import torch
@@ -568,22 +583,20 @@ def mask_rooflines(line, eng, pk, pk_kind, traffic, H, IMG_W):
     ma_ms = time_kernel(lambda: ops.mask_assemble(protos, cofs, boxes, 0.5, layout='hwc', out=pos))
     ma_bytes = Hm * Wm * 32 * 2 + N * 128 * 4 + N * 16 + N * Hm * Wm * 4
     gbs = ma_bytes / (ma_ms * 1e-3) / 1e9
-    tr = traffic.get('mask_assemble', {})
     line['roofline_mask_assembly'] = dict(bound='hbm', kernel='mask_assemble%s_kernel, %s (writes every output element; no memset)'
                                                               % ('_mma' if tensor_dot else '', fam), achieved=gbs,
                                           peak=float(pk['hbm_gbs']), unit='GB/s', frac=gbs / float(pk['hbm_gbs']),
-                                          traffic=tr.get('dram_bytes_per_launch'), traffic_source=tr.get('source'), ms=ma_ms,
+                                          ms=ma_ms,
                                           algorithmic_bytes=ma_bytes, peak_source=pk_kind + ' hbm_gbs',
                                           note='protos fp16 HWC read once + fp32 pos_masks [100,400,672] written; L2 flushed between launches')
     # (b) the path the engine runs: fused assembly + bilinear resize + threshold + bit-pack (no pos_masks traffic)
     mf_ms = time_kernel(lambda: ops.mask_assemble_pack(protos, cofs, boxes, 0.5, (H, IMG_W), 0.4, layout='hwc', out=bits))
     mf_bytes = Hm * Wm * 32 * 2 + N * 128 * 4 + N * 16 + bits.numel() * 4
     mgbs = mf_bytes / (mf_ms * 1e-3) / 1e9
-    tr = traffic.get('mask_fused', {})
     line['roofline_mask_fused'] = dict(bound='hbm', kernel='smb_mask_assemble_pack = memset + mask_fused_pack%s_kernel, %s'
                                                            % ('_mma' if tensor_dot else '', fam), achieved=mgbs,
                                        peak=float(pk['hbm_gbs']), unit='GB/s', frac=mgbs / float(pk['hbm_gbs']),
-                                       traffic=tr.get('dram_bytes_per_launch'), traffic_source=tr.get('source'), ms=mf_ms,
+                                       ms=mf_ms,
                                        algorithmic_bytes=mf_bytes, peak_source=pk_kind + ' hbm_gbs',
                                        note='protos fp16 read once + bit-packed [100,800,42] int32 masks written')
     line['roofline_mask_assembly']['other_family'] = dict(kernels=other['kernels'], ms=other['dense_ms'])
@@ -670,6 +683,8 @@ def main():
     ap.add_argument('--workload', default='A', choices=sorted(WORKLOADS))
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-library-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the result arrays of the last timed step to DIR/<name>.npy')
     ap.add_argument('--in-flight', type=int, default=int(os.environ.get('SMB_IN_FLIGHT', '0')),
                     help='forwards in flight per GPU (independent forwards on separate streams); 0 = the workload default, '
                          '1 = strictly serial')

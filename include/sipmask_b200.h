@@ -1,5 +1,5 @@
 /*
- * sipmask_b200 - C ABI of the B200-native SipMask inference hot path.
+ * sipmask_b200 - C ABI of the H100-native (sm_90a) SipMask inference hot path.
  *
  * Drop-in boundary (SURVEY.md §8b).  Every entry point replaces one native
  * (pybind) entry point or one python/ATen call sequence of the reference
@@ -33,14 +33,14 @@ typedef struct CUstream_st* smb_stream_t; /* == cudaStream_t */
 #define SMB_EINVAL (-1)   /* bad argument / unsupported shape */
 #define SMB_ECUDA (-2)    /* CUDA runtime / driver error      */
 #define SMB_EWORKSPACE (-3) /* workspace too small            */
-#define SMB_EARCH (-4)    /* device is not sm_100             */
+#define SMB_EARCH (-4)    /* device is not sm_90              */
 
 #define SMB_F32 0
 #define SMB_F16 1
 
 const char* smb_last_error(void);
 int smb_version(void);
-/* 0 if the current device can run the sm_100a kernels, SMB_EARCH otherwise. */
+/* 0 if the current device can run the sm_90a kernels, SMB_EARCH otherwise. */
 int smb_check_device(void);
 
 /* ------------------------------------------------------------------ mask assembly
@@ -216,14 +216,14 @@ int smb_track_step(const float* host_det, const int64_t* host_labels, const floa
 int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev,
                         int max_rows, int row_elems, float* dst, smb_stream_t stream);
 
-/* ------------------------------------------------------------------ convolution engine (tcgen05)
+/* ------------------------------------------------------------------ convolution engine (wgmma)
  * Replaces every nn.Conv2d (+ folded eval BatchNorm, bias, residual add, ReLU) on the path
  * (models/backbones/resnet.py:203-239, models/necks/fpn.py:138-178, ops/conv_module.py:124-132,
  * anchor_heads/sipmask_head.py:241-287) with one implicit-GEMM kernel:
  *   D[pixels, Cout] = sum_{taps, Cin} A[pixel + tap, Cin] * Wt[Cout, tap, Cin]
  * A is the NHWC fp16 activation read through TMA tensor maps (one 2D-patch box per tap; zero
  * fill outside the image gives the padding), W is [Cout, taps*Cin] fp16 K-major, the fp32
- * accumulator lives in TMEM (tcgen05.mma cta_group::1, M=128), the epilogue applies
+ * accumulators live in registers (two warpgroups of wgmma.m64nNk16, M=128), the epilogue applies
  * scale/bias (folded BN), residual, ReLU, optional GroupNorm statistics, and writes NHWC.
  */
 typedef struct smb_conv_plan smb_conv_plan_t;

@@ -6,7 +6,7 @@
     /root/reference exists (the build container); the GPU box uses the prebuilt file.
   * oracle/_ref/libsipmask_ref_cuda.so   - the reference's own CUDA kernels CropSplitKernelForward
     (ops/crop/src/crop_split_cuda_kernel.cu:19-88) and deformable_im2col_gpu_kernel
-    (ops/dcn/src/deform_conv_cuda_kernel.cu:84-277), compiled by plain nvcc for sm_100a from where they lie,
+    (ops/dcn/src/deform_conv_cuda_kernel.cu:84-277), compiled by plain nvcc for sm_90a from where they lie,
     through the wrappers in oracle/ref_cuda/ (shim headers stand in for ATen; no arithmetic there).  The GPU
     tests pin the oracle's restatement AND the smb kernels against them (tests/test_gpu_ref_cuda.py).
   * oracle/lib/liboracle_c.so            - plain-C restatement (oracle/csrc/oracle_c.c) of the
@@ -54,7 +54,7 @@ def build_ref_nms():
 
 
 def build_ref_cuda():
-    """nvcc -gencode arch=compute_100a,code=sm_100a on the reference's crop_split / deform_conv kernel sources (read in
+    """nvcc -gencode arch=compute_90a,code=sm_90a on the reference's crop_split / deform_conv kernel sources (read in
     place, never copied) -> oracle/_ref/libsipmask_ref_cuda.so.  Returns None when /root/reference is absent and no
     prebuilt file exists (the GPU box uses the prebuilt file that travels with the snapshot)."""
     os.makedirs(OUT, exist_ok=True)
@@ -71,11 +71,11 @@ def build_ref_cuda():
     objs = []
     for w, ref in units:
         obj = os.path.join(OUT, w[:-3] + '.o')
-        subprocess.check_call([NVCC, '-gencode', 'arch=compute_100a,code=sm_100a', '-O2', '-w', '-Xcompiler', '-fPIC',
+        subprocess.check_call([NVCC, '-gencode', 'arch=compute_90a,code=sm_90a', '-O2', '-w', '-Xcompiler', '-fPIC',
                                '-I', os.path.join(wrap, 'shim'), '-DREF_SRC="%s"' % ref, '-c', os.path.join(wrap, w),
                                '-o', obj])
         objs.append(obj)
-    subprocess.check_call([NVCC, '-shared', '-o', dst] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'])
+    subprocess.check_call([NVCC, '-shared', '-o', dst] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'])
     return dst
 
 

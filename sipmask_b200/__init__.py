@@ -1,4 +1,4 @@
-"""sipmask_b200 - B200-native (sm_100a) implementation of SipMask's per-image inference hot path.
+"""sipmask_b200 - H100-native (sm_90a) implementation of SipMask's per-image inference hot path.
 
 Public surface (mirrors the reference's operator / registry API, SURVEY.md §8b):
     sipmask_b200.ops        CropSplit, crop_split, nms, multiclass_nms_idx, fast_nms, mask_assemble, ...

@@ -1,13 +1,12 @@
 """ctypes loader for libsipmask_b200.so (the C ABI declared in include/sipmask_b200.h).
 
-There is NO fallback: if the library is missing or the device is not sm_100 every op raises.
+There is NO fallback: if the library is missing or the device is not sm_90 every op raises.
 """
 import ctypes
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# SMB_LIB_PATH: an instrumented build of the same sources (tools/build_trace_lib.sh), for profiling tools only
-LIB_PATH = os.environ.get('SMB_LIB_PATH') or os.path.join(HERE, 'lib', 'libsipmask_b200.so')
+LIB_PATH = os.path.join(HERE, 'lib', 'libsipmask_b200.so')
 
 F32, F16 = 0, 1
 

@@ -1,4 +1,4 @@
-"""In-tree build of libsipmask_b200.so (sm_100a only): nvcc cross-compiles without a GPU."""
+"""In-tree build of libsipmask_b200.so (sm_90a only): nvcc cross-compiles without a GPU."""
 import glob
 import os
 import subprocess
@@ -8,9 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'lib', 'libsipmask_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-Xptxas', '-v']
-FLAGS += os.environ.get('SMB_NVCC_EXTRA', '').split()       # e.g. -DSMB_TS_FINE for tools/conv_timeline.py (then build -f)
 
 
 def sources():
@@ -41,7 +40,7 @@ def build(verbose=False, force=False):
     for src, log, p in procs:
         rc = p.wait()
         log.close()
-        # keep the ptxas -v resource usage (tracked as evidence), drop the run-dependent timing lines
+        # keep the ptxas -v resource usage (registers / spills per kernel), drop the run-dependent timing lines
         kept = [l for l in open(log.name) if 'Compile time' not in l]
         open(log.name, 'w').writelines(kept)
         if rc != 0 or verbose:
@@ -50,7 +49,7 @@ def build(verbose=False, force=False):
             raise RuntimeError('nvcc failed on %s' % src)
     if rebuilt or not os.path.exists(LIB):
         tmp = LIB + '.tmp.so'                      # link next to the target, then rename: the library is never half-written
-        subprocess.check_call([NVCC, '-shared', '-o', tmp] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'])
+        subprocess.check_call([NVCC, '-shared', '-o', tmp] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'])
         os.replace(tmp, LIB)
     return LIB
 

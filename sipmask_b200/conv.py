@@ -1,4 +1,4 @@
-"""Host side of the tcgen05 convolution engine: weight packing (BN folding, K-major fp16) and plan objects.
+"""Host side of the wgmma convolution engine: weight packing (BN folding, K-major fp16) and plan objects.
 
 Reference modules replaced: nn.Conv2d (+ eval BatchNorm2d, bias, residual add, ReLU) in
 MM/mmdet/models/backbones/resnet.py:203-239, MM/mmdet/models/necks/fpn.py:138-178,

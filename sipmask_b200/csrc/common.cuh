@@ -1,4 +1,4 @@
-// Shared helpers for the sipmask_b200 CUDA sources (sm_100a only).
+// Shared helpers for the sipmask_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -72,8 +72,8 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  static int enabled = -1;                                  // SMB_PDL_AUX=1 turns the attribute on; measured SLOWER for the
-                                                            // elementwise / NMS kernels (r01: 639 vs 656 img/s), so off by default
+  static int enabled = -1;                                  // SMB_PDL_AUX=1 turns the attribute on for the elementwise / NMS
+                                                            // kernels; off by default
   if (enabled < 0) {
     const char* e = getenv("SMB_PDL_AUX");
     enabled = e ? atoi(e) : 0;

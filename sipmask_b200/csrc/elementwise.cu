@@ -1,4 +1,4 @@
-// Bandwidth-bound helper kernels around the tcgen05 convolution (all NHWC fp16 unless noted), sm_100a.
+// Bandwidth-bound helper kernels around the wgmma convolution (all NHWC fp16 unless noted), sm_90a.
 //
 // Reference (SipMask-mmdetection/mmdet/):
 //   ops/norm.py:43-49 + ops/conv_module.py:124-132            GroupNorm(32) + ReLU after tower convs
@@ -49,7 +49,7 @@ __global__ void gn_apply_kernel(__half* __restrict__ x, int n_img, int hw, int C
       const int c = v * 8 + j;
       const int g = c / cpg;
       // int64 -> fp32 with ONE rounding; the 2^-20 / 2^-16 scales are exact, so this equals the former double-precision
-      // product bit for bit without FP64 instructions (B200 issues those at a small fraction of the fp32 rate)
+      // product bit for bit without FP64 instructions (the GPU issues those at a fraction of the fp32 rate)
       const float s = __ll2float_rn(stats[((size_t)img * G + g) * 2]) * (1.0f / kGnSumScale);
       const float ss = __ll2float_rn(stats[((size_t)img * G + g) * 2 + 1]) * (1.0f / kGnSqScale);
       const float mean = s * inv_cnt;
@@ -376,8 +376,7 @@ __global__ void gn_apply_multi_kernel(MultiDesc d, int n_img, int C, int pitch, 
 // Same arithmetic, thread-stationary in the channel vector: a CTA owns kGnRows consecutive pixel rows of ONE (level, image),
 // a thread one 8-channel vector (v = tid % vecs) of every (256 / vecs)-th of those rows.  Level lookup, statistics (two
 // int64 loads, conversions, rsqrt) and gamma / beta (four 16-byte loads) are evaluated once per thread instead of once per
-// 16-byte vector (gn_apply_multi_kernel: ~150 instructions per vector, 67 % issue-bound at 10 us for 23 MB in the r02 ncu
-// capture); the row loop is a load, 8 x (sub, mul, fma, max), a store.  start[] holds the prefix of CTAs per level.
+// 16-byte vector (gn_apply_multi_kernel: ~150 instructions per vector, issue-bound); the row loop is a load, 8 x (sub, mul, fma, max), a store.  start[] holds the prefix of CTAs per level.
 constexpr int kGnRows = 64;
 __global__ void __launch_bounds__(256) gn_apply_rows_kernel(MultiDesc d, int n_img, int C, int pitch, const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, float eps, int relu) {

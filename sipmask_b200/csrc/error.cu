@@ -18,8 +18,8 @@ extern "C" int smb_check_device(void) {
   SMB_CUDA_OK(cudaGetDevice(&dev));
   cudaDeviceProp p;
   SMB_CUDA_OK(cudaGetDeviceProperties(&p, dev));
-  if (p.major != 10) {
-    smb::set_error("device %d is sm_%d%d; this library contains sm_100a code only", dev, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    smb::set_error("device %d is sm_%d%d; this library contains sm_90a code only", dev, p.major, p.minor);
     return SMB_EARCH;
   }
   return SMB_OK;

@@ -1,4 +1,4 @@
-// Fused SipMask mask assembly for sm_100a.
+// Fused SipMask mask assembly for sm_90a.
 //
 // Reference (SipMask-mmdetection/mmdet/):
 //   models/anchor_heads/sipmask_head.py:609-633   4x sgemm -> 4x sigmoid -> stack -> CropSplit -> permute
@@ -591,8 +591,8 @@ __device__ __forceinline__ void run_values(const float (&acc)[4], const BoxP& b,
 // keeping the row's 32 fragment registers live cost a CTA per SM).
 // Tile = TH_ rows x TW_ pixels, TH_ * TW_ = 512 (8 x 64, 4 x 128 or 2 x 256): a warp owns one 64-pixel segment of one
 // tile row; wider tiles make the zero / value stores of a detection longer contiguous runs (256 / 512 / 1024 bytes).
-// 64 registers: four CTAs per SM, so the 550 - 600 CTAs of a 400 x 672 prototype map are ONE wave (at 80 registers the
-// second wave ran on a quarter of the SMs and the kernel took as long as the scalar one, profiles/r02_ncu_mask_mma_v1_summary.txt).
+// 64 registers: four CTAs per SM (528 slots on 132 SMs for the 550 - 600 CTAs of a 400 x 672 prototype map; at three CTAs
+// per SM the second wave would run on a fraction of the SMs).
 template <bool HWC, typename OT, int TH_, int TW_>
 __global__ void __launch_bounds__(MA_THREADS2, 4) mask_assemble_mma_kernel(
     const __half* __restrict__ protos, const float* __restrict__ cofs, const float* __restrict__ boxes,
@@ -1178,7 +1178,7 @@ extern "C" int smb_crop_split_forward(const void* data, const void* rois, void* 
   SMB_CHECK_ARG(H > 0 && W > 0 && N >= 0, "smb_crop_split_forward: bad shape");
   const long long count = (long long)H * W * N;
   if (count == 0) return SMB_OK;
-  const int blocks = (int)min((long long)148 * 16, (count + 255) / 256);
+  const int blocks = (int)min((long long)132 * 16, (count + 255) / 256);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == SMB_F32)
     crop_split_kernel<float><<<blocks, 256, 0, st>>>((const float*)data, (const float*)rois, (float*)out, count, H, W, N);
@@ -1197,7 +1197,7 @@ extern "C" int smb_crop_split_backward(const void* top_grad, const void* rois, v
   SMB_CHECK_ARG(H > 0 && W > 0 && N >= 0, "smb_crop_split_backward: bad shape");
   const long long count = (long long)H * W * N;
   if (count == 0) return SMB_OK;
-  const int blocks = (int)min((long long)148 * 16, (count + 255) / 256);
+  const int blocks = (int)min((long long)132 * 16, (count + 255) / 256);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == SMB_F32)
     crop_split_backward_kernel<float><<<blocks, 256, 0, st>>>((const float*)top_grad, (const float*)rois, (float*)bottom_grad, count, H, W, N);
@@ -1215,7 +1215,7 @@ extern "C" int smb_crop_split_gt(const void* data, const void* rois, void* out, 
   SMB_CHECK_ARG(H > 0 && W > 0 && N >= 0, "smb_crop_split_gt: bad shape");
   const long long count = (long long)H * W * N;
   if (count == 0) return SMB_OK;
-  const int blocks = (int)min((long long)148 * 16, (count + 255) / 256);
+  const int blocks = (int)min((long long)132 * 16, (count + 255) / 256);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == SMB_F32)
     crop_mask_kernel<float><<<blocks, 256, 0, st>>>((const float*)data, (const float*)rois, (float*)out, count, H, W, N);

@@ -1,4 +1,4 @@
-// Device-side detection post-processing for sm_100a: per-level top-k + box decode, single-class NMS,
+// Device-side detection post-processing for sm_90a: per-level top-k + box decode, single-class NMS,
 // batched multi-class NMS, fast NMS.  No host synchronisation, no D2H copies.
 //
 // Reference (SipMask-mmdetection/mmdet/):
@@ -889,7 +889,7 @@ extern "C" int smb_multiclass_nms(const float* boxes, const float* scores, const
                                                                    (float*)(ws + w.cscore), (unsigned long long*)(ws + w.keys),
                                                                    (float4*)(ws + w.sbox), (int*)(ws + w.m)));
     SMB_LAUNCH_OK("mc_prepare_kernel");
-    SMB_CUDA_OK(launch_pdl(mc_mask_kernel, dim3(148 * 16), dim3(64), 0, st, (const float4*)(ws + w.sbox), (const int*)(ws + w.m), n, num_classes, nbmax, iou_thr,
+    SMB_CUDA_OK(launch_pdl(mc_mask_kernel, dim3(132 * 16), dim3(64), 0, st, (const float4*)(ws + w.sbox), (const int*)(ws + w.m), n, num_classes, nbmax, iou_thr,
                                             cmp_ge, (unsigned long long*)(ws + w.mask)));
     SMB_LAUNCH_OK("mc_mask_kernel");
     SMB_CUDA_OK(launch_pdl(mc_sweep_kernel, dim3(num_classes), dim3(NT), 0, st, (const unsigned long long*)(ws + w.mask), (const unsigned long long*)(ws + w.keys),
@@ -962,14 +962,14 @@ extern "C" int smb_decode_topk(int num_levels, const smb_level_t* host_levels, i
   float* s = (float*)workspace;
   int* sel = (int*)((char*)workspace + s_bytes);
   const int total = L.loc_off[L.num];
-  SMB_CUDA_OK(launch_pdl(level_score_kernel, dim3(min(cdiv(total, 8), 148 * 8)), dim3(256), 0, st, L, num_classes, s));
+  SMB_CUDA_OK(launch_pdl(level_score_kernel, dim3(min(cdiv(total, 8), 132 * 8)), dim3(256), 0, st, L, num_classes, s));
   SMB_LAUNCH_OK("level_score_kernel");
   SMB_CUDA_OK(launch_pdl(level_topk_kernel, dim3(num_levels), dim3(NT), 0, st, L, nms_pre, s, sel));
   SMB_LAUNCH_OK("level_topk_kernel");
   const int ncand = L.cand_off[L.num];
   const float i0 = host_scale4 ? host_scale4[0] : 1.f, i1 = host_scale4 ? host_scale4[1] : 1.f;
   const float i2 = host_scale4 ? host_scale4[2] : 1.f, i3 = host_scale4 ? host_scale4[3] : 1.f;
-  SMB_CUDA_OK(launch_pdl(gather_decode_kernel, dim3(min(cdiv(ncand, 8), 148 * 8)), dim3(256), 0, st, L, num_classes, img_h, img_w, i0, i1, i2, i3,
+  SMB_CUDA_OK(launch_pdl(gather_decode_kernel, dim3(min(cdiv(ncand, 8), 132 * 8)), dim3(256), 0, st, L, num_classes, img_h, img_w, i0, i1, i2, i3,
                                                                     host_scale4 ? 1 : 0, sel, cand_boxes, cand_scores,
                                                                     cand_ctr, cand_loc));
   SMB_LAUNCH_OK("gather_decode_kernel");

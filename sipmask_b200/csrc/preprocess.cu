@@ -122,7 +122,7 @@ static int preprocess_impl(const uint8_t* src, int src_h, int src_w, int src_pit
   a.m0 = host_mean3[0]; a.m1 = host_mean3[1]; a.m2 = host_mean3[2];
   const long long total = s2d ? (long long)(H / 2 + 3) * (W / 2 + 4) : (long long)(H + 6) * (W + 8);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (s2d) preprocess_u8_s2d_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, (__half*)out, H, W);
   else preprocess_u8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, (__half*)out, H, W);
   SMB_LAUNCH_OK("preprocess_u8_kernel");

@@ -86,7 +86,7 @@ extern "C" int smb_conv3x3s2_relu_f32(const float* in, const float* weight, cons
   const int Ho = (H - 3) / 2 + 1, Wo = (W - 3) / 2 + 1;
   const long long total = (long long)N * Ho * Wo;
   int bx = (int)((total + 127) / 128);
-  if (bx > 148 * 32) bx = 148 * 32;
+  if (bx > 132 * 32) bx = 132 * 32;
   dim3 grid(bx, (Cout + RS_CO - 1) / RS_CO);
   const size_t smem = (size_t)RS_CO * Cin * 9 * sizeof(float);
   static bool attr_done = false;

@@ -3,8 +3,8 @@
 // Replaces the per-frame tail of SipMaskHead.get_bboxes in SipMask-VIS
 // (SipMask-VIS/mmdet/models/anchor_heads/sipmask_head.py:612-667, compute_comp_scores :544-562, bbox_overlaps
 // core/bbox/geometry.py:4-63).  The association is sequential in frame order and tiny (<= 10 detections x a few dozen tracked
-// objects); in python/numpy it costs ~150 us per frame, which at 8 GPUs x 2600 frames/s per GPU is the bottleneck of the
-// whole clip (r2: 11.2 k instead of 21 k frames/s).  Here it is ~2 us per frame.
+// objects); in python/numpy it costs ~150 us of host time per frame, which caps a clip sharded over several GPUs at a few
+// thousand frames/s.  Here it is ~2 us per frame.
 //
 //   comp[i][0]   = logsoftmax_i[0] + c0*log(score_i)            + c2            (dummy column: IoU 0, label match 1)
 //   comp[i][j+1] = logsoftmax_i[j+1] + c0*log(score_i) + c1*IoU(det_i, prev_j) + c2*[label_i == prev_label_j]

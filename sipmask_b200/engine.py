@@ -1,4 +1,4 @@
-"""SipMask inference engine: the whole per-image hot path as a fixed sequence of sm_100a kernel launches.
+"""SipMask inference engine: the whole per-image hot path as a fixed sequence of sm_90a kernel launches.
 
     image (NCHW fp32) -> NHWC8 fp16 -> ResNet-50/101 (caffe, folded BN) -> FPN P3..P7 -> FCOS towers (conv+GN+ReLU)
     -> FeatureAlign (DCN) -> cls/centerness/reg/coefficient heads -> prototype branch -> decode/top-k -> NMS ->
@@ -324,9 +324,9 @@ class SipMaskEngine(object):
         self.level_views = list(zip(clscof_l, regctr_l))
         si = 0
         cls_feats, reg_feats = list(feats), list(feats)
-        # The cls and reg towers are independent chains of 202-tile GEMMs (1.36 waves each on 148 SMs).  They are
+        # The cls and reg towers are independent chains of 202-tile GEMMs (1.5 waves each on 132 SMs).  They are
         # captured on two streams with their persistent grids capped at half the GPU, so together they keep every SM
-        # busy (2.73 waves for a pair instead of 2 + 2).
+        # busy (3.06 waves for a pair instead of 2 + 2).
         two = self.two_streams
         if two:
             self._marker('fork')

@@ -1,4 +1,4 @@
-"""Drop-in heads with the reference's registry / module API, computed by the sm_100a kernels.
+"""Drop-in heads with the reference's registry / module API, computed by the sm_90a kernels.
 
     SipMaskHead  <- MM/mmdet/models/anchor_heads/sipmask_head.py:107-287,500-662
     FCOSHead     <- MM/mmdet/models/anchor_heads/fcos_head.py:15-135,190-291
@@ -10,7 +10,7 @@ Same constructor keywords, same parameter names (a reference checkpoint `load_st
 `SingleStageDetector.simple_test` (MM/mmdet/models/detectors/single_stage.py:75-93).
 
 The nn.Conv2d / nn.GroupNorm members only hold parameters; nothing here calls their forward.  Inference only:
-`loss()` raises (training stays with the reference implementation).  CUDA sm_100 required - no CPU path.
+`loss()` raises (training stays with the reference implementation).  CUDA sm_90 required - no CPU path.
 """
 import numpy as np
 import torch

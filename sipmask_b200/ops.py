@@ -6,7 +6,7 @@ and `mmdet.core` entry points, backed by the C ABI (PyTorch tensors in, PyTorch 
   multiclass_nms_idx       <- MM/mmdet/core/post_processing/bbox_nms.py:79-146
   fast_nms                 <- MM/mmdet/models/anchor_heads/sipmask_head.py:868-910
   mask_assemble            <- MM/mmdet/models/anchor_heads/sipmask_head.py:609-627 (fused)
-All tensors must be CUDA tensors on an sm_100 device; there is no CPU path.
+All tensors must be CUDA tensors on an sm_90 device; there is no CPU path.
 """
 import ctypes
 
@@ -493,7 +493,7 @@ class DeformConv(nn.Module):
     `weight` parameter ([out, in, kh, kw], uniform(-1/sqrt(fan_in), +)), `forward(x[N,C,H,W], offset[N,dg*2*k*k,H,W])`.
 
     Replaces deform_conv_cuda.deform_conv_forward_cuda (ops/dcn/src/deform_conv_cuda.cpp:152-260: im2col kernel + addmm)
-    by `smb_deform_im2col` (channel-last bilinear gather, fp16 columns) + the tcgen05 GEMM (fp32 accumulate).  The hot
+    by `smb_deform_im2col` (channel-last bilinear gather, fp16 columns) + the wgmma GEMM (fp32 accumulate).  The hot
     path only uses 3x3 / stride 1 / padding 1 / dilation 1 / groups 1 (FeatureAlign `conv_adaption`, sipmask_head.py:35-41,
     and DeformConvPack in the ++ backbone, resnet.py:146-168); other geometries raise.  NCHW in, NCHW out, x.dtype kept."""
 

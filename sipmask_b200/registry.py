@@ -1,4 +1,4 @@
-"""Registry hook: make `type='SipMaskHead'` / `type='FCOSHead'` in an mmdetection config build the sm_100a heads.
+"""Registry hook: make `type='SipMaskHead'` / `type='FCOSHead'` in an mmdetection config build the sm_90a heads.
 
 The reference registers its heads with `@HEADS.register_module` (MM/mmdet/models/anchor_heads/sipmask_head.py:107-108,
 MM/mmdet/utils/registry.py:24-48); duplicate names raise KeyError unless `force=True` (registry.py:39-42).
@@ -16,7 +16,7 @@ def register(force=True):
 
 
 def register_ops(force=True):
-    """Point `mmdet.ops.{CropSplit, DeformConv, nms}` at the sm_100a operators (same call signatures;
+    """Point `mmdet.ops.{CropSplit, DeformConv, nms}` at the sm_90a operators (same call signatures;
     MM/mmdet/ops/__init__.py:5-22 exports)."""
     import mmdet.ops as mmops
     from . import ops

@@ -2,12 +2,12 @@
 
 The reference moves data synchronously: `scatter` uploads the image (MM/mmdet/apis/inference.py:83) and every detection's
 mask is copied back one by one (`masks[i].cpu().numpy()`, sipmask_head.py:645-657).  Here the upload of image i+1 and
-the download of result i-1 run on their own streams (the B200 has independent H2D / D2H copy engines) while the
+the download of result i-1 run on their own streams (the GPU has independent H2D / D2H copy engines) while the
 CUDA-graph replay of image i runs on a compute stream; device staging buffers decouple the three.
 Per image: one 12.9 MB H2D (fp32 NCHW 800x1344) and one 13.4 MB D2H (fixed-shape record + bit-packed masks).
 
 Images in flight.  One 800x1344 image is ~75 short convolution launches, most of them latency-bound chains that leave
-SMs idle (layer3/4 have 33 / 9 M-tiles for 148 SMs).  `make_engines(..., in_flight=n)` builds n engines that share ONE
+SMs idle (layer3/4 have 33 / 9 M-tiles for 132 SMs).  `make_engines(..., in_flight=n)` builds n engines that share ONE
 copy of the packed weights but own their activations and CUDA graph; `EnginePool` / `PipelinedRunner` replay them
 round-robin on n streams with the persistent conv grids capped (64 CTAs), so the images fill each other's bubbles.
 Every forward is still one image (imgs_per_gpu == 1, base.py:118-119); only the throughput changes.
@@ -17,7 +17,7 @@ import torch
 from . import conv as C
 from .engine import SipMaskEngine
 
-# tuning measured on B200 (profiles/r01_inflight_sweep.txt): grid cap / planner min_tiles per number of images in flight
+# grid cap / planner min_tiles per number of images in flight
 _TUNING = {1: dict(max_ctas=None, head_max_ctas=None, min_tiles=48)}
 
 

@@ -35,13 +35,13 @@ def test_ops_fail_loudly_without_cuda():
         ops.mask_assemble(torch.zeros(32, 4, 4), torch.zeros(1, 128), torch.zeros(1, 4), 0.5)
 
 
-def test_sass_contains_blackwell_instructions():
-    """The conv kernel must be real tcgen05/TMA code (B200_PROFILING.md 'What proves a Blackwell-native kernel')."""
+def test_sass_contains_hopper_instructions():
+    """The conv kernel must be real wgmma / TMA code: warpgroup MMAs (HGMMA) fed by tensor-memory-accelerator loads."""
     import shutil
     import subprocess
     from sipmask_b200 import build
     if shutil.which('cuobjdump') is None:
         pytest.skip('cuobjdump not available')
     sass = subprocess.run(['cuobjdump', '-sass', build.LIB], capture_output=True, text=True).stdout
-    for mnemonic in ('UTCHMMA', 'UTMALDG', 'LDTM'):
+    for mnemonic in ('HGMMA', 'UTMALDG', 'WARPGROUP.ARRIVE'):
         assert mnemonic in sass, mnemonic

@@ -1,4 +1,4 @@
-"""GPU parity tests for the tcgen05 implicit-GEMM convolution and the NHWC helper kernels (run with -m gpu).
+"""GPU parity tests for the wgmma implicit-GEMM convolution and the NHWC helper kernels (run with -m gpu).
 References are plain PyTorch ops in float64 on the fp16-rounded operands (the fp32-accumulating tensor-core result
 must then agree to fp16 output rounding)."""
 import numpy as np
@@ -50,8 +50,8 @@ def _check(out, ref, tol=2e-3):
     (25, 42, 512, 128, 1, 1),
     (20, 20, 768, 512, 1, 1),       # sip_mask_lat0
     (9, 5, 2304, 256, 1, 1),        # DCN GEMM (K = 9*256)
-    (104, 208, 256, 256, 3, 1),     # 169 M-tiles (odd): 2-CTA clusters multicast the weight tile, last cluster has a dummy CTA
-    (200, 336, 64, 256, 1, 1),      # layer1 conv3 shape: 525 M-tiles, one k-block, cluster path
+    (104, 208, 256, 256, 3, 1),     # 169 M-tiles: more tiles than SMs, uneven last wave
+    (200, 336, 64, 256, 1, 1),      # layer1 conv3 shape: 525 M-tiles, one k-block
     (120, 160, 128, 512, 3, 1),     # 2 N-tiles x 150 M-tiles
 ])
 def test_conv_matches_reference(H, W, cin, cout, k, stride):
@@ -67,7 +67,7 @@ def test_conv_matches_reference(H, W, cin, cout, k, stride):
     torch.cuda.synchronize()
     assert torch.isfinite(out.float()).all()
     _check(out, _ref_conv(x, wk, k, stride))
-    # running twice must give the same answer (barrier phases / TMEM reuse)
+    # running twice must give the same answer (barrier phases of the persistent pipeline)
     out2 = out.clone()
     plan.run()
     torch.cuda.synchronize()
@@ -273,39 +273,12 @@ def test_multi_level_conv_and_helpers_match_single_level():
         assert (c1.float() - cols[i].float()).abs().max().item() <= 2e-3 * (c1.float().abs().max().item() + 1), i
 
 
-@pytest.mark.parametrize('H,W,cin,cout,stride,res', [(200, 336, 64, 256, 1, True), (50, 84, 256, 512, 2, False),
-                                                     (13, 21, 256, 2048, 1, True), (8, 160, 128, 256, 1, False)])
-def test_small_1x1_kernel_matches_persistent_kernel(H, W, cin, cout, stride, res, monkeypatch):
-    """conv1x1_small_kernel (one 128 x 128 tile per CTA, 2-3 CTAs per SM; SMB_CONV_SMALL=1) is an alternative execution of the
-    short-K 1x1 convolutions: bit-identical to the persistent kernel (same MMA order over K, same epilogue arithmetic)."""
+def _bias_residual_relu_variants(H, W, cin, cout, k, stride, res, seed, variants):
+    """One convolution with the fused epilogue (acc + bias, + residual, ReLU, round to fp16) under several planner settings
+    (min_tiles, max_ctas): every variant is bit-identical to the first (the per-element arithmetic and the K order do not
+    depend on the tiling or the schedule), and the result equals the float64 reference to fp16 output rounding."""
     from sipmask_b200 import conv
-    g = torch.Generator().manual_seed(H + cout)
-    x = _nhwc(torch.randn(1, cin, H, W, generator=g))
-    w = torch.randn(cout, cin, 1, 1, generator=g) / (cin ** 0.5)
-    wk, _ = conv.pack_weight(w, device='cuda')
-    bias = torch.randn(cout, generator=g).cuda()
-    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    r = _nhwc(torch.randn(1, cout, Ho, Wo, generator=g)) if res else None
-    outs = []
-    for small in ('0', '1'):
-        monkeypatch.setenv('SMB_CONV_SMALL', small)
-        out = torch.zeros((1, Ho, Wo, cout), dtype=torch.float16, device='cuda')
-        conv.ConvPlan(x, wk, out, 1, stride, relu=True, bias=bias, residual=r).run()
-        torch.cuda.synchronize()
-        outs.append(out)
-    assert torch.equal(outs[0], outs[1])
-    _check(outs[1], _ref_conv(x, wk, 1, stride, bias=bias, residual=r, relu=True))
-
-
-@pytest.mark.parametrize('H,W,cin,cout,k,stride,res', [(200, 336, 64, 256, 1, 1, True), (100, 168, 256, 64, 1, 1, False),
-                                                       (50, 84, 256, 512, 1, 2, False), (25, 42, 256, 256, 3, 1, False),
-                                                       (13, 21, 512, 2048, 1, 1, True), (37, 53, 128, 128, 3, 1, False)])
-def test_split_epilogue_matches_lockstep_epilogue(H, W, cin, cout, k, stride, res, monkeypatch):
-    """epilogue_split (the two warp groups drain alternate 64-channel chunks) against the lockstep epilogue of the same kernel
-    (SMB_CONV_EPI_SPLIT=0): the per-element arithmetic (acc + bias, + residual, ReLU, round) is the same sequence, so the
-    outputs are bit-identical."""
-    from sipmask_b200 import conv
-    g = torch.Generator().manual_seed(H * 3 + cout + k)
+    g = torch.Generator().manual_seed(seed)
     x = _nhwc(torch.randn(1, cin, H, W, generator=g))
     w = torch.randn(cout, cin, k, k, generator=g) / ((cin * k * k) ** 0.5)
     wk, _ = conv.pack_weight(w, device='cuda')
@@ -313,12 +286,36 @@ def test_split_epilogue_matches_lockstep_epilogue(H, W, cin, cout, k, stride, re
     Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
     r = _nhwc(torch.randn(1, cout, Ho, Wo, generator=g)) if res else None
     outs = []
-    for split in ('0', '1'):
-        monkeypatch.setenv('SMB_CONV_EPI_SPLIT', split)
+    for min_tiles, max_ctas in variants:
         out = torch.zeros((1, Ho, Wo, cout), dtype=torch.float16, device='cuda')
-        conv.ConvPlan(x, wk, out, k, stride, relu=True, bias=bias, residual=r).run()
+        prev = conv.set_min_tiles(min_tiles)
+        try:
+            plan = conv.ConvPlan(x, wk, out, k, stride, relu=True, bias=bias, residual=r)
+        finally:
+            conv.set_min_tiles(prev)
+        if max_ctas:
+            plan.set_max_ctas(max_ctas)
+        plan.run()
         torch.cuda.synchronize()
         outs.append(out)
     for o in outs[1:]:
         assert torch.equal(outs[0], o)
     _check(outs[0], _ref_conv(x, wk, k, stride, bias=bias, residual=r, relu=True))
+
+
+@pytest.mark.parametrize('H,W,cin,cout,stride,res', [(200, 336, 64, 256, 1, True), (50, 84, 256, 512, 2, False),
+                                                     (13, 21, 256, 2048, 1, True), (8, 160, 128, 256, 1, False)])
+def test_small_1x1_kernel_matches_persistent_kernel(H, W, cin, cout, stride, res):
+    """Short-K 1x1 convolutions (ResNet conv1 / conv3 / shortcut, K <= 256: one to four k-blocks per tile) with bias,
+    residual and ReLU: the full grid (one CTA per SM, at most a few tiles each) against 7 persistent CTAs that each loop over
+    many tiles, so the operand ring wraps across tile boundaries and the producer runs ahead into the next tile."""
+    _bias_residual_relu_variants(H, W, cin, cout, 1, stride, res, H + cout, [(48, None), (48, 7)])
+
+
+@pytest.mark.parametrize('H,W,cin,cout,k,stride,res', [(200, 336, 64, 256, 1, 1, True), (100, 168, 256, 64, 1, 1, False),
+                                                       (50, 84, 256, 512, 1, 2, False), (25, 42, 256, 256, 3, 1, False),
+                                                       (13, 21, 512, 2048, 1, 1, True), (37, 53, 128, 128, 3, 1, False)])
+def test_split_epilogue_matches_lockstep_epilogue(H, W, cin, cout, k, stride, res):
+    """The epilogue split over 64-channel N tiles (each CTA drains one 64-column slice of the output channels) against the
+    widest N tile the plan allows (one CTA drains 128 / 256 columns together), on the bottleneck / shortcut / tower shapes."""
+    _bias_residual_relu_variants(H, W, cin, cout, k, stride, res, H * 3 + cout + k, [(1, None), (1 << 30, None)])

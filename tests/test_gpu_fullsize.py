@@ -13,8 +13,7 @@ tests/test_gpu_engine.py covers):
 Stated tolerance: labels of matched pairs are equal by construction; matched fraction >= 0.95; box L-inf <= 1.0 px; score
 |diff| <= 2e-3; head outputs relative L2 <= 5e-3; mask IoU over matches: pooled (sum of intersections / sum of unions) >= 0.995,
 mean >= 0.99, min >= 0.80 (the minimum is set by masks of a few dozen pixels, where one threshold flip costs several percent).
-Measured on B200 (r2, gpurun_out/parity_fullsize_*.json -> profiles/r02_parity_fullsize.json): matched 98-100 %, box L-inf
-0.03-0.35 px, score diff <= 4e-4, head rel-L2 <= 2.2e-3, mean mask IoU 0.9965-0.9970, min 0.875 / 0.947 / 0.989.  (north_star's "mask IoU >= 0.999, indices
+(The post-processing's "mask IoU >= 0.999, indices
 bit-exact" holds for the post-processing given identical head outputs - tests/test_gpu_postproc.py, test_gpu_engine.py; an
 fp16 backbone cannot reproduce an fp32 one bit for bit, so near-tie candidates at the max_per_img / NMS boundaries differ.)
 """

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): CUDA post-processing kernels, called through the
+"""GPU parity tests (run with -m gpu on an H100): CUDA post-processing kernels, called through the
 C ABI, against the CPU oracle on the same seeded inputs and against the reference-generated fixtures."""
 import os
 

@@ -107,35 +107,3 @@ def test_fp16_hi_lo_coefficient_split_keeps_fp32_logits():
             seq = seq + p[:, k].astype(np.float32) * cc[:, k]
         assert (np.abs(seq.astype(np.float64) - exact) <= bound).all(), scale
 
-
-def test_bench_traffic_json_derives_from_the_committed_ncu_capture():
-    """bench.py fills roofline_mask_*.traffic from profiles/r02_ncu_traffic.json; those entries must be the per-launch
-    dram__bytes of the committed `ncu --set full` export of the same kernels (profiles/r02_ncu_mask_mma_raw.csv)."""
-    import csv
-    import json
-    prof = os.path.join(ROOT, 'profiles')
-    rows = list(csv.reader(open(os.path.join(prof, 'r02_ncu_mask_mma_raw.csv'))))
-    hdr, units = rows[0], rows[1]
-    idx = {h: i for i, h in enumerate(hdr)}
-    scale = {'byte': 1.0, 'kbyte': 1e3, 'mbyte': 1e6, 'gbyte': 1e9}
-
-    def launches(pattern):
-        out = []
-        for r in rows[2:]:
-            if len(r) == len(hdr) and pattern in r[idx['Kernel Name']]:
-                rd = float(r[idx['dram__bytes_read.sum']].replace(',', '')) * scale[units[idx['dram__bytes_read.sum']].lower()]
-                wr = float(r[idx['dram__bytes_write.sum']].replace(',', '')) * scale[units[idx['dram__bytes_write.sum']].lower()]
-                regs = int(float(r[idx['launch__registers_per_thread']]))
-                out.append((rd, wr, regs))
-        return out
-
-    traffic = json.load(open(os.path.join(prof, 'r02_ncu_traffic.json')))
-    for key, pattern in (('mask_assemble', 'mask_assemble_mma_kernel'), ('mask_fused', 'mask_fused_pack_mma_kernel')):
-        ls = launches(pattern)
-        assert ls and all(regs == 64 for _, _, regs in ls)                       # the product build: four CTAs per SM
-        e = traffic[key]
-        assert pattern in e['kernel']
-        assert min(rd for rd, _, _ in ls) * 0.98 <= e['dram_read_bytes'] <= max(rd for rd, _, _ in ls) * 1.02
-        assert min(rd + wr for rd, wr, _ in ls) * 0.95 <= e['dram_bytes_per_launch'] <= max(rd + wr for rd, wr, _ in ls) * 1.05
-        # reads = the fp16 prototype map (400 x 672 x 32 x 2 bytes) plus coefficients / boxes: no wasted re-reads
-        assert 17.0e6 <= e["dram_read_bytes"] <= 19.0e6
