@@ -111,7 +111,7 @@ int smb_mask_assemble_pack(const void* protos, int protos_dtype, int layout_hwc,
 /* fp16 prototypes run the tensor-core variants of smb_mask_assemble / smb_mask_assemble_pack (mma.sync dot products with
  * the fp32 coefficients split into fp16 hi + lo; same crop geometry, mask values within ~1e-6 of the scalar kernels).
  * on = 1 / 0 selects them / the scalar-fmaf kernels for later calls, on < 0 only queries; returns the previous setting
- * (initial value: environment SMB_MASK_MMA, else the build default). */
+ * (initial value: 1).  fp32 prototypes always run the scalar kernels. */
 int smb_mask_set_tensor_dot(int on);
 
 /* ------------------------------------------------------------------ CropSplit (operator API)
@@ -229,7 +229,7 @@ int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, con
 typedef struct smb_conv_plan smb_conv_plan_t;
 
 typedef struct {
-  int N, H, W, Cin;          /* input  NHWC (Cin % 64 == 0, or Cin == 8-padded stem handled internally) */
+  int N, H, W, Cin;          /* input  NHWC (Cin % 64 == 0; the 3-channel stem uses smb_stem_plan_create_s2d) */
   int Cout;                  /* multiple of 16, <= 256 per N-tile (larger Cout is tiled) */
   int kh, kw, stride, pad;   /* 1x1/3x3 stride 1|2, pad = k/2 ; 7x7/2 stem uses the dedicated plan */
   int relu;                  /* apply ReLU in the epilogue */
@@ -288,7 +288,8 @@ int smb_offset_conv1x1(const float* bbox, int bbox_pitch, float scale, const flo
                        long long npix, smb_stream_t stream);
 
 /* Multi-level (batched over feature-pyramid levels, shared parameters) variants of the three kernels above:
- * one launch instead of one per level.  Pointer arrays are HOST arrays of device pointers. */
+ * one launch instead of one per level.  Pointer arrays are HOST arrays of device pointers.
+ * smb_groupnorm_relu_apply_multi supports C in {256, 512, 1024, 2048} (SMB_EINVAL otherwise). */
 int smb_groupnorm_relu_apply_multi(int num_levels, void* const* xs, const void* const* stats, const int* Hs, const int* Ws,
                                    int n_img, int C, int pitch, const float* gamma, const float* beta, float eps, int relu,
                                    smb_stream_t stream);
@@ -307,27 +308,22 @@ int smb_maxpool3x3s2(const void* x, void* y, int N, int H, int W, int C, smb_str
 int smb_upsample_bilinear(const void* x, int in_pitch, void* y, int out_pitch, int out_choff,
                           int N, int H, int W, int C, int factor, int relu, smb_stream_t stream);
 
-/* Image preparation: NCHW fp32 -> zero-padded NHWC8 fp16 [N, H+6, W+8, 8] for the 7x7/2 stem. */
-int smb_image_to_nhwc8(const float* img, void* out, int N, int H, int W, smb_stream_t stream);
+/* Stem 7x7/2 conv (3->64) + folded BN + ReLU (backbones/resnet.py:448-460) in space-to-depth form (K = 256): the
+ * zero-padded image (pixel (y,x) at (y+3, x+3)) is stored as [N, H/2+3, W/2+4, 16] fp16 with element
+ * (Y, X, (dy*2+dx)*4 + c) = padded pixel (2Y+dy, 2X+dx) channel c (c == 3: zero), the weights as [64, 4*64] with
+ * K = a*64 + b*16 + (dy*2+dx)*4 + c for filter tap (r, s) = (2a+dy, 2b+dx). */
+int smb_stem_plan_create_s2d(int N, int H, int W, const void* img_s2d16, const void* weight256, void* out,
+                             smb_conv_plan_t** plan_out);
+/* Image preparation: NCHW fp32 -> the stem's space-to-depth input above (H, W even). */
+int smb_image_to_s2d16(const float* img_nchw_f32, void* out_s2d16, int N, int H, int W, smb_stream_t stream);
 
 /* Test-time image pipeline on the device (SURVEY.md 8f-3; transforms.py:97-110 Resize(keep_ratio), :335-363 Normalize
  * (std = 1, to_rgb = False), :274-300 Pad(32); mmcv.imrescale -> cv2.resize(INTER_LINEAR) restated bit-exactly):
  *   src       : uint8 BGR HWC [src_h, src_w, 3] device image, row pitch in bytes
  *   dst_h/w   : resized size (mmcv rule: int(h * s + 0.5), s = min(max_long / max(h, w), max_short / min(h, w)))
- *   out_nhwc8 : the stem's input [H+6, W+8, 8] fp16 (pixel (y,x) at (y+3, x+3)), H x W = padded size >= dst; everything
- *               outside the resized image is zero (= zero padding AFTER mean subtraction, as in the reference) */
-int smb_preprocess_u8(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
-                      const float* host_mean3, void* out_nhwc8, int H, int W, smb_stream_t stream);
-
-/* Stem 7x7/2 conv (3->64) + folded BN + ReLU on the padded NHWC8 image (backbones/resnet.py:448-460). */
-int smb_stem_plan_create(int N, int H, int W, const void* img_nhwc8, const void* weight448, void* out,
-                         smb_conv_plan_t** plan_out);
-/* Space-to-depth form of the same stem (K = 256 instead of 448): the image is stored as [N, H/2+3, W/2+4, 16] fp16 with
- * element (Y, X, (dy*2+dx)*4 + c) = padded pixel (2Y+dy, 2X+dx) channel c (smb_image_to_s2d16 / smb_preprocess_u8_s2d), the
- * weights as [64, 4*64] with K = a*64 + b*16 + (dy*2+dx)*4 + c for filter tap (r, s) = (2a+dy, 2b+dx). */
-int smb_stem_plan_create_s2d(int N, int H, int W, const void* img_s2d16, const void* weight256, void* out,
-                             smb_conv_plan_t** plan_out);
-int smb_image_to_s2d16(const float* img_nchw_f32, void* out_s2d16, int N, int H, int W, smb_stream_t stream);
+ *   out_s2d16 : the stem's space-to-depth input [H/2+3, W/2+4, 16] fp16 of the padded H x W image (H, W even, padded
+ *               size >= dst); everything outside the resized image is zero (= zero padding AFTER mean subtraction, as in
+ *               the reference) */
 int smb_preprocess_u8_s2d(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
                           const float* host_mean3, void* out_s2d16, int H, int W, smb_stream_t stream);
 

@@ -44,7 +44,7 @@ SYMBOLS = [
     'smb_gather_rows_f32', 'smb_gather_det_inputs', 'smb_gather_track_feats', 'smb_track_step', 'smb_conv_plan_create', 'smb_conv_plan_create_multi', 'smb_conv_plan_destroy', 'smb_conv_plan_set_max_ctas', 'smb_conv_set_min_tiles',
     'smb_conv_run',
     'smb_groupnorm_relu_apply', 'smb_groupnorm_stats', 'smb_deform_im2col', 'smb_offset_conv1x1', 'smb_groupnorm_relu_apply_multi', 'smb_offset_conv1x1_multi', 'smb_deform_im2col_multi', 'smb_maxpool3x3s2',
-    'smb_upsample_bilinear', 'smb_image_to_nhwc8', 'smb_preprocess_u8', 'smb_stem_plan_create', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
+    'smb_upsample_bilinear', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
 ]
 
 

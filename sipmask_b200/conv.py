@@ -38,20 +38,6 @@ def pack_weight(w, bn=None, eps=1e-5, cout_pad=None, device=None):
     return wk, bias
 
 
-def pack_stem_weight(w, bn, eps=1e-5, device=None):
-    """7x7 stem [64,3,7,7] -> [64, 7*64] : K = r*64 + s*8 + c (s<7, c<3 real, rest zero)."""
-    gamma, beta, mean, var = [t.detach().float() for t in bn]
-    s = gamma / torch.sqrt(var + eps)
-    w = w.detach().float() * s.view(-1, 1, 1, 1)
-    out = w.new_zeros(64, 7, 8, 8)
-    out[:, :, :7, :3] = w.permute(0, 2, 3, 1)           # [co, r, s, c]
-    wk = out.reshape(64, 448).to(torch.float16).contiguous()
-    bias = (beta - mean * s).contiguous()
-    if device is not None:
-        wk, bias = wk.to(device), bias.to(device)
-    return wk, bias
-
-
 def pack_stem_weight_s2d(w, bn, eps=1e-5, device=None):
     """7x7 stem [64,3,7,7] -> [64, 4*64] for the space-to-depth stem: K = a*64 + b*16 + (dy*2+dx)*4 + c holds filter tap
     (r, s) = (2a+dy, 2b+dx), channel c (taps with r == 7 or s == 7 and c == 3 are zero)."""
@@ -176,37 +162,23 @@ class ConvPlanMulti(ConvPlan):
 
 
 class StemPlan(ConvPlan):
-    """7x7/2 stem + folded BN + ReLU (resnet.py:448-460) on the padded NHWC8 image [N,H+6,W+8,8] with weights [64,448]
-    (pack_stem_weight), or - s2d=True - on the space-to-depth image [N,H/2+3,W/2+4,16] with weights [64,256]
-    (pack_stem_weight_s2d): the same convolution with 43 % fewer operand bytes."""
+    """7x7/2 stem + folded BN + ReLU (resnet.py:448-460) on the space-to-depth image [N,H/2+3,W/2+4,16]
+    (image_to_s2d16 / preprocess_u8) with weights [64,256] (pack_stem_weight_s2d)."""
 
-    def __init__(self, img8, weight, bias, out, N, H, W, s2d=False):
+    def __init__(self, img8, weight, bias, out, N, H, W):
         self._keep = (img8, weight, bias, out)
         self.bias, self.residual, self.gn_stats, self.alpha = bias, None, None, 1.0
         self.handle = ctypes.c_void_p()
         self.dev = img8.device
-        assert tuple(img8.shape) == ((N, H // 2 + 3, W // 2 + 4, 16) if s2d else (N, H + 6, W + 8, 8)) and img8.is_contiguous()
-        assert tuple(weight.shape) == (64, 256 if s2d else 448)
+        assert tuple(img8.shape) == (N, H // 2 + 3, W // 2 + 4, 16) and img8.is_contiguous()
+        assert tuple(weight.shape) == (64, 256)
         with torch.cuda.device(self.dev):
-            if s2d:
-                L.check(L.lib().smb_stem_plan_create_s2d(N, H, W, L.ptr(img8), L.ptr(weight), L.ptr(out),
-                                                         ctypes.byref(self.handle)), 'smb_stem_plan_create_s2d')
-            else:
-                L.check(L.lib().smb_stem_plan_create(N, H, W, L.ptr(img8), L.ptr(weight), L.ptr(out),
-                                                     ctypes.byref(self.handle)), 'smb_stem_plan_create')
+            L.check(L.lib().smb_stem_plan_create_s2d(N, H, W, L.ptr(img8), L.ptr(weight), L.ptr(out),
+                                                     ctypes.byref(self.handle)), 'smb_stem_plan_create_s2d')
         self.out = out
 
 
 # ------------------------------------------------------------------------------------- small wrappers
-@L.device_guard
-def image_to_nhwc8(img, out=None):
-    N, _, H, W = img.shape
-    if out is None:
-        out = torch.empty((N, H + 6, W + 8, 8), dtype=torch.float16, device=img.device)
-    L.check(L.lib().smb_image_to_nhwc8(L.ptr(img.contiguous()), L.ptr(out), N, H, W, L.stream_ptr()), 'smb_image_to_nhwc8')
-    return out
-
-
 @L.device_guard
 def image_to_s2d16(img, out=None):
     """img [N,3,H,W] fp32 -> the stem's space-to-depth input [N, H/2+3, W/2+4, 16] fp16 (smb_image_to_s2d16)."""
@@ -219,22 +191,16 @@ def image_to_s2d16(img, out=None):
 
 @L.device_guard
 def preprocess_u8(src, resized_hw, out, mean):
-    """uint8 BGR HWC CUDA image -> resized (cv2 INTER_LINEAR, bit-exact) - mean -> zero-padded fp16 stem input: `out` is
-    either the NHWC8 buffer [1, H+6, W+8, 8] (smb_preprocess_u8) or the space-to-depth buffer [1, H/2+3, W/2+4, 16]
-    (smb_preprocess_u8_s2d); the layout is taken from its shape."""
+    """uint8 BGR HWC CUDA image -> resized (cv2 INTER_LINEAR, bit-exact) - mean -> zero-padded fp16 stem input in the
+    space-to-depth layout `out` [1, H/2+3, W/2+4, 16] (smb_preprocess_u8_s2d)."""
     assert src.is_cuda and src.dtype == torch.uint8 and src.dim() == 3 and src.shape[2] == 3 and src.stride(2) == 1 \
         and src.stride(1) == 3
-    assert out.dtype == torch.float16 and out.is_contiguous() and out.shape[0] == 1 and out.shape[3] in (8, 16)
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.shape[0] == 1 and out.shape[3] == 16
     m = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    if out.shape[3] == 16:
-        H, W = 2 * (out.shape[1] - 3), 2 * (out.shape[2] - 4)
-        L.check(L.lib().smb_preprocess_u8_s2d(L.ptr(src), int(src.shape[0]), int(src.shape[1]), int(src.stride(0)),
-                                              int(resized_hw[0]), int(resized_hw[1]), m, L.ptr(out), H, W, L.stream_ptr()),
-                'smb_preprocess_u8_s2d')
-        return out
-    H, W = out.shape[1] - 6, out.shape[2] - 8
-    L.check(L.lib().smb_preprocess_u8(L.ptr(src), int(src.shape[0]), int(src.shape[1]), int(src.stride(0)), int(resized_hw[0]),
-                                      int(resized_hw[1]), m, L.ptr(out), H, W, L.stream_ptr()), 'smb_preprocess_u8')
+    H, W = 2 * (out.shape[1] - 3), 2 * (out.shape[2] - 4)
+    L.check(L.lib().smb_preprocess_u8_s2d(L.ptr(src), int(src.shape[0]), int(src.shape[1]), int(src.stride(0)),
+                                          int(resized_hw[0]), int(resized_hw[1]), m, L.ptr(out), H, W, L.stream_ptr()),
+            'smb_preprocess_u8_s2d')
     return out
 
 

@@ -56,35 +56,16 @@ struct DeviceOnce {
   }
 };
 
-// Programmatic dependent launch (PDL): a kernel launched through launch_pdl may start while the previous kernel in the
-// stream is still draining; it must call pdl_wait() before its first global-memory access (the wait returns once the
-// previous grid has completed and its writes are visible).  Chains of short kernels lose the ~1-2 us launch gap each.
+// Programmatic dependent launch (PDL).  The elementwise / NMS kernels are launched with plain <<<>>>, so for them
+// griddepcontrol.wait is a no-op (the stream already orders them after the previous kernel).  launch_dependents is not:
+// smb_conv_run launches conv_gemm_kernel with the PDL attribute, and the signal lets that next convolution be scheduled
+// and run its prologue (shared-memory carve-up, mbarrier init) while this kernel is still running.  The convolution
+// executes griddepcontrol.wait before it touches global memory, so it still sees every write of this kernel.
 __device__ __forceinline__ void pdl_wait() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  static int enabled = -1;                                  // SMB_PDL_AUX=1 turns the attribute on for the elementwise / NMS
-                                                            // kernels; off by default
-  if (enabled < 0) {
-    const char* e = getenv("SMB_PDL_AUX");
-    enabled = e ? atoi(e) : 0;
-  }
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = enabled ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // GroupNorm statistics are accumulated as 64-bit fixed point (deterministic integer atomics)

@@ -617,50 +617,10 @@ extern "C" int smb_conv_plan_create(const smb_conv_desc_t* d, const void* in, co
   return smb_conv_plan_create_multi(d, 1, &lv, weight, plan_out);
 }
 
-// 7x7/2 stem on the padded NHWC8 image written by smb_image_to_nhwc8:
-//   img8 [N, H+6, W+8, 8] fp16 (pixel (y,x) stored at (y+3, x+3)); K = 7 filter rows x (8 pixels x 8 ch).
-//   Output pixel (oy,ox), filter row r reads padded row 2*oy + r, pixels 2*ox .. 2*ox+7 (128 contiguous bytes).
-extern "C" int smb_stem_plan_create(int N, int H, int W, const void* img_nhwc8, const void* weight448, void* out,
-                                    smb_conv_plan_t** plan_out) {
-  SMB_CHECK_ARG(img_nhwc8 && weight448 && out && plan_out, "smb_stem_plan_create: null pointer");
-  SMB_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "smb_stem_plan_create: H, W must be even (images are padded to /32)");
-  smb_conv_plan* pl = new smb_conv_plan();
-  memset(&pl->p, 0, sizeof(ConvParams));
-  ConvParams& p = pl->p;
-  LevelDesc& L = p.lv[0];
-  const int Ho = H / 2, Wo = W / 2, Hp = H + 6, Wp = W + 8;
-  p.n_img = N; p.num_levels = 1;
-  L.H_out = Ho; L.W_out = Wo;
-  choose_patch(Ho, Wo, &L.BH, &L.BW);
-  L.tiles_x = cdiv(Wo, L.BW); L.tiles_y = cdiv(Ho, L.BH);
-  L.tile_start = 0; L.map0 = 0; L.out = out;
-  p.tiles_m = N * L.tiles_x * L.tiles_y;
-  p.num_taps = 7; p.kb_per_tap = 1;
-  p.Cout = 64;
-  p.out_pitch = 64; p.out_f32 = 0; p.alpha = 1.f; p.relu = 1;
-  p.gn_group = 0;
-  pl->has_bias = 1;
-  const uint64_t rowb = (uint64_t)Wp * 16;
-  const uint32_t box[4] = {64, (uint32_t)L.BW, (uint32_t)L.BH, 1};
-  int rc = SMB_OK;
-  for (int par = 0; par < 2 && rc == SMB_OK; ++par) {
-    const int rows = (Hp - par + 1) / 2;
-    uint64_t dims[4] = {64, (uint64_t)Wo, (uint64_t)rows, (uint64_t)N};
-    uint64_t strides[3] = {32, rowb * 2, rowb * Hp};     // 2-pixel step along x: overlapping 8-pixel windows
-    rc = encode_map(&p.amap[par], (char*)const_cast<void*>(img_nhwc8) + par * rowb, 4, dims, strides, box);
-  }
-  for (int i = 2; i < kMaxMaps; ++i) p.amap[i] = p.amap[i & 1];
-  for (int r = 0; r < 7; ++r) { p.tap_map[r] = r & 1; p.tap_dy[r] = r >> 1; p.tap_dx[r] = 0; }
-  if (rc == SMB_OK) rc = finish_plan(pl, 64, 448, weight448);
-  if (rc != SMB_OK) { delete pl; return rc; }
-  *plan_out = pl;
-  return SMB_OK;
-}
-
 // 7x7/2 stem on the SPACE-TO-DEPTH image written by smb_image_to_s2d16 / smb_preprocess_u8_s2d:
 //   q [N, H/2+3, W/2+4, 16] fp16, q(Y, X, (dy*2+dx)*4 + c) = padded pixel (2Y+dy, 2X+dx) channel c.
 //   out(oy, ox) = sum_{a,b<4} sum_{dy,dx,c} w[2a+dy][2b+dx][c] * q(oy+a, ox+b, (dy,dx,c)) : a 4x4 stride-1 convolution
-//   over 16 channels, K = 4 filter rows x (4 cells x 16 ch = 128 contiguous bytes) = 256 instead of the 448 of the
+//   over 16 channels, K = 4 filter rows x (4 cells x 16 ch = 128 contiguous bytes) = 256 instead of the 448 of a
 //   pixel-window form (7 rows x 8 pixels x 8 ch) - 43 % fewer operand bytes and MMAs.
 extern "C" int smb_stem_plan_create_s2d(int N, int H, int W, const void* img_s2d16, const void* weight256, void* out,
                                         smb_conv_plan_t** plan_out) {

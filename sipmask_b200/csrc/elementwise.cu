@@ -267,27 +267,7 @@ __global__ void copy_channels_kernel(const __half* __restrict__ x, int in_pitch,
   }
 }
 
-// --------------------------------------------------------------------------------------- image -> NHWC8
-// img [N,3,H,W] fp32 -> out [N, H+6, W+8, 8] fp16, pixel (y,x) at (y+3, x+3), zeros elsewhere / in ch 3..7.
-__global__ void image_to_nhwc8_kernel(const float* __restrict__ img, __half* __restrict__ out, int N, int H, int W) {
-  pdl_wait();
-  const int Hp = H + 6, Wp = W + 8;
-  const long long total = (long long)N * Hp * Wp;
-  for (unsigned t = blockIdx.x * blockDim.x + threadIdx.x; t < (unsigned)total; t += blockDim.x * gridDim.x) {   // 32-bit index math: 64-bit div/mod costs ~100 instructions each
-    const int xp = (int)(t % Wp);
-    const int yp = (int)((t / Wp) % Hp);
-    const int n = (int)(t / ((long long)Wp * Hp));
-    const int x = xp - 3, y = yp - 3;
-    float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (x >= 0 && x < W && y >= 0 && y < H) {
-      const size_t plane = (size_t)H * W;
-      const float* p = img + (size_t)n * 3 * plane + (size_t)y * W + x;
-      f[0] = p[0]; f[1] = p[plane]; f[2] = p[2 * plane];
-    }
-    *reinterpret_cast<uint4*>(out + (size_t)t * 8) = pack8(f);
-  }
-}
-
+// --------------------------------------------------------------------------------------- image -> stem input
 // img [N,3,H,W] fp32 -> out [N, H/2+3, W/2+4, 16] fp16: the stem's space-to-depth layout, element (Y, X, (dy*2+dx)*4 + c) =
 // image pixel (2Y+dy-3, 2X+dx-3), channel c; zeros outside the image and in c == 3.
 __global__ void image_to_s2d16_kernel(const float* __restrict__ img, __half* __restrict__ out, int N, int H, int W) {
@@ -336,47 +316,11 @@ __device__ __forceinline__ int find_level(const MultiDesc& d, long long t) {
   return l;
 }
 
-// GroupNorm(32) + ReLU in place; a[l] = x (fp16 [n_img*hw, C]), b[l] = stats (int64 fixed point).  C/32 % 8 == 0.
-__global__ void gn_apply_multi_kernel(MultiDesc d, int n_img, int C, int pitch, const float* __restrict__ gamma,
-                                      const float* __restrict__ beta, float eps, int relu) {
-  pdl_wait();
-  const int vecs = C >> 3;
-  const int cpg = C / 32;
-  const long long total = d.start[d.num];
-  for (unsigned t = blockIdx.x * blockDim.x + threadIdx.x; t < (unsigned)total; t += blockDim.x * gridDim.x) {   // 32-bit index math: 64-bit div/mod costs ~100 instructions each
-    const int l = find_level(d, t);
-    const unsigned q = t - (unsigned)d.start[l];
-    const int hw = d.H[l] * d.W[l];
-    const int v = (int)(q % vecs);
-    const unsigned row = q / (unsigned)vecs;
-    const int img = (int)(row / hw);
-    const int g = (v * 8) / cpg;
-    const long long* st = reinterpret_cast<const long long*>(d.b[l]) + ((size_t)img * 32 + g) * 2;
-    const float inv_cnt = 1.0f / ((float)hw * (float)cpg);
-    // int64 -> fp32 with one rounding, exact power-of-two scales: same bits as the double-precision product, no FP64 issue
-    const float mean = __ll2float_rn(st[0]) * (1.0f / kGnSumScale) * inv_cnt;
-    const float ex2 = __ll2float_rn(st[1]) * (1.0f / kGnSqScale) * inv_cnt;
-    const float rstd = rsqrtf(fmaxf(ex2 - mean * mean, 0.f) + eps);
-    uint4* p = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(d.c[l]) + (size_t)row * pitch + v * 8);
-    float f[8];
-    unpack8(*p, f);
-    const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + v * 8)), g1 = __ldg(reinterpret_cast<const float4*>(gamma + v * 8) + 1);
-    const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta + v * 8)), b1 = __ldg(reinterpret_cast<const float4*>(beta + v * 8) + 1);
-    const float ga[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-    const float be[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float y = (f[j] - mean) * rstd * ga[j] + be[j];
-      f[j] = relu ? fmaxf(y, 0.f) : y;
-    }
-    *p = pack8(f);
-  }
-}
-
-// Same arithmetic, thread-stationary in the channel vector: a CTA owns kGnRows consecutive pixel rows of ONE (level, image),
-// a thread one 8-channel vector (v = tid % vecs) of every (256 / vecs)-th of those rows.  Level lookup, statistics (two
-// int64 loads, conversions, rsqrt) and gamma / beta (four 16-byte loads) are evaluated once per thread instead of once per
-// 16-byte vector (gn_apply_multi_kernel: ~150 instructions per vector, issue-bound); the row loop is a load, 8 x (sub, mul, fma, max), a store.  start[] holds the prefix of CTAs per level.
+// GroupNorm(32) + ReLU in place over all levels; a[l] = x (fp16 [n_img*hw, C]), b[l] = stats (int64 fixed point).
+// Thread-stationary in the channel vector: a CTA owns kGnRows consecutive pixel rows of ONE (level, image), a thread one
+// 8-channel vector (v = tid % vecs) of every (256 / vecs)-th of those rows.  Level lookup, statistics (two int64 loads,
+// conversions, rsqrt) and gamma / beta (four 16-byte loads) are evaluated once per thread, not once per 16-byte vector;
+// the row loop is a load, 8 x (sub, mul, fma, max), a store.  start[] holds the prefix of CTAs per level.
 constexpr int kGnRows = 64;
 __global__ void __launch_bounds__(256) gn_apply_rows_kernel(MultiDesc d, int n_img, int C, int pitch, const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, float eps, int relu) {
@@ -393,6 +337,7 @@ __global__ void __launch_bounds__(256) gn_apply_rows_kernel(MultiDesc d, int n_i
   const int g = (v * 8) / cpg;
   const long long* st = reinterpret_cast<const long long*>(d.b[l]) + ((size_t)img * 32 + g) * 2;
   const float inv_cnt = 1.0f / ((float)hw * (float)cpg);
+  // int64 -> fp32 with one rounding, exact power-of-two scales: same bits as the double-precision product, no FP64 issue
   const float mean = __ll2float_rn(st[0]) * (1.0f / kGnSumScale) * inv_cnt;
   const float ex2 = __ll2float_rn(st[1]) * (1.0f / kGnSqScale) * inv_cnt;
   const float rstd = rsqrtf(fmaxf(ex2 - mean * mean, 0.f) + eps);
@@ -408,7 +353,7 @@ __global__ void __launch_bounds__(256) gn_apply_rows_kernel(MultiDesc d, int n_i
     unpack8(*p, f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float y = (f[j] - mean) * rstd * ga[j] + be[j];   // the expression of gn_apply_multi_kernel: same bits
+      const float y = (f[j] - mean) * rstd * ga[j] + be[j];
       f[j] = relu ? fmaxf(y, 0.f) : y;
     }
     *p = pack8(f);
@@ -552,8 +497,7 @@ extern "C" int smb_maxpool3x3s2(const void* x, void* y, int N, int H, int W, int
   SMB_CHECK_ARG(x && y && C % 8 == 0, "smb_maxpool3x3s2: bad argument");
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
   const long long total = (long long)N * Ho * Wo * (C / 8);
-  SMB_CUDA_OK(launch_pdl(maxpool3x3s2_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x,
-                         (__half*)y, N, H, W, C, Ho, Wo));
+  maxpool3x3s2_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, N, H, W, C, Ho, Wo);
   SMB_LAUNCH_OK("maxpool3x3s2_kernel");
   return SMB_OK;
 }
@@ -564,27 +508,17 @@ extern "C" int smb_upsample_bilinear(const void* x, int in_pitch, void* y, int o
                 "smb_upsample_bilinear: bad argument");
   if (factor == 1) {
     const long long npix = (long long)N * H * W;
-    SMB_CUDA_OK(launch_pdl(copy_channels_kernel, dim3(grid_for(npix * (C / 8), 256)), dim3(256), 0, (cudaStream_t)stream,
-                           (const __half*)x, in_pitch, (__half*)y, out_pitch, out_choff, npix, C, relu));
+    copy_channels_kernel<<<grid_for(npix * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>((const __half*)x, in_pitch, (__half*)y,
+                                                                                          out_pitch, out_choff, npix, C, relu);
     SMB_LAUNCH_OK("copy_channels_kernel");
     return SMB_OK;
   }
   const long long total = (long long)N * H * factor * W * factor * (C / 8);
-  SMB_CUDA_OK(launch_pdl(upsample_bilinear_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x,
-                         in_pitch, (__half*)y, out_pitch, out_choff, N, H, W, C, factor, relu));
+  upsample_bilinear_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>((const __half*)x, in_pitch, (__half*)y, out_pitch,
+                                                                                  out_choff, N, H, W, C, factor, relu);
   SMB_LAUNCH_OK("upsample_bilinear_kernel");
   return SMB_OK;
 }
-
-extern "C" int smb_image_to_nhwc8(const float* img, void* out, int N, int H, int W, smb_stream_t stream) {
-  SMB_CHECK_ARG(img && out && N > 0 && H > 0 && W > 0, "smb_image_to_nhwc8: bad argument");
-  const long long total = (long long)N * (H + 6) * (W + 8);
-  SMB_CUDA_OK(launch_pdl(image_to_nhwc8_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, img, (__half*)out, N,
-                         H, W));
-  SMB_LAUNCH_OK("image_to_nhwc8_kernel");
-  return SMB_OK;
-}
-
 
 // ------------------------------------------------------------------------------------------ multi-level C ABI
 static int fill_multi(MultiDesc* d, int num, const int* Hs, const int* Ws, long long items_per_pixel, int n_img) {
@@ -602,7 +536,7 @@ static int fill_multi(MultiDesc* d, int num, const int* Hs, const int* Ws, long 
 extern "C" int smb_image_to_s2d16(const float* img, void* out, int N, int H, int W, smb_stream_t stream) {
   SMB_CHECK_ARG(img && out && N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "smb_image_to_s2d16: bad argument");
   const long long total = (long long)N * (H / 2 + 3) * (W / 2 + 4);
-  SMB_CUDA_OK(launch_pdl(image_to_s2d16_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, img, (__half*)out, N, H, W));
+  image_to_s2d16_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(img, (__half*)out, N, H, W);
   SMB_LAUNCH_OK("image_to_s2d16_kernel");
   return SMB_OK;
 }
@@ -611,29 +545,21 @@ extern "C" int smb_groupnorm_relu_apply_multi(int num_levels, void* const* xs, c
                                               const int* Ws, int n_img, int C, int pitch, const float* gamma,
                                               const float* beta, float eps, int relu, smb_stream_t stream) {
   SMB_CHECK_ARG(xs && stats && Hs && Ws && gamma && beta, "smb_groupnorm_relu_apply_multi: null pointer");
-  SMB_CHECK_ARG(C % 256 == 0 && pitch % 8 == 0 && n_img > 0, "smb_groupnorm_relu_apply_multi: C must be a multiple of 256");
+  // one CTA thread per 8-channel vector of a row, (256 / vecs) rows at a time: 256 % (C / 8) == 0
+  SMB_CHECK_ARG((C == 256 || C == 512 || C == 1024 || C == 2048) && pitch % 8 == 0 && n_img > 0,
+                "smb_groupnorm_relu_apply_multi: C=%d unsupported (256, 512, 1024 or 2048)", C);
   MultiDesc d;
   SMB_CHECK_ARG(fill_multi(&d, num_levels, Hs, Ws, C / 8, n_img) == 0, "smb_groupnorm_relu_apply_multi: bad levels");
   for (int l = 0; l < num_levels; ++l) { d.c[l] = xs[l]; d.b[l] = stats[l]; d.a[l] = nullptr; d.scale[l] = 1.f; }
-  static int rows_kernel = -1;                               // SMB_GN_ROWS=0 keeps the one-vector-per-thread kernel
-  if (rows_kernel < 0) { const char* e = getenv("SMB_GN_ROWS"); rows_kernel = e ? atoi(e) : 1; }
-  const int vecs = C / 8;
-  if (rows_kernel && vecs <= 256 && 256 % vecs == 0) {
-    long long ctas = 0;
-    for (int l = 0; l < num_levels; ++l) {                   // start[] = prefix of CTAs: n_img * ceil(hw / kGnRows) per level
-      d.start[l] = ctas;
-      ctas += (long long)n_img * (((long long)Hs[l] * Ws[l] + kGnRows - 1) / kGnRows);
-    }
-    d.start[num_levels] = ctas;
-    SMB_CHECK_ARG(ctas < (1LL << 31), "smb_groupnorm_relu_apply_multi: too many rows");
-    SMB_CUDA_OK(launch_pdl(gn_apply_rows_kernel, dim3((unsigned)ctas), dim3(256), 0, (cudaStream_t)stream, d, n_img, C, pitch, gamma,
-                           beta, eps, relu));
-    SMB_LAUNCH_OK("gn_apply_rows_kernel");
-    return SMB_OK;
+  long long ctas = 0;
+  for (int l = 0; l < num_levels; ++l) {                     // start[] = prefix of CTAs: n_img * ceil(hw / kGnRows) per level
+    d.start[l] = ctas;
+    ctas += (long long)n_img * (((long long)Hs[l] * Ws[l] + kGnRows - 1) / kGnRows);
   }
-  SMB_CUDA_OK(launch_pdl(gn_apply_multi_kernel, dim3(grid_for(d.start[num_levels], 256)), dim3(256), 0, (cudaStream_t)stream, d, n_img, C,
-                         pitch, gamma, beta, eps, relu));
-  SMB_LAUNCH_OK("gn_apply_multi_kernel");
+  d.start[num_levels] = ctas;
+  SMB_CHECK_ARG(ctas < (1LL << 31), "smb_groupnorm_relu_apply_multi: too many rows");
+  gn_apply_rows_kernel<<<(unsigned)ctas, 256, 0, (cudaStream_t)stream>>>(d, n_img, C, pitch, gamma, beta, eps, relu);
+  SMB_LAUNCH_OK("gn_apply_rows_kernel");
   return SMB_OK;
 }
 
@@ -644,8 +570,7 @@ extern "C" int smb_offset_conv1x1_multi(int num_levels, const float* const* bbox
   MultiDesc d;
   SMB_CHECK_ARG(fill_multi(&d, num_levels, Hs, Ws, n_off, n_img) == 0, "smb_offset_conv1x1_multi: bad levels");
   for (int l = 0; l < num_levels; ++l) { d.a[l] = bboxes[l]; d.c[l] = offs[l]; d.b[l] = nullptr; d.scale[l] = scales[l]; }
-  SMB_CUDA_OK(launch_pdl(offset_conv_multi_kernel, dim3(grid_for(d.start[num_levels], 256)), dim3(256), 0, (cudaStream_t)stream, d,
-                         bbox_pitch, weight, n_off));
+  offset_conv_multi_kernel<<<grid_for(d.start[num_levels], 256), 256, 0, (cudaStream_t)stream>>>(d, bbox_pitch, weight, n_off);
   SMB_LAUNCH_OK("offset_conv_multi_kernel");
   return SMB_OK;
 }
@@ -659,8 +584,8 @@ extern "C" int smb_deform_im2col_multi(int num_levels, const void* const* xs, co
   MultiDesc d;
   SMB_CHECK_ARG(fill_multi(&d, num_levels, Hs, Ws, 1, n_img) == 0, "smb_deform_im2col_multi: bad levels");
   for (int l = 0; l < num_levels; ++l) { d.a[l] = xs[l]; d.b[l] = offs[l]; d.c[l] = cols[l]; d.scale[l] = 1.f; }
-  SMB_CUDA_OK(launch_pdl(deform_im2col_multi_kernel, dim3(grid_for(d.start[num_levels] * 32, 256)), dim3(256), 0, (cudaStream_t)stream,
-                         d, off_pitch, C, deformable_groups));
+  deform_im2col_multi_kernel<<<grid_for(d.start[num_levels] * 32, 256), 256, 0, (cudaStream_t)stream>>>(d, off_pitch, C,
+                                                                                                        deformable_groups);
   SMB_LAUNCH_OK("deform_im2col_multi_kernel");
   return SMB_OK;
 }

@@ -10,13 +10,6 @@
 // HBM-bound: algorithmic bytes = protos (H*W*32*sizeof) + out (N*H*W*sizeof).
 #include "common.cuh"
 
-#ifndef SMB_MASK_MMA_DEFAULT
-#define SMB_MASK_MMA_DEFAULT 1
-#endif
-#ifndef SMB_MASK_TILE_DEFAULT
-#define SMB_MASK_TILE_DEFAULT 0
-#endif
-
 namespace smb {
 
 struct __align__(16) BoxP {
@@ -589,17 +582,16 @@ __device__ __forceinline__ void run_values(const float (&acc)[4], const BoxP& b,
 // Dense pos_masks, tensor-core dots.  Same tiling / listing / zero-fill as mask_assemble_kernel; a warp owns one tile row
 // (its A fragments are re-read from shared memory per 16-pixel run and group: 8 LDS.32 against ~70 other instructions;
 // keeping the row's 32 fragment registers live cost a CTA per SM).
-// Tile = TH_ rows x TW_ pixels, TH_ * TW_ = 512 (8 x 64, 4 x 128 or 2 x 256): a warp owns one 64-pixel segment of one
-// tile row; wider tiles make the zero / value stores of a detection longer contiguous runs (256 / 512 / 1024 bytes).
+// Tile = MA_TH rows x MA_TW pixels: a warp owns one 64-pixel segment of one tile row.
 // 64 registers: four CTAs per SM (528 slots on 132 SMs for the 550 - 600 CTAs of a 400 x 672 prototype map; at three CTAs
 // per SM the second wave would run on a fraction of the SMs).
-template <bool HWC, typename OT, int TH_, int TW_>
+template <bool HWC, typename OT>
 __global__ void __launch_bounds__(MA_THREADS2, 4) mask_assemble_mma_kernel(
     const __half* __restrict__ protos, const float* __restrict__ cofs, const float* __restrict__ boxes,
     float sx1, float sy1, float sx2, float sy2, OT* __restrict__ out, int H, int W, int N) {
-  static_assert(TH_ * TW_ == 512 && TW_ % 64 == 0 && TH_ * (TW_ / 64) == MA_THREADS2 / 32, "one warp per 64-pixel row segment");
-  constexpr int SEGS = TW_ / 64;                              // 64-pixel segments (warps) per tile row
-  extern __shared__ __align__(16) unsigned char s_p[];        // [TH_ * TW_] swizzled pixels (32 KB)
+  static_assert(MA_TW % 64 == 0 && MA_TH * (MA_TW / 64) == MA_THREADS2 / 32, "one warp per 64-pixel row segment");
+  constexpr int SEGS = MA_TW / 64;                            // 64-pixel segments (warps) per tile row
+  extern __shared__ __align__(16) unsigned char s_p[];        // [MA_TH * MA_TW] swizzled pixels (32 KB)
   __shared__ BoxP s_box[MA_LIST];
   __shared__ int s_det[MA_LIST];
   __shared__ int s_cnt;
@@ -607,8 +599,8 @@ __global__ void __launch_bounds__(MA_THREADS2, 4) mask_assemble_mma_kernel(
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
-  const int y0t = blockIdx.y * TH_, x0t = blockIdx.x * TW_;
-  const int SRa = min(TH_, H - y0t), SCa = min(TW_, W - x0t);
+  const int y0t = blockIdx.y * MA_TH, x0t = blockIdx.x * MA_TW;
+  const int SRa = min(MA_TH, H - y0t), SCa = min(MA_TW, W - x0t);
   stage_window<__half, HWC>(protos, s_p, H, W, y0t, x0t, SRa, SCa, MA_THREADS2);
   const int wrow = warp / SEGS, wseg = (warp % SEGS) * 64;   // this warp's tile row and first tile column
   const int h = y0t + wrow;
@@ -616,8 +608,8 @@ __global__ void __launch_bounds__(MA_THREADS2, 4) mask_assemble_mma_kernel(
   const float hf = (float)h;
   const float tile_x0 = (float)x0t, tile_x1 = (float)(x0t + SCa - 1), tile_y0 = (float)y0t, tile_y1 = (float)(y0t + SRa - 1);
   const float seg_x0 = (float)(x0t + wseg);
-  // zero-fill role: thread t < 128 owns 4 pixels: row t / (TW_ / 4), columns 4 * (t % (TW_ / 4)) ..
-  const int zr = threadIdx.x / (TW_ / 4), zc = (threadIdx.x % (TW_ / 4)) * 4;
+  // zero-fill role: thread t < 128 owns 4 pixels: row t / (MA_TW / 4), columns 4 * (t % (MA_TW / 4)) ..
+  const int zr = threadIdx.x / (MA_TW / 4), zc = (threadIdx.x % (MA_TW / 4)) * 4;
   const bool z_vec = threadIdx.x < 128 && zr < SRa && zc + 3 < SCa && ((W & 3) == 0);
   const bool z_tail = threadIdx.x < 128 && zr < SRa && !z_vec && zc < SCa;
   const int MT = min(4, (SCa - wseg + 15) >> 4);            // 16-pixel runs of this warp's segment (the last one may be
@@ -964,18 +956,11 @@ __global__ void crop_mask_kernel(const T* __restrict__ data, const T* __restrict
 
 using namespace smb;
 
-// fp16 prototypes: tensor-core kernels (1, default) or the scalar-fmaf kernels (0); SMB_MASK_MMA overrides the default
-static int g_mask_mma = -1;
-static int mask_mma_enabled() {
-  if (g_mask_mma < 0) {
-    const char* e = getenv("SMB_MASK_MMA");
-    g_mask_mma = e ? (atoi(e) != 0) : SMB_MASK_MMA_DEFAULT;
-  }
-  return g_mask_mma;
-}
+// fp16 prototypes: tensor-core kernels (1, default) or the scalar-fmaf kernels (0)
+static int g_mask_mma = 1;
 
 extern "C" int smb_mask_set_tensor_dot(int on) {
-  const int prev = mask_mma_enabled();
+  const int prev = g_mask_mma;
   if (on >= 0) g_mask_mma = on ? 1 : 0;
   return prev;
 }
@@ -1004,18 +989,10 @@ extern "C" int smb_mask_assemble(const void* protos, int protos_dtype, int layou
   mask_assemble_kernel<PT, HWC, OT><<<grid, block, ma_smem, st>>>((const PT*)protos, cofs, boxes, s0, s1, s2, s3, \
                                                                   (OT*)out, H, W, N)
   const int key = (protos_dtype << 2) | ((layout_hwc ? 1 : 0) << 1) | out_dtype;
-  if (protos_dtype == SMB_F16 && mask_mma_enabled()) {
-    static int tile = -1;                                    // SMB_MASK_TILE: 0 = 8 x 64, 1 = 4 x 128, 2 = 2 x 256 pixels
-    if (tile < 0) { const char* e = getenv("SMB_MASK_TILE"); tile = e ? atoi(e) : SMB_MASK_TILE_DEFAULT; if (tile < 0 || tile > 2) tile = 0; }
-#define MAM_LAUNCH3(HWC, OT, TH_, TW_)                                                                                   \
-  mask_assemble_mma_kernel<HWC, OT, TH_, TW_><<<dim3(cdiv(W, TW_), cdiv(H, TH_)), block, 512 * 64, st>>>(                \
-      (const __half*)protos, cofs, boxes, s0, s1, s2, s3, (OT*)out, H, W, N)
-#define MAM_LAUNCH(HWC, OT)                                  \
-  do {                                                       \
-    if (tile == 1) MAM_LAUNCH3(HWC, OT, 4, 128);             \
-    else if (tile == 2) MAM_LAUNCH3(HWC, OT, 2, 256);        \
-    else MAM_LAUNCH3(HWC, OT, 8, 64);                        \
-  } while (0)
+  if (protos_dtype == SMB_F16 && g_mask_mma) {
+#define MAM_LAUNCH(HWC, OT)                                                                                      \
+  mask_assemble_mma_kernel<HWC, OT><<<grid, block, ma_smem, st>>>((const __half*)protos, cofs, boxes, s0, s1, s2, s3, \
+                                                                  (OT*)out, H, W, N)
     switch (key & 3) {
       case 0: MAM_LAUNCH(false, float); break;
       case 1: MAM_LAUNCH(false, __half); break;
@@ -1023,7 +1000,6 @@ extern "C" int smb_mask_assemble(const void* protos, int protos_dtype, int layou
       case 3: MAM_LAUNCH(true, __half); break;
     }
 #undef MAM_LAUNCH
-#undef MAM_LAUNCH3
     SMB_LAUNCH_OK("mask_assemble_mma_kernel");
     return SMB_OK;
   }
@@ -1123,9 +1099,7 @@ extern "C" int smb_mask_assemble_pack(const void* protos, int protos_dtype, int 
   const int px_budget = (int)((48 * 1024) / px_bytes);
   auto win_rows = [&](int ty) { return (int)ceilf((float)(ty - 1) * rs.ry) + 2; };
   auto win_cols = [&](int tw) { return (int)ceilf((float)(tw * 32 - 1) * rs.rx) + 2; };
-  static int ty_max = -1;                                    // SMB_MASK_FUSED_TY: output rows per tile (1 .. 16, default 16)
-  if (ty_max < 0) { const char* e = getenv("SMB_MASK_FUSED_TY"); ty_max = e ? atoi(e) : MF_TY_MAX; if (ty_max < 1 || ty_max > MF_TY_MAX) ty_max = MF_TY_MAX; }
-  int TW = 4, TY = ty_max;
+  int TW = 4, TY = MF_TY_MAX;
   while (TW > 1 && win_rows(TY) * win_cols(TW) > px_budget) TW >>= 1;
   while (TY > 1 && win_rows(TY) * win_cols(TW) > px_budget) TY >>= 1;
   // rounded up to a multiple of 4 pixels: the arrays carved out of shared memory after the window (s_val, s_box, ...) are
@@ -1135,7 +1109,7 @@ extern "C" int smb_mask_assemble_pack(const void* protos, int protos_dtype, int 
                 "pixels per 32-pixel word)", H, W, full_h, full_w, win_cap);
   dim3 grid(cdiv(cdiv(vw, 32), TW), cdiv(vh, TY)), block(MF_THREADS);
   const float s0 = host_box_scale4[0], s1 = host_box_scale4[1], s2 = host_box_scale4[2], s3 = host_box_scale4[3];
-  const bool mma = protos_dtype == SMB_F16 && mask_mma_enabled();
+  const bool mma = protos_dtype == SMB_F16 && g_mask_mma;
   // value tiles: two (double-buffered, one detection each) for the scalar kernel, four (a group of detections) for the
   // tensor-core kernel
   const size_t smem = (size_t)win_cap * (px_bytes + (mma ? 16 : 8)) + (mma ? MFM_LIST : MF_LIST) * (sizeof(BoxP) + sizeof(int)) +

@@ -885,21 +885,21 @@ extern "C" int smb_multiclass_nms(const float* boxes, const float* scores, const
     SMB_CUDA_OK(cudaMemsetAsync(ws_count, 0, sizeof(int) * (num_classes + 1), st));
   } else {
     const int nbmax = (n + 63) / 64;
-    SMB_CUDA_OK(launch_pdl(mc_prepare_kernel, dim3(num_classes), dim3(NT), sizeof(McPrepSmem), st, boxes, scores, ctr, n, num_classes, score_thr, (int*)(ws + w.cidx),
+    mc_prepare_kernel<<<num_classes, NT, sizeof(McPrepSmem), st>>>(boxes, scores, ctr, n, num_classes, score_thr, (int*)(ws + w.cidx),
                                                                    (float*)(ws + w.cscore), (unsigned long long*)(ws + w.keys),
-                                                                   (float4*)(ws + w.sbox), (int*)(ws + w.m)));
+                                                                   (float4*)(ws + w.sbox), (int*)(ws + w.m));
     SMB_LAUNCH_OK("mc_prepare_kernel");
-    SMB_CUDA_OK(launch_pdl(mc_mask_kernel, dim3(132 * 16), dim3(64), 0, st, (const float4*)(ws + w.sbox), (const int*)(ws + w.m), n, num_classes, nbmax, iou_thr,
-                                            cmp_ge, (unsigned long long*)(ws + w.mask)));
+    mc_mask_kernel<<<132 * 16, 64, 0, st>>>((const float4*)(ws + w.sbox), (const int*)(ws + w.m), n, num_classes, nbmax, iou_thr,
+                                            cmp_ge, (unsigned long long*)(ws + w.mask));
     SMB_LAUNCH_OK("mc_mask_kernel");
-    SMB_CUDA_OK(launch_pdl(mc_sweep_kernel, dim3(num_classes), dim3(NT), 0, st, (const unsigned long long*)(ws + w.mask), (const unsigned long long*)(ws + w.keys),
+    mc_sweep_kernel<<<num_classes, NT, 0, st>>>((const unsigned long long*)(ws + w.mask), (const unsigned long long*)(ws + w.keys),
                                                 (const int*)(ws + w.cidx), (const float*)(ws + w.cscore), (const int*)(ws + w.m), n,
-                                                nbmax, (int*)(ws + w.idx), (float*)(ws + w.score), ws_count));
+                                                nbmax, (int*)(ws + w.idx), (float*)(ws + w.score), ws_count);
     SMB_LAUNCH_OK("mc_sweep_kernel");
   }
-  SMB_CUDA_OK(launch_pdl(finalize_kernel, dim3(1), dim3(NT), 0, st, boxes, n, num_classes, max_num, 0, (const int*)(ws + w.idx), (const float*)(ws + w.score),
+  finalize_kernel<<<1, NT, 0, st>>>(boxes, n, num_classes, max_num, 0, (const int*)(ws + w.idx), (const float*)(ws + w.score),
                                     ws_count, nn, (unsigned long long*)(ws + w.gkey), (int*)(ws + w.gval), det_out,
-                                    (long long*)label_out, (long long*)idx_out, count_out));
+                                    (long long*)label_out, (long long*)idx_out, count_out);
   SMB_LAUNCH_OK("finalize_kernel");
   return SMB_OK;
 }
@@ -931,9 +931,9 @@ extern "C" int smb_fast_nms(const float* boxes, const float* scores, const float
   fast_nms_class_kernel<<<num_classes, NT, sizeof(FastSmem), st>>>(boxes, scores, ctr, n, num_classes, score_thr, iou_thr, top_k,
                                                                    (int*)(ws + o_idx), (float*)(ws + o_score), (int*)(ws + o_count));
   SMB_LAUNCH_OK("fast_nms_class_kernel");
-  SMB_CUDA_OK(launch_pdl(finalize_kernel, dim3(1), dim3(NT), 0, st, boxes, n, num_classes, max_num, 1, (const int*)(ws + o_idx), (const float*)(ws + o_score),
+  finalize_kernel<<<1, NT, 0, st>>>(boxes, n, num_classes, max_num, 1, (const int*)(ws + o_idx), (const float*)(ws + o_score),
                                     (const int*)(ws + o_count), top_k, (unsigned long long*)(ws + o_gkey), (int*)(ws + o_gval),
-                                    det_out, (long long*)label_out, (long long*)idx_out, count_out));
+                                    det_out, (long long*)label_out, (long long*)idx_out, count_out);
   SMB_LAUNCH_OK("finalize_kernel");
   return SMB_OK;
 }
@@ -962,16 +962,16 @@ extern "C" int smb_decode_topk(int num_levels, const smb_level_t* host_levels, i
   float* s = (float*)workspace;
   int* sel = (int*)((char*)workspace + s_bytes);
   const int total = L.loc_off[L.num];
-  SMB_CUDA_OK(launch_pdl(level_score_kernel, dim3(min(cdiv(total, 8), 132 * 8)), dim3(256), 0, st, L, num_classes, s));
+  level_score_kernel<<<min(cdiv(total, 8), 132 * 8), 256, 0, st>>>(L, num_classes, s);
   SMB_LAUNCH_OK("level_score_kernel");
-  SMB_CUDA_OK(launch_pdl(level_topk_kernel, dim3(num_levels), dim3(NT), 0, st, L, nms_pre, s, sel));
+  level_topk_kernel<<<num_levels, NT, 0, st>>>(L, nms_pre, s, sel);
   SMB_LAUNCH_OK("level_topk_kernel");
   const int ncand = L.cand_off[L.num];
   const float i0 = host_scale4 ? host_scale4[0] : 1.f, i1 = host_scale4 ? host_scale4[1] : 1.f;
   const float i2 = host_scale4 ? host_scale4[2] : 1.f, i3 = host_scale4 ? host_scale4[3] : 1.f;
-  SMB_CUDA_OK(launch_pdl(gather_decode_kernel, dim3(min(cdiv(ncand, 8), 132 * 8)), dim3(256), 0, st, L, num_classes, img_h, img_w, i0, i1, i2, i3,
+  gather_decode_kernel<<<min(cdiv(ncand, 8), 132 * 8), 256, 0, st>>>(L, num_classes, img_h, img_w, i0, i1, i2, i3,
                                                                     host_scale4 ? 1 : 0, sel, cand_boxes, cand_scores,
-                                                                    cand_ctr, cand_loc));
+                                                                    cand_ctr, cand_loc);
   SMB_LAUNCH_OK("gather_decode_kernel");
   return SMB_OK;
 }
@@ -988,9 +988,9 @@ extern "C" int smb_gather_det_inputs(const float* cof_src, int cof_pitch, const 
   memset(&lm, 0, sizeof(lm));
   lm.num = num_levels; lm.n_img = n_img; lm.img = img;
   for (int l = 0; l < num_levels; ++l) lm.loc_off[l + 1] = lm.loc_off[l] + host_level_hw[l];
-  SMB_CUDA_OK(launch_pdl(gather_det_inputs_kernel, dim3(cdiv(max_rows * row_elems, 256)), dim3(256), 0, (cudaStream_t)stream,
-                         cof_src, cof_pitch, cand_loc, (const long long*)idx, det, count_dev, max_rows, row_elems, det_cofs,
-                         det_boxes, (long long*)loc_out, lm));
+  gather_det_inputs_kernel<<<cdiv(max_rows * row_elems, 256), 256, 0, (cudaStream_t)stream>>>(
+      cof_src, cof_pitch, cand_loc, (const long long*)idx, det, count_dev, max_rows, row_elems, det_cofs, det_boxes,
+      (long long*)loc_out, lm);
   SMB_LAUNCH_OK("gather_det_inputs_kernel");
   return SMB_OK;
 }
@@ -1000,8 +1000,8 @@ extern "C" int smb_gather_track_feats(const float* track, int h, int w, int C, c
                                       smb_stream_t stream) {
   SMB_CHECK_ARG(track && det && count_dev && out && h > 0 && w > 0 && C > 0 && max_rows > 0 && feat_stride > 0.f,
                 "smb_gather_track_feats: bad argument");
-  SMB_CUDA_OK(launch_pdl(gather_track_feats_kernel, dim3(cdiv(max_rows * C, 256)), dim3(256), 0, (cudaStream_t)stream, track, h, w,
-                         C, det, count_dev, max_rows, scale_x, scale_y, feat_stride, out));
+  gather_track_feats_kernel<<<cdiv(max_rows * C, 256), 256, 0, (cudaStream_t)stream>>>(track, h, w, C, det, count_dev, max_rows,
+                                                                                         scale_x, scale_y, feat_stride, out);
   SMB_LAUNCH_OK("gather_track_feats_kernel");
   return SMB_OK;
 }
@@ -1009,8 +1009,8 @@ extern "C" int smb_gather_track_feats(const float* track, int h, int w, int C, c
 extern "C" int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev, int max_rows,
                                    int row_elems, float* dst, smb_stream_t stream) {
   SMB_CHECK_ARG(src && idx && count_dev && dst && max_rows > 0 && row_elems > 0, "smb_gather_rows_f32: bad argument");
-  SMB_CUDA_OK(launch_pdl(gather_rows_kernel, dim3(cdiv(max_rows * row_elems, 256)), dim3(256), 0, (cudaStream_t)stream, src, src_pitch, (const long long*)idx,
-                                                                                         count_dev, max_rows, row_elems, dst));
+  gather_rows_kernel<<<cdiv(max_rows * row_elems, 256), 256, 0, (cudaStream_t)stream>>>(src, src_pitch, (const long long*)idx,
+                                                                                         count_dev, max_rows, row_elems, dst);
   SMB_LAUNCH_OK("gather_rows_kernel");
   return SMB_OK;
 }

@@ -1,5 +1,5 @@
 // Test-time image pipeline on the device (SURVEY.md 8f-3): uint8 BGR HWC image -> keep-ratio bilinear resize ->
-// mean subtraction -> zero pad -> the stem's NHWC8 fp16 layout, in one kernel.
+// mean subtraction -> zero pad -> the stem's space-to-depth fp16 layout, in one kernel.
 //
 // Reference: Resize(keep_ratio) / Normalize(std=1, to_rgb=False) / Pad(32) / ImageToTensor on the host CPU
 // (SipMask-mmdetection/mmdet/datasets/pipelines/transforms.py:97-110, 274-300, 335-363), i.e. mmcv -> cv2.resize(INTER_LINEAR),
@@ -75,18 +75,6 @@ __device__ __forceinline__ void pre_pixel(const PreArgs& a, int x, int y, float*
   }
 }
 
-// out [H+6, W+8, 8] fp16: pixel (y, x) at (y+3, x+3); zeros in the halo, the padding and channels 3..7
-__global__ void preprocess_u8_kernel(PreArgs a, __half* __restrict__ out, int H, int W) {
-  const int Hp = H + 6, Wp = W + 8;
-  const long long total = (long long)Hp * Wp;
-  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)blockDim.x * gridDim.x) {
-    const int xp = (int)(t % Wp), yp = (int)(t / Wp);
-    float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    pre_pixel(a, xp - 3, yp - 3, f);
-    *reinterpret_cast<uint4*>(out + t * 8) = pack8h(f);
-  }
-}
-
 // Space-to-depth layout of the 7x7/2 stem: out [H/2+3, W/2+4, 16] fp16, element (Y, X, (dy*2+dx)*4 + c) = padded pixel
 // (2Y+dy, 2X+dx) = image pixel (2Y+dy-3, 2X+dx-3), channel c (c == 3: zero).  One thread = one 32-byte (Y, X) cell.
 __global__ void preprocess_u8_s2d_kernel(PreArgs a, __half* __restrict__ out, int H, int W) {
@@ -110,31 +98,20 @@ __global__ void preprocess_u8_s2d_kernel(PreArgs a, __half* __restrict__ out, in
 
 using namespace smb;
 
-static int preprocess_impl(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
-                           const float* host_mean3, void* out, int H, int W, int s2d, smb_stream_t stream) {
-  SMB_CHECK_ARG(src && host_mean3 && out, "smb_preprocess_u8: null pointer");
+extern "C" int smb_preprocess_u8_s2d(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
+                                     const float* host_mean3, void* out, int H, int W, smb_stream_t stream) {
+  SMB_CHECK_ARG(src && host_mean3 && out, "smb_preprocess_u8_s2d: null pointer");
   SMB_CHECK_ARG(src_h > 0 && src_w > 0 && src_pitch_bytes >= 3 * src_w && dst_h > 0 && dst_w > 0 && dst_h <= H && dst_w <= W,
-                "smb_preprocess_u8: bad shape (src %dx%d -> %dx%d inside %dx%d)", src_h, src_w, dst_h, dst_w, H, W);
-  SMB_CHECK_ARG(!s2d || (H % 2 == 0 && W % 2 == 0), "smb_preprocess_u8_s2d: H, W must be even");
+                "smb_preprocess_u8_s2d: bad shape (src %dx%d -> %dx%d inside %dx%d)", src_h, src_w, dst_h, dst_w, H, W);
+  SMB_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "smb_preprocess_u8_s2d: H, W must be even");
   PreArgs a;
   a.src = src; a.sh = src_h; a.sw = src_w; a.pitch = src_pitch_bytes; a.dh = dst_h; a.dw = dst_w;
   a.scale_y = 1.0 / ((double)dst_h / src_h); a.scale_x = 1.0 / ((double)dst_w / src_w);
   a.m0 = host_mean3[0]; a.m1 = host_mean3[1]; a.m2 = host_mean3[2];
-  const long long total = s2d ? (long long)(H / 2 + 3) * (W / 2 + 4) : (long long)(H + 6) * (W + 8);
+  const long long total = (long long)(H / 2 + 3) * (W / 2 + 4);
   int blocks = (int)((total + 255) / 256);
   if (blocks > 132 * 16) blocks = 132 * 16;
-  if (s2d) preprocess_u8_s2d_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, (__half*)out, H, W);
-  else preprocess_u8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, (__half*)out, H, W);
-  SMB_LAUNCH_OK("preprocess_u8_kernel");
+  preprocess_u8_s2d_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, (__half*)out, H, W);
+  SMB_LAUNCH_OK("preprocess_u8_s2d_kernel");
   return SMB_OK;
-}
-
-extern "C" int smb_preprocess_u8(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
-                                 const float* host_mean3, void* out_nhwc8, int H, int W, smb_stream_t stream) {
-  return preprocess_impl(src, src_h, src_w, src_pitch_bytes, dst_h, dst_w, host_mean3, out_nhwc8, H, W, 0, stream);
-}
-
-extern "C" int smb_preprocess_u8_s2d(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
-                                     const float* host_mean3, void* out_s2d16, int H, int W, smb_stream_t stream) {
-  return preprocess_impl(src, src_h, src_w, src_pitch_bytes, dst_h, dst_w, host_mean3, out_s2d16, H, W, 1, stream);
 }

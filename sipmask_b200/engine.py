@@ -1,16 +1,17 @@
 """SipMask inference engine: the whole per-image hot path as a fixed sequence of sm_90a kernel launches.
 
-    image (NCHW fp32) -> NHWC8 fp16 -> ResNet-50/101 (caffe, folded BN) -> FPN P3..P7 -> FCOS towers (conv+GN+ReLU)
-    -> FeatureAlign (DCN) -> cls/centerness/reg/coefficient heads -> prototype branch -> decode/top-k -> NMS ->
-    mask assembly -> x2 upsample + threshold (bit-packed)
+    image (NCHW fp32) -> space-to-depth fp16 -> ResNet-50/101 (caffe, folded BN) -> FPN P3..P7 -> FCOS towers
+    (conv+GN+ReLU) -> FeatureAlign (DCN) -> cls/centerness/reg/coefficient heads -> prototype branch -> decode/top-k ->
+    NMS -> mask assembly -> x2 upsample + threshold (bit-packed)
 
 Reference call stack replaced (SipMask-mmdetection/mmdet/): detectors/single_stage.py:75-93,
 backbones/resnet.py:501-512, necks/fpn.py:138-178, anchor_heads/sipmask_head.py:241-287,500-662.
 Weights come from a reference-keyed state_dict (SURVEY.md §8b); all buffers are allocated once, TMA descriptors
-are baked into per-layer plans, and the launch sequence can be replayed as one CUDA graph.
+are baked into per-layer plans, and the launch sequence can be replayed as one CUDA graph.  Independent branches run on
+side streams: the projection shortcut of residual stages 2-4, P5 -> P6 -> P7, the reg tower next to the cls tower, the
+prototype branch next to FeatureAlign / the cls heads, and (batch > 1) the per-image post-processing chains.
 """
 import ctypes
-import os
 
 import numpy as np
 import torch
@@ -25,8 +26,8 @@ ARCH = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
 class SipMaskEngine(object):
     def __init__(self, state_dict, img_hw, batch=1, depth=50, stacked_convs=4, gn=True, ssd_flag=False, num_classes=81,
                  strides=(8, 16, 32, 64, 128), test_cfg=None, img_shape=None, scale_factor=1.0, device='cuda',
-                 mask_thr=0.4, use_graph=True, pos_dtype=torch.float32, head_only=False, feat_sizes=None, in_channels=256,
-                 fcos=False, prefix_head='bbox_head.', build_postproc=True, two_streams=True, share_weights=None,
+                 mask_thr=0.4, use_graph=True, head_only=False, feat_sizes=None, in_channels=256,
+                 fcos=False, prefix_head='bbox_head.', build_postproc=True, share_weights=None,
                  max_ctas=None, head_max_ctas=None, backbone_dcn=False, ori_shape=None, legacy_interp=False, vis=False):
         self.dev = torch.device(device)
         if self.dev.index is None:
@@ -36,9 +37,6 @@ class SipMaskEngine(object):
         self.N, (self.H, self.W) = batch, img_hw
         self.head_only, self.feat_sizes, self.in_channels, self.fcos = head_only, feat_sizes, in_channels, fcos
         self.hp, self.build_post = prefix_head, build_postproc
-        self.two_streams = two_streams and os.environ.get('SMB_TWO_STREAMS', '1') != '0'
-        self.fork_branches = self.two_streams and os.environ.get('SMB_FORK_BRANCHES', '1') != '0'
-        self.fork_from_layer = int(os.environ.get('SMB_FORK_FROM_LAYER', '1'))      # 0-based residual stage index
         # batch > 1: N images per forward (the reference's forward_test asserts imgs_per_gpu == 1, base.py:118-119, but
         # get_bboxes loops over images, sipmask_head.py:517-540; BASELINE config 4 is a bs=32 throughput mode)
         assert head_only or (self.H % 32 == 0 and self.W % 32 == 0), 'images are padded to a multiple of 32 (Pad size_divisor=32)'
@@ -59,7 +57,6 @@ class SipMaskEngine(object):
         self.ori_shape = tuple(ori_shape) if ori_shape is not None else self.img_shape
         self.legacy_interp = legacy_interp
         self.mask_thr = 0.5 if (vis and mask_thr == 0.4) else mask_thr      # VIS thresholds at 0.5 (VIS/...:764), MM at 0.4
-        self.pos_dtype = pos_dtype
         self.sd = {k: v for k, v in state_dict.items()}
         self.ops = []            # list of zero-argument callables = the launch sequence
         self.op_names = []
@@ -74,7 +71,7 @@ class SipMaskEngine(object):
         self._wcache = ({} if share_weights is None else share_weights if isinstance(share_weights, dict)
                         else share_weights._wcache)
         self.max_ctas = max_ctas                   # persistent-grid cap of every conv (None: all SMs)
-        self.head_max_ctas = head_max_ctas         # cap inside the two-stream head section (None: env / 100)
+        self.head_max_ctas = head_max_ctas         # cap inside the two-stream head section (None: 100)
         self.conv_plans = []
         self.conv_meta = []
         self.conv_flops = 0.0
@@ -150,27 +147,19 @@ class SipMaskEngine(object):
                 self._build_head(self.fpn_outs)
             return
         self.img = self._t(N, 3, H, W, dtype=torch.float32)
-        # ---- stem
-        # stem input: space-to-depth [N,H/2+3,W/2+4,16] (K = 256) by default, the 8-pixel-window NHWC8 form (K = 448) with
-        # SMB_STEM_S2D=0 (kept for A/B timing); the op keeps its round-1 name 'image_to_nhwc8' either way
-        s2d = os.environ.get('SMB_STEM_S2D', '1') != '0'
-        img8 = self._t(N, H // 2 + 3, W // 2 + 4, 16) if s2d else self._t(N, H + 6, W + 8, 8)
+        # ---- stem: space-to-depth input [N,H/2+3,W/2+4,16], K = 256
+        img8 = self._t(N, H // 2 + 3, W // 2 + 4, 16)
         self.img8 = img8
-        if s2d:
-            self._add(lambda: C.image_to_s2d16(self.img, img8), name='image_to_nhwc8')
-            wk, b = self._once('stem_s2d', lambda: C.pack_stem_weight_s2d(self._w('backbone.conv1.weight'), self._bn('backbone.bn1'),
-                                                                          device=self.dev))
-        else:
-            self._add(lambda: C.image_to_nhwc8(self.img, img8), name='image_to_nhwc8')
-            wk, b = self._once('stem', lambda: C.pack_stem_weight(self._w('backbone.conv1.weight'), self._bn('backbone.bn1'),
-                                                                  device=self.dev))
+        self._add(lambda: C.image_to_s2d16(self.img, img8), name='image_to_s2d16')
+        wk, b = self._once('stem_s2d', lambda: C.pack_stem_weight_s2d(self._w('backbone.conv1.weight'), self._bn('backbone.bn1'),
+                                                                      device=self.dev))
         s1 = self._t(N, H // 2, W // 2, 64)
-        stem = C.StemPlan(img8, wk, b, s1, N, H, W, s2d=s2d)
+        stem = C.StemPlan(img8, wk, b, s1, N, H, W)
         self._keep += [stem, wk, b]
         self.conv_plans.append(stem)
-        fl = 2.0 * N * (H // 2) * (W // 2) * 64 * 147                                 # algorithmic 7x7x3 (executed K is 256 / 448)
+        fl = 2.0 * N * (H // 2) * (W // 2) * 64 * 147                                 # algorithmic 7x7x3 (executed K is 256)
         self.conv_flops += fl
-        self.conv_meta.append(dict(name='stem', M=N * (H // 2) * (W // 2), N=64, K=256 if s2d else 448, k=7, stride=2, flops=fl,
+        self.conv_meta.append(dict(name='stem', M=N * (H // 2) * (W // 2), N=64, K=256, k=7, stride=2, flops=fl,
                                    res=False, gn=False))
         self._add(stem.run, name='conv')
         x = self._t(N, H // 4, W // 4, 64)
@@ -183,7 +172,7 @@ class SipMaskEngine(object):
                 stride = 2 if (j == 0 and i > 0) else 1
                 # the projection shortcut only depends on the block input: it runs on the side stream next to conv1/conv2
                 # (layers 2-4 are short latency-bound launches that leave most SMs idle)
-                side = self.fork_branches and j == 0 and i >= self.fork_from_layer
+                side = j == 0 and i >= 1
                 if side:
                     self._marker('fork')
                     self._tag = 1
@@ -211,22 +200,18 @@ class SipMaskEngine(object):
         c3, c4, c5 = feats[1], feats[2], feats[3]
         # ---- FPN (fpn.py:138-178): laterals top-down with the nearest-upsample add fused into the epilogue
         lat5 = self._conv(c5, 'neck.lateral_convs.2.conv.weight', 1, bias_key='neck.lateral_convs.2.conv.bias')
-        if self.fork_branches:
-            # P5 -> P6 -> P7 is a chain of tiny convolutions (9 / 3 / 1 M-tiles): side stream, next to the P4 / P3 laterals
-            self._marker('fork')
-            self._tag = 1
-            p5, p6, p7 = self._fpn_top(lat5)
-            self._tag = 0
+        # P5 -> P6 -> P7 is a chain of tiny convolutions (9 / 3 / 1 M-tiles): side stream, next to the P4 / P3 laterals
+        self._marker('fork')
+        self._tag = 1
+        p5, p6, p7 = self._fpn_top(lat5)
+        self._tag = 0
         lat4 = self._conv(c4, 'neck.lateral_convs.1.conv.weight', 1, bias_key='neck.lateral_convs.1.conv.bias',
                           residual=lat5, residual_upsample=True)
         lat3 = self._conv(c3, 'neck.lateral_convs.0.conv.weight', 1, bias_key='neck.lateral_convs.0.conv.bias',
                           residual=lat4, residual_upsample=True)
         p3 = self._conv(lat3, 'neck.fpn_convs.0.conv.weight', 3, bias_key='neck.fpn_convs.0.conv.bias')
         p4 = self._conv(lat4, 'neck.fpn_convs.1.conv.weight', 3, bias_key='neck.fpn_convs.1.conv.bias')
-        if self.fork_branches:
-            self._marker('join')
-        else:
-            p5, p6, p7 = self._fpn_top(lat5)
+        self._marker('join')
         self.fpn_outs = [p3, p4, p5, p6, p7]
         self._build_head(self.fpn_outs)
 
@@ -327,28 +312,25 @@ class SipMaskEngine(object):
         # The cls and reg towers are independent chains of 202-tile GEMMs (1.5 waves each on 132 SMs).  They are
         # captured on two streams with their persistent grids capped at half the GPU, so together they keep every SM
         # busy (3.06 waves for a pair instead of 2 + 2).
-        two = self.two_streams
-        if two:
-            self._marker('fork')
-            cap = self.head_max_ctas if self.head_max_ctas is not None else int(os.environ.get('SMB_HEAD_MAX_CTAS', '100'))
-            if self.max_ctas:
-                cap = min(cap, self.max_ctas) if cap else self.max_ctas
-            self._max_ctas = cap or None
+        self._marker('fork')
+        cap = self.head_max_ctas if self.head_max_ctas is not None else 100
+        if self.max_ctas:
+            cap = min(cap, self.max_ctas) if cap else self.max_ctas
+        self._max_ctas = cap or None
         self._tag = 0
         for i in range(self.stacked - 1):
             cls_feats = self._tower_conv(cls_feats, hp + 'cls_convs.%d.conv.weight' % i, hp + 'cls_convs.%d.gn' % i,
                                          hp + 'cls_convs.%d.conv.bias' % i, [self.gn_arena[si, l] for l in range(nl)])
             si += 1
-        self._tag = 1 if two else 0
+        self._tag = 1
         for i in range(self.stacked):
             reg_feats = self._tower_conv(reg_feats, hp + 'reg_convs.%d.conv.weight' % i, hp + 'reg_convs.%d.gn' % i,
                                          hp + 'reg_convs.%d.conv.bias' % i, [self.gn_arena[si, l] for l in range(nl)])
             si += 1
         # fcos_reg | fcos_centerness on the reg tower (sipmask_head.py:261,265), raw fp32 (Scale applied by consumers)
         self._conv_multi(reg_feats, wk_reg, 3, outs=regctr_l, bias=b_reg, cout_real=5)
-        if two:
-            self._marker('join')
-            self._marker('fork')
+        self._marker('join')
+        self._marker('fork')
         self._tag = 0
         # FeatureAlign: offsets from scale*fcos_reg, DCN 3x3 dg=4, GN, ReLU (sipmask_head.py:49-55)
         offs = [self._t(N, h, w, 72, dtype=torch.float32) for h, w in sizes]
@@ -367,7 +349,7 @@ class SipMaskEngine(object):
         # fcos_cls | sip_cof on the aligned feature (sipmask_head.py:264,271)
         self._conv_multi(aligned, wk_cls, 3, outs=clscof_l, bias=b_cls)
         # prototype branch on the side stream, next to FeatureAlign / the cls heads
-        self._tag = 1 if two else 0
+        self._tag = 1
         # prototype input: reg feature of levels 0..2 at P3 resolution (sipmask_head.py:275-281)
         h3, w3 = sizes[0]
         cat = self._t(N, h3, w3, 768)
@@ -378,8 +360,7 @@ class SipMaskEngine(object):
         m1 = self._conv(m0, hp + 'sip_mask_lat.weight', 3, relu=True, bias_key=hp + 'sip_mask_lat.bias')
         self.protos = self._t(N, 4 * h3, 4 * w3, 32)
         self._add(lambda: C.upsample_bilinear(m1, 4, out=self.protos), name='upsample')
-        if two:
-            self._marker('join')
+        self._marker('join')
         self._tag = 0
         if self.vis:
             # tracking branch (VIS/...:274-287,296-312): track_convs on levels 0..2 -> bilinear x1 / x2 / x4 to P3 resolution ->
@@ -484,7 +465,7 @@ class SipMaskEngine(object):
         self._keep.append(level_hw)
         # the per-image decode -> NMS -> gather -> mask chains are independent (get_bboxes loops over images,
         # sipmask_head.py:517-540): with a batch they are spread over a few streams of the captured graph
-        pp_streams = min(N, int(os.environ.get('SMB_POSTPROC_STREAMS', '4'))) if N > 1 else 0
+        pp_streams = min(N, 4) if N > 1 else 0
         if pp_streams:
             self._marker('fork')
         for n in range(N):
@@ -624,7 +605,7 @@ class SipMaskEngine(object):
     def forward_raw(self, img_u8, mean=(102.9801, 115.9465, 122.7717)):
         """img_u8: uint8 BGR HWC CUDA image straight from the decoder.  Resize (keep ratio, mmcv.imrescale rule towards this
         engine's img_shape) + mean subtraction + padding + layout run in ONE kernel that writes the stem's input
-        (SURVEY.md 8f-3); the rest of the step is the CUDA graph without its `image_to_nhwc8` node.  The resized size must
+        (SURVEY.md 8f-3); the rest of the step is the CUDA graph without its `image_to_s2d16` node.  The resized size must
         equal the engine's img_shape (one engine per input resolution); batch 1."""
         assert self.N == 1, 'forward_raw preprocesses one image'
         if torch.cuda.current_device() != self.dev.index:
@@ -633,7 +614,7 @@ class SipMaskEngine(object):
         C.preprocess_u8(img_u8, self.img_shape[:2], self.img8, mean)
         if self.use_graph:
             if getattr(self, 'graph_raw', None) is None:
-                names = set(self.op_names) - {'image_to_nhwc8', 'fork', 'join'}
+                names = set(self.op_names) - {'image_to_s2d16', 'fork', 'join'}
                 self._run_ops(only=names)
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()
@@ -642,7 +623,7 @@ class SipMaskEngine(object):
                 self.graph_raw = g
             self.graph_raw.replay()
         else:
-            self._run_ops(only=set(self.op_names) - {'image_to_nhwc8', 'fork', 'join'})
+            self._run_ops(only=set(self.op_names) - {'image_to_s2d16', 'fork', 'join'})
         return self._result()
 
     # head outputs in the reference's layout (for parity tests / the drop-in head)

@@ -133,7 +133,7 @@ def test_conv_fp32_heads_alpha_and_fpn_residual():
         _check(out, _ref_conv(xin, wk, 1, 1, bias=b, residual=up))
 
 
-@pytest.mark.parametrize('H,W', [(64, 96), (160, 224)])
+@pytest.mark.parametrize('H,W', [(64, 96), (160, 224), (96, 128), (224, 352)])
 def test_stem_matches_reference(H, W):
     from sipmask_b200 import conv, synth
     g = torch.Generator().manual_seed(7)
@@ -141,26 +141,23 @@ def test_stem_matches_reference(H, W):
     w = torch.randn(64, 3, 7, 7, generator=g) * 0.01
     bn = (torch.rand(64, generator=g) + 0.5, torch.randn(64, generator=g) * 0.1, torch.randn(64, generator=g) * 0.1,
           torch.rand(64, generator=g) + 0.5)
-    wk, bias = conv.pack_stem_weight(w, bn, device='cuda')
-    img8 = conv.image_to_nhwc8(img)
+    wk, bias = conv.pack_stem_weight_s2d(w, bn, device='cuda')
+    q = conv.image_to_s2d16(img)
+    Hq, Wq = H // 2 + 3, W // 2 + 4
+    assert q.shape == (2, Hq, Wq, 16)
+    # host-built layout: the fp16 image zero-padded by 3 (to [H+6, W+8], 4 channels), q(Y, X, (dy*2+dx)*4 + c) = padded
+    # pixel (2Y+dy, 2X+dx, c)
+    p = torch.zeros(2, H + 6, W + 8, 4)
+    p[:, 3:3 + H, 3:3 + W, :3] = img.cpu().half().float().permute(0, 2, 3, 1)
+    want_q = p.view(2, Hq, 2, Wq, 2, 4).permute(0, 1, 3, 2, 4, 5).reshape(2, Hq, Wq, 16)
+    assert torch.equal(q.float().cpu(), want_q)
     out = torch.empty((2, H // 2, W // 2, 64), dtype=torch.float16, device='cuda')
-    conv.StemPlan(img8, wk, bias, out, 2, H, W).run()
+    conv.StemPlan(q, wk, bias, out, 2, H, W).run()
     torch.cuda.synchronize()
     s = (bn[0] / torch.sqrt(bn[3] + 1e-5)).cuda()
     wq = (w.cuda() * s.view(-1, 1, 1, 1)).half().double()
     y = F.conv2d(img.half().double(), wq, stride=2, padding=3) + bias.double().view(1, -1, 1, 1)
     _check(out, y.clamp(min=0).permute(0, 2, 3, 1))
-    # space-to-depth form (K = 256): same convolution, same fp16 weights, different summation grouping only
-    wk2, bias2 = conv.pack_stem_weight_s2d(w, bn, device='cuda')
-    q = conv.image_to_s2d16(img)
-    assert q.shape == (2, H // 2 + 3, W // 2 + 4, 16)
-    p8 = img8.float()                                           # [2, H+6, W+8, 8]: padded pixels, channels 0..2 real
-    want_q = p8.view(2, H // 2 + 3, 2, W // 2 + 4, 2, 8)[..., :4].permute(0, 1, 3, 2, 4, 5).reshape(2, H // 2 + 3, W // 2 + 4, 16)
-    assert torch.equal(q.float(), want_q)                       # q(Y, X, (dy*2+dx)*4 + c) = padded pixel (2Y+dy, 2X+dx, c)
-    out2 = torch.empty_like(out)
-    conv.StemPlan(q, wk2, bias2, out2, 2, H, W, s2d=True).run()
-    torch.cuda.synchronize()
-    _check(out2, y.clamp(min=0).permute(0, 2, 3, 1))
     # max pool 3x3/2 pad 1 (resnet.py:460)
     mp = conv.maxpool3x3s2(out)
     ref = F.max_pool2d(out.float().permute(0, 3, 1, 2), 3, 2, 1).permute(0, 2, 3, 1)

@@ -107,3 +107,18 @@ def test_fp16_hi_lo_coefficient_split_keeps_fp32_logits():
             seq = seq + p[:, k].astype(np.float32) * cc[:, k]
         assert (np.abs(seq.astype(np.float64) - exact) <= bound).all(), scale
 
+
+
+def test_groupnorm_apply_multi_rejects_unsupported_channels():
+    """The multi-level GroupNorm apply covers C in {256, 512, 1024, 2048}; any other C is refused before a launch (the
+    argument checks run first, so the placeholder pointers are never dereferenced)."""
+    import ctypes
+    from sipmask_b200 import _lib
+    lib = _lib.lib()
+    ptrs = (ctypes.c_void_p * 1)(16)
+    hw = (ctypes.c_int * 1)(4)
+    for C in (128, 768, 4096):
+        rc = lib.smb_groupnorm_relu_apply_multi(1, ptrs, ptrs, hw, hw, 1, C, C, ctypes.c_void_p(16), ctypes.c_void_p(16),
+                                                ctypes.c_float(1e-5), 1, None)
+        assert rc == -1, C
+        assert b'unsupported' in lib.smb_last_error()

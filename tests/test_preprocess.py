@@ -37,22 +37,24 @@ def test_oracle_pipeline_matches_cv2_steps():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('h,w', [(480, 640), (375, 500), (800, 1333), (1080, 1920)])
+@pytest.mark.parametrize('h,w', [(480, 640), (375, 500), (800, 1333), (1080, 1920), (427, 640), (333, 500), (64, 48),
+                                 (720, 1280)])
 def test_device_preprocess_bit_exact(h, w):
     from sipmask_b200 import conv as C
     img = _img(h, w, 3 * h + w)
     x, meta = P.preprocess(img)
     nh, nw = meta['img_shape'][:2]
     H, W = meta['pad_shape'][:2]
-    out = torch.full((1, H + 6, W + 8, 8), 7.0, dtype=torch.float16, device='cuda')
+    Hq, Wq = H // 2 + 3, W // 2 + 4
+    out = torch.full((1, Hq, Wq, 16), 7.0, dtype=torch.float16, device='cuda')
     C.preprocess_u8(torch.from_numpy(img).cuda(), (nh, nw), out, P.MEAN_BGR)
-    want = torch.empty_like(out)
-    C.image_to_nhwc8(torch.from_numpy(x).cuda(), want)                          # the fp32 path of the engine
-    assert torch.equal(out, want)
-    # space-to-depth layout of the stem (engine default)
-    out2 = torch.full((1, H // 2 + 3, W // 2 + 4, 16), 7.0, dtype=torch.float16, device='cuda')
-    C.preprocess_u8(torch.from_numpy(img).cuda(), (nh, nw), out2, P.MEAN_BGR)
-    assert torch.equal(out2, C.image_to_s2d16(torch.from_numpy(x).cuda()))
+    assert torch.equal(out, C.image_to_s2d16(torch.from_numpy(x).cuda()))      # the fp32 path of the engine
+    # the oracle's image in the stem's space-to-depth layout, built on the host: zero-padded by 3 (to [H+6, W+8], 4
+    # channels), q(Y, X, (dy*2+dx)*4 + c) = padded pixel (2Y+dy, 2X+dx, c)
+    p = np.zeros((H + 6, W + 8, 4), np.float16)
+    p[3:3 + H, 3:3 + W, :3] = x[0].transpose(1, 2, 0)
+    want = p.reshape(Hq, 2, Wq, 2, 4).transpose(0, 2, 1, 3, 4).reshape(1, Hq, Wq, 16)
+    assert np.array_equal(out.cpu().numpy(), want)
 
 
 @pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""Graph-replay time of the head section (first fork .. last join) under different stream / grid-cap settings."""
+"""Graph-replay time of the head section (first fork .. last join) for several persistent-grid caps (head_max_ctas)."""
 import os
 import sys
 import torch
@@ -10,19 +10,14 @@ from sipmask_b200.engine import SipMaskEngine  # noqa: E402
 
 sd = synth.detector_state_dict(50, seed=1, cls_bias=bench.CLS_BIAS)
 img = synth.synthetic_image(bench.H, bench.W, seed=0).cuda()
-for two, cap in ((False, '0'), (True, '74'), (True, '0'), (True, '100')):
-    os.environ['SMB_HEAD_MAX_CTAS'] = cap
+for cap in (74, 0, 100):
     eng = SipMaskEngine(sd, (bench.H, bench.W), test_cfg=bench.TEST_CFG, img_shape=(bench.H, bench.IMG_W, 3), use_graph=False,
-                        two_streams=two)
+                        head_max_ctas=cap)
     eng.forward(img)
     torch.cuda.synchronize()
     names = eng.op_names
-    if two:
-        first = names.index('fork')
-        last = len(names) - 1 - names[::-1].index('join')
-    else:
-        first = names.index('memset') + 1
-        last = max(i for i, n in enumerate(names) if n == 'upsample')
+    first = names.index('fork', names.index('memset'))
+    last = len(names) - 1 - names[::-1].index('join')
     sub = list(range(first, last + 1))
     full_ops, full_tags, full_names = eng.ops, eng.op_tags, eng.op_names
     eng.ops = [full_ops[i] for i in sub]
@@ -42,5 +37,5 @@ for two, cap in ((False, '0'), (True, '74'), (True, '0'), (True, '100')):
         g.replay()
     e1.record()
     torch.cuda.synchronize()
-    print('two_streams=%s cap=%s: head section %.1f us (%d ops)' % (two, cap, e0.elapsed_time(e1) / 20 * 1e3, len(sub)))
+    print('head_max_ctas=%s: head section %.1f us (%d ops)' % (cap, e0.elapsed_time(e1) / 20 * 1e3, len(sub)))
     del eng, g

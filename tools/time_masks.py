@@ -1,7 +1,8 @@
-"""Times the two mask ABI calls (dense pos_masks, fused bit-packed) at the BASELINE config-A sizes for the CURRENT
-environment (SMB_MASK_MMA / SMB_MASK_TILE / SMB_MASK_FUSED_TY are read once per process): N = 100 detections with
-32-512 px boxes on a 400 x 672 x 32 fp16 prototype map, L2 flushed between launches, CUDA events, median of 12.
-Prints one JSON line."""
+"""Times the two mask ABI calls (dense pos_masks, fused bit-packed) at the BASELINE config-A sizes for one kernel family:
+N = 100 detections with 32-512 px boxes on a 400 x 672 x 32 fp16 prototype map, L2 flushed between launches, CUDA
+events, median of 12.  Prints one JSON line.
+
+usage: python tools/time_masks.py [tensor|scalar]      (default: tensor)"""
 import json
 import os
 import statistics
@@ -12,6 +13,9 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from sipmask_b200 import ops  # noqa: E402
 
+family = sys.argv[1] if len(sys.argv) > 1 else 'tensor'
+assert family in ('tensor', 'scalar'), 'family must be tensor or scalar'
+ops.set_mask_tensor_dot(family == 'tensor')
 dev = 'cuda'
 H, W, IMG_W, N = 800, 1344, 1333, 100
 Hm, Wm = H // 2, W // 2
@@ -43,6 +47,6 @@ dense = time_kernel(lambda: ops.mask_assemble(protos, cofs, boxes, 0.5, layout='
 fused = time_kernel(lambda: ops.mask_assemble_pack(protos, cofs, boxes, 0.5, (H, IMG_W), 0.4, layout='hwc', out=bits))
 dense_bytes = Hm * Wm * 64 + N * 528 + N * Hm * Wm * 4
 fused_bytes = Hm * Wm * 64 + N * 528 + bits.numel() * 4
-print(json.dumps(dict(env={k: v for k, v in os.environ.items() if k.startswith('SMB_MASK')}, tensor_dot=ops.set_mask_tensor_dot(None),
+print(json.dumps(dict(family=family,
                       dense_ms=dense, dense_gbs=dense_bytes / dense / 1e6, fused_ms=fused, fused_gbs=fused_bytes / fused / 1e6,
                       checksum=[int(bits.ne(0).sum()), float(pos.sum())])))
