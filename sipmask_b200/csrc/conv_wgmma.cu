@@ -28,7 +28,10 @@ constexpr int kMaxTaps = 9;
 constexpr int kMaxMaps = 8;
 constexpr int kMaxLevels = 5;
 constexpr int kConsumerWarps = 8;
-constexpr int kThreads = 32 * (kConsumerWarps + 1);   // + the TMA producer warp
+// + a producer warpgroup: warp 8 issues the TMA loads, warps 9-11 exist only so that the CTA is whole warpgroups, which
+// setmaxnreg needs to move registers from the producer (40 per thread) to the consumers (232 instead of 168)
+constexpr int kThreads = 32 * (kConsumerWarps + 4);
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int kProducerWarp = kConsumerWarps;
 constexpr int kABytes = 128 * 64 * 2;                // one A stage: 128 pixels x 64 channels fp16
 constexpr size_t kSmemBudget = 220 * 1024;           // operand stages + barriers (227 KB per block on sm_90)
@@ -271,50 +274,67 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
   }
   const int cq = 2 * (lane & 3);
   float gsum = 0.f, gsq = 0.f;                       // GroupNorm partials of the current 16-channel group (gn_group 16)
+  // The output may alias the residual as far as the compiler knows, so a residual load written after a store cannot be
+  // issued before it: one 8-channel block at a time, every residual load would wait a full memory round trip.  The
+  // bias and residual operands of kEpiChunk blocks are therefore loaded together, then combined and stored (at N = 256
+  // next to 128 accumulators: this is what the consumers' 232 registers are for).
+  constexpr int kEpiChunk = 8;
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    const int ch0 = tc.n0 + 8 * j;                   // first channel of this 8-channel block (warp-uniform)
-    if (ch0 >= p.Cout) break;
-    const int ch = ch0 + cq;
-    float b0 = 0.f, b1 = 0.f;
-    if (p.bias) { b0 = __ldg(p.bias + ch); b1 = __ldg(p.bias + ch + 1); }
-    float s = 0.f, q = 0.f;
+  for (int j0 = 0; j0 < N / 8; j0 += kEpiChunk) {
+    if (tc.n0 + 8 * j0 >= p.Cout) break;
+    float2 bb[kEpiChunk], rr[kEpiChunk][2];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      float f0 = acc[4 * j + 2 * i] + b0, f1 = acc[4 * j + 2 * i + 1] + b1;
-      if (p.alpha != 1.0f) { f0 *= p.alpha; f1 *= p.alpha; }
-      if (res_row[i]) {
-        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(res_row[i] + ch));
-        f0 += r.x; f1 += r.y;
-      }
-      if (valid[i]) { s += f0 + f1; q += f0 * f0 + f1 * f1; }
-      if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-      if (valid[i]) {
-        if (p.out_f32) {
-          *reinterpret_cast<float2*>(reinterpret_cast<float*>(L.out) + pix[i] * p.out_pitch + ch) = make_float2(f0, f1);
-        } else {
-          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(L.out) + pix[i] * p.out_pitch + ch) = __floats2half2_rn(f0, f1);
-        }
-      }
+    for (int jj = 0; jj < kEpiChunk; ++jj) {
+      const int ch = tc.n0 + 8 * (j0 + jj) + cq;
+      bb[jj] = make_float2(0.f, 0.f);
+      rr[jj][0] = rr[jj][1] = make_float2(0.f, 0.f);
+      if (ch - cq >= p.Cout) continue;
+      if (p.bias) bb[jj] = make_float2(__ldg(p.bias + ch), __ldg(p.bias + ch + 1));
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+        if (res_row[i]) rr[jj][i] = __half22float2(*reinterpret_cast<const __half2*>(res_row[i] + ch));
     }
-    if (p.gn_group) {
-      // per-(image, group) sum / sum of squares of the conv output (pre-activation): fp32 over the warp's 16 rows, then
-      // 64-bit fixed-point integer atomics (associative -> bit-reproducible run to run, whatever the tile order).
-      gsum += s; gsq += q;
-      if (p.gn_group == 8 || (j & 1)) {
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
-          gsq += __shfl_xor_sync(0xffffffffu, gsq, o);
+    for (int jj = 0; jj < kEpiChunk; ++jj) {
+      const int j = j0 + jj;
+      const int ch0 = tc.n0 + 8 * j;                 // first channel of this 8-channel block (warp-uniform)
+      if (ch0 >= p.Cout) break;
+      const int ch = ch0 + cq;
+      float s = 0.f, q = 0.f;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float f0 = acc[4 * j + 2 * i] + bb[jj].x, f1 = acc[4 * j + 2 * i + 1] + bb[jj].y;
+        if (p.alpha != 1.0f) { f0 *= p.alpha; f1 *= p.alpha; }
+        if (res_row[i]) { f0 += rr[jj][i].x; f1 += rr[jj][i].y; }
+        if (valid[i]) { s += f0 + f1; q += f0 * f0 + f1 * f1; }
+        if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+        if (valid[i]) {
+          if (p.out_f32) {
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(L.out) + pix[i] * p.out_pitch + ch) = make_float2(f0, f1);
+          } else {
+            *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(L.out) + pix[i] * p.out_pitch + ch) = __floats2half2_rn(f0, f1);
+          }
         }
-        if (lane == 0) {
-          const int ngroups = p.Cout / p.gn_group;
-          unsigned long long* st = reinterpret_cast<unsigned long long*>(L.gn_stats) +
-                                   ((size_t)tc.img * ngroups + ch0 / p.gn_group) * 2;
-          atomicAdd(st, (unsigned long long)__float2ll_rn(gsum * kGnSumScale));
-          atomicAdd(st + 1, (unsigned long long)__float2ll_rn(gsq * kGnSqScale));
+      }
+      if (p.gn_group) {
+        // per-(image, group) sum / sum of squares of the conv output (pre-activation): fp32 over the warp's 16 rows, then
+        // 64-bit fixed-point integer atomics (associative -> bit-reproducible run to run, whatever the tile order).
+        gsum += s; gsq += q;
+        if (p.gn_group == 8 || (j & 1)) {
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
+            gsq += __shfl_xor_sync(0xffffffffu, gsq, o);
+          }
+          if (lane == 0) {
+            const int ngroups = p.Cout / p.gn_group;
+            unsigned long long* st = reinterpret_cast<unsigned long long*>(L.gn_stats) +
+                                     ((size_t)tc.img * ngroups + ch0 / p.gn_group) * 2;
+            atomicAdd(st, (unsigned long long)__float2ll_rn(gsum * kGnSumScale));
+            atomicAdd(st + 1, (unsigned long long)__float2ll_rn(gsq * kGnSqScale));
+          }
+          gsum = 0.f; gsq = 0.f;
         }
-        gsum = 0.f; gsq = 0.f;
       }
     }
   }
@@ -347,9 +367,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   const int total_units = p.tiles_m * p.n_tiles_n;
   const int kblocks = p.num_taps * p.kb_per_tap;
 
-  if (warp == kProducerWarp) {
+  if (warp >= kProducerWarp) {
     // ===================== TMA producer (one lane) =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == kProducerWarp && lane == 0) {
       for (int i = 0; i < kMaxMaps; ++i) tma_prefetch_desc(&p.amap[i]);
       tma_prefetch_desc(&p.bmap);
       int s = 0;
@@ -374,6 +395,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     }
   } else {
     // ===================== consumers: warpgroup wg computes pixels 64*wg .. 64*wg+63 of the tile =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
     const int wg = warp >> 2;
     const uint32_t sA0 = smem_u32(sA) + (uint32_t)wg * (64 * 128), sB0 = smem_u32(sB);
     float acc[N / 2];
