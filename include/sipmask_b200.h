@@ -304,9 +304,11 @@ int smb_deform_im2col_multi(int num_levels, const void* const* xs, const float* 
 int smb_maxpool3x3s2(const void* x, void* y, int N, int H, int W, int C, smb_stream_t stream);
 
 /* Bilinear upsample by an integer factor, align_corners=False (sipmask_head.py:279,285), NHWC fp16,
- * writing into a channel slice of a wider tensor (out_pitch, out_choff) so torch.cat is free. */
+ * writing into a channel slice of a wider tensor (out_pitch, out_choff) so torch.cat is free.  y is [N, out_h, out_w]
+ * pixels: normally out_h = H*factor, out_w = W*factor; otherwise the upsampled image is cropped or its last row / column
+ * repeated, and nothing is written outside y.  factor 1 (a channel-slice copy) needs out_h = H, out_w = W. */
 int smb_upsample_bilinear(const void* x, int in_pitch, void* y, int out_pitch, int out_choff,
-                          int N, int H, int W, int C, int factor, int relu, smb_stream_t stream);
+                          int N, int H, int W, int out_h, int out_w, int C, int factor, int relu, smb_stream_t stream);
 
 /* Stem 7x7/2 conv (3->64) + folded BN + ReLU (backbones/resnet.py:448-460) in space-to-depth form (K = 256): the
  * zero-padded image (pixel (y,x) at (y+3, x+3)) is stored as [N, H/2+3, W/2+4, 16] fp16 with element

@@ -261,8 +261,10 @@ def upsample_bilinear(x, factor, out=None, out_choff=0, relu=False):
     N, H, W, C = x.shape
     if out is None:
         out = torch.empty((N, H * factor, W * factor, C), dtype=torch.float16, device=x.device)
-    L.check(L.lib().smb_upsample_bilinear(L.ptr(x), x.stride(2), L.ptr(out), out.stride(2), int(out_choff), N, H, W, C,
-                                          int(factor), int(relu), L.stream_ptr()), 'smb_upsample_bilinear')
+    assert out.shape[0] == N and out.stride(3) == 1 and out.stride(1) == out.shape[2] * out.stride(2)
+    L.check(L.lib().smb_upsample_bilinear(L.ptr(x), x.stride(2), L.ptr(out), out.stride(2), int(out_choff), N, H, W,
+                                          out.shape[1], out.shape[2], C, int(factor), int(relu), L.stream_ptr()),
+            'smb_upsample_bilinear')
     return out
 
 

@@ -247,8 +247,29 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int unit) 
 
 // Epilogue of one consumer warp: rows (warp%4)*16 + lane/4 + {0, 8} of its warpgroup's 64-pixel half of the tile.
 // Per element: acc + bias, * alpha, + residual -> GroupNorm statistics (pre-activation) -> ReLU -> fp16 / fp32 store.
+// GroupNorm partials of one tile: [consumer warp][group within the N tile (<= 256 / 8)][sum, sum of squares], fixed point
+typedef unsigned long long GnPart[kConsumerWarps][32][2];
+
+// After every consumer warp has written its partials of the tile: one global atomic per (group, statistic) of the tile
+// instead of one per warp.  When all SMs run tower convolutions, per-warp atomics on the same few addresses serialised
+// in L2 and stretched every tile.  Integer sums are exact, so the statistics are the same bits.
+__device__ __forceinline__ void gn_flush(const ConvParams& p, const TileCoord& tc, GnPart& gn_part, int N) {
+  asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory");       // partials of all consumer warps written
+  const int t = threadIdx.x, ngl = min(N, p.Cout - tc.n0) / p.gn_group;
+  if (t < 2 * ngl) {
+    unsigned long long v = 0;
+#pragma unroll
+    for (int w = 0; w < kConsumerWarps; ++w) v += gn_part[w][t >> 1][t & 1];
+    const int ngroups = p.Cout / p.gn_group;
+    atomicAdd(reinterpret_cast<unsigned long long*>(p.lv[tc.lvl].gn_stats) +
+                  ((size_t)tc.img * ngroups + tc.n0 / p.gn_group + (t >> 1)) * 2 + (t & 1), v);
+  }
+  asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory");       // read before the next tile overwrites
+}
+
 template <int N>
-__device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp, int lane) {
+__device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp, int lane,
+                                         GnPart& gn_part) {
   const LevelDesc& L = p.lv[tc.lvl];
   const int bw_shift = 31 - __clz(L.BW);            // BW is a power of two (choose_patch)
   bool valid[2];
@@ -318,7 +339,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
       }
       if (p.gn_group) {
         // per-(image, group) sum / sum of squares of the conv output (pre-activation): fp32 over the warp's 16 rows, then
-        // 64-bit fixed-point integer atomics (associative -> bit-reproducible run to run, whatever the tile order).
+        // 64-bit fixed point, summed over the tile by gn_flush (integer sums: bit-reproducible whatever the tile order).
         gsum += s; gsq += q;
         if (p.gn_group == 8 || (j & 1)) {
 #pragma unroll
@@ -327,11 +348,9 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
             gsq += __shfl_xor_sync(0xffffffffu, gsq, o);
           }
           if (lane == 0) {
-            const int ngroups = p.Cout / p.gn_group;
-            unsigned long long* st = reinterpret_cast<unsigned long long*>(L.gn_stats) +
-                                     ((size_t)tc.img * ngroups + ch0 / p.gn_group) * 2;
-            atomicAdd(st, (unsigned long long)__float2ll_rn(gsum * kGnSumScale));
-            atomicAdd(st + 1, (unsigned long long)__float2ll_rn(gsq * kGnSqScale));
+            unsigned long long* part = gn_part[warp][(ch0 - tc.n0) / p.gn_group];
+            part[0] = (unsigned long long)__float2ll_rn(gsum * kGnSumScale);
+            part[1] = (unsigned long long)__float2ll_rn(gsq * kGnSqScale);
           }
           gsum = 0.f; gsq = 0.f;
         }
@@ -343,6 +362,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
 template <int N>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
+  __shared__ GnPart gn_part;                         // 4 KB beside the <= 220 KB of operand stages
   // the 128-byte swizzle atoms (8 rows x 128 B) must start on 1024-byte boundaries
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -424,7 +444,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       wgmma_wait<0>();
       fence_regs<N / 2>(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      epilogue<N>(p, tc, acc, wg, warp, lane);
+      epilogue<N>(p, tc, acc, wg, warp, lane, gn_part);
+      if (p.gn_group) gn_flush(p, tc, gn_part, N);
     }
   }
 }

@@ -214,11 +214,13 @@ __global__ void maxpool3x3s2_kernel(const __half* __restrict__ x, __half* __rest
 // ------------------------------------------------------------------------------------ bilinear upsample
 // PyTorch upsample_bilinear2d, align_corners=False, scale_factor = factor (integer):
 //   src = max((dst + 0.5) / factor - 0.5, 0); i0 = (int)src; i1 = i0 + (i0 < in-1); l1 = src - i0
+// The output is Ho x Wo (the destination tensor's extent).  It is H*factor x W*factor when the pyramid levels are exact
+// multiples of each other; otherwise the upsampled image is cropped, or its last row / column repeated (i0 clamped to
+// in-1), so that nothing is written outside the destination.
 __global__ void upsample_bilinear_kernel(const __half* __restrict__ x, int in_pitch, __half* __restrict__ y, int out_pitch,
-                                         int out_choff, int N, int H, int W, int C, int factor, int relu) {
+                                         int out_choff, int N, int H, int W, int Ho, int Wo, int C, int factor, int relu) {
   pdl_wait();
   const int vecs = C >> 3;
-  const int Ho = H * factor, Wo = W * factor;
   const float rs = 1.0f / (float)factor;
   const long long total = (long long)N * Ho * Wo * vecs;
   for (unsigned t = blockIdx.x * blockDim.x + threadIdx.x; t < (unsigned)total; t += blockDim.x * gridDim.x) {   // 32-bit index math: 64-bit div/mod costs ~100 instructions each
@@ -229,7 +231,7 @@ __global__ void upsample_bilinear_kernel(const __half* __restrict__ x, int in_pi
     const int n = (int)(q / Ho);
     float sy = ((float)oy + 0.5f) * rs - 0.5f; sy = sy < 0.f ? 0.f : sy;
     float sx = ((float)ox + 0.5f) * rs - 0.5f; sx = sx < 0.f ? 0.f : sx;
-    const int y0 = (int)sy, x0 = (int)sx;
+    const int y0 = min((int)sy, H - 1), x0 = min((int)sx, W - 1);
     const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
     const float ly = sy - (float)y0, lx = sx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
     const __half* b = x + (size_t)n * H * W * in_pitch + v * 8;
@@ -503,9 +505,11 @@ extern "C" int smb_maxpool3x3s2(const void* x, void* y, int N, int H, int W, int
 }
 
 extern "C" int smb_upsample_bilinear(const void* x, int in_pitch, void* y, int out_pitch, int out_choff, int N, int H, int W,
-                                     int C, int factor, int relu, smb_stream_t stream) {
-  SMB_CHECK_ARG(x && y && C % 8 == 0 && in_pitch % 8 == 0 && out_pitch % 8 == 0 && out_choff % 8 == 0 && factor >= 1,
+                                     int out_h, int out_w, int C, int factor, int relu, smb_stream_t stream) {
+  SMB_CHECK_ARG(x && y && C % 8 == 0 && in_pitch % 8 == 0 && out_pitch % 8 == 0 && out_choff % 8 == 0 && factor >= 1 &&
+                    H > 0 && W > 0 && out_h > 0 && out_w > 0,
                 "smb_upsample_bilinear: bad argument");
+  SMB_CHECK_ARG(factor > 1 || (out_h == H && out_w == W), "smb_upsample_bilinear: a copy (factor 1) needs out_h == H, out_w == W");
   if (factor == 1) {
     const long long npix = (long long)N * H * W;
     copy_channels_kernel<<<grid_for(npix * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>((const __half*)x, in_pitch, (__half*)y,
@@ -513,9 +517,9 @@ extern "C" int smb_upsample_bilinear(const void* x, int in_pitch, void* y, int o
     SMB_LAUNCH_OK("copy_channels_kernel");
     return SMB_OK;
   }
-  const long long total = (long long)N * H * factor * W * factor * (C / 8);
+  const long long total = (long long)N * out_h * out_w * (C / 8);
   upsample_bilinear_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>((const __half*)x, in_pitch, (__half*)y, out_pitch,
-                                                                                  out_choff, N, H, W, C, factor, relu);
+                                                                                  out_choff, N, H, W, out_h, out_w, C, factor, relu);
   SMB_LAUNCH_OK("upsample_bilinear_kernel");
   return SMB_OK;
 }
