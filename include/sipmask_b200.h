@@ -87,6 +87,30 @@ int smb_mask_rescore(const float* feat, int N, int C, int h, int w, const float*
                      int num_classes, const int64_t* labels, const float* det, const int* n_valid, float* scores,
                      smb_stream_t stream);
 
+/* The same rescoring on tensor cores, for a batch of images (the engine's path): fp16 masks, weights and activations,
+ * fp32 accumulation (mma.sync.m16n8k16), layers 1+2 fused so that layer 1 never reaches memory.
+ *   pos_masks : [n_img*max_rows, H, W] fp16 cropped stride-2 masks, row r = img*max_rows + j
+ *   count     : device int [n_img]; rows j >= clamp(count[img], 0, max_rows) do no work and score exactly 0
+ *   labels    : int64 [n_img*max_rows] (0-based; a label outside [0, num_classes) scores 0), det [n_img*max_rows, 5]
+ *   scores    : fp32 [n_img*max_rows] = det[:,4] * max_p relu(mask_scoring(conv6(...(conv1(mask)))))[label]
+ *   weights   : HOST struct of device pointers.  conv_w[i]: fp16 [Cout_i, 9*Cin_i] with K = (r*3 + s)*Cin_i + ci (the
+ *               convolution engine's packing, conv.pack_weight), (Cin, Cout) = (1,16) (16,16) (16,16) (16,32) (32,64)
+ *               (64,128); conv_b[i]: fp32 [Cout_i]; score_w: fp16 [>= num_classes, 128] (mask_scoring 1x1, row = class);
+ *               score_b: fp32 [num_classes].
+ * H, W >= 127 (127 -> 63 -> 31 -> 15 -> 7 -> 3 -> 1).  SMB_EINVAL without a launch for null pointers, smaller masks or a
+ * workspace smaller than smb_mask_rescore_f16_workspace_bytes(n_img*max_rows, H, W) (which is 0 for invalid shapes). */
+typedef struct {
+  const void* conv_w[6];
+  const float* conv_b[6];
+  const void* score_w;
+  const float* score_b;
+  int num_classes;
+} smb_rescore_weights_t;
+size_t smb_mask_rescore_f16_workspace_bytes(int R, int H, int W);
+int smb_mask_rescore_f16(const void* pos_masks, int n_img, int max_rows, int H, int W, const int* count,
+                         const smb_rescore_weights_t* host_weights, const int64_t* labels, const float* det, float* scores,
+                         void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
 /* COCO RLE of bit-packed masks on the device (replaces the per-detection `masks[i].cpu().numpy()` + pycocotools
  * `mask_util.encode(order='F')` tail, sipmask_head.py:645-657; SURVEY.md 8f-1).
  *   mask_bits : [N, mask_h, words] uint32 (pixel x = bit x&31 of word x>>5), cropped to the top-left H x W (= ori_shape)

@@ -34,12 +34,17 @@ class ConvLevel(ctypes.Structure):
                 ('res_w', ctypes.c_int)]
 
 
+class RescoreWeights(ctypes.Structure):
+    _fields_ = [('conv_w', ctypes.c_void_p * 6), ('conv_b', ctypes.c_void_p * 6), ('score_w', ctypes.c_void_p),
+                ('score_b', ctypes.c_void_p), ('num_classes', ctypes.c_int)]
+
+
 _lib = None
 
 # every symbol include/sipmask_b200.h declares (checked by tests/test_abi.py)
 SYMBOLS = [
     'smb_last_error', 'smb_version', 'smb_check_device', 'smb_mask_assemble', 'smb_mask_upsample2_threshold', 'smb_mask_upsample2_threshold_pack', 'smb_mask_resize_threshold', 'smb_mask_resize_threshold_pack', 'smb_mask_assemble_pack', 'smb_mask_set_tensor_dot',
-    'smb_crop_split_forward', 'smb_crop_split_backward', 'smb_crop_split_gt', 'smb_mask_rle_counts', 'smb_rle_to_string', 'smb_conv3x3s2_relu_f32', 'smb_mask_rescore', 'smb_nms', 'smb_decode_workspace_bytes', 'smb_decode_topk',
+    'smb_crop_split_forward', 'smb_crop_split_backward', 'smb_crop_split_gt', 'smb_mask_rle_counts', 'smb_rle_to_string', 'smb_conv3x3s2_relu_f32', 'smb_mask_rescore', 'smb_mask_rescore_f16_workspace_bytes', 'smb_mask_rescore_f16', 'smb_nms', 'smb_decode_workspace_bytes', 'smb_decode_topk',
     'smb_multiclass_nms_workspace_bytes', 'smb_multiclass_nms', 'smb_fast_nms_workspace_bytes', 'smb_fast_nms',
     'smb_gather_rows_f32', 'smb_gather_det_inputs', 'smb_gather_track_feats', 'smb_track_step', 'smb_conv_plan_create', 'smb_conv_plan_create_multi', 'smb_conv_plan_destroy', 'smb_conv_plan_set_max_ctas', 'smb_conv_set_min_tiles',
     'smb_conv_run',
@@ -56,7 +61,8 @@ def lib():
                            '(there is no CPU / PyTorch fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
         L.smb_last_error.restype = ctypes.c_char_p
-        for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes'):
+        for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes',
+                  'smb_mask_rescore_f16_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

@@ -28,7 +28,8 @@ class SipMaskEngine(object):
                  strides=(8, 16, 32, 64, 128), test_cfg=None, img_shape=None, scale_factor=1.0, device='cuda',
                  mask_thr=0.4, use_graph=True, head_only=False, feat_sizes=None, in_channels=256,
                  fcos=False, prefix_head='bbox_head.', build_postproc=True, share_weights=None,
-                 max_ctas=None, head_max_ctas=None, backbone_dcn=False, ori_shape=None, legacy_interp=False, vis=False):
+                 max_ctas=None, head_max_ctas=None, backbone_dcn=False, ori_shape=None, legacy_interp=False, vis=False,
+                 rescoring_flag=False):
         self.dev = torch.device(device)
         if self.dev.index is None:
             self.dev = torch.device('cuda', torch.cuda.current_device())
@@ -58,6 +59,10 @@ class SipMaskEngine(object):
         self.legacy_interp = legacy_interp
         self.mask_thr = 0.5 if (vis and mask_thr == 0.4) else mask_thr      # VIS thresholds at 0.5 (VIS/...:764), MM at 0.4
         self.sd = {k: v for k, v in state_dict.items()}
+        # SipMask++ mask rescoring (sipmask_head.py:200-219,635-643): a mask score per detection in the result record
+        self.rescoring = rescoring_flag
+        if rescoring_flag:
+            self._check_rescoring()
         self.ops = []            # list of zero-argument callables = the launch sequence
         self.op_names = []
         self.op_tags = []        # 0 = main stream, 1 = side stream, 'fork' / 'join' = stream dependencies
@@ -75,10 +80,22 @@ class SipMaskEngine(object):
         self.conv_plans = []
         self.conv_meta = []
         self.conv_flops = 0.0
+        self.rescore_flops = 0.0                   # mask rescoring, kept apart from the convolution roofline
         with torch.cuda.device(self.dev):
             self._build()
         self.graph = None
         self.use_graph = use_graph
+
+    def _check_rescoring(self):
+        if self.vis:
+            raise ValueError('rescoring_flag=True: the SipMask-VIS head has no mask rescoring')
+        keys = ['%sconvs_scoring.%d.conv.%s' % (self.hp, i, k) for i in range(6) for k in ('weight', 'bias')]
+        missing = [k for k in keys + [self.hp + 'mask_scoring.weight', self.hp + 'mask_scoring.bias'] if k not in self.sd]
+        if missing:
+            raise ValueError('rescoring_flag=True needs the SipMask++ scoring weights; missing: %s' % ', '.join(missing))
+        h3, w3 = self.feat_sizes[0] if self.head_only else (self.H // 8, self.W // 8)
+        if min(4 * h3, 4 * w3) < 127:               # prototypes are 4x P3; six valid stride-2 3x3 convs need 127 pixels
+            raise ValueError('rescoring_flag=True needs prototypes of at least 127 x 127, got %d x %d' % (4 * h3, 4 * w3))
 
     # ------------------------------------------------------------------------------------------ helpers
     def _t(self, *shape, dtype=torch.float16, zero=False):
@@ -461,6 +478,17 @@ class SipMaskEngine(object):
         self.det_cofs = self._t(N, self.max_num, 128, dtype=torch.float32)
         self.det_boxes4 = self._t(N, self.max_num, 4, dtype=torch.float32)
         self.det_track = self._t(N, self.max_num, 512, dtype=torch.float32) if self.vis else None
+        if self.rescoring:
+            # dense fp16 cropped masks of every detection slot, for the one batched rescoring op after the per-image chains
+            self.pos_masks = self._t(N, self.max_num, Hm, Wm)
+            self.mask_scores = self._t(N, self.max_num, dtype=torch.float32, zero=True)
+            hp = self.hp
+            self._rescore_w = self._once('rescore', lambda: ops.RescoreWeights(
+                [self._w('%sconvs_scoring.%d.conv.weight' % (hp, i)) for i in range(6)],
+                [self._w('%sconvs_scoring.%d.conv.bias' % (hp, i)) for i in range(6)],
+                self._w(hp + 'mask_scoring.weight'), self._w(hp + 'mask_scoring.bias'), self.dev))
+            self._rescore_ws = self._t(ops.mask_rescore_f16_workspace_bytes(N * self.max_num, Hm, Wm), dtype=torch.uint8)
+            self.rescore_flops = float(N * self.max_num * ops.rescore_flops_per_row(Hm, Wm))    # at full detection counts
         level_hw = (ctypes.c_int * nl)(*[h * w for h, w in self.level_sizes])
         self._keep.append(level_hw)
         # the per-image decode -> NMS -> gather -> mask chains are independent (get_bboxes loops over images,
@@ -526,6 +554,13 @@ class SipMaskEngine(object):
                                                    ctypes.c_float(ry), ctypes.c_float(rx), oh, ow,
                                                    ctypes.c_float(self.mask_thr), L.stream_ptr()), 'smb_mask_assemble_pack')
             self._add(masks, 2, name='mask_fused')
+            if self.rescoring:
+                def dense(n=n):
+                    # the same rois as mask_fused; rows past the count have zero boxes and are skipped by the rescoring
+                    L.check(lib.smb_mask_assemble(L.ptr(self.protos[n]), L.F16, 1, L.ptr(self.det_cofs[n]),
+                                                  L.ptr(self.det_boxes4[n]), self._box_scale4, L.ptr(self.pos_masks[n]), L.F16,
+                                                  Hm, Wm, self.max_num, L.stream_ptr()), 'smb_mask_assemble')
+                self._add(dense, 1, name='mask_dense')
             if self.vis:
                 th, tw = self.track_feats.shape[1], self.track_feats.shape[2]
 
@@ -538,6 +573,9 @@ class SipMaskEngine(object):
         if pp_streams:
             self._marker('join')
         self._tag = 0
+        if self.rescoring:
+            self._add(lambda: ops.mask_rescore_f16(self.pos_masks, self.count, self._rescore_w, self.labels, self.det,
+                                                   workspace=self._rescore_ws, out=self.mask_scores), 5, name='rescore')
 
     # ---------------------------------------------------------------------------------------------- run
     def _run_ops(self, only=None):
@@ -600,6 +638,8 @@ class SipMaskEngine(object):
         r = dict(det_bboxes=self.det, det_labels=self.labels, count=self.count, mask_bits=self.mask_bits, idxs_keep=self.idx)
         if self.vis:
             r['track_feats'] = self.det_track          # [N,max,512] box-centre tracking features (zeros after count)
+        if self.rescoring:
+            r['mask_scores'] = self.mask_scores        # [N,max] fp32 SipMask++ mask scores (zeros after count)
         return r
 
     def forward_raw(self, img_u8, mean=(102.9801, 115.9465, 122.7717)):

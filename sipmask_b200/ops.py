@@ -487,6 +487,74 @@ def mask_rescore(pos_masks, conv_weights, conv_biases, w1x1, b1x1, labels, det, 
     return scores
 
 
+RESCORE_CHANNELS = (1, 16, 16, 16, 32, 64, 128)       # convs_scoring (sipmask_head.py:200-215)
+
+
+def rescore_flops_per_row(H, W):
+    """Algorithmic FLOPs of one detection through the six stride-2 convolutions and its own mask_scoring row (36.5 M at
+    272 x 272)."""
+    fl, h, w = 0, H, W
+    for cin, cout in zip(RESCORE_CHANNELS[:-1], RESCORE_CHANNELS[1:]):
+        h, w = (h - 3) // 2 + 1, (w - 3) // 2 + 1
+        fl += 2 * h * w * cout * 9 * cin
+    return fl + 2 * h * w * RESCORE_CHANNELS[-1]
+
+
+class RescoreWeights(object):
+    """convs_scoring (6 x [Cout, Cin, 3, 3] + bias) and mask_scoring ([C, 128(, 1, 1)] + bias) packed for
+    smb_mask_rescore_f16: fp16 [Cout, 9 * Cin] via conv.pack_weight, fp32 biases; `struct` points at the device tensors."""
+
+    def __init__(self, conv_weights, conv_biases, w1x1, b1x1, device):
+        from . import conv as C
+        if len(conv_weights) != 6 or len(conv_biases) != 6:
+            raise ValueError('rescoring needs six convs_scoring layers, got %d' % len(conv_weights))
+        for i, w in enumerate(conv_weights):
+            want = (RESCORE_CHANNELS[i + 1], RESCORE_CHANNELS[i], 3, 3)
+            if tuple(w.shape) != want:
+                raise ValueError('convs_scoring.%d: weight shape %s, expected %s' % (i, tuple(w.shape), want))
+        if w1x1.shape[1] != RESCORE_CHANNELS[-1]:
+            raise ValueError('mask_scoring: %d input channels, expected 128' % w1x1.shape[1])
+        self.conv_w = [C.pack_weight(w, device=device)[0] for w in conv_weights]
+        self.conv_b = [b.detach().float().contiguous().to(device) for b in conv_biases]
+        self.num_classes = int(w1x1.shape[0])
+        self.score_w = C.pack_weight(w1x1.reshape(self.num_classes, -1, 1, 1), device=device)[0]
+        self.score_b = b1x1.detach().float().contiguous().to(device)
+        self.struct = L.RescoreWeights()
+        for i in range(6):
+            self.struct.conv_w[i] = self.conv_w[i].data_ptr()
+            self.struct.conv_b[i] = self.conv_b[i].data_ptr()
+        self.struct.score_w, self.struct.score_b = self.score_w.data_ptr(), self.score_b.data_ptr()
+        self.struct.num_classes = self.num_classes
+
+
+def mask_rescore_f16_workspace_bytes(rows, H, W):
+    return int(L.lib().smb_mask_rescore_f16_workspace_bytes(int(rows), int(H), int(W)))
+
+
+@L.device_guard
+def mask_rescore_f16(pos_masks, count, weights, labels, det, workspace=None, out=None):
+    """SipMask++ rescoring on tensor cores (smb_mask_rescore_f16): pos_masks [n_img, max_rows, H, W] fp16 cropped stride-2
+    masks, count device int32 [n_img], weights a RescoreWeights, labels int64 [n_img, max_rows], det [n_img, max_rows, 5]
+    -> mask_scores fp32 [n_img, max_rows] (exactly 0 after count)."""
+    _need_cuda(pos_masks, count, labels, det)
+    if pos_masks.dtype != torch.float16 or pos_masks.dim() != 4 or not pos_masks.is_contiguous():
+        raise L.SmbError('mask_rescore_f16: pos_masks must be a contiguous fp16 [n_img, max_rows, H, W] tensor')
+    n_img, max_rows, H, W = pos_masks.shape
+    if tuple(labels.shape) != (n_img, max_rows) or tuple(det.shape) != (n_img, max_rows, 5) or count.numel() != n_img:
+        raise L.SmbError('mask_rescore_f16: labels / det / count do not match pos_masks %s' % (tuple(pos_masks.shape),))
+    count = count.to(torch.int32).contiguous()
+    labels, det = labels.long().contiguous(), det.float().contiguous()
+    if workspace is None:
+        workspace = torch.empty(max(mask_rescore_f16_workspace_bytes(n_img * max_rows, H, W), 1), dtype=torch.uint8,
+                                device=pos_masks.device)
+    if out is None:
+        out = torch.empty((n_img, max_rows), dtype=torch.float32, device=pos_masks.device)
+    L.check(L.lib().smb_mask_rescore_f16(L.ptr(pos_masks), n_img, max_rows, H, W, L.ptr(count), ctypes.byref(weights.struct),
+                                         L.ptr(labels), L.ptr(det), L.ptr(out), L.ptr(workspace),
+                                         ctypes.c_size_t(workspace.numel()), L.stream_ptr()), 'smb_mask_rescore_f16')
+    return out
+
+
 # ----------------------------------------------------------------------------------- DeformConv (operator API)
 class DeformConv(nn.Module):
     """Drop-in for `mmdet.ops.DeformConv` (MM/mmdet/ops/dcn/deform_conv.py:192-255): same constructor keywords, same

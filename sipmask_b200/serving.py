@@ -137,6 +137,9 @@ class PipelinedRunner(object):
         if engine.vis:                            # SipMask-VIS: the 512-d tracking features travel with the record
             for o in self.out_dev:
                 o['trk'] = torch.empty_like(engine.det_track)
+        if engine.rescoring:                      # SipMask++: the mask scores travel with the record
+            for o in self.out_dev:
+                o['msc'] = torch.empty_like(engine.mask_scores)
         self.out_host = [{k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in o.items()} for o in self.out_dev]
         self.ev_in_ready = [torch.cuda.Event() for _ in range(ns)]      # H2D of slot finished
         self.ev_in_free = [torch.cuda.Event() for _ in range(ns)]       # compute consumed the slot's input
@@ -199,6 +202,8 @@ class PipelinedRunner(object):
             o['bits'].copy_(eng.mask_bits, non_blocking=True)
             if 'trk' in o:
                 o['trk'].copy_(eng.det_track, non_blocking=True)
+            if 'msc' in o:
+                o['msc'].copy_(eng.mask_scores, non_blocking=True)
             self.ev_out_ready[k].record(cs)
         with torch.cuda.stream(self.s_d2h):
             self.s_d2h.wait_event(self.ev_out_ready[k])
@@ -217,6 +222,8 @@ class PipelinedRunner(object):
         rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'], mask_bits=o['bits'])
         if 'trk' in o:
             rec['track_feats'] = o['trk']
+        if 'msc' in o:
+            rec['mask_scores'] = o['msc']
         r = fn(rec)
         if self.ev_hold[slot] is None:
             self.ev_hold[slot] = torch.cuda.Event()
