@@ -212,6 +212,31 @@ int smb_fast_nms(const float* boxes, const float* scores, const float* ctr, int 
                  float* det_out, int64_t* label_out, int64_t* idx_out, int* count_out,
                  void* workspace, size_t workspace_bytes, smb_stream_t stream);
 
+/* ------------------------------------------------------------------ SipMask-benchmark post-processing
+ * (SipMask-benchmark/fcos_core/modeling/rpn/sipmask/inference.py:90-190, csrc/cuda/ml_nms.cu).
+ * smb_pair_decode_topk: candidates are (location, class) pairs with sigmoid(cls) > score_thr.  Per level, when more than
+ *   nms_pre pass, the nms_pre with the largest sigmoid(cls) * sigmoid(ctr) are kept (ties -> lower pair index loc*C + c).
+ *   Output order: level by level, ascending pair index inside a level.  Sigmoids are 1 / (1 + exp(-x)) with exp in
+ *   double rounded to float and IEEE float add / divide.  box = location -/+ relu(box * box_scale) * box_mul, clipped to
+ *   [0, img_w-1] x [0, img_h-1]; score = sqrt(sigmoid(cls) * sigmoid(ctr)); label = class (0-based); loc =
+ *   level-concatenated location.  *n_cand (device) = number of candidates; slots past it hold zeros and label / loc -1.
+ *   n_slots >= smb_pair_decode_slots(...) = sum_l min(h_l * w_l * C, nms_pre).  The workspace holds one key per pair.
+ *   1 <= nms_pre <= 5120, C <= 1024, h*w*C < 2^31 per level.
+ * smb_ml_nms_topk: label-aware NMS over n = min(*n_dev, cap) candidates (cap <= 5120): descending score, ties by ascending
+ *   index, suppress when IoU (+1 areas) > iou_thr within a label.  Survivors in ascending candidate order; when more than
+ *   max_per_img (> 0) survive, keep scores >= the max_per_img-th largest (ties can keep more).  The first out_cap kept rows
+ *   go to det_out [out_cap,5] (box, score), label_out / idx_out int64 [out_cap] (candidate row); *count_out =
+ *   min(kept, out_cap), *kept_total_out = kept.  Rows past the count: zeros, label / idx -1. */
+int smb_pair_decode_slots(int num_levels, const smb_level_t* host_levels, int num_classes, int nms_pre);
+size_t smb_pair_decode_workspace_bytes(int num_levels, const smb_level_t* host_levels, int num_classes, int nms_pre);
+int smb_pair_decode_topk(int num_levels, const smb_level_t* host_levels, int num_classes, float score_thr, int nms_pre,
+                         int img_h, int img_w, float* cand_boxes, float* cand_scores, int* cand_labels, int* cand_loc,
+                         int* n_cand, int n_slots, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+size_t smb_ml_nms_workspace_bytes(int cap);
+int smb_ml_nms_topk(const float* boxes, const float* scores, const int* labels, const int* n_dev, int cap, float iou_thr,
+                    int max_per_img, int out_cap, float* det_out, int64_t* label_out, int64_t* idx_out, int* count_out,
+                    int* kept_total_out, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
 /* The gather between NMS and mask assembly (mlvl_cofs[idxs_keep], det_bboxes[:, :4]; sipmask_head.py:612,623) in one launch:
  * det_cofs[i,:] = cof_src[cand_loc[idx[i]],:] (row pitch cof_pitch floats), det_boxes[i,:] = det[i,:4] for i < *count,
  * zeros after; loc_out (may be NULL) receives the level-concatenated location of each kept detection (-1 after count).
@@ -320,6 +345,11 @@ int smb_groupnorm_relu_apply_multi(int num_levels, void* const* xs, const void* 
 int smb_offset_conv1x1_multi(int num_levels, const float* const* bboxes, int bbox_pitch, const float* scales,
                              const float* weight, int n_off, float* const* offs, const int* Hs, const int* Ws, int n_img,
                              smb_stream_t stream);
+/* The same offsets from relu(scale * bbox) (SipMask-benchmark FeatureAlign input with NORM_REG_TARGETS,
+ * SipMask-benchmark/fcos_core/modeling/rpn/sipmask/sipmask.py:161-171). */
+int smb_offset_conv1x1_relu_multi(int num_levels, const float* const* bboxes, int bbox_pitch, const float* scales,
+                                  const float* weight, int n_off, float* const* offs, const int* Hs, const int* Ws, int n_img,
+                                  smb_stream_t stream);
 int smb_deform_im2col_multi(int num_levels, const void* const* xs, const float* const* offs, int off_pitch,
                             void* const* cols, const int* Hs, const int* Ws, int n_img, int C, int deformable_groups,
                             smb_stream_t stream);

@@ -45,10 +45,11 @@ _lib = None
 SYMBOLS = [
     'smb_last_error', 'smb_version', 'smb_check_device', 'smb_mask_assemble', 'smb_mask_upsample2_threshold', 'smb_mask_upsample2_threshold_pack', 'smb_mask_resize_threshold', 'smb_mask_resize_threshold_pack', 'smb_mask_assemble_pack', 'smb_mask_set_tensor_dot',
     'smb_crop_split_forward', 'smb_crop_split_backward', 'smb_crop_split_gt', 'smb_mask_rle_counts', 'smb_rle_to_string', 'smb_conv3x3s2_relu_f32', 'smb_mask_rescore', 'smb_mask_rescore_f16_workspace_bytes', 'smb_mask_rescore_f16', 'smb_nms', 'smb_decode_workspace_bytes', 'smb_decode_topk',
-    'smb_multiclass_nms_workspace_bytes', 'smb_multiclass_nms', 'smb_fast_nms_workspace_bytes', 'smb_fast_nms',
+    'smb_multiclass_nms_workspace_bytes', 'smb_multiclass_nms', 'smb_pair_decode_slots', 'smb_pair_decode_workspace_bytes',
+    'smb_pair_decode_topk', 'smb_ml_nms_workspace_bytes', 'smb_ml_nms_topk', 'smb_fast_nms_workspace_bytes', 'smb_fast_nms',
     'smb_gather_rows_f32', 'smb_gather_det_inputs', 'smb_gather_track_feats', 'smb_track_step', 'smb_conv_plan_create', 'smb_conv_plan_create_multi', 'smb_conv_plan_destroy', 'smb_conv_plan_set_max_ctas', 'smb_conv_set_min_tiles',
     'smb_conv_run',
-    'smb_groupnorm_relu_apply', 'smb_groupnorm_stats', 'smb_deform_im2col', 'smb_offset_conv1x1', 'smb_groupnorm_relu_apply_multi', 'smb_offset_conv1x1_multi', 'smb_deform_im2col_multi', 'smb_maxpool3x3s2',
+    'smb_groupnorm_relu_apply', 'smb_groupnorm_stats', 'smb_deform_im2col', 'smb_offset_conv1x1', 'smb_groupnorm_relu_apply_multi', 'smb_offset_conv1x1_multi', 'smb_offset_conv1x1_relu_multi', 'smb_deform_im2col_multi', 'smb_maxpool3x3s2',
     'smb_upsample_bilinear', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
 ]
 
@@ -62,7 +63,7 @@ def lib():
         L = ctypes.CDLL(LIB_PATH)
         L.smb_last_error.restype = ctypes.c_char_p
         for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes',
-                  'smb_mask_rescore_f16_workspace_bytes'):
+                  'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

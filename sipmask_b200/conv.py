@@ -288,12 +288,13 @@ def groupnorm_relu_apply_multi(xs, stats, gamma, beta, eps=1e-5, relu=True):
 
 
 @L.device_guard
-def offset_conv1x1_multi(bboxes, scales, weight, offs):
+def offset_conv1x1_multi(bboxes, scales, weight, offs, relu=False):
+    """relu=True: offsets from relu(scale * bbox) (smb_offset_conv1x1_relu_multi)."""
     N = bboxes[0].shape[0]
     sc = (ctypes.c_float * len(scales))(*[float(v) for v in scales])
-    L.check(L.lib().smb_offset_conv1x1_multi(len(bboxes), _parr(bboxes), bboxes[0].stride(2), sc, L.ptr(weight),
-                                             weight.shape[0], _parr(offs), _iarr([b.shape[1] for b in bboxes]),
-                                             _iarr([b.shape[2] for b in bboxes]), N, L.stream_ptr()),
+    fn = L.lib().smb_offset_conv1x1_relu_multi if relu else L.lib().smb_offset_conv1x1_multi
+    L.check(fn(len(bboxes), _parr(bboxes), bboxes[0].stride(2), sc, L.ptr(weight), weight.shape[0], _parr(offs),
+               _iarr([b.shape[1] for b in bboxes]), _iarr([b.shape[2] for b in bboxes]), N, L.stream_ptr()),
             'smb_offset_conv1x1_multi')
     return offs
 

@@ -362,7 +362,9 @@ __global__ void __launch_bounds__(256) gn_apply_rows_kernel(MultiDesc d, int n_i
   }
 }
 
-// offsets for all levels: a[l] = raw fcos_reg (fp32, pitch bbox_pitch), c[l] = offsets fp32 [hw, n_off], scale[l] = Scale_l
+// offsets for all levels: a[l] = raw fcos_reg (fp32, pitch bbox_pitch), c[l] = offsets fp32 [hw, n_off], scale[l] = Scale_l;
+// RELU: the offsets are computed from relu(scale * x) (SipMask-benchmark, NORM_REG_TARGETS)
+template <bool RELU>
 __global__ void offset_conv_multi_kernel(MultiDesc d, int bbox_pitch, const float* __restrict__ w, int n_off) {
   pdl_wait();
   const long long total = d.start[d.num];
@@ -374,7 +376,10 @@ __global__ void offset_conv_multi_kernel(MultiDesc d, int bbox_pitch, const floa
     const float* b = reinterpret_cast<const float*>(d.a[l]) + (size_t)pix * bbox_pitch;
     float acc = 0.f;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) acc = fmaf(__fmul_rn(b[k], d.scale[l]), w[o * 4 + k], acc);
+    for (int k = 0; k < 4; ++k) {
+      const float x = __fmul_rn(b[k], d.scale[l]);
+      acc = fmaf(RELU ? fmaxf(x, 0.f) : x, w[o * 4 + k], acc);
+    }
     reinterpret_cast<float*>(d.c[l])[q] = acc;
   }
 }
@@ -567,16 +572,31 @@ extern "C" int smb_groupnorm_relu_apply_multi(int num_levels, void* const* xs, c
   return SMB_OK;
 }
 
-extern "C" int smb_offset_conv1x1_multi(int num_levels, const float* const* bboxes, int bbox_pitch, const float* scales,
-                                        const float* weight, int n_off, float* const* offs, const int* Hs, const int* Ws,
-                                        int n_img, smb_stream_t stream) {
+static int offset_conv1x1_multi(int num_levels, const float* const* bboxes, int bbox_pitch, const float* scales,
+                                const float* weight, int n_off, float* const* offs, const int* Hs, const int* Ws, int n_img,
+                                bool relu, smb_stream_t stream) {
   SMB_CHECK_ARG(bboxes && scales && weight && offs && Hs && Ws && n_off > 0, "smb_offset_conv1x1_multi: bad argument");
   MultiDesc d;
   SMB_CHECK_ARG(fill_multi(&d, num_levels, Hs, Ws, n_off, n_img) == 0, "smb_offset_conv1x1_multi: bad levels");
   for (int l = 0; l < num_levels; ++l) { d.a[l] = bboxes[l]; d.c[l] = offs[l]; d.b[l] = nullptr; d.scale[l] = scales[l]; }
-  offset_conv_multi_kernel<<<grid_for(d.start[num_levels], 256), 256, 0, (cudaStream_t)stream>>>(d, bbox_pitch, weight, n_off);
+  if (relu)
+    offset_conv_multi_kernel<true><<<grid_for(d.start[num_levels], 256), 256, 0, (cudaStream_t)stream>>>(d, bbox_pitch, weight, n_off);
+  else
+    offset_conv_multi_kernel<false><<<grid_for(d.start[num_levels], 256), 256, 0, (cudaStream_t)stream>>>(d, bbox_pitch, weight, n_off);
   SMB_LAUNCH_OK("offset_conv_multi_kernel");
   return SMB_OK;
+}
+
+extern "C" int smb_offset_conv1x1_multi(int num_levels, const float* const* bboxes, int bbox_pitch, const float* scales,
+                                        const float* weight, int n_off, float* const* offs, const int* Hs, const int* Ws,
+                                        int n_img, smb_stream_t stream) {
+  return offset_conv1x1_multi(num_levels, bboxes, bbox_pitch, scales, weight, n_off, offs, Hs, Ws, n_img, false, stream);
+}
+
+extern "C" int smb_offset_conv1x1_relu_multi(int num_levels, const float* const* bboxes, int bbox_pitch, const float* scales,
+                                             const float* weight, int n_off, float* const* offs, const int* Hs, const int* Ws,
+                                             int n_img, smb_stream_t stream) {
+  return offset_conv1x1_multi(num_levels, bboxes, bbox_pitch, scales, weight, n_off, offs, Hs, Ws, n_img, true, stream);
 }
 
 extern "C" int smb_deform_im2col_multi(int num_levels, const void* const* xs, const float* const* offs, int off_pitch,

@@ -792,6 +792,288 @@ __global__ void gather_track_feats_kernel(const float* __restrict__ track, int h
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// SipMask-benchmark post-processing (SipMask-benchmark/fcos_core/modeling/rpn/sipmask/inference.py:90-190,
+// csrc/cuda/ml_nms.cu:13-72,132-135).  Candidates are (location, class) PAIRS, not locations.
+// ---------------------------------------------------------------------------------------------
+// Sigmoid with one rounding per step: exp in double rounded to float, then IEEE add and divide.  A CPU restatement
+// (float64 exp -> float32, float32 arithmetic) gives the same bits, so the pair selection can be checked exactly.
+__device__ __forceinline__ float sigmoid_rn(float x) {
+  const float e = (float)exp(-(double)x);
+  return __fdiv_rn(1.0f, __fadd_rn(1.0f, e));
+}
+
+struct PairLevels {
+  smb_level_t lv[MAXLVL];
+  int loc_off[MAXLVL + 1];    // level-concatenated location offsets
+  long long pair_off[MAXLVL + 1];   // level-concatenated pair offsets (h*w*C per level)
+  int sel_cap[MAXLVL];        // min(h*w*C, nms_pre): capacity of the level's slice of `sel`
+  int sel_off[MAXLVL + 1];
+  int num;
+};
+
+// key[pair] = bits(sigmoid(cls) * sigmoid(ctr)) + 1 if sigmoid(cls) > thr, else 0 (inference.py:90-95).  Positive floats
+// order like their bit patterns, so a larger key is a larger score.  One warp per location.
+__global__ void pair_key_kernel(PairLevels L, int C, float thr, unsigned* __restrict__ keys) {
+  pdl_wait();
+  const int total = L.loc_off[L.num];
+  const int warps_per_block = blockDim.x >> 5;
+  const int lane = threadIdx.x & 31;
+  for (int loc = blockIdx.x * warps_per_block + (threadIdx.x >> 5); loc < total; loc += gridDim.x * warps_per_block) {
+    int l = 0;
+    while (loc >= L.loc_off[l + 1]) ++l;
+    const int i = loc - L.loc_off[l];
+    const smb_level_t& lv = L.lv[l];
+    const float* row = lv.cls + (size_t)i * lv.cls_pitch;
+    const float ct = sigmoid_rn(lv.ctr[(size_t)i * lv.ctr_pitch]);
+    unsigned* out = keys + L.pair_off[l] + (size_t)i * C;
+    for (int c = lane; c < C; c += 32) {
+      const float s = sigmoid_rn(row[c]);
+      out[c] = (s > thr) ? __float_as_uint(__fmul_rn(s, ct)) + 1u : 0u;
+    }
+  }
+}
+
+// One CTA per level: the pairs that pass, or, when more than nms_pre pass, the nms_pre largest keys with ties going to
+// the lower pair index.  Writes the selected pair indices in ascending order and their number (<= sel_cap[l]).
+constexpr int PAIR_RUN = 16;       // consecutive pairs per thread in the ordered compaction
+__global__ void __launch_bounds__(NT) pair_select_kernel(PairLevels L, int nms_pre, const unsigned* __restrict__ keys,
+                                                         int* __restrict__ sel, int* __restrict__ sel_count) {
+  pdl_wait();
+  __shared__ unsigned s_hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_k;
+  __shared__ int s_warp[33];
+  const int l = blockIdx.x;
+  const int n = (int)(L.pair_off[l + 1] - L.pair_off[l]);
+  const unsigned* kl = keys + L.pair_off[l];
+  const int cap = L.sel_cap[l];
+  int* out = sel + L.sel_off[l];
+  // number of passing pairs
+  int mine = 0;
+  for (int i = threadIdx.x; i < n; i += NT) mine += kl[i] != 0u;
+  int n_pass;
+  block_exscan(mine, s_warp, &n_pass);
+  // threshold key T and the number of pairs equal to T that may still be taken (lowest indices first)
+  unsigned T = 1u;
+  int budget = 0x7fffffff;
+  if (n_pass > cap) {
+    // radix-select the cap-th smallest of ~key (= the cap-th largest key) over 4 bytes
+    if (threadIdx.x == 0) { s_prefix = 0ull; s_k = cap; }
+    __syncthreads();
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      for (int i = threadIdx.x; i < 256; i += NT) s_hist[i] = 0u;
+      __syncthreads();
+      const unsigned long long prefix = s_prefix;
+      const unsigned himask = (shift == 24) ? 0u : (0xffffffffu << (shift + 8));
+      for (int i = threadIdx.x; i < n; i += NT) {
+        const unsigned k = ~kl[i];
+        if ((k & himask) == (unsigned)prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1u);
+      }
+      select_digit(s_hist, &s_k, &s_prefix, prefix, shift);
+    }
+    T = ~(unsigned)s_prefix;
+    budget = s_k;                       // rank of the cap-th key among the keys equal to T
+  }
+  // ordered compaction: thread t owns PAIR_RUN consecutive pairs of each chunk
+  int running = 0, tie_running = 0;
+  for (int base = 0; base < n; base += NT * PAIR_RUN) {
+    const int i0 = base + threadIdx.x * PAIR_RUN;
+    unsigned k[PAIR_RUN];
+    int ties = 0;
+#pragma unroll
+    for (int j = 0; j < PAIR_RUN; ++j) {
+      k[j] = (i0 + j < n) ? kl[i0 + j] : 0u;
+      ties += k[j] == T;
+    }
+    int tie_tot;
+    int tie_rank = tie_running + block_exscan(ties, s_warp, &tie_tot);
+    unsigned take = 0u;
+    int cnt = 0;
+#pragma unroll
+    for (int j = 0; j < PAIR_RUN; ++j) {
+      bool f = k[j] > T;
+      if (k[j] == T && k[j] != 0u) { f = tie_rank < budget; ++tie_rank; }
+      if (f) { take |= 1u << j; ++cnt; }
+    }
+    int tot;
+    int pos = running + block_exscan(cnt, s_warp, &tot);
+#pragma unroll
+    for (int j = 0; j < PAIR_RUN; ++j)
+      if ((take >> j) & 1u) {
+        if (pos < cap) out[pos] = i0 + j;
+        ++pos;
+      }
+    running += tot;
+    tie_running += tie_tot;
+  }
+  if (threadIdx.x == 0) sel_count[l] = min(running, cap);
+}
+
+// One thread per output slot: level-major, ascending pair index inside a level.  Box = location -/+ relu(box * scale) *
+// mul, clipped to [0, w-1] x [0, h-1] (inference.py:125-141, bounding_box.py:214-224); score = sqrt(cls * ctr).
+// Slots past the candidate count get zero boxes / scores and label -1.
+__global__ void pair_decode_kernel(PairLevels L, int C, int img_h, int img_w, const int* __restrict__ sel,
+                                   const int* __restrict__ sel_count, int n_slots, float* __restrict__ cand_boxes,
+                                   float* __restrict__ cand_scores, int* __restrict__ cand_labels, int* __restrict__ cand_loc,
+                                   int* __restrict__ n_cand) {
+  pdl_wait();
+  int off[MAXLVL + 1];
+  off[0] = 0;
+  for (int l = 0; l < L.num; ++l) off[l + 1] = off[l] + min(max(sel_count[l], 0), L.sel_cap[l]);
+  const int total = off[L.num];
+  if (blockIdx.x == 0 && threadIdx.x == 0) *n_cand = total;
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < n_slots; q += gridDim.x * blockDim.x) {
+    if (q >= total) {
+      *reinterpret_cast<float4*>(cand_boxes + (size_t)q * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      cand_scores[q] = 0.f;
+      cand_labels[q] = -1;
+      cand_loc[q] = -1;
+      continue;
+    }
+    int l = 0;
+    while (q >= off[l + 1]) ++l;
+    const int p = sel[L.sel_off[l] + (q - off[l])];
+    const int i = p / C, c = p - i * C;
+    const smb_level_t& lv = L.lv[l];
+    const float s = __fmul_rn(sigmoid_rn(lv.cls[(size_t)i * lv.cls_pitch + c]), sigmoid_rn(lv.ctr[(size_t)i * lv.ctr_pitch]));
+    const int y = i / lv.w, x = i - y * lv.w;
+    const float px = (float)(x * lv.stride + lv.stride / 2), py = (float)(y * lv.stride + lv.stride / 2);
+    const float* d = lv.box + (size_t)i * lv.box_pitch;
+    float dd[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) dd[k] = __fmul_rn(fmaxf(__fmul_rn(d[k], lv.box_scale), 0.f), lv.box_mul);
+    const float mw = (float)(img_w - 1), mh = (float)(img_h - 1);
+    const float x1 = fminf(fmaxf(__fsub_rn(px, dd[0]), 0.f), mw), y1 = fminf(fmaxf(__fsub_rn(py, dd[1]), 0.f), mh);
+    const float x2 = fminf(fmaxf(__fadd_rn(px, dd[2]), 0.f), mw), y2 = fminf(fmaxf(__fadd_rn(py, dd[3]), 0.f), mh);
+    *reinterpret_cast<float4*>(cand_boxes + (size_t)q * 4) = make_float4(x1, y1, x2, y2);
+    cand_scores[q] = __fsqrt_rn(s);
+    cand_labels[q] = c;
+    cand_loc[q] = L.loc_off[l] + i;
+  }
+}
+
+// Label-aware NMS, stage 1 (one CTA): n = clamp(*n_dev, 0, cap) candidates sorted by descending score, ties by ascending
+// index.  Writes the mc_* layout of one list so that mc_sweep_kernel can run the sweep.
+__global__ void __launch_bounds__(NT) ml_prepare_kernel(const float* __restrict__ boxes, const float* __restrict__ scores,
+                                                        const int* __restrict__ labels, const int* __restrict__ n_dev, int cap,
+                                                        int* __restrict__ w_cidx, float* __restrict__ w_cscore,
+                                                        unsigned long long* __restrict__ w_keys, float4* __restrict__ w_sbox,
+                                                        int* __restrict__ w_slab, int* __restrict__ w_m) {
+  pdl_wait();
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw);     // [next pow2 of MAXN]
+  const int n = min(max(*n_dev, 0), cap);
+  if (threadIdx.x == 0) *w_m = n;
+  if (n == 0) return;
+  int P = 1;
+  while (P < n) P <<= 1;
+  for (int i = threadIdx.x; i < P; i += NT) keys[i] = (i < n) ? desc_key(scores[i], (unsigned)i) : ~0ull;
+  bitonic_sort(keys, P);
+  for (int r = threadIdx.x; r < n; r += NT) {
+    const unsigned long long k = keys[r];
+    const int i = (int)(k & 0xffffffffu);
+    w_keys[r] = k;
+    w_sbox[r] = *reinterpret_cast<const float4*>(boxes + (size_t)i * 4);
+    w_slab[r] = labels[i];
+    w_cidx[r] = r;                   // positions are candidate indices: the sweep returns kept candidates ascending
+    w_cscore[r] = scores[r];
+  }
+}
+
+// Stage 2: suppression bit-matrix over 64x64 tiles of the upper triangle; IoU is 0 across labels (ml_nms.cu:13-24).
+__global__ void __launch_bounds__(64) ml_mask_kernel(const float4* __restrict__ w_sbox, const int* __restrict__ w_slab,
+                                                     const int* __restrict__ w_m, int nbmax, float iou_thr,
+                                                     unsigned long long* __restrict__ mask) {
+  pdl_wait();
+  __shared__ float4 s_col[64];
+  __shared__ int s_lab[64];
+  const int m = min(*w_m, nbmax * 64);
+  const int nb = (m + 63) >> 6;
+  const int total = nb * (nb + 1) / 2;
+  for (int t = blockIdx.x; t < total; t += gridDim.x) {
+    int u = t, rb = 0;
+    while (u >= nb - rb) { u -= nb - rb; ++rb; }
+    const int cb = rb + u;
+    const int col = cb * 64 + threadIdx.x;
+    s_col[threadIdx.x] = (col < m) ? w_sbox[col] : make_float4(0.f, 0.f, 0.f, 0.f);
+    s_lab[threadIdx.x] = (col < m) ? w_slab[col] : -1;
+    __syncthreads();
+    const int row = rb * 64 + threadIdx.x;
+    if (row < m) {
+      const float4 a = w_sbox[row];
+      const int la = w_slab[row];
+      unsigned long long bits = 0ull;
+      const int lim = min(64, m - cb * 64);
+      const int start = (rb == cb) ? threadIdx.x + 1 : 0;
+      for (int q = start; q < lim; ++q) {
+        const float v = (s_lab[q] != la) ? 0.f : iou_ref(a, s_col[q], 1.0f);
+        if (v > iou_thr) bits |= 1ull << q;
+      }
+      mask[(size_t)row * nbmax + cb] = bits;
+    }
+    __syncthreads();
+  }
+}
+
+// Stage 4 (one CTA): survivors (ascending candidate index) -> k-th-value cut at max_per_img (keep score >= the
+// max_per_img-th largest, inference.py:182-190; ties can keep more) -> first out_cap rows, count = min(kept, out_cap),
+// kept_total = kept.  Rows past the count: zeros, label / index -1.
+__global__ void __launch_bounds__(NT) ml_finalize_kernel(const float* __restrict__ boxes, const int* __restrict__ labels,
+                                                         const int* __restrict__ ws_idx, const float* __restrict__ ws_score,
+                                                         const int* __restrict__ ws_count, int cap, int max_per_img,
+                                                         int out_cap, float* __restrict__ det_out,
+                                                         long long* __restrict__ label_out, long long* __restrict__ idx_out,
+                                                         int* __restrict__ count_out, int* __restrict__ kept_total_out) {
+  pdl_wait();
+  __shared__ unsigned s_hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_k;
+  __shared__ int s_warp[33];
+  const int K = min(max(*ws_count, 0), cap);
+  float thr = -INFINITY;
+  if (max_per_img > 0 && K > max_per_img) {
+    if (threadIdx.x == 0) { s_prefix = 0ull; s_k = max_per_img; }
+    __syncthreads();
+    for (int shift = 56; shift >= 32; shift -= 8) {
+      for (int i = threadIdx.x; i < 256; i += NT) s_hist[i] = 0u;
+      __syncthreads();
+      const unsigned long long prefix = s_prefix;
+      const unsigned long long himask = (shift == 56) ? 0ull : (~0ull << (shift + 8));
+      for (int g = threadIdx.x; g < K; g += NT) {
+        const unsigned long long k = desc_key(ws_score[g], 0u);
+        if ((k & himask) == prefix) atomicAdd(&s_hist[(unsigned)(k >> shift) & 255u], 1u);
+      }
+      select_digit(s_hist, &s_k, &s_prefix, prefix, shift);
+    }
+    thr = key_score(s_prefix);
+  }
+  int running = 0;
+  for (int base = 0; base < K; base += NT) {
+    const int g = base + threadIdx.x;
+    const float s = (g < K) ? ws_score[g] : 0.f;
+    const int f = (g < K) && (s >= thr);
+    int tot;
+    const int pos = running + block_exscan(f, s_warp, &tot);
+    if (f && pos < out_cap) {
+      const int i = ws_idx[g];
+      const float4 b = *reinterpret_cast<const float4*>(boxes + (size_t)i * 4);
+      det_out[pos * 5 + 0] = b.x; det_out[pos * 5 + 1] = b.y; det_out[pos * 5 + 2] = b.z; det_out[pos * 5 + 3] = b.w;
+      det_out[pos * 5 + 4] = s;
+      label_out[pos] = labels[i];
+      idx_out[pos] = i;
+    }
+    running += tot;
+  }
+  const int count = min(running, out_cap);
+  for (int r = count + threadIdx.x; r < out_cap; r += NT) {
+    for (int q = 0; q < 5; ++q) det_out[r * 5 + q] = 0.f;
+    label_out[r] = -1;
+    idx_out[r] = -1;
+  }
+  if (threadIdx.x == 0) { *count_out = count; *kept_total_out = running; }
+}
+
 static int fill_levels(Levels* L, int num_levels, const smb_level_t* host_levels, int nms_pre) {
   if (num_levels < 1 || num_levels > MAXLVL) return -1;
   L->num = num_levels;
@@ -1012,5 +1294,155 @@ extern "C" int smb_gather_rows_f32(const float* src, int src_pitch, const int64_
   gather_rows_kernel<<<cdiv(max_rows * row_elems, 256), 256, 0, (cudaStream_t)stream>>>(src, src_pitch, (const long long*)idx,
                                                                                          count_dev, max_rows, row_elems, dst);
   SMB_LAUNCH_OK("gather_rows_kernel");
+  return SMB_OK;
+}
+
+// ------------------------------------------------------------------------------------ SipMask-benchmark entry points
+static int fill_pair_levels(PairLevels* L, int num_levels, const smb_level_t* host_levels, int C, int nms_pre) {
+  if (num_levels < 1 || num_levels > MAXLVL || C < 1 || C > 1024 || nms_pre < 1 || nms_pre > MAXN) return -1;
+  L->num = num_levels;
+  L->loc_off[0] = 0;
+  L->pair_off[0] = 0;
+  L->sel_off[0] = 0;
+  for (int l = 0; l < num_levels; ++l) {
+    L->lv[l] = host_levels[l];
+    const long long hw = (long long)host_levels[l].h * host_levels[l].w;
+    const long long np = hw * C;
+    if (host_levels[l].h <= 0 || host_levels[l].w <= 0 || np >= (1LL << 31) - (long long)NT * PAIR_RUN) return -1;
+    if (!host_levels[l].cls || !host_levels[l].ctr || !host_levels[l].box) return -1;
+    L->loc_off[l + 1] = L->loc_off[l] + (int)hw;
+    L->pair_off[l + 1] = L->pair_off[l] + np;
+    L->sel_cap[l] = (int)(np < nms_pre ? np : nms_pre);
+    L->sel_off[l + 1] = L->sel_off[l] + L->sel_cap[l];
+    if ((long long)L->loc_off[l + 1] >= (1LL << 31)) return -1;
+  }
+  return 0;
+}
+
+struct PairWs {
+  size_t keys, sel, count, total;
+};
+static PairWs pair_ws_layout(const PairLevels& L) {
+  PairWs w;
+  size_t off = 0;
+  w.keys = off;  off = align_up(off + (size_t)L.pair_off[L.num] * sizeof(unsigned), 256);
+  w.sel = off;   off = align_up(off + (size_t)L.sel_off[L.num] * sizeof(int), 256);
+  w.count = off; off = align_up(off + (size_t)MAXLVL * sizeof(int), 256);
+  w.total = off;
+  return w;
+}
+
+extern "C" int smb_pair_decode_slots(int num_levels, const smb_level_t* host_levels, int num_classes, int nms_pre) {
+  PairLevels L;
+  if (!host_levels || fill_pair_levels(&L, num_levels, host_levels, num_classes, nms_pre)) return SMB_EINVAL;
+  return L.sel_off[L.num];
+}
+
+extern "C" size_t smb_pair_decode_workspace_bytes(int num_levels, const smb_level_t* host_levels, int num_classes,
+                                                  int nms_pre) {
+  PairLevels L;
+  if (!host_levels || fill_pair_levels(&L, num_levels, host_levels, num_classes, nms_pre)) return 0;
+  return pair_ws_layout(L).total;
+}
+
+extern "C" int smb_pair_decode_topk(int num_levels, const smb_level_t* host_levels, int num_classes, float score_thr,
+                                    int nms_pre, int img_h, int img_w, float* cand_boxes, float* cand_scores,
+                                    int* cand_labels, int* cand_loc, int* n_cand, int n_slots, void* workspace,
+                                    size_t workspace_bytes, smb_stream_t stream) {
+  PairLevels L;
+  SMB_CHECK_ARG(host_levels && fill_pair_levels(&L, num_levels, host_levels, num_classes, nms_pre) == 0,
+                "smb_pair_decode_topk: bad levels (1..%d levels, 1 <= C <= 1024, 1 <= nms_pre <= %d, h*w*C < 2^31)",
+                MAXLVL, MAXN);
+  SMB_CHECK_ARG(cand_boxes && cand_scores && cand_labels && cand_loc && n_cand && workspace,
+                "smb_pair_decode_topk: null pointer");
+  SMB_CHECK_ARG(img_h > 0 && img_w > 0, "smb_pair_decode_topk: img %dx%d", img_h, img_w);
+  SMB_CHECK_ARG(n_slots >= L.sel_off[L.num], "smb_pair_decode_topk: n_slots=%d < %d", n_slots, L.sel_off[L.num]);
+  const PairWs w = pair_ws_layout(L);
+  if (workspace_bytes < w.total) {
+    set_error("smb_pair_decode_topk: workspace %zu < %zu", workspace_bytes, w.total);
+    return SMB_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  unsigned* keys = (unsigned*)(ws + w.keys);
+  int* sel = (int*)(ws + w.sel);
+  int* cnt = (int*)(ws + w.count);
+  const int total = L.loc_off[L.num];
+  pair_key_kernel<<<min(cdiv(total, 8), 132 * 16), 256, 0, st>>>(L, num_classes, score_thr, keys);
+  SMB_LAUNCH_OK("pair_key_kernel");
+  pair_select_kernel<<<num_levels, NT, 0, st>>>(L, nms_pre, keys, sel, cnt);
+  SMB_LAUNCH_OK("pair_select_kernel");
+  pair_decode_kernel<<<max(1, min(cdiv(n_slots, 256), 132 * 4)), 256, 0, st>>>(L, num_classes, img_h, img_w, sel, cnt, n_slots,
+                                                                             cand_boxes, cand_scores, cand_labels, cand_loc,
+                                                                             n_cand);
+  SMB_LAUNCH_OK("pair_decode_kernel");
+  return SMB_OK;
+}
+
+struct MlWs {
+  size_t cidx, cscore, keys, sbox, slab, m, mask, idx, score, count, total;
+};
+static MlWs ml_ws_layout(int cap) {
+  MlWs w;
+  const int nbmax = (cap + 63) / 64;
+  size_t off = 0;
+  w.cidx = off;   off = align_up(off + (size_t)cap * sizeof(int), 256);
+  w.cscore = off; off = align_up(off + (size_t)cap * sizeof(float), 256);
+  w.keys = off;   off = align_up(off + (size_t)cap * sizeof(unsigned long long), 256);
+  w.sbox = off;   off = align_up(off + (size_t)cap * sizeof(float4), 256);
+  w.slab = off;   off = align_up(off + (size_t)cap * sizeof(int), 256);
+  w.m = off;      off = align_up(off + sizeof(int), 256);
+  w.mask = off;   off = align_up(off + (size_t)cap * nbmax * sizeof(unsigned long long), 256);
+  w.idx = off;    off = align_up(off + (size_t)cap * sizeof(int), 256);
+  w.score = off;  off = align_up(off + (size_t)cap * sizeof(float), 256);
+  w.count = off;  off = align_up(off + sizeof(int), 256);
+  w.total = off;
+  return w;
+}
+
+extern "C" size_t smb_ml_nms_workspace_bytes(int cap) {
+  if (cap < 1 || cap > MAXN) return 0;
+  return ml_ws_layout(cap).total;
+}
+
+extern "C" int smb_ml_nms_topk(const float* boxes, const float* scores, const int* labels, const int* n_dev, int cap,
+                               float iou_thr, int max_per_img, int out_cap, float* det_out, int64_t* label_out,
+                               int64_t* idx_out, int* count_out, int* kept_total_out, void* workspace,
+                               size_t workspace_bytes, smb_stream_t stream) {
+  SMB_CHECK_ARG(cap >= 1 && cap <= MAXN, "smb_ml_nms_topk: cap=%d outside [1,%d]", cap, MAXN);
+  SMB_CHECK_ARG(out_cap >= 1 && out_cap <= MAXN, "smb_ml_nms_topk: out_cap=%d outside [1,%d]", out_cap, MAXN);
+  SMB_CHECK_ARG(boxes && scores && labels && n_dev && det_out && label_out && idx_out && count_out && kept_total_out &&
+                workspace, "smb_ml_nms_topk: null pointer");
+  const MlWs w = ml_ws_layout(cap);
+  if (workspace_bytes < w.total) {
+    set_error("smb_ml_nms_topk: workspace %zu < %zu", workspace_bytes, w.total);
+    return SMB_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  int P = 1;
+  while (P < cap) P <<= 1;
+  const size_t prep_smem = (size_t)P * sizeof(unsigned long long);
+  static DeviceOnce attr_once;
+  if (attr_once.first()) {
+    SMB_CUDA_OK(cudaFuncSetAttribute(ml_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(8192 * sizeof(unsigned long long))));
+  }
+  const int nbmax = (cap + 63) / 64;
+  ml_prepare_kernel<<<1, NT, prep_smem, st>>>(boxes, scores, labels, n_dev, cap, (int*)(ws + w.cidx), (float*)(ws + w.cscore),
+                                              (unsigned long long*)(ws + w.keys), (float4*)(ws + w.sbox), (int*)(ws + w.slab),
+                                              (int*)(ws + w.m));
+  SMB_LAUNCH_OK("ml_prepare_kernel");
+  ml_mask_kernel<<<132 * 8, 64, 0, st>>>((const float4*)(ws + w.sbox), (const int*)(ws + w.slab), (const int*)(ws + w.m), nbmax,
+                                         iou_thr, (unsigned long long*)(ws + w.mask));
+  SMB_LAUNCH_OK("ml_mask_kernel");
+  mc_sweep_kernel<<<1, NT, 0, st>>>((const unsigned long long*)(ws + w.mask), (const unsigned long long*)(ws + w.keys),
+                                    (const int*)(ws + w.cidx), (const float*)(ws + w.cscore), (const int*)(ws + w.m), cap, nbmax,
+                                    (int*)(ws + w.idx), (float*)(ws + w.score), (int*)(ws + w.count));
+  SMB_LAUNCH_OK("mc_sweep_kernel");
+  ml_finalize_kernel<<<1, NT, 0, st>>>(boxes, labels, (const int*)(ws + w.idx), (const float*)(ws + w.score),
+                                       (const int*)(ws + w.count), cap, max_per_img, out_cap, det_out, (long long*)label_out,
+                                       (long long*)idx_out, count_out, kept_total_out);
+  SMB_LAUNCH_OK("ml_finalize_kernel");
   return SMB_OK;
 }

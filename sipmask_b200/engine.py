@@ -29,7 +29,14 @@ class SipMaskEngine(object):
                  mask_thr=0.4, use_graph=True, head_only=False, feat_sizes=None, in_channels=256,
                  fcos=False, prefix_head='bbox_head.', build_postproc=True, share_weights=None,
                  max_ctas=None, head_max_ctas=None, backbone_dcn=False, ori_shape=None, legacy_interp=False, vis=False,
-                 rescoring_flag=False):
+                 rescoring_flag=False, benchmark=False):
+        # SipMask-benchmark checkpoints (keys from sipmask_b200.benchmark.convert_state_dict): FrozenBatchNorm without eps,
+        # tower / DCN convs with bias before GN, relu'd regression, pair candidates, label-aware NMS, k-th-value cut
+        self.benchmark = benchmark
+        if benchmark:
+            from .benchmark import check_options
+            check_options(vis=vis, rescoring=rescoring_flag)
+        self.bn_eps = 0.0 if benchmark else 1e-5
         self.dev = torch.device(device)
         if self.dev.index is None:
             self.dev = torch.device('cuda', torch.cuda.current_device())
@@ -48,7 +55,8 @@ class SipMaskEngine(object):
         self.backbone_dcn = backbone_dcn           # SipMask++: DeformConvPack (dg=1) as conv2 of every 3rd block of stages 2-4
         self.ncls = num_classes - 1
         self.strides = tuple(strides)
-        self.cfg = dict(nms_pre=1000, score_thr=0.05, nms=dict(type='nms', iou_thr=0.5), max_per_img=100)
+        # BM: INFERENCE_TH, PRE_NMS_TOP_N, NMS_TH, DETECTIONS_PER_IMG (fcos_core/config/defaults.py:295-297,487)
+        self.cfg = dict(nms_pre=1000, score_thr=0.05, nms=dict(type='nms', iou_thr=0.6 if benchmark else 0.5), max_per_img=100)
         if test_cfg:
             self.cfg.update(test_cfg)
         self.img_shape = tuple(img_shape) if img_shape is not None else (self.H, self.W, 3)
@@ -127,7 +135,8 @@ class SipMaskEngine(object):
         if weight is None:
             ck = (wkey, bn, bias_key, cout_pad)
             if ck not in self._wcache:           # tower weights are shared by the five pyramid levels
-                weight, b = C.pack_weight(self._w(wkey), bn=self._bn(bn) if bn else None, cout_pad=cout_pad, device=self.dev)
+                weight, b = C.pack_weight(self._w(wkey), bn=self._bn(bn) if bn else None, eps=self.bn_eps, cout_pad=cout_pad,
+                                          device=self.dev)
                 if bias_key is not None:
                     b = self._w(bias_key)
                     if cout_pad and cout_pad != b.numel():
@@ -169,7 +178,7 @@ class SipMaskEngine(object):
         self.img8 = img8
         self._add(lambda: C.image_to_s2d16(self.img, img8), name='image_to_s2d16')
         wk, b = self._once('stem_s2d', lambda: C.pack_stem_weight_s2d(self._w('backbone.conv1.weight'), self._bn('backbone.bn1'),
-                                                                      device=self.dev))
+                                                                      eps=self.bn_eps, device=self.dev))
         s1 = self._t(N, H // 2, W // 2, 64)
         stem = C.StemPlan(img8, wk, b, s1, N, H, W)
         self._keep += [stem, wk, b]
@@ -276,8 +285,9 @@ class SipMaskEngine(object):
         """ConvModule: conv3x3 -> GN(32) -> ReLU (conv_module.py:124-132) for all pyramid levels in one launch;
         GN statistics come out of the GEMM epilogue (per level, per image)."""
         if self.gn:
-            w, _ = self._packed(wkey)
-            ys = self._conv_multi(xs, w, 3, gn_stats=stats)
+            # BM towers keep the conv bias before GN (sipmask.py:71-82); the epilogue adds it before the statistics
+            w, b = self._packed(wkey, bias_key if self.benchmark else None)
+            ys = self._conv_multi(xs, w, 3, bias=b if self.benchmark else None, gn_stats=stats)
             gamma = self._w(gn_prefix + '.weight').to(self.dev)
             beta = self._w(gn_prefix + '.bias').to(self.dev)
             self._keep += [gamma, beta]
@@ -351,12 +361,16 @@ class SipMaskEngine(object):
         self._tag = 0
         # FeatureAlign: offsets from scale*fcos_reg, DCN 3x3 dg=4, GN, ReLU (sipmask_head.py:49-55)
         offs = [self._t(N, h, w, 72, dtype=torch.float32) for h, w in sizes]
-        self._add(lambda: C.offset_conv1x1_multi(regctr_l, self.scales, w_off, offs), name='offset_conv')
+        # BM: offsets from relu(scale * bbox_pred) (sipmask.py:161-171)
+        self._add(lambda: C.offset_conv1x1_multi(regctr_l, self.scales, w_off, offs, relu=self.benchmark), name='offset_conv')
         cols = [self._t(N, h, w, 2304) for h, w in sizes]
         self._add(lambda: C.deform_im2col_multi(cls_feats, offs, 4, cols), name='deform_im2col')
         if self.gn:
             stats = [self.gn_arena[si, l] for l in range(nl)]
-            aligned = self._conv_multi(cols, wk_dcn, 1, gn_stats=stats)
+            b_dcn = None
+            if self.benchmark:            # DeformConv(bias=True) before GN (sipmask.py:26-30,44)
+                b_dcn = self._once('head.b_dcn', lambda: self._w(hp + 'feat_align.conv_adaption.bias').to(self.dev))
+            aligned = self._conv_multi(cols, wk_dcn, 1, bias=b_dcn, gn_stats=stats)
             gamma = self._w(hp + 'feat_align.norm.weight').to(self.dev)
             beta = self._w(hp + 'feat_align.norm.bias').to(self.dev)
             self._keep += [gamma, beta]
@@ -394,7 +408,10 @@ class SipMaskEngine(object):
                                           out_dtype=torch.float32)
         self._max_ctas = self.max_ctas
         if self.build_post:
-            self._build_postproc()
+            if self.benchmark:
+                self._build_postproc_bm()
+            else:
+                self._build_postproc()
 
     def _build_fcos_head(self, feats):
         """Plain FCOS head (MM/mmdet/models/anchor_heads/fcos_head.py:118-135): 4+4 tower ConvModules, fcos_cls and
@@ -577,6 +594,90 @@ class SipMaskEngine(object):
             self._add(lambda: ops.mask_rescore_f16(self.pos_masks, self.count, self._rescore_w, self.labels, self.det,
                                                    workspace=self._rescore_ws, out=self.mask_scores), 5, name='rescore')
 
+    def _build_postproc_bm(self):
+        """SipMask-benchmark post-processing per image (SipMask-benchmark/fcos_core/modeling/rpn/sipmask/inference.py:
+        66-222): pair candidates -> label-aware NMS + k-th-value cut -> coefficient gather -> mask assembly.  Boxes stay in
+        resized-image coordinates, rois = boxes / 2, masks are resized by 2 / sf with sf = min(h / ori_h, w / ori_w) and
+        pasted into the ori_shape canvas.  `kept_total` [N] holds the number the reference keeps; the record holds the first
+        max_per_img of them (ties at the k-th value can keep more)."""
+        N, cfg, lib = self.N, self.cfg, L.lib()
+        nl = len(self.level_sizes)
+        CCp, ncls = self.clscof.shape[-1], self.ncls
+        nms_pre = int(cfg['nms_pre'])
+        self.max_num = int(cfg['max_per_img'])
+        img_h, img_w = int(self.img_shape[0]), int(self.img_shape[1])
+        oh, ow = int(self.ori_shape[0]), int(self.ori_shape[1])
+        self.mask_hw = (oh, ow)
+        sf = np.minimum(img_h / oh, img_w / ow)                                 # inference.py:196
+        Hm, Wm = self.protos.shape[1], self.protos.shape[2]
+        fh, fw, ry, rx = ops.resize_spec(Hm, Wm, float(2 / sf), self.legacy_interp)
+        self._box_scale4 = L.f4([0.5] * 4)
+        words = (ow + 31) // 32
+        self.det = self._t(N, self.max_num, 5, dtype=torch.float32)
+        self.labels = self._t(N, self.max_num, dtype=torch.long)
+        self.idx = self._t(N, self.max_num, dtype=torch.long)
+        self.count = self._t(N, dtype=torch.int32, zero=True)
+        self.kept_total = self._t(N, dtype=torch.int32, zero=True)
+        self.mask_bits = self._t(N, self.max_num, oh, words, dtype=torch.int32)
+        self.loc_kept = self._t(N, self.max_num, dtype=torch.long)
+        self.det_cofs = self._t(N, self.max_num, 128, dtype=torch.float32)
+        self.det_boxes4 = self._t(N, self.max_num, 4, dtype=torch.float32)
+        level_hw = (ctypes.c_int * nl)(*[h * w for h, w in self.level_sizes])
+        self._keep.append(level_hw)
+        pp_streams = min(N, 4) if N > 1 else 0
+        if pp_streams:
+            self._marker('fork')
+        for n in range(N):
+            self._tag = (n % pp_streams) + 1 if pp_streams else 0
+            lv = (L.Level * nl)()
+            for l, (h, w) in enumerate(self.level_sizes):
+                cc, rc = self.level_views[l][0][n], self.level_views[l][1][n]
+                lv[l] = L.Level(cc.data_ptr(), rc.data_ptr() + 4 * 4, rc.data_ptr(), CCp, 16, 16, h, w, int(self.strides[l]),
+                                float(self.scales[l]), float(self.strides[l]))
+            self._keep.append(lv)
+            ncand = lib.smb_pair_decode_slots(nl, lv, ncls, nms_pre)
+            if ncand < 0 or ncand > 5120:
+                raise ValueError('benchmark: %d candidate slots (nms_pre=%d) exceed the NMS capacity 5120' % (ncand, nms_pre))
+            self.ncand = ncand
+            ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, ncls, nms_pre)
+            ws = self._t(ws_bytes, dtype=torch.uint8)
+            cb, cs = self._t(ncand, 4, dtype=torch.float32), self._t(ncand, dtype=torch.float32)
+            cl, cloc = self._t(ncand, dtype=torch.int32), self._t(ncand, dtype=torch.int32)
+            nc = self._t(1, dtype=torch.int32)
+
+            def decode(lv=lv, ws=ws, ws_bytes=ws_bytes, cb=cb, cs=cs, cl=cl, cloc=cloc, nc=nc, ncand=ncand):
+                L.check(lib.smb_pair_decode_topk(nl, lv, ncls, ctypes.c_float(cfg['score_thr']), nms_pre, img_h, img_w,
+                                                 L.ptr(cb), L.ptr(cs), L.ptr(cl), L.ptr(cloc), L.ptr(nc), ncand, L.ptr(ws),
+                                                 ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_pair_decode_topk')
+            self._add(decode, 3, name='decode_topk')
+            nws_bytes = lib.smb_ml_nms_workspace_bytes(ncand)
+            nws = self._t(nws_bytes, dtype=torch.uint8)
+
+            def nms(n=n, nws=nws, nws_bytes=nws_bytes, cb=cb, cs=cs, cl=cl, nc=nc, ncand=ncand):
+                L.check(lib.smb_ml_nms_topk(L.ptr(cb), L.ptr(cs), L.ptr(cl), L.ptr(nc), ncand, ctypes.c_float(cfg['nms']['iou_thr']),
+                                            self.max_num, self.max_num, L.ptr(self.det[n]), L.ptr(self.labels[n]),
+                                            L.ptr(self.idx[n]), L.ptr(self.count[n:n + 1]), L.ptr(self.kept_total[n:n + 1]),
+                                            L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()), 'smb_ml_nms_topk')
+            self._add(nms, 4, name='nms')
+            cof_src = self.clscof[:, ncls:ncls + 128]
+
+            def gather(n=n, cof_src=cof_src, cloc=cloc):
+                L.check(lib.smb_gather_det_inputs(L.ptr(cof_src), CCp, L.ptr(cloc), L.ptr(self.idx[n]), L.ptr(self.det[n]),
+                                                  L.ptr(self.count[n:n + 1]), self.max_num, 128, L.ptr(self.det_cofs[n]),
+                                                  L.ptr(self.det_boxes4[n]), L.ptr(self.loc_kept[n]), nl if N > 1 else 0,
+                                                  level_hw, N, n, L.stream_ptr()), 'smb_gather_det_inputs')
+            self._add(gather, 1, name='gather_cofs')
+
+            def masks(n=n):
+                L.check(lib.smb_mask_assemble_pack(L.ptr(self.protos[n]), L.F16, 1, L.ptr(self.det_cofs[n]), L.ptr(self.det_boxes4[n]),
+                                                   self._box_scale4, L.ptr(self.mask_bits[n]), Hm, Wm, self.max_num, fh, fw,
+                                                   ctypes.c_float(ry), ctypes.c_float(rx), oh, ow,
+                                                   ctypes.c_float(self.mask_thr), L.stream_ptr()), 'smb_mask_assemble_pack')
+            self._add(masks, 2, name='mask_fused')
+        if pp_streams:
+            self._marker('join')
+        self._tag = 0
+
     # ---------------------------------------------------------------------------------------------- run
     def _run_ops(self, only=None):
         """Issue the launch sequence on the current stream (+ the side stream between fork / join markers).
@@ -673,7 +774,10 @@ class SipMaskEngine(object):
         for l, (cc, rc) in enumerate(self.level_views):
             outs['cls'].append(cc[..., :ncls].permute(0, 3, 1, 2))
             outs['cof'].append(cc[..., ncls:ncls + 128].permute(0, 3, 1, 2))
-            outs['bbox'].append((rc[..., :4] * self.scales[l]).permute(0, 3, 1, 2) * self.strides[l])
+            d = rc[..., :4] * self.scales[l]
+            if self.benchmark:
+                d = torch.relu(d)                     # NORM_REG_TARGETS (sipmask.py:161-167)
+            outs['bbox'].append(d.permute(0, 3, 1, 2) * self.strides[l])
             outs['ctr'].append(rc[..., 4:5].permute(0, 3, 1, 2))
         outs['feat_masks'] = self.protos.permute(0, 3, 1, 2)
         if self.vis:

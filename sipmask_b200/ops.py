@@ -155,13 +155,8 @@ def nms(dets, iou_thr, device_id=None, cmp_ge=False):
 
 
 # ------------------------------------------------------------------------------------- decode + top-k
-@L.device_guard
-def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale_factor=None, box_scales=None):
-    """Per-level tensors channel-last fp32: cls [h,w,C], box [h,w,4] (distances x stride), ctr [h,w,1|].
-
-    Returns cand_boxes [n,4], cand_scores [n,C], cand_ctr [n], cand_loc [n] int32."""
+def _levels(cls_list, box_list, ctr_list, strides, box_scales):
     nl = len(cls_list)
-    C = cls_list[0].shape[-1]
     lv = (L.Level * nl)()
     keep_alive = []
     for i in range(nl):
@@ -177,6 +172,17 @@ def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale
         bs, bm = (1.0, 1.0) if box_scales is None else (float(box_scales[i]), float(strides[i]))
         lv[i] = L.Level(c.data_ptr(), t2.data_ptr(), b.data_ptr(), c.stride(1), t2.stride(1), b.stride(1), h, w,
                         int(strides[i]), bs, bm)
+    return lv, keep_alive
+
+
+@L.device_guard
+def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale_factor=None, box_scales=None):
+    """Per-level tensors channel-last fp32: cls [h,w,C], box [h,w,4] (distances x stride), ctr [h,w,1|].
+
+    Returns cand_boxes [n,4], cand_scores [n,C], cand_ctr [n], cand_loc [n] int32."""
+    nl = len(cls_list)
+    C = cls_list[0].shape[-1]
+    lv, keep_alive = _levels(cls_list, box_list, ctr_list, strides, box_scales)
     lib = L.lib()
     dev = cls_list[0].device
     ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, int(nms_pre))
@@ -194,6 +200,58 @@ def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale
                                 L.ptr(scores), L.ptr(ctr), L.ptr(loc), L.ptr(ws), ctypes.c_size_t(ws_bytes),
                                 L.stream_ptr()), 'smb_decode_topk')
     return boxes, scores, ctr, loc
+
+
+@L.device_guard
+def pair_decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre=1000, score_thr=0.05, box_scales=None):
+    """SipMask-benchmark candidate selection (smb_pair_decode_topk).  Per-level channel-last fp32 tensors as decode_topk:
+    cls [h,w,C] logits, ctr [h,w,1|], box [h,w,4]; distances are relu(box * box_scales[l]) * strides[l] when box_scales is
+    given (raw bbox_pred), else relu(box).  Returns (boxes [n,4], scores [n] = sqrt(cls * ctr), labels [n] int32 0-based,
+    loc [n] int32, n_cand device int32 [1]); n is the slot capacity, rows past n_cand are zero / -1."""
+    nl = len(cls_list)
+    C = cls_list[0].shape[-1]
+    lv, keep_alive = _levels(cls_list, box_list, ctr_list, strides, box_scales)
+    lib = L.lib()
+    dev = cls_list[0].device
+    n = lib.smb_pair_decode_slots(nl, lv, C, int(nms_pre))
+    if n < 0:
+        raise L.SmbError('pair_decode_topk: unsupported levels / nms_pre=%d' % nms_pre)
+    ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, C, int(nms_pre))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    boxes = torch.empty((n, 4), dtype=torch.float32, device=dev)
+    scores = torch.empty((n,), dtype=torch.float32, device=dev)
+    labels = torch.empty((n,), dtype=torch.int32, device=dev)
+    loc = torch.empty((n,), dtype=torch.int32, device=dev)
+    n_cand = torch.empty((1,), dtype=torch.int32, device=dev)
+    L.check(lib.smb_pair_decode_topk(nl, lv, C, ctypes.c_float(score_thr), int(nms_pre), int(img_shape[0]), int(img_shape[1]),
+                                     L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(loc), L.ptr(n_cand), n, L.ptr(ws),
+                                     ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_pair_decode_topk')
+    return boxes, scores, labels, loc, n_cand
+
+
+@L.device_guard
+def ml_nms_topk(boxes, scores, labels, n_cand, iou_thr=0.6, max_per_img=100, out_cap=None):
+    """SipMask-benchmark label-aware NMS + k-th-value cut (smb_ml_nms_topk) over the first *n_cand rows of boxes [cap,4],
+    scores [cap], labels [cap] int32.  Returns (det [out_cap,5], labels int64, idx int64, count int32 [1], kept_total
+    int32 [1]); out_cap defaults to cap."""
+    _need_cuda(boxes, scores, labels, n_cand)
+    boxes, scores = boxes.float().contiguous(), scores.float().contiguous()
+    labels, n_cand = labels.to(torch.int32).contiguous(), n_cand.to(torch.int32).contiguous()
+    cap = boxes.shape[0]
+    out_cap = cap if out_cap is None else int(out_cap)
+    dev = boxes.device
+    lib = L.lib()
+    ws_bytes = lib.smb_ml_nms_workspace_bytes(cap)
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    det = torch.empty((out_cap, 5), dtype=torch.float32, device=dev)
+    lab = torch.empty((out_cap,), dtype=torch.long, device=dev)
+    idx = torch.empty((out_cap,), dtype=torch.long, device=dev)
+    cnt = torch.empty((1,), dtype=torch.int32, device=dev)
+    total = torch.empty((1,), dtype=torch.int32, device=dev)
+    L.check(lib.smb_ml_nms_topk(L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(n_cand), cap, ctypes.c_float(iou_thr),
+                                int(max_per_img), out_cap, L.ptr(det), L.ptr(lab), L.ptr(idx), L.ptr(cnt), L.ptr(total),
+                                L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_ml_nms_topk')
+    return det, lab, idx, cnt, total
 
 
 # ------------------------------------------------------------------------------------ multi-class NMS
