@@ -251,18 +251,16 @@ class SipMaskModule(torch.nn.Module):
         eng = self._engine(features)
         eng.load_features(features)
         eng._run_ops()
-        ncls = self.num_classes - 1
         out = []
         for n, (h, w) in enumerate(images.image_sizes):
-            cls = [cc[n][..., :ncls] for cc, _ in eng.level_views]
-            box = [rc[n][..., :4] for _, rc in eng.level_views]
-            ctr = [rc[n][..., 4:5] for _, rc in eng.level_views]
-            b, sc, lab, loc, nc = ops.pair_decode_topk(cls, box, ctr, self.strides, (h, w), self.nms_pre, self.thr,
+            views = [{k: t[n] for k, t in v.items()} for v in eng.level_views]
+            b, sc, lab, loc, nc = ops.pair_decode_topk([v['cls'] for v in views], [v['box'] for v in views],
+                                                       [v['ctr'] for v in views], self.strides, (h, w), self.nms_pre, self.thr,
                                                        box_scales=eng.scales)
             det, dl, idx, cnt, _ = ops.ml_nms_topk(b, sc, lab, nc, self.nms_thr, self.max_per_img)
             k = int(cnt.item())
             det, dl, idx = det[:k], dl[:k], idx[:k]
-            cof_all = torch.cat([cc[n][..., ncls:ncls + 128].reshape(-1, 128) for cc, _ in eng.level_views])
+            cof_all = torch.cat([v['cof'].reshape(-1, 128) for v in views])
             cofs = cof_all[loc.long()[idx]]
             ow, oh = (img_metas[n] if img_metas is not None else (w, h))
             sf = np.minimum(h / oh, w / ow)                                  # inference.py:196

@@ -129,37 +129,58 @@ class SipMaskEngine(object):
         self.op_names.append(kind)
         self.op_tags.append(kind)
 
-    def _conv(self, x, wkey, k, stride=1, relu=False, bn=None, bias_key=None, residual=None, residual_upsample=False,
-              gn_stats=None, out=None, out_dtype=torch.float16, cout_pad=None, weight=None, bias=None, cin=None,
-              cout_real=None):
-        if weight is None:
-            ck = (wkey, bn, bias_key, cout_pad)
-            if ck not in self._wcache:           # tower weights are shared by the five pyramid levels
-                weight, b = C.pack_weight(self._w(wkey), bn=self._bn(bn) if bn else None, eps=self.bn_eps, cout_pad=cout_pad,
-                                          device=self.dev)
-                if bias_key is not None:
-                    b = self._w(bias_key)
-                    if cout_pad and cout_pad != b.numel():
-                        b = torch.cat([b, b.new_zeros(cout_pad - b.numel())])
-                    b = b.to(self.dev).contiguous()
-                self._wcache[ck] = (weight, b)
-            weight, bias = self._wcache[ck]
-        N, H, W, _ = x.shape
-        Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
-        if out is None:
-            out = self._t(N, Ho, Wo, weight.shape[0], dtype=out_dtype)
-        plan = C.ConvPlan(x, weight, out, k, stride, relu=relu, bias=bias, residual=residual,
-                          residual_upsample=residual_upsample, gn_stats=gn_stats, cin=cin)
-        if self._max_ctas:
+    def _once(self, key, fn):
+        if key not in self._wcache:
+            self._wcache[key] = fn()
+        return self._wcache[key]
+
+    def _packed(self, wkey, bn=None, bias_key=None, cout_pad=None):
+        """(packed weight, fp32 bias) of one convolution, once per weight cache: BN `bn` folded in, or the bias `bias_key`
+        zero-padded to cout_pad."""
+        def pack():
+            weight, b = C.pack_weight(self._w(wkey), bn=self._bn(bn) if bn else None, eps=self.bn_eps, cout_pad=cout_pad,
+                                      device=self.dev)
+            if bias_key is not None:
+                b = self._w(bias_key)
+                if cout_pad and cout_pad != b.numel():
+                    b = torch.cat([b, b.new_zeros(cout_pad - b.numel())])
+                b = b.to(self.dev).contiguous()
+            return weight, b
+        return self._once((wkey, bn, bias_key, cout_pad), pack)
+
+    def _add_conv(self, plan, weight, name, M, k, stride=1, res=False, gn=False, cout_real=None, k_real=None, cap=True):
+        """Registers a convolution plan: CTA cap (`cap`), kept alive, its launch, its algorithmic FLOPs in conv_flops and
+        its GEMM shape in conv_meta."""
+        if cap and self._max_ctas:
             plan.set_max_ctas(self._max_ctas)
         self._keep.append(plan)
         self.conv_plans.append(plan)
-        fl = 2.0 * N * Ho * Wo * (cout_real or weight.shape[0]) * weight.shape[1]                 # algorithmic FLOPs
+        fl = 2.0 * M * (cout_real or weight.shape[0]) * (k_real or weight.shape[1])
         self.conv_flops += fl
-        self.conv_meta.append(dict(name=wkey or 'shared', M=N * Ho * Wo, N=weight.shape[0], K=weight.shape[1], k=k, stride=stride,
-                                   flops=fl, res=residual is not None, gn=gn_stats is not None))
+        self.conv_meta.append(dict(name=name, M=M, N=weight.shape[0], K=weight.shape[1], k=k, stride=stride, flops=fl,
+                                   res=res, gn=gn))
         self._add(plan.run, name='conv')
+
+    def _conv(self, x, wkey, k, stride=1, relu=False, bn=None, bias_key=None, residual=None, residual_upsample=False,
+              out_dtype=torch.float16, cout_pad=None, cout_real=None):
+        weight, bias = self._packed(wkey, bn, bias_key, cout_pad)
+        N, H, W, _ = x.shape
+        Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
+        out = self._t(N, Ho, Wo, weight.shape[0], dtype=out_dtype)
+        plan = C.ConvPlan(x, weight, out, k, stride, relu=relu, bias=bias, residual=residual,
+                          residual_upsample=residual_upsample)
+        self._add_conv(plan, weight, wkey, N * Ho * Wo, k, stride, res=residual is not None, cout_real=cout_real)
         return out
+
+    def _conv_multi(self, xs, weight, k, outs=None, relu=False, bias=None, gn_stats=None, cout_real=None):
+        """One stride-1 convolution over several pyramid levels (one launch)."""
+        N = xs[0].shape[0]
+        if outs is None:
+            outs = [self._t(N, x.shape[1], x.shape[2], weight.shape[0]) for x in xs]
+        plan = C.ConvPlanMulti(xs, weight, outs, k, relu=relu, bias=bias, gn_stats=gn_stats)
+        self._add_conv(plan, weight, 'multi-level x%d' % len(xs), N * sum(x.shape[1] * x.shape[2] for x in xs), k,
+                       gn=gn_stats is not None, cout_real=cout_real)
+        return outs
 
     # -------------------------------------------------------------------------------------------- build
     def _build(self):
@@ -180,14 +201,8 @@ class SipMaskEngine(object):
         wk, b = self._once('stem_s2d', lambda: C.pack_stem_weight_s2d(self._w('backbone.conv1.weight'), self._bn('backbone.bn1'),
                                                                       eps=self.bn_eps, device=self.dev))
         s1 = self._t(N, H // 2, W // 2, 64)
-        stem = C.StemPlan(img8, wk, b, s1, N, H, W)
-        self._keep += [stem, wk, b]
-        self.conv_plans.append(stem)
-        fl = 2.0 * N * (H // 2) * (W // 2) * 64 * 147                                 # algorithmic 7x7x3 (executed K is 256)
-        self.conv_flops += fl
-        self.conv_meta.append(dict(name='stem', M=N * (H // 2) * (W // 2), N=64, K=256, k=7, stride=2, flops=fl,
-                                   res=False, gn=False))
-        self._add(stem.run, name='conv')
+        # algorithmic K is 7x7x3 (executed K is 256); the stem runs on all SMs
+        self._add_conv(C.StemPlan(img8, wk, b, s1, N, H, W), wk, 'stem', N * (H // 2) * (W // 2), 7, 2, k_real=147, cap=False)
         x = self._t(N, H // 4, W // 4, 64)
         self._add(lambda s1=s1, x=x: C.maxpool3x3s2(s1, x), name='maxpool')
         # ---- residual stages (caffe style: stride on conv1, resnet.py:125-130)
@@ -249,66 +264,60 @@ class SipMaskEngine(object):
         p7 = self._conv(p6r, 'neck.fpn_convs.4.conv.weight', 3, 2, bias_key='neck.fpn_convs.4.conv.bias')
         return p5, p6, p7
 
-    def _once(self, key, fn):
-        if key not in self._wcache:
-            self._wcache[key] = fn()
-        return self._wcache[key]
+    def _tower(self, xs, name, n, slot):
+        """ConvModules <hp><name>.0 .. n-1: conv3x3 -> GN(32) -> ReLU (conv_module.py:124-132), each for all pyramid levels
+        in one launch; the GN statistics of conv i come out of the GEMM epilogue into gn_arena[slot + i] (per level, per
+        image)."""
+        for i in range(n):
+            p = '%s%s.%d.' % (self.hp, name, i)
+            if self.gn:
+                # BM towers keep the conv bias before GN (sipmask.py:71-82); the epilogue adds it before the statistics
+                w, b = self._packed(p + 'conv.weight', bias_key=p + 'conv.bias' if self.benchmark else None)
+                stats = [self.gn_arena[slot + i, l] for l in range(len(xs))]
+                xs = self._conv_multi(xs, w, 3, bias=b, gn_stats=stats)
+                self._gn_relu(xs, stats, p + 'gn')
+            else:
+                w, b = self._packed(p + 'conv.weight', bias_key=p + 'conv.bias')
+                xs = self._conv_multi(xs, w, 3, relu=True, bias=b)
+        return xs
 
-    def _packed(self, wkey, bias_key=None, cout_pad=None):
-        ck = (wkey, None, bias_key, cout_pad)
-        if ck not in self._wcache:
-            weight, b = C.pack_weight(self._w(wkey), cout_pad=cout_pad, device=self.dev)
-            if bias_key is not None:
-                b = self._w(bias_key).to(self.dev).contiguous()
-            self._wcache[ck] = (weight, b)
-        return self._wcache[ck]
+    def _gn_relu(self, xs, stats, prefix):
+        gamma = self._w(prefix + '.weight').to(self.dev)
+        beta = self._w(prefix + '.bias').to(self.dev)
+        self._keep += [gamma, beta]
+        self._add(lambda: C.groupnorm_relu_apply_multi(xs, stats, gamma, beta, 1e-5, True), name='gn_apply')
 
-    def _conv_multi(self, xs, weight, k, outs=None, relu=False, bias=None, gn_stats=None, out_dtype=torch.float16,
-                    cout_real=None):
-        N = xs[0].shape[0]
-        if outs is None:
-            outs = [self._t(N, x.shape[1], x.shape[2], weight.shape[0], dtype=out_dtype) for x in xs]
-        plan = C.ConvPlanMulti(xs, weight, outs, k, relu=relu, bias=bias, gn_stats=gn_stats)
-        if self._max_ctas:
-            plan.set_max_ctas(self._max_ctas)
-        self._keep.append(plan)
-        self.conv_plans.append(plan)
-        npix = sum(x.shape[1] * x.shape[2] for x in xs)
-        fl = 2.0 * N * npix * (cout_real or weight.shape[0]) * weight.shape[1]
-        self.conv_flops += fl
-        self.conv_meta.append(dict(name='multi-level x%d' % len(xs), M=N * npix, N=weight.shape[0], K=weight.shape[1], k=k, stride=1,
-                                   flops=fl, res=False, gn=gn_stats is not None))
-        self._add(plan.run, name='conv')
-        return outs
-
-    def _tower_conv(self, xs, wkey, gn_prefix, bias_key, stats):
-        """ConvModule: conv3x3 -> GN(32) -> ReLU (conv_module.py:124-132) for all pyramid levels in one launch;
-        GN statistics come out of the GEMM epilogue (per level, per image)."""
-        if self.gn:
-            # BM towers keep the conv bias before GN (sipmask.py:71-82); the epilogue adds it before the statistics
-            w, b = self._packed(wkey, bias_key if self.benchmark else None)
-            ys = self._conv_multi(xs, w, 3, bias=b if self.benchmark else None, gn_stats=stats)
-            gamma = self._w(gn_prefix + '.weight').to(self.dev)
-            beta = self._w(gn_prefix + '.bias').to(self.dev)
-            self._keep += [gamma, beta]
-            self._add(lambda: C.groupnorm_relu_apply_multi(ys, stats, gamma, beta, 1e-5, True), name='gn_apply')
-            return ys
-        w, b = self._packed(wkey, bias_key)
-        return self._conv_multi(xs, w, 3, relu=True, bias=b)
+    def _head_buffers(self, feats, n_stats, cls_pitch):
+        """What both heads allocate: one int64 fixed-point statistics arena for every (conv, level) GroupNorm, zeroed once per
+        forward; the Scale values; the fp32 head outputs, channel-last, ONE allocation each in level-major order
+        [level][image][h*w][C]: clscof (C = cls_pitch) and regctr (C = 16).  Every level is a contiguous [N,h,w,C] tensor
+        for the GEMM epilogue, and with N == 1 the buffer is the level-concatenated [tot, C] table a candidate's location
+        index addresses directly.  Returns the per-level [N,h,w,C] views of clscof and of regctr."""
+        N = self.N
+        sizes = self.level_sizes = [(f.shape[1], f.shape[2]) for f in feats]
+        self.gn_arena = self._t(n_stats, len(sizes), N, 32, 2, dtype=torch.int64, zero=True)
+        self._add(lambda: self.gn_arena.zero_(), 0, name='memset')
+        self.scales = [float(self._w(self.hp + 'scales.%d.scale' % i)) for i in range(len(sizes))]
+        tot = sum(h * w for h, w in sizes)
+        self.clscof = self._t(N * tot, cls_pitch, dtype=torch.float32)
+        self.regctr = self._t(N * tot, 16, dtype=torch.float32)
+        cls_l, reg_l, o = [], [], 0
+        for h, w in sizes:
+            cls_l.append(self.clscof[N * o:N * (o + h * w)].view(N, h, w, cls_pitch))
+            reg_l.append(self.regctr[N * o:N * (o + h * w)].view(N, h, w, 16))
+            o += h * w
+        return cls_l, reg_l
 
     def _build_head(self, feats):
-        N = self.N
-        hp = self.hp
-        sizes = [(f.shape[1], f.shape[2]) for f in feats]
-        self.level_sizes = sizes
-        tot = sum(h * w for h, w in sizes)
-        nl = len(feats)
-        n_tower = (self.stacked - 1) + self.stacked + 1 + ((self.stacked - 1) if self.vis else 0)
-        # one int64 fixed-point statistics arena for every (conv, level) GroupNorm, zeroed once per forward
-        self.gn_arena = self._t(n_tower, nl, N, 32, 2, dtype=torch.int64, zero=True)
-        self._add(lambda: self.gn_arena.zero_(), 0, name='memset')
-        ncls, CC = self.ncls, self.ncls + 128
+        N, hp, ncls = self.N, self.hp, self.ncls
+        CC = ncls + 128
         CCp = (CC + 15) // 16 * 16
+        si = 2 * self.stacked - 1                        # GN statistics slot of FeatureAlign, after the cls and reg towers
+        cls_l, reg_l = self._head_buffers(feats, si + 1 + ((self.stacked - 1) if self.vis else 0), CCp)
+        # clscof = [cls | 128 coefficients | pad], regctr = [4 raw box distances | centerness | pad]
+        self.level_views = [dict(cls=c[..., :ncls], cof=c[..., ncls:CC], box=r[..., :4], ctr=r[..., 4:5])
+                            for c, r in zip(cls_l, reg_l)]
+        self.cof_src = self.clscof[:, ncls:CC]          # coefficients of every location, row pitch CCp
         w_cls = torch.cat([self._w(hp + 'fcos_cls.weight'), self._w(hp + 'sip_cof.weight')], 0)
         b_cls = torch.cat([self._w(hp + 'fcos_cls.bias'), self._w(hp + 'sip_cof.bias')], 0)
         wk_cls = self._once('head.wk_cls', lambda: C.pack_weight(w_cls, cout_pad=CCp, device=self.dev)[0])
@@ -322,20 +331,6 @@ class SipMaskEngine(object):
         w_off = self._once('head.w_off',
                            lambda: self._w(hp + 'feat_align.conv_offset.weight').view(72, 4).contiguous().to(self.dev))
         self._keep += [wk_cls, b_cls, wk_reg, b_reg, wk_dcn, w_off]
-        self.scales = [float(self._w(hp + 'scales.%d.scale' % i)) for i in range(nl)]
-        # fp32 head outputs, channel-last, ONE allocation in level-major order [level][image][h*w][C] with C = 80+128 (-> 208)
-        # and 16 = 4 reg | 1 ctr | pad: every level is a contiguous [N,h,w,C] tensor for the GEMM epilogue, and with N == 1
-        # the buffer is the level-concatenated [tot, C] table a candidate's location index addresses directly
-        self.clscof = self._t(N * tot, CCp, dtype=torch.float32)
-        self.regctr = self._t(N * tot, 16, dtype=torch.float32)
-        offs0 = [sum(h * w for h, w in sizes[:l]) for l in range(nl)]
-        clscof_l = [self.clscof[N * offs0[l]:N * (offs0[l] + sizes[l][0] * sizes[l][1])].view(N, sizes[l][0], sizes[l][1], CCp)
-                    for l in range(nl)]
-        regctr_l = [self.regctr[N * offs0[l]:N * (offs0[l] + sizes[l][0] * sizes[l][1])].view(N, sizes[l][0], sizes[l][1], 16)
-                    for l in range(nl)]
-        self.level_views = list(zip(clscof_l, regctr_l))
-        si = 0
-        cls_feats, reg_feats = list(feats), list(feats)
         # The cls and reg towers are independent chains of 202-tile GEMMs (1.5 waves each on 132 SMs).  They are
         # captured on two streams with their persistent grids capped at half the GPU, so together they keep every SM
         # busy (3.06 waves for a pair instead of 2 + 2).
@@ -345,44 +340,36 @@ class SipMaskEngine(object):
             cap = min(cap, self.max_ctas) if cap else self.max_ctas
         self._max_ctas = cap or None
         self._tag = 0
-        for i in range(self.stacked - 1):
-            cls_feats = self._tower_conv(cls_feats, hp + 'cls_convs.%d.conv.weight' % i, hp + 'cls_convs.%d.gn' % i,
-                                         hp + 'cls_convs.%d.conv.bias' % i, [self.gn_arena[si, l] for l in range(nl)])
-            si += 1
+        cls_feats = self._tower(feats, 'cls_convs', self.stacked - 1, 0)
         self._tag = 1
-        for i in range(self.stacked):
-            reg_feats = self._tower_conv(reg_feats, hp + 'reg_convs.%d.conv.weight' % i, hp + 'reg_convs.%d.gn' % i,
-                                         hp + 'reg_convs.%d.conv.bias' % i, [self.gn_arena[si, l] for l in range(nl)])
-            si += 1
+        reg_feats = self._tower(feats, 'reg_convs', self.stacked, self.stacked - 1)
         # fcos_reg | fcos_centerness on the reg tower (sipmask_head.py:261,265), raw fp32 (Scale applied by consumers)
-        self._conv_multi(reg_feats, wk_reg, 3, outs=regctr_l, bias=b_reg, cout_real=5)
+        self._conv_multi(reg_feats, wk_reg, 3, outs=reg_l, bias=b_reg, cout_real=5)
         self._marker('join')
         self._marker('fork')
         self._tag = 0
         # FeatureAlign: offsets from scale*fcos_reg, DCN 3x3 dg=4, GN, ReLU (sipmask_head.py:49-55)
-        offs = [self._t(N, h, w, 72, dtype=torch.float32) for h, w in sizes]
+        offs = [self._t(N, h, w, 72, dtype=torch.float32) for h, w in self.level_sizes]
+        boxes = [v['box'] for v in self.level_views]
         # BM: offsets from relu(scale * bbox_pred) (sipmask.py:161-171)
-        self._add(lambda: C.offset_conv1x1_multi(regctr_l, self.scales, w_off, offs, relu=self.benchmark), name='offset_conv')
-        cols = [self._t(N, h, w, 2304) for h, w in sizes]
+        self._add(lambda: C.offset_conv1x1_multi(boxes, self.scales, w_off, offs, relu=self.benchmark), name='offset_conv')
+        cols = [self._t(N, h, w, 2304) for h, w in self.level_sizes]
         self._add(lambda: C.deform_im2col_multi(cls_feats, offs, 4, cols), name='deform_im2col')
         if self.gn:
-            stats = [self.gn_arena[si, l] for l in range(nl)]
+            stats = [self.gn_arena[si, l] for l in range(len(feats))]
             b_dcn = None
             if self.benchmark:            # DeformConv(bias=True) before GN (sipmask.py:26-30,44)
                 b_dcn = self._once('head.b_dcn', lambda: self._w(hp + 'feat_align.conv_adaption.bias').to(self.dev))
             aligned = self._conv_multi(cols, wk_dcn, 1, bias=b_dcn, gn_stats=stats)
-            gamma = self._w(hp + 'feat_align.norm.weight').to(self.dev)
-            beta = self._w(hp + 'feat_align.norm.bias').to(self.dev)
-            self._keep += [gamma, beta]
-            self._add(lambda: C.groupnorm_relu_apply_multi(aligned, stats, gamma, beta, 1e-5, True), name='gn_apply')
+            self._gn_relu(aligned, stats, hp + 'feat_align.norm')
         else:
             aligned = self._conv_multi(cols, wk_dcn, 1, relu=True)
         # fcos_cls | sip_cof on the aligned feature (sipmask_head.py:264,271)
-        self._conv_multi(aligned, wk_cls, 3, outs=clscof_l, bias=b_cls)
+        self._conv_multi(aligned, wk_cls, 3, outs=cls_l, bias=b_cls)
         # prototype branch on the side stream, next to FeatureAlign / the cls heads
         self._tag = 1
         # prototype input: reg feature of levels 0..2 at P3 resolution (sipmask_head.py:275-281)
-        h3, w3 = sizes[0]
+        h3, w3 = self.level_sizes[0]
         cat = self._t(N, h3, w3, 768)
         for l in range(3):
             self._add(lambda l=l: C.upsample_bilinear(reg_feats[l], 2 ** l, out=cat, out_choff=256 * l), name='upsample')
@@ -396,35 +383,24 @@ class SipMaskEngine(object):
         if self.vis:
             # tracking branch (VIS/...:274-287,296-312): track_convs on levels 0..2 -> bilinear x1 / x2 / x4 to P3 resolution ->
             # concat 768 -> sipmask_track 1x1 -> 512, fp32 (the features enter dot products of the association)
-            tfe = list(feats[:3])
-            for i in range(self.stacked - 1):
-                tfe = self._tower_conv(tfe, hp + 'track_convs.%d.conv.weight' % i, hp + 'track_convs.%d.gn' % i,
-                                       hp + 'track_convs.%d.conv.bias' % i, [self.gn_arena[si + 1 + i, l] for l in range(3)])
+            tfe = self._tower(feats[:3], 'track_convs', self.stacked - 1, si + 1)
             cat_t = self._t(N, h3, w3, 768)
             for l in range(3):
-                self._add(lambda l=l, tfe=tfe, cat_t=cat_t: C.upsample_bilinear(tfe[l], 2 ** l, out=cat_t, out_choff=256 * l),
-                          name='upsample')
+                self._add(lambda l=l: C.upsample_bilinear(tfe[l], 2 ** l, out=cat_t, out_choff=256 * l), name='upsample')
             self.track_feats = self._conv(cat_t, hp + 'sipmask_track.weight', 1, bias_key=hp + 'sipmask_track.bias',
                                           out_dtype=torch.float32)
         self._max_ctas = self.max_ctas
         if self.build_post:
-            if self.benchmark:
-                self._build_postproc_bm()
-            else:
-                self._build_postproc()
+            self._build_postproc()
 
     def _build_fcos_head(self, feats):
         """Plain FCOS head (MM/mmdet/models/anchor_heads/fcos_head.py:118-135): 4+4 tower ConvModules, fcos_cls and
         fcos_centerness on the cls tower, fcos_reg on the reg tower (exp(scale * x) is applied by the caller)."""
-        N, hp = self.N, self.hp
-        sizes = [(f.shape[1], f.shape[2]) for f in feats]
-        self.level_sizes = sizes
-        nl = len(feats)
-        tot = sum(h * w for h, w in sizes)
-        self.gn_arena = self._t(2 * self.stacked, nl, N, 32, 2, dtype=torch.int64, zero=True)
-        self._add(lambda: self.gn_arena.zero_(), 0, name='memset')
-        ncls = self.ncls
+        hp, ncls = self.hp, self.ncls
         CCp = (ncls + 1 + 15) // 16 * 16
+        cls_l, reg_l = self._head_buffers(feats, 2 * self.stacked, CCp)
+        # clscof = [cls | centerness | pad], regctr = [4 raw box distances | pad]
+        self.level_views = [dict(cls=c[..., :ncls], ctr=c[..., ncls:ncls + 1], box=r[..., :4]) for c, r in zip(cls_l, reg_l)]
         w_cls = torch.cat([self._w(hp + 'fcos_cls.weight'), self._w(hp + 'fcos_centerness.weight')], 0)
         b_cls = torch.cat([self._w(hp + 'fcos_cls.bias'), self._w(hp + 'fcos_centerness.bias')], 0)
         wk_cls, _ = C.pack_weight(w_cls, cout_pad=CCp, device=self.dev)
@@ -432,23 +408,8 @@ class SipMaskEngine(object):
         wk_reg, _ = C.pack_weight(self._w(hp + 'fcos_reg.weight'), cout_pad=16, device=self.dev)
         b_reg = torch.cat([self._w(hp + 'fcos_reg.bias'), torch.zeros(12)]).to(self.dev)
         self._keep += [wk_cls, b_cls, wk_reg, b_reg]
-        self.scales = [float(self._w(hp + 'scales.%d.scale' % i)) for i in range(nl)]
-        self.clscof = self._t(N * tot, CCp, dtype=torch.float32)      # [cls(80) | centerness(1) | pad], level-major
-        self.regctr = self._t(N * tot, 16, dtype=torch.float32)       # [reg(4) | pad]
-        offs0 = [sum(h * w for h, w in sizes[:l]) for l in range(nl)]
-        cls_l = [self.clscof[N * offs0[l]:N * (offs0[l] + sizes[l][0] * sizes[l][1])].view(N, sizes[l][0], sizes[l][1], CCp) for l in range(nl)]
-        reg_l = [self.regctr[N * offs0[l]:N * (offs0[l] + sizes[l][0] * sizes[l][1])].view(N, sizes[l][0], sizes[l][1], 16) for l in range(nl)]
-        self.level_views = list(zip(cls_l, reg_l))
-        si = 0
-        cls_feats, reg_feats = list(feats), list(feats)
-        for i in range(self.stacked):
-            cls_feats = self._tower_conv(cls_feats, hp + 'cls_convs.%d.conv.weight' % i, hp + 'cls_convs.%d.gn' % i,
-                                         hp + 'cls_convs.%d.conv.bias' % i, [self.gn_arena[si, l] for l in range(nl)])
-            si += 1
-        for i in range(self.stacked):
-            reg_feats = self._tower_conv(reg_feats, hp + 'reg_convs.%d.conv.weight' % i, hp + 'reg_convs.%d.gn' % i,
-                                         hp + 'reg_convs.%d.conv.bias' % i, [self.gn_arena[si, l] for l in range(nl)])
-            si += 1
+        cls_feats = self._tower(feats, 'cls_convs', self.stacked, 0)
+        reg_feats = self._tower(feats, 'reg_convs', self.stacked, self.stacked)
         self._conv_multi(cls_feats, wk_cls, 3, outs=cls_l, bias=b_cls, cout_real=ncls + 1)
         self._conv_multi(reg_feats, wk_reg, 3, outs=reg_l, bias=b_reg, cout_real=4)
 
@@ -459,38 +420,58 @@ class SipMaskEngine(object):
 
     # ------------------------------------------------------------------------------- post-processing
     def _build_postproc(self):
-        """decode -> NMS -> coefficient gather -> mask assembly -> x2 upsample/threshold/bit-pack, image by image
-        (get_bboxes loops over images, sipmask_head.py:517-540), all on device with fixed-shape outputs."""
-        N, dev = self.N, self.dev
-        cfg = self.cfg
-        nl = len(self.level_sizes)
-        CCp = self.clscof.shape[-1]
-        ncls = self.ncls
+        """candidates -> NMS -> coefficient gather -> mask assembly -> resize / threshold / bit-pack into the ori_shape
+        canvas, image by image (get_bboxes loops over images, sipmask_head.py:517-540), all on device with fixed-shape
+        outputs.  Only the candidates and the NMS depend on the checkpoint tree (_mm_candidates, _bm_candidates).
+        MM: rescale=True semantics, boxes / scale_factor and masks resized by 2 / scale_factor (sipmask_head.py:587-588,
+        629-633,648-654).  BM (SipMask-benchmark/fcos_core/modeling/rpn/sipmask/inference.py:66-222): boxes stay in
+        resized-image coordinates, rois = boxes / 2, masks are resized by 2 / sf with sf = min(h / ori_h, w / ori_w)."""
+        N, cfg, lib = self.N, self.cfg, L.lib()
+        nl, ncls = len(self.level_sizes), self.ncls
         nms_pre = int(cfg['nms_pre'])
-        self.max_num = 100 if self.ssd else int(cfg['max_per_img'])      # MM's fast_nms hard-codes 100 (sipmask_head.py:903)
-        fast = self.ssd or self.vis                                         # VIS: fast_nms with cfg.max_per_img (VIS/...:986)
-        ncand = sum(min(h * w, nms_pre) if nms_pre > 0 else h * w for h, w in self.level_sizes)
-        self.ncand = ncand
-        lib = L.lib()
+        oh, ow = int(self.ori_shape[0]), int(self.ori_shape[1])
+        self.mask_hw = (oh, ow)
+        Hm, Wm = self.protos.shape[1], self.protos.shape[2]
         sf = np.atleast_1d(np.asarray(self.scale_factor, dtype=np.float32))
         s4 = (sf if sf.size == 4 else np.repeat(sf, 4)).astype(np.float32)
-        self._sf4 = L.f4(s4)
-        self._box_scale4 = L.f4(s4 / 2.0)
-        Hm, Wm = self.protos.shape[1], self.protos.shape[2]
-        oh, ow = int(self.ori_shape[0]), int(self.ori_shape[1])        # rescale=True: masks live in the ori_shape canvas
-        self.mask_hw = (oh, ow)
-        from .postproc import mask_up_factors
-        fh, fw, ry, rx = ops.resize_spec(Hm, Wm, mask_up_factors(self.scale_factor, self.ssd), self.legacy_interp)
+        levels = []                                     # per image: the smb_level_t array over its head outputs
+        for n in range(N):
+            lv, views = ops.level_descs([v['cls'][n] for v in self.level_views], [v['box'][n] for v in self.level_views],
+                                        [v['ctr'][n] for v in self.level_views], self.strides, self.scales)
+            self._keep += [lv, views]
+            levels.append(lv)
+        if self.benchmark:
+            self.max_num = int(cfg['max_per_img'])
+            self.ncand = lib.smb_pair_decode_slots(nl, levels[0], ncls, nms_pre)
+            if self.ncand < 0 or self.ncand > 5120:
+                raise ValueError('benchmark: %d candidate slots (nms_pre=%d) exceed the NMS capacity 5120' % (self.ncand, nms_pre))
+            self._box_scale4 = L.f4([0.5] * 4)
+            up = float(2 / np.minimum(int(self.img_shape[0]) / oh, int(self.img_shape[1]) / ow))     # inference.py:196
+            self.cand_scores = self._t(N, self.ncand, dtype=torch.float32)
+            self.cand_labels = self._t(N, self.ncand, dtype=torch.int32)
+            self.n_cand = self._t(N, dtype=torch.int32)
+            # the number the reference keeps; the record holds the first max_per_img (ties at the k-th value keep more)
+            self.kept_total = self._t(N, dtype=torch.int32, zero=True)
+            candidates = self._bm_candidates
+        else:
+            self.max_num = 100 if self.ssd else int(cfg['max_per_img'])      # MM's fast_nms hard-codes 100 (sipmask_head.py:903)
+            self.ncand = sum(min(h * w, nms_pre) if nms_pre > 0 else h * w for h, w in self.level_sizes)
+            self._sf4 = L.f4(s4)
+            self._box_scale4 = L.f4(s4 / 2.0)
+            from .postproc import mask_up_factors
+            up = mask_up_factors(self.scale_factor, self.ssd)
+            self.cand_scores = self._t(N, self.ncand, ncls, dtype=torch.float32)
+            self.cand_ctr = self._t(N, self.ncand, dtype=torch.float32)
+            candidates = self._mm_candidates
+        self.cand_boxes = self._t(N, self.ncand, 4, dtype=torch.float32)
+        self.cand_loc = self._t(N, self.ncand, dtype=torch.int32)
+        fh, fw, ry, rx = ops.resize_spec(Hm, Wm, up, self.legacy_interp)
         words = (ow + 31) // 32
         self.det = self._t(N, self.max_num, 5, dtype=torch.float32)
         self.labels = self._t(N, self.max_num, dtype=torch.long)
         self.idx = self._t(N, self.max_num, dtype=torch.long)
         self.count = self._t(N, dtype=torch.int32, zero=True)
         self.mask_bits = self._t(N, self.max_num, oh, words, dtype=torch.int32)
-        self.cand_boxes = self._t(N, ncand, 4, dtype=torch.float32)
-        self.cand_scores = self._t(N, ncand, ncls, dtype=torch.float32)
-        self.cand_ctr = self._t(N, ncand, dtype=torch.float32)
-        self.cand_loc = self._t(N, ncand, dtype=torch.int32)
         self.loc_kept = self._t(N, self.max_num, dtype=torch.long)
         self.det_cofs = self._t(N, self.max_num, 128, dtype=torch.float32)
         self.det_boxes4 = self._t(N, self.max_num, 4, dtype=torch.float32)
@@ -508,64 +489,26 @@ class SipMaskEngine(object):
             self.rescore_flops = float(N * self.max_num * ops.rescore_flops_per_row(Hm, Wm))    # at full detection counts
         level_hw = (ctypes.c_int * nl)(*[h * w for h, w in self.level_sizes])
         self._keep.append(level_hw)
-        # the per-image decode -> NMS -> gather -> mask chains are independent (get_bboxes loops over images,
-        # sipmask_head.py:517-540): with a batch they are spread over a few streams of the captured graph
+        # the per-image chains are independent (get_bboxes loops over images, sipmask_head.py:517-540): with a batch they
+        # are spread over a few streams of the captured graph
         pp_streams = min(N, 4) if N > 1 else 0
         if pp_streams:
             self._marker('fork')
         for n in range(N):
             self._tag = (n % pp_streams) + 1 if pp_streams else 0
-            lv = (L.Level * nl)()
-            for l, (h, w) in enumerate(self.level_sizes):
-                cc = self.level_views[l][0][n]                 # [h,w,CCp] of image n (contiguous)
-                rc = self.level_views[l][1][n]
-                lv[l] = L.Level(cc.data_ptr(), rc.data_ptr() + 4 * 4, rc.data_ptr(), CCp, 16, 16, h, w, int(self.strides[l]),
-                                float(self.scales[l]), float(self.strides[l]))
-            ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, nms_pre)
-            ws = self._t(ws_bytes, dtype=torch.uint8)
-            self._keep.append(lv)
+            cand_loc = candidates(n, levels[n])
 
-            def decode(n=n, lv=lv, ws=ws, ws_bytes=ws_bytes):
-                L.check(lib.smb_decode_topk(nl, lv, ncls, nms_pre, int(self.img_shape[0]), int(self.img_shape[1]), self._sf4,
-                                            L.ptr(self.cand_boxes[n]), L.ptr(self.cand_scores[n]), L.ptr(self.cand_ctr[n]),
-                                            L.ptr(self.cand_loc[n]), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
-                        'smb_decode_topk')
-            self._add(decode, 3, name='decode_topk')
-            iou_thr = float(cfg['nms']['iou_thr'])
-            if not fast:
-                nws_bytes = lib.smb_multiclass_nms_workspace_bytes(ncand, ncls)
-                nws = self._t(nws_bytes, dtype=torch.uint8)
-
-                def nms(n=n, nws=nws, nws_bytes=nws_bytes):
-                    L.check(lib.smb_multiclass_nms(L.ptr(self.cand_boxes[n]), L.ptr(self.cand_scores[n]), L.ptr(self.cand_ctr[n]),
-                                                   ncand, ncls, ctypes.c_float(cfg['score_thr']), ctypes.c_float(iou_thr),
-                                                   self.max_num, 0, L.ptr(self.det[n]), L.ptr(self.labels[n]), L.ptr(self.idx[n]),
-                                                   L.ptr(self.count[n:n + 1]), L.ptr(nws), ctypes.c_size_t(nws_bytes),
-                                                   L.stream_ptr()), 'smb_multiclass_nms')
-            else:
-                nws_bytes = lib.smb_fast_nms_workspace_bytes(ncand, ncls, 200)
-                nws = self._t(nws_bytes, dtype=torch.uint8)
-
-                def nms(n=n, nws=nws, nws_bytes=nws_bytes):
-                    L.check(lib.smb_fast_nms(L.ptr(self.cand_boxes[n]), L.ptr(self.cand_scores[n]), L.ptr(self.cand_ctr[n]), ncand,
-                                             ncls, ctypes.c_float(cfg['score_thr']), ctypes.c_float(iou_thr), 200, self.max_num,
-                                             L.ptr(self.det[n]), L.ptr(self.labels[n]), L.ptr(self.idx[n]),
-                                             L.ptr(self.count[n:n + 1]), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()),
-                            'smb_fast_nms')
-            self._add(nms, 4 if not fast else 2, name='nms')
-            cof_src = self.clscof[:, ncls:ncls + 128]                          # coefficient columns, row pitch CCp
-
-            def gather(n=n, cof_src=cof_src):
+            def gather(n=n, cand_loc=cand_loc):
                 # candidate row -> level-concatenated location -> coefficient row (mlvl_cofs[idxs_keep], sipmask_head.py:612)
-                # and det[:, :4] -> contiguous rois input, one launch (was index_select + gather + copy_)
-                L.check(lib.smb_gather_det_inputs(L.ptr(cof_src), CCp, L.ptr(self.cand_loc[n]), L.ptr(self.idx[n]),
+                # and det[:, :4] -> contiguous rois input, one launch
+                L.check(lib.smb_gather_det_inputs(L.ptr(self.cof_src), self.cof_src.stride(0), L.ptr(cand_loc), L.ptr(self.idx[n]),
                                                   L.ptr(self.det[n]), L.ptr(self.count[n:n + 1]), self.max_num, 128,
                                                   L.ptr(self.det_cofs[n]), L.ptr(self.det_boxes4[n]), L.ptr(self.loc_kept[n]),
                                                   nl if N > 1 else 0, level_hw, N, n, L.stream_ptr()), 'smb_gather_det_inputs')
             self._add(gather, 1, name='gather_cofs')
 
             def masks(n=n):
-                # fused: prototypes -> sub-region dot/sigmoid/crop -> x2 bilinear -> threshold -> bit-pack (no pos_masks tensor)
+                # fused: prototypes -> sub-region dot/sigmoid/crop -> resize -> threshold -> bit-pack (no pos_masks tensor)
                 L.check(lib.smb_mask_assemble_pack(L.ptr(self.protos[n]), L.F16, 1, L.ptr(self.det_cofs[n]), L.ptr(self.det_boxes4[n]),
                                                    self._box_scale4, L.ptr(self.mask_bits[n]), Hm, Wm, self.max_num, fh, fw,
                                                    ctypes.c_float(ry), ctypes.c_float(rx), oh, ow,
@@ -594,89 +537,70 @@ class SipMaskEngine(object):
             self._add(lambda: ops.mask_rescore_f16(self.pos_masks, self.count, self._rescore_w, self.labels, self.det,
                                                    workspace=self._rescore_ws, out=self.mask_scores), 5, name='rescore')
 
-    def _build_postproc_bm(self):
-        """SipMask-benchmark post-processing per image (SipMask-benchmark/fcos_core/modeling/rpn/sipmask/inference.py:
-        66-222): pair candidates -> label-aware NMS + k-th-value cut -> coefficient gather -> mask assembly.  Boxes stay in
-        resized-image coordinates, rois = boxes / 2, masks are resized by 2 / sf with sf = min(h / ori_h, w / ori_w) and
-        pasted into the ori_shape canvas.  `kept_total` [N] holds the number the reference keeps; the record holds the first
-        max_per_img of them (ties at the k-th value can keep more)."""
-        N, cfg, lib = self.N, self.cfg, L.lib()
-        nl = len(self.level_sizes)
-        CCp, ncls = self.clscof.shape[-1], self.ncls
-        nms_pre = int(cfg['nms_pre'])
-        self.max_num = int(cfg['max_per_img'])
-        img_h, img_w = int(self.img_shape[0]), int(self.img_shape[1])
-        oh, ow = int(self.ori_shape[0]), int(self.ori_shape[1])
-        self.mask_hw = (oh, ow)
-        sf = np.minimum(img_h / oh, img_w / ow)                                 # inference.py:196
-        Hm, Wm = self.protos.shape[1], self.protos.shape[2]
-        fh, fw, ry, rx = ops.resize_spec(Hm, Wm, float(2 / sf), self.legacy_interp)
-        self._box_scale4 = L.f4([0.5] * 4)
-        words = (ow + 31) // 32
-        self.det = self._t(N, self.max_num, 5, dtype=torch.float32)
-        self.labels = self._t(N, self.max_num, dtype=torch.long)
-        self.idx = self._t(N, self.max_num, dtype=torch.long)
-        self.count = self._t(N, dtype=torch.int32, zero=True)
-        self.kept_total = self._t(N, dtype=torch.int32, zero=True)
-        self.mask_bits = self._t(N, self.max_num, oh, words, dtype=torch.int32)
-        self.loc_kept = self._t(N, self.max_num, dtype=torch.long)
-        self.det_cofs = self._t(N, self.max_num, 128, dtype=torch.float32)
-        self.det_boxes4 = self._t(N, self.max_num, 4, dtype=torch.float32)
-        level_hw = (ctypes.c_int * nl)(*[h * w for h, w in self.level_sizes])
-        self._keep.append(level_hw)
-        pp_streams = min(N, 4) if N > 1 else 0
-        if pp_streams:
-            self._marker('fork')
-        for n in range(N):
-            self._tag = (n % pp_streams) + 1 if pp_streams else 0
-            lv = (L.Level * nl)()
-            for l, (h, w) in enumerate(self.level_sizes):
-                cc, rc = self.level_views[l][0][n], self.level_views[l][1][n]
-                lv[l] = L.Level(cc.data_ptr(), rc.data_ptr() + 4 * 4, rc.data_ptr(), CCp, 16, 16, h, w, int(self.strides[l]),
-                                float(self.scales[l]), float(self.strides[l]))
-            self._keep.append(lv)
-            ncand = lib.smb_pair_decode_slots(nl, lv, ncls, nms_pre)
-            if ncand < 0 or ncand > 5120:
-                raise ValueError('benchmark: %d candidate slots (nms_pre=%d) exceed the NMS capacity 5120' % (ncand, nms_pre))
-            self.ncand = ncand
-            ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, ncls, nms_pre)
-            ws = self._t(ws_bytes, dtype=torch.uint8)
-            cb, cs = self._t(ncand, 4, dtype=torch.float32), self._t(ncand, dtype=torch.float32)
-            cl, cloc = self._t(ncand, dtype=torch.int32), self._t(ncand, dtype=torch.int32)
-            nc = self._t(1, dtype=torch.int32)
+    def _mm_candidates(self, n, lv):
+        """MM candidates of image n: decode + per-level top-k (smb_decode_topk), then multi-class NMS, or fast NMS for SSD
+        and VIS (fast_nms with cfg.max_per_img, VIS/...:986).  Returns the candidate -> location table."""
+        cfg, lib, ncls, ncand = self.cfg, L.lib(), self.ncls, self.ncand
+        nl, nms_pre, iou_thr = len(lv), int(cfg['nms_pre']), float(cfg['nms']['iou_thr'])
+        boxes, scores, ctr, loc = self.cand_boxes[n], self.cand_scores[n], self.cand_ctr[n], self.cand_loc[n]
+        det, labels, idx, count = self.det[n], self.labels[n], self.idx[n], self.count[n:n + 1]
+        ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, nms_pre)
+        ws = self._t(ws_bytes, dtype=torch.uint8)
 
-            def decode(lv=lv, ws=ws, ws_bytes=ws_bytes, cb=cb, cs=cs, cl=cl, cloc=cloc, nc=nc, ncand=ncand):
-                L.check(lib.smb_pair_decode_topk(nl, lv, ncls, ctypes.c_float(cfg['score_thr']), nms_pre, img_h, img_w,
-                                                 L.ptr(cb), L.ptr(cs), L.ptr(cl), L.ptr(cloc), L.ptr(nc), ncand, L.ptr(ws),
-                                                 ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_pair_decode_topk')
-            self._add(decode, 3, name='decode_topk')
-            nws_bytes = lib.smb_ml_nms_workspace_bytes(ncand)
+        def decode():
+            L.check(lib.smb_decode_topk(nl, lv, ncls, nms_pre, int(self.img_shape[0]), int(self.img_shape[1]), self._sf4,
+                                        L.ptr(boxes), L.ptr(scores), L.ptr(ctr), L.ptr(loc), L.ptr(ws), ctypes.c_size_t(ws_bytes),
+                                        L.stream_ptr()), 'smb_decode_topk')
+        self._add(decode, 3, name='decode_topk')
+        if not (self.ssd or self.vis):
+            nws_bytes = lib.smb_multiclass_nms_workspace_bytes(ncand, ncls)
             nws = self._t(nws_bytes, dtype=torch.uint8)
 
-            def nms(n=n, nws=nws, nws_bytes=nws_bytes, cb=cb, cs=cs, cl=cl, nc=nc, ncand=ncand):
-                L.check(lib.smb_ml_nms_topk(L.ptr(cb), L.ptr(cs), L.ptr(cl), L.ptr(nc), ncand, ctypes.c_float(cfg['nms']['iou_thr']),
-                                            self.max_num, self.max_num, L.ptr(self.det[n]), L.ptr(self.labels[n]),
-                                            L.ptr(self.idx[n]), L.ptr(self.count[n:n + 1]), L.ptr(self.kept_total[n:n + 1]),
-                                            L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()), 'smb_ml_nms_topk')
+            def nms():
+                L.check(lib.smb_multiclass_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls, ctypes.c_float(cfg['score_thr']),
+                                               ctypes.c_float(iou_thr), self.max_num, 0, L.ptr(det), L.ptr(labels), L.ptr(idx),
+                                               L.ptr(count), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()),
+                        'smb_multiclass_nms')
             self._add(nms, 4, name='nms')
-            cof_src = self.clscof[:, ncls:ncls + 128]
+        else:
+            nws_bytes = lib.smb_fast_nms_workspace_bytes(ncand, ncls, 200)
+            nws = self._t(nws_bytes, dtype=torch.uint8)
 
-            def gather(n=n, cof_src=cof_src, cloc=cloc):
-                L.check(lib.smb_gather_det_inputs(L.ptr(cof_src), CCp, L.ptr(cloc), L.ptr(self.idx[n]), L.ptr(self.det[n]),
-                                                  L.ptr(self.count[n:n + 1]), self.max_num, 128, L.ptr(self.det_cofs[n]),
-                                                  L.ptr(self.det_boxes4[n]), L.ptr(self.loc_kept[n]), nl if N > 1 else 0,
-                                                  level_hw, N, n, L.stream_ptr()), 'smb_gather_det_inputs')
-            self._add(gather, 1, name='gather_cofs')
+            def nms():
+                L.check(lib.smb_fast_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls, ctypes.c_float(cfg['score_thr']),
+                                         ctypes.c_float(iou_thr), 200, self.max_num, L.ptr(det), L.ptr(labels), L.ptr(idx),
+                                         L.ptr(count), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()), 'smb_fast_nms')
+            self._add(nms, 2, name='nms')
+        return loc
 
-            def masks(n=n):
-                L.check(lib.smb_mask_assemble_pack(L.ptr(self.protos[n]), L.F16, 1, L.ptr(self.det_cofs[n]), L.ptr(self.det_boxes4[n]),
-                                                   self._box_scale4, L.ptr(self.mask_bits[n]), Hm, Wm, self.max_num, fh, fw,
-                                                   ctypes.c_float(ry), ctypes.c_float(rx), oh, ow,
-                                                   ctypes.c_float(self.mask_thr), L.stream_ptr()), 'smb_mask_assemble_pack')
-            self._add(masks, 2, name='mask_fused')
-        if pp_streams:
-            self._marker('join')
-        self._tag = 0
+    def _bm_candidates(self, n, lv):
+        """BM candidates of image n: (location, class) pairs above score_thr, the top nms_pre per level
+        (smb_pair_decode_topk), then label-aware NMS and the k-th-value cut (smb_ml_nms_topk), which also writes
+        kept_total[n].  Returns the candidate -> location table."""
+        cfg, lib, ncls, ncand = self.cfg, L.lib(), self.ncls, self.ncand
+        nl, nms_pre = len(lv), int(cfg['nms_pre'])
+        boxes, scores, labels, loc = self.cand_boxes[n], self.cand_scores[n], self.cand_labels[n], self.cand_loc[n]
+        n_cand = self.n_cand[n:n + 1]
+        ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, ncls, nms_pre)
+        ws = self._t(ws_bytes, dtype=torch.uint8)
+
+        def decode():
+            L.check(lib.smb_pair_decode_topk(nl, lv, ncls, ctypes.c_float(cfg['score_thr']), nms_pre, int(self.img_shape[0]),
+                                             int(self.img_shape[1]), L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(loc),
+                                             L.ptr(n_cand), ncand, L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
+                    'smb_pair_decode_topk')
+        self._add(decode, 3, name='decode_topk')
+        nws_bytes = lib.smb_ml_nms_workspace_bytes(ncand)
+        nws = self._t(nws_bytes, dtype=torch.uint8)
+
+        def nms():
+            L.check(lib.smb_ml_nms_topk(L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(n_cand), ncand,
+                                        ctypes.c_float(cfg['nms']['iou_thr']), self.max_num, self.max_num, L.ptr(self.det[n]),
+                                        L.ptr(self.labels[n]), L.ptr(self.idx[n]), L.ptr(self.count[n:n + 1]),
+                                        L.ptr(self.kept_total[n:n + 1]), L.ptr(nws), ctypes.c_size_t(nws_bytes),
+                                        L.stream_ptr()), 'smb_ml_nms_topk')
+        self._add(nms, 4, name='nms')
+        return loc
 
     # ---------------------------------------------------------------------------------------------- run
     def _run_ops(self, only=None):
@@ -770,15 +694,14 @@ class SipMaskEngine(object):
     # head outputs in the reference's layout (for parity tests / the drop-in head)
     def head_outputs(self):
         outs = dict(cls=[], bbox=[], ctr=[], cof=[])
-        ncls = self.ncls
-        for l, (cc, rc) in enumerate(self.level_views):
-            outs['cls'].append(cc[..., :ncls].permute(0, 3, 1, 2))
-            outs['cof'].append(cc[..., ncls:ncls + 128].permute(0, 3, 1, 2))
-            d = rc[..., :4] * self.scales[l]
+        for l, v in enumerate(self.level_views):
+            outs['cls'].append(v['cls'].permute(0, 3, 1, 2))
+            outs['cof'].append(v['cof'].permute(0, 3, 1, 2))
+            d = v['box'] * self.scales[l]
             if self.benchmark:
                 d = torch.relu(d)                     # NORM_REG_TARGETS (sipmask.py:161-167)
             outs['bbox'].append(d.permute(0, 3, 1, 2) * self.strides[l])
-            outs['ctr'].append(rc[..., 4:5].permute(0, 3, 1, 2))
+            outs['ctr'].append(v['ctr'].permute(0, 3, 1, 2))
         outs['feat_masks'] = self.protos.permute(0, 3, 1, 2)
         if self.vis:
             outs['track_feats'] = self.track_feats.permute(0, 3, 1, 2)

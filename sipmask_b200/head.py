@@ -329,14 +329,12 @@ class FCOSHead(_HeadBase):
     @torch.no_grad()
     def forward(self, feats):
         """-> (cls_scores, bbox_preds, centernesses), lists of 5 NCHW fp32 tensors (fcos_head.py:118-135)."""
-        ncls = self.cls_out_channels
-
         def collect(eng):
             cls, box, ctr = [], [], []
-            for l, (cc, rc) in enumerate(eng.level_views):
-                cls.append(cc[..., :ncls].permute(0, 3, 1, 2))
-                ctr.append(cc[..., ncls:ncls + 1].permute(0, 3, 1, 2))
-                box.append((rc[..., :4] * eng.scales[l]).exp().permute(0, 3, 1, 2))     # scale(x).float().exp() (:134)
+            for l, v in enumerate(eng.level_views):
+                cls.append(v['cls'].permute(0, 3, 1, 2))
+                ctr.append(v['ctr'].permute(0, 3, 1, 2))
+                box.append((v['box'] * eng.scales[l]).exp().permute(0, 3, 1, 2))     # scale(x).float().exp() (:134)
             return cls, box, ctr
         return tuple(self._run_images(feats, collect))
 

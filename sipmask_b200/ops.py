@@ -155,7 +155,10 @@ def nms(dets, iou_thr, device_id=None, cmp_ge=False):
 
 
 # ------------------------------------------------------------------------------------- decode + top-k
-def _levels(cls_list, box_list, ctr_list, strides, box_scales):
+def level_descs(cls_list, box_list, ctr_list, strides, box_scales):
+    """smb_level_t array for one image's per-level channel-last fp32 views (cls [h,w,C], box [h,w,4], ctr [h,w,1|]):
+    pointers and row pitches from the views, (box_scales[l], strides[l]) as the box scale when box_scales is given.
+    Returns (levels, views to keep alive while the array is in use)."""
     nl = len(cls_list)
     lv = (L.Level * nl)()
     keep_alive = []
@@ -166,7 +169,7 @@ def _levels(cls_list, box_list, ctr_list, strides, box_scales):
         assert c.stride(-1) == 1 and b.stride(-1) == 1
         h, w = c.shape[0], c.shape[1]
         assert c.stride(0) == w * c.stride(1) and b.stride(0) == w * b.stride(1)
-        t2 = t.reshape(h, w, -1)
+        t2 = t if t.dim() == 3 else t.reshape(h, w, -1)      # a reshape would renumber the strides of a 1-wide level
         assert t2.stride(0) == w * t2.stride(1)
         keep_alive.append(t2)
         bs, bm = (1.0, 1.0) if box_scales is None else (float(box_scales[i]), float(strides[i]))
@@ -182,7 +185,7 @@ def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale
     Returns cand_boxes [n,4], cand_scores [n,C], cand_ctr [n], cand_loc [n] int32."""
     nl = len(cls_list)
     C = cls_list[0].shape[-1]
-    lv, keep_alive = _levels(cls_list, box_list, ctr_list, strides, box_scales)
+    lv, keep_alive = level_descs(cls_list, box_list, ctr_list, strides, box_scales)
     lib = L.lib()
     dev = cls_list[0].device
     ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, int(nms_pre))
@@ -210,7 +213,7 @@ def pair_decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre=1
     loc [n] int32, n_cand device int32 [1]); n is the slot capacity, rows past n_cand are zero / -1."""
     nl = len(cls_list)
     C = cls_list[0].shape[-1]
-    lv, keep_alive = _levels(cls_list, box_list, ctr_list, strides, box_scales)
+    lv, keep_alive = level_descs(cls_list, box_list, ctr_list, strides, box_scales)
     lib = L.lib()
     dev = cls_list[0].device
     n = lib.smb_pair_decode_slots(nl, lv, C, int(nms_pre))
