@@ -17,6 +17,10 @@
 //    wgmma.m64nNk16 (fp32 accumulators in registers) for 64 of the tile's 128 pixels and then running the epilogue
 //    (scale / bias / residual / GN statistics / ReLU -> global NHWC store) on its own accumulators; warp 8 is the TMA
 //    producer, which runs ahead into the next tile while the consumers drain the current one.
+//  * fp16-output plans without an upsampled residual (epi_tma) take the epilogue through shared memory: warp 9 loads the
+//    residual of each 64-pixel x 32-channel chunk by TMA into a slot, the consumer warps read it with ldmatrix, write their
+//    results over it with stmatrix and hand the slot back, and warp 9 stores it by TMA.  The consumers never wait on a
+//    global load or store.  fp32-output (head) and nearest-upsampled-residual (FPN lateral) plans store from registers.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -28,13 +32,30 @@ constexpr int kMaxTaps = 9;
 constexpr int kMaxMaps = 8;
 constexpr int kMaxLevels = 5;
 constexpr int kConsumerWarps = 8;
-// + a producer warpgroup: warp 8 issues the TMA loads, warps 9-11 exist only so that the CTA is whole warpgroups, which
-// setmaxnreg needs to move registers from the producer (40 per thread) to the consumers (232 instead of 168)
+// + a producer warpgroup: warp 8 issues the operand TMA loads, warp 9 the epilogue's residual loads and output stores
+// (epi_tma plans), warps 10-11 exist only so that the CTA is whole warpgroups, which setmaxnreg needs to move registers
+// from the producer (40 per thread) to the consumers (232 instead of 168)
 constexpr int kThreads = 32 * (kConsumerWarps + 4);
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int kProducerWarp = kConsumerWarps;
+constexpr int kEpiWarp = kConsumerWarps + 1;
 constexpr int kABytes = 128 * 64 * 2;                // one A stage: 128 pixels x 64 channels fp16
-constexpr size_t kSmemBudget = 220 * 1024;           // operand stages + barriers (227 KB per block on sm_90)
+constexpr size_t kSmemBudget = 220 * 1024;           // epilogue slots + operand stages + barriers (227 KB per block on sm_90)
+// Epilogue slots (epi_tma plans): per consumer warpgroup a ring of kEpiSlots chunks of 64 pixels x 32 channels fp16, one
+// 64-byte row per pixel in the TMA 64-byte swizzle.  32 channels keep every N at its operand ring (static_asserts below).
+constexpr int kEpiSlots = 3;
+constexpr int kEpiSlotBytes = 64 * 32 * 2;
+constexpr int kEpiBytes = 2 * kEpiSlots * kEpiSlotBytes;
+
+// operand stages of an N-channel tile: what is left of the budget after the epilogue slots, 1 KB alignment slack and
+// 256 B of epilogue barriers, 16 B of barriers per stage, at most 8
+constexpr int ring_stages(int n_tile) {
+  const int s = (int)((kSmemBudget - kEpiBytes - 1024 - 256) / ((size_t)kABytes + (size_t)n_tile * 128 + 16));
+  return s > 8 ? 8 : s;
+}
+static_assert(ring_stages(256) == 4 && ring_stages(128) == 6 && ring_stages(64) == 8,
+              "the epilogue slots must not cost any N tile an operand stage");
+static_assert(4 * kEpiSlots * 8 <= 256, "epilogue barriers exceed their reserve");
 
 // One pyramid level (or the only tensor) of a launch.  Convolutions whose weights are shared by several feature-pyramid
 // levels (the FCOS towers and heads, sipmask_head.py:250-257) run as ONE launch over the union of the levels' tiles.
@@ -51,6 +72,10 @@ struct LevelDesc {
 struct ConvParams {
   CUtensorMap amap[kMaxMaps];
   CUtensorMap bmap;
+  // epi_tma plans: output per level and the same-shape residual (single-level plans, encoded per launch), as boxes of
+  // {32 ch, min(BW, 64), max(BH / 2, 1), 1}: one consumer warpgroup's 64 pixels of a chunk, rows in accumulator order
+  CUtensorMap omap[kMaxLevels];
+  CUtensorMap rmap;
   LevelDesc lv[kMaxLevels];
   int num_levels;
   int tap_map[kMaxTaps], tap_dx[kMaxTaps], tap_dy[kMaxTaps];
@@ -63,7 +88,9 @@ struct ConvParams {
   int res_pitch, res_mode;        // res_mode: 0 none, 1 same shape, 2 nearest-upsampled coarser map
   int gn_group;                   // channels per GroupNorm group (8 or 16), 0 = no statistics
   int relu;
+  int epi_tma;                    // epilogue through shared memory and TMA (fp16 output, res_mode 0 / 1)
 };
+static_assert(sizeof(ConvParams) <= 4096, "ConvParams must fit the 4 KB kernel-parameter space");
 
 // ------------------------------------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -106,6 +133,27 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// generic-proxy writes to shared memory (stmatrix) -> visible to a later TMA store
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// lane l addresses row l % 8 of 8x8 matrix l / 8; register m holds row lane / 4, columns 2 (lane % 4) + {0, 1} of matrix m
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t* r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t* r) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
 }
 
 // K-major, 128-byte swizzle wgmma shared-memory matrix descriptor (sm_90):
@@ -359,6 +407,91 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
   }
 }
 
+// The same per-element arithmetic and GroupNorm partials as epilogue(), for epi_tma plans, one 32-channel chunk at a time
+// through the warpgroup's slot ring (slot es, phase eph, carried across tiles): wait until warp 9 has filled the slot
+// (residual) or freed it, ldmatrix the residual, stmatrix the fp16 results over it, hand the slot to warp 9's TMA store.
+// Slot layout: pixel row r (0..63, accumulator row order) at r * 64 bytes, its 16-byte channel quad q at
+// ((q ^ (r >> 1) & 3) * 16): the TMA 64-byte swizzle (address bits [4,6) ^= bits [7,9)).
+template <int N>
+__device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp,
+                                             int lane, GnPart& gn_part, uint32_t slots, uint64_t* epi_full,
+                                             uint64_t* epi_ready, int& es, uint32_t& eph) {
+  const LevelDesc& L = p.lv[tc.lvl];
+  const int bw_shift = 31 - __clz(L.BW);
+  bool valid[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+    valid[i] = (tc.x0 + (row & (L.BW - 1)) < L.W_out) && (tc.y0 + (row >> bw_shift) < L.H_out);
+  }
+  // ldmatrix / stmatrix x4 number h covers the warp's 16 rows x 8-channel blocks 2h, 2h + 1 of the chunk: lane supplies
+  // row (lane & 7) + 8 * ((lane >> 3) & 1) of block 2h + (lane >> 4); register m = 2 * (block & 1) + i of that call.
+  const int mrow = (warp & 3) * 16 + 8 * ((lane >> 3) & 1) + (lane & 7);
+  const uint32_t row_addr = slots + (uint32_t)wg * (kEpiSlots * kEpiSlotBytes) + (uint32_t)mrow * 64;
+  const uint32_t q0 = (uint32_t)((0 + (lane >> 4)) ^ ((mrow >> 1) & 3)) << 4;
+  const uint32_t q1 = (uint32_t)((2 + (lane >> 4)) ^ ((mrow >> 1) & 3)) << 4;
+  const int cq = 2 * (lane & 3);
+  const int nchunks = (min(N, p.Cout - tc.n0) + 31) >> 5;
+  float gsum = 0.f, gsq = 0.f;
+#pragma unroll
+  for (int c = 0; c < N / 32; ++c) {
+    if (c >= nchunks) break;
+    mbar_wait(&epi_full[wg * kEpiSlots + es], eph);
+    const uint32_t sa = row_addr + (uint32_t)es * kEpiSlotBytes;
+    uint32_t rh[8], oh[8];                           // residual / output: block jj, row half i in register 2 jj + i
+    if (p.res_mode) { ldmatrix_x4(sa + q0, rh); ldmatrix_x4(sa + q1, rh + 4); }
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * c + jj;
+      const int ch0 = tc.n0 + 8 * j;                 // warp-uniform; blocks past Cout are clipped by the TMA store
+      const int ch = ch0 + cq;
+      float2 bb = make_float2(0.f, 0.f);
+      if (p.bias && ch0 < p.Cout) bb = make_float2(__ldg(p.bias + ch), __ldg(p.bias + ch + 1));
+      float s = 0.f, q = 0.f;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float f0 = acc[4 * j + 2 * i] + bb.x, f1 = acc[4 * j + 2 * i + 1] + bb.y;
+        if (p.alpha != 1.0f) { f0 *= p.alpha; f1 *= p.alpha; }
+        if (p.res_mode) {
+          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rh[2 * jj + i]));
+          f0 += r.x; f1 += r.y;
+        }
+        if (valid[i]) { s += f0 + f1; q += f0 * f0 + f1 * f1; }
+        if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+        const __half2 h = __floats2half2_rn(f0, f1);
+        oh[2 * jj + i] = *reinterpret_cast<const uint32_t*>(&h);
+      }
+      if (p.gn_group && ch0 < p.Cout) {
+        gsum += s; gsq += q;
+        if (p.gn_group == 8 || (j & 1)) {
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
+            gsq += __shfl_xor_sync(0xffffffffu, gsq, o);
+          }
+          if (lane == 0) {
+            unsigned long long* part = gn_part[warp][(ch0 - tc.n0) / p.gn_group];
+            part[0] = (unsigned long long)__float2ll_rn(gsum * kGnSumScale);
+            part[1] = (unsigned long long)__float2ll_rn(gsq * kGnSqScale);
+          }
+          gsum = 0.f; gsq = 0.f;
+        }
+      }
+    }
+    stmatrix_x4(sa + q0, oh);
+    stmatrix_x4(sa + q1, oh + 4);
+    fence_proxy_async_smem();
+    mbar_arrive(&epi_ready[wg * kEpiSlots + es]);
+    if (++es == kEpiSlots) { es = 0; eph ^= 1; }
+  }
+}
+
+// Box origin of warpgroup wg's 64 pixels of a tile: the lower / upper half of the patch rows, or of the 1 x 128 row.
+__device__ __forceinline__ void epi_box_origin(const LevelDesc& L, int x0, int y0, int wg, int& x, int& y) {
+  if (L.BW > 64) { x = x0 + 64 * wg; y = y0; }
+  else { x = x0; y = y0 + wg * (L.BH >> 1); }
+}
+
 template <int N>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -369,13 +502,17 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   constexpr int kBBytes = N * 128;                   // one B stage: N output channels x 64 k fp16
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
   const int nstages = p.stages;
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + (size_t)nstages * kABytes;
+  uint8_t* epi_slots = smem;                         // [warpgroup][kEpiSlots] x 4 KB, 1024-byte aligned
+  uint8_t* sA = smem + kEpiBytes;
+  uint8_t* sB = sA + (size_t)nstages * kABytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + (size_t)nstages * kBBytes);
   uint64_t* empty_bar = full_bar + nstages;
+  uint64_t* epi_full = empty_bar + nstages;          // [warpgroup][slot]: residual landed / slot free (warp 9)
+  uint64_t* epi_ready = epi_full + 2 * kEpiSlots;    // [warpgroup][slot]: results written (the warpgroup's 128 threads)
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < nstages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerWarps); }
+    for (int i = 0; i < 2 * kEpiSlots; ++i) { mbar_init(&epi_full[i], 1); mbar_init(&epi_ready[i], 128); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -412,6 +549,59 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           }
         }
       }
+    } else if (warp == kEpiWarp && lane == 0 && p.epi_tma) {
+      // ===================== epilogue copies (one lane): the consumers' chunk sequence, kEpiSlots chunks ahead ==========
+      // Step k stores the chunk that last used slot k % kEpiSlots (once both warpgroups have written it), waits until the
+      // stores have read their slots, then fills the slot for chunk k: the residual by TMA, or just a release.  Chunk 0..
+      // kEpiSlots-1 of a tile are thus loaded while the consumers still run its MMAs.  kEpiSlots extra steps store the
+      // last chunks.
+      __shared__ int4 pend[kEpiSlots];               // chunk in each slot: {channel, x0, y0, image * 8 + level}
+      for (int l = 0; l < p.num_levels; ++l) tma_prefetch_desc(&p.omap[l]);
+      if (p.res_mode) tma_prefetch_desc(&p.rmap);
+      int s = 0, c = 0, nchunks = 0, filled = 0;
+      uint32_t ph = 0;
+      int unit = blockIdx.x;
+      TileCoord tc = {};
+      for (int step = 0;; ++step) {
+        const bool fill = unit < total_units;
+        if (!fill && step >= filled + kEpiSlots) break;
+        if (step >= kEpiSlots && step - kEpiSlots < filled) {
+          const int4 q = pend[s];
+          const LevelDesc& L = p.lv[q.w & 7];
+#pragma unroll
+          for (int wg = 0; wg < 2; ++wg) {
+            int x, y;
+            epi_box_origin(L, q.y, q.z, wg, x, y);
+            mbar_wait(&epi_ready[wg * kEpiSlots + s], ph ^ 1);
+            tma_store_4d(&p.omap[q.w & 7], epi_slots + (wg * kEpiSlots + s) * kEpiSlotBytes, q.x, x, y, q.w >> 3);
+          }
+          bulk_commit();
+        }
+        if (fill) {
+          if (c == 0) {
+            tc = decode_tile(p, unit);
+            nchunks = (min(N, p.Cout - tc.n0) + 31) >> 5;
+          }
+          bulk_wait_read_all();                        // the store above has read the slot
+#pragma unroll
+          for (int wg = 0; wg < 2; ++wg) {
+            uint64_t* bar = &epi_full[wg * kEpiSlots + s];
+            if (p.res_mode) {
+              int x, y;
+              epi_box_origin(p.lv[0], tc.x0, tc.y0, wg, x, y);
+              mbar_expect_tx(bar, kEpiSlotBytes);      // out-of-bounds fill counts toward the bytes
+              tma_load_4d(epi_slots + (wg * kEpiSlots + s) * kEpiSlotBytes, &p.rmap, bar, tc.n0 + 32 * c, x, y, tc.img);
+            } else {
+              mbar_arrive(bar);
+            }
+          }
+          pend[s] = make_int4(tc.n0 + 32 * c, tc.x0, tc.y0, tc.img * 8 + tc.lvl);
+          ++filled;
+          if (++c == nchunks) { c = 0; unit += gridDim.x; }
+        }
+        if (++s == kEpiSlots) { s = 0; ph ^= 1; }
+      }
+      bulk_wait_read_all();                          // the slots stay allocated until the last store has read them
     }
   } else {
     // ===================== consumers: warpgroup wg computes pixels 64*wg .. 64*wg+63 of the tile =====================
@@ -421,8 +611,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     float acc[N / 2];
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-    int s = 0;
-    uint32_t ph = 0;
+    int s = 0, es = 0;
+    uint32_t ph = 0, eph = 0;
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
       const TileCoord tc = decode_tile(p, unit);
       int prev = -1;
@@ -444,7 +634,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       wgmma_wait<0>();
       fence_regs<N / 2>(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      epilogue<N>(p, tc, acc, wg, warp, lane, gn_part);
+      if (p.epi_tma)
+        epilogue_tma<N>(p, tc, acc, wg, warp, lane, gn_part, smem_u32(epi_slots), epi_full, epi_ready, es, eph);
+      else
+        epilogue<N>(p, tc, acc, wg, warp, lane, gn_part);
       if (p.gn_group) gn_flush(p, tc, gn_part, N);
     }
   }
@@ -468,14 +661,14 @@ static EncodeTiledFn get_encode() {
 }
 
 static int encode_map(CUtensorMap* m, void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                      const uint32_t* box) {
+                      const uint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return SMB_ECUDA; }
   cuuint64_t d[5]; cuuint64_t s[4]; cuuint32_t b[5]; cuuint32_t es[5];
   for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; es[i] = 1; }
   for (int i = 0; i < rank - 1; ++i) s[i] = strides_bytes[i];
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, base, d, s, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed (%d): rank=%d dims=[%llu,%llu,%llu,%llu] strides=[%llu,%llu,%llu] box=[%u,%u,%u,%u]",
               (int)r, rank, (unsigned long long)d[0], (unsigned long long)d[1], (unsigned long long)(rank > 2 ? d[2] : 0),
@@ -484,6 +677,17 @@ static int encode_map(CUtensorMap* m, void* base, int rank, const uint64_t* dims
     return SMB_ECUDA;
   }
   return SMB_OK;
+}
+
+// Output (or same-shape residual) of one level as seen by the shared-memory epilogue: [N, H_out, W_out, pitch] fp16, the
+// first Cout channels, in boxes of one consumer warpgroup's 64 pixels x 32 channels (rows past the level's edge and
+// channels past Cout are clipped on store, zero-filled on load).
+static int encode_epi_map(CUtensorMap* m, const void* base, const ConvParams& p, const LevelDesc& L, int pitch) {
+  const uint64_t px = (uint64_t)pitch * 2;
+  const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)L.W_out, (uint64_t)L.H_out, (uint64_t)p.n_img};
+  const uint64_t strides[3] = {px, px * L.W_out, px * L.W_out * L.H_out};
+  const uint32_t box[4] = {32, (uint32_t)(L.BW < 64 ? L.BW : 64), (uint32_t)(L.BH > 1 ? L.BH / 2 : 1), 1};
+  return encode_map(m, const_cast<void*>(base), 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
 }  // namespace smb
@@ -536,10 +740,17 @@ static int finish_plan(smb_conv_plan* pl, int Cout, int Ktotal, const void* weig
   p.n_tile = n_tile;
   p.n_tiles_n = cdiv(Cout, n_tile);
   const size_t stage = (size_t)kABytes + (size_t)n_tile * 128;
-  int stages = (int)((kSmemBudget - 1024 - 256) / (stage + 16));
-  if (stages > 8) stages = 8;
-  p.stages = stages;
-  pl->smem_bytes = (size_t)stages * (stage + 16) + 1024;       // + barriers + alignment slack
+  p.stages = ring_stages(n_tile);
+  pl->smem_bytes = kEpiBytes + (size_t)p.stages * (stage + 16) + 4 * kEpiSlots * 8 + 1024;   // + barriers + alignment slack
+  // Shared-memory / TMA epilogue for fp16 outputs whose rows TMA can address (16-byte aligned bases and pitch) and whose
+  // residual, if any, is the same-shape tensor of a single-level plan.
+  p.epi_tma = !p.out_f32 && p.out_pitch % 8 == 0 && (p.res_mode == 0 || (p.res_mode == 1 && p.num_levels == 1));
+  for (int l = 0; l < p.num_levels; ++l)
+    if ((uintptr_t)p.lv[l].out % 16) p.epi_tma = 0;
+  for (int l = 0; l < p.num_levels && p.epi_tma; ++l) {
+    const int rc = encode_epi_map(&p.omap[l], p.lv[l].out, p, p.lv[l], p.out_pitch);
+    if (rc) return rc;
+  }
   // weights: [Cout, Ktotal] K-major
   uint64_t dims[2] = {(uint64_t)Ktotal, (uint64_t)Cout};
   uint64_t strides[1] = {(uint64_t)Ktotal * 2};
@@ -719,6 +930,16 @@ extern "C" int smb_conv_run(const smb_conv_plan_t* plan, const float* bias, cons
     if (plan->has_residual) {
       SMB_CHECK_ARG(residual, "smb_conv_run: plan expects a residual");
       p.lv[0].residual = (const __half*)residual;
+      // the residual's TMA map goes into this launch's parameters (a captured graph keeps them by value); a residual
+      // TMA cannot address (not 16-byte aligned) takes the register epilogue
+      if (p.epi_tma && p.res_mode == 1) {
+        if ((uintptr_t)residual % 16) {
+          p.epi_tma = 0;
+        } else {
+          const int rc = encode_epi_map(&p.rmap, residual, p, p.lv[0], p.res_pitch);
+          if (rc) return rc;
+        }
+      }
     }
     if (plan->gn_stats) {
       SMB_CHECK_ARG(gn_stats, "smb_conv_run: plan expects a gn_stats buffer");
