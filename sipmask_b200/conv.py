@@ -90,6 +90,7 @@ class ConvPlan(object):
         d.in_pitch = in_pitch
         d.out_pitch = out_pitch
         self._keep = (x, weight, out, bias, residual, gn_stats)
+        self.desc = d                                  # what the kernel is told (read by the layer audit)
         self.bias, self.residual, self.gn_stats, self.alpha = bias, residual, gn_stats, float(alpha)
         self.handle = ctypes.c_void_p()
         self.dev = x.device
@@ -152,6 +153,7 @@ class ConvPlanMulti(ConvPlan):
         d.in_pitch = in_pitch
         d.out_pitch = out_pitch
         self._keep = (xs, weight, outs, bias, gn_stats, lv)
+        self.desc, self.levels = d, lv                 # descriptor and level table the kernel is told (read by the layer audit)
         self.bias, self.residual, self.gn_stats, self.alpha = bias, None, None, float(alpha)
         self.handle = ctypes.c_void_p()
         self.dev = xs[0].device

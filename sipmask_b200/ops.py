@@ -592,6 +592,25 @@ def mask_rescore_f16_workspace_bytes(rows, H, W):
     return int(L.lib().smb_mask_rescore_f16_workspace_bytes(int(rows), int(H), int(W)))
 
 
+def mask_rescore_f16_layers(workspace, rows, H, W):
+    """The activations of layers 2-5 that smb_mask_rescore_f16 leaves in its uint8 `workspace` for `rows` masks of H x W:
+    fp16 views [rows, h, w, C] with C = 16, 16, 32, 64 (h = (h_prev - 3) // 2 + 1 from the mask size), each starting on a
+    256-byte boundary.  They span exactly mask_rescore_f16_workspace_bytes(rows, H, W) bytes."""
+    hs, ws = [int(H)], [int(W)]
+    for _ in range(5):
+        hs.append((hs[-1] - 3) // 2 + 1)
+        ws.append((ws[-1] - 3) // 2 + 1)
+    views, o = [], 0
+    for l in range(2, 6):
+        n = int(rows) * hs[l] * ws[l] * RESCORE_CHANNELS[l]
+        views.append(workspace[o:o + 2 * n].view(torch.float16).view(int(rows), hs[l], ws[l], RESCORE_CHANNELS[l]))
+        o = (o + 2 * n + 255) // 256 * 256
+    if o != mask_rescore_f16_workspace_bytes(rows, H, W) or workspace.numel() < o:
+        raise L.SmbError('mask_rescore_f16_layers: layout of %d bytes does not match the %d-byte workspace of %d x %d x %d '
+                         '(buffer %d bytes)' % (o, mask_rescore_f16_workspace_bytes(rows, H, W), rows, H, W, workspace.numel()))
+    return views
+
+
 @L.device_guard
 def mask_rescore_f16(pos_masks, count, weights, labels, det, workspace=None, out=None):
     """SipMask++ rescoring on tensor cores (smb_mask_rescore_f16): pos_masks [n_img, max_rows, H, W] fp16 cropped stride-2

@@ -127,8 +127,7 @@ def test_fp16_epilogue_into_channel_slice():
 @pytest.mark.parametrize('H,W', [(64, 96), (224, 352)])
 def test_stem_fp16_epilogue_is_deterministic(H, W):
     """The stem (N = 64, K = 256, 2100 tiles at 800 x 1344) stores through shared memory: same bits on every run, and
-    within fp16 rounding of a float64 reference."""
-    import torch.nn.functional as F
+    within the per-element convolution bound of the float64 value of its operands."""
     from sipmask_b200 import conv
     g = torch.Generator().manual_seed(H + W)
     img = torch.randn(2, 3, H, W, generator=g).cuda()
@@ -145,9 +144,7 @@ def test_stem_fp16_epilogue_is_deterministic(H, W):
     plan.run()
     torch.cuda.synchronize()
     assert torch.equal(out, first)
-    s = bn[0] / torch.sqrt(bn[3] + 1e-5)
-    wf = (w * s.view(-1, 1, 1, 1)).half().double().cuda()
-    y = F.conv2d(img.half().double(), wf, stride=2, padding=3) + bias.double().view(1, -1, 1, 1)
-    y = y.clamp(min=0).permute(0, 2, 3, 1)
-    err = (out.double() - y).abs().max().item()
-    assert err <= 2e-3 * y.abs().max().item() + 1e-3, err
+    # element by element: a 4x4 valid convolution over the space-to-depth input, weights viewed as [64, 4, 4, 16]
+    from oracle import numerics as NU
+    y, m = NU.conv_reference(q, wk, 4, 1, bias=bias, pad=0, out_hw=out.shape[1:3])
+    NU.check_conv(out, y, m, 256, relu=True, what='stem %dx%d' % (H, W))

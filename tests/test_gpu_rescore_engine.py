@@ -88,9 +88,22 @@ def _kernel_inputs(hw, seed=0):
 def test_mask_rescore_f16_matches_fp32_chain(hw):
     from sipmask_b200 import ops
     cw, cb, w1, b1 = _scoring_weights()
+    from oracle import numerics as NU
     wt = ops.RescoreWeights(cw, cb, w1, b1, 'cuda')
     pos, labels, det, count = _kernel_inputs(hw)
-    got = ops.mask_rescore_f16(pos.cuda(), count.cuda(), wt, labels.cuda(), det.cuda()).cpu()
+    R = pos.shape[0] * pos.shape[1]
+    need = ops.mask_rescore_f16_workspace_bytes(R, hw[0], hw[1])
+    ws = torch.full((need,), 0xFF, dtype=torch.uint8, device='cuda')        # unwritten fp16 reads back as 0xFFFF
+    layers = ops.mask_rescore_f16_layers(ws, R, hw[0], hw[1])
+    assert [t.shape[3] for t in layers] == [16, 16, 32, 64] and all(t.data_ptr() % 256 == 0 for t in layers)
+    end = layers[-1].data_ptr() + layers[-1].numel() * 2 - ws.data_ptr()          # the views tile the whole workspace
+    assert (end + 255) // 256 * 256 == need
+    gotd = ops.mask_rescore_f16(pos.cuda(), count.cuda(), wt, labels.cuda(), det.cuda(), workspace=ws)
+    # layer by layer: layer 2 from float64 layer 1, layers 3-5 and the score teacher-forced from the device's layers
+    res = NU.check_rescore_chain(pos.cuda(), count.cuda(), wt.conv_w, wt.conv_b, wt.score_w, wt.score_b, labels.cuda(),
+                                 det.cuda(), layers, gotd)
+    print('rescore %dx%d: %s' % (hw[0], hw[1], ', '.join('%s %.3g' % kv for kv in res.items())))
+    got = gotd.cpu()
     want = ops.mask_rescore(pos[0, :5].float().cuda(), [w.cuda() for w in cw], [b.cuda() for b in cb], w1.cuda(), b1.cuda(),
                             labels[0, :5].cuda(), det[0, :5].cuda()).cpu()
     assert (got[0, :5] != 0).any()
