@@ -427,6 +427,25 @@ int smb_image_to_s2d16(const float* img_nchw_f32, void* out_s2d16, int N, int H,
 int smb_preprocess_u8_s2d(const uint8_t* src, int src_h, int src_w, int src_pitch_bytes, int dst_h, int dst_w,
                           const float* host_mean3, void* out_s2d16, int H, int W, smb_stream_t stream);
 
+/* One image of a batched preprocessing launch, read from DEVICE memory when the kernel runs (so a captured CUDA graph
+ * serves new images and sizes: the host rewrites the rows between replays).
+ *   src              : absolute device pointer of the image's uint8 BGR HWC pixels, row pitch src_pitch_bytes (>= 3 * src_w)
+ *   dst_h, dst_w     : the resized size (the image's img_shape), <= the canvas H x W
+ *   mean[3]          : subtracted per channel (kept in the row, so a captured graph never holds a stale mean)
+ * A filler row (dst_h == 0 or dst_w == 0) writes an all-zero canvas and reads nothing (src may be null): a partial batch
+ * fills its remaining images with such rows.  The rows are not validated on the device; the caller validates them. */
+typedef struct {
+  const uint8_t* src;
+  int src_h, src_w, src_pitch_bytes;
+  int dst_h, dst_w;
+  float mean[3];
+} smb_raw_src_t;
+
+/* smb_preprocess_u8_s2d for a batch: out_s2d16 [N, H/2+3, W/2+4, 16] fp16, canvas n from rows[n] (device pointer to N
+ * rows), one launch over all N canvases.  Same kernel as smb_preprocess_u8_s2d (which passes its one row by value), so
+ * every canvas is bit-identical to the single-image entry point.  Reads sum(src bytes), writes N*(H/2+3)*(W/2+4)*32 bytes. */
+int smb_preprocess_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out_s2d16, int H, int W, smb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -42,6 +42,12 @@ class ImgGeom(ctypes.Structure):
                 ('track_sx', ctypes.c_float), ('track_sy', ctypes.c_float)]
 
 
+class RawSrc(ctypes.Structure):
+    """smb_raw_src_t: one image of a batched preprocessing launch (include/sipmask_b200.h)."""
+    _fields_ = [('src', ctypes.c_void_p), ('src_h', ctypes.c_int), ('src_w', ctypes.c_int), ('src_pitch_bytes', ctypes.c_int),
+                ('dst_h', ctypes.c_int), ('dst_w', ctypes.c_int), ('mean', ctypes.c_float * 3)]
+
+
 class RescoreWeights(ctypes.Structure):
     _fields_ = [('conv_w', ctypes.c_void_p * 6), ('conv_b', ctypes.c_void_p * 6), ('score_w', ctypes.c_void_p),
                 ('score_b', ctypes.c_void_p), ('num_classes', ctypes.c_int)]
@@ -60,7 +66,7 @@ SYMBOLS = [
     'smb_groupnorm_relu_apply', 'smb_groupnorm_stats', 'smb_deform_im2col', 'smb_offset_conv1x1', 'smb_groupnorm_relu_apply_multi', 'smb_offset_conv1x1_multi', 'smb_offset_conv1x1_relu_multi', 'smb_deform_im2col_multi', 'smb_maxpool3x3s2',
     'smb_upsample_bilinear', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
     'smb_mask_assemble_dev', 'smb_mask_assemble_pack_dev', 'smb_decode_topk_dev', 'smb_pair_decode_topk_dev',
-    'smb_gather_track_feats_dev',
+    'smb_gather_track_feats_dev', 'smb_preprocess_u8_s2d_dev',
 ]
 
 

@@ -51,6 +51,18 @@ struct PreArgs {
   double scale_y, scale_x;
   float m0, m1, m2;
 };
+// The per-pixel arguments of one source row.  A filler row (dst_h == 0 or dst_w == 0) gets dh = dw = 0: every pixel is
+// outside the image, so nothing is read and its canvas is all zero.
+__device__ __forceinline__ PreArgs pre_args(const smb_raw_src_t& r) {
+  PreArgs a;
+  const bool fill = r.dst_h <= 0 || r.dst_w <= 0;
+  a.src = r.src; a.sh = r.src_h; a.sw = r.src_w; a.pitch = r.src_pitch_bytes;
+  a.dh = fill ? 0 : r.dst_h; a.dw = fill ? 0 : r.dst_w;
+  a.scale_y = fill ? 1.0 : 1.0 / ((double)r.dst_h / r.src_h);
+  a.scale_x = fill ? 1.0 : 1.0 / ((double)r.dst_w / r.src_w);
+  a.m0 = r.mean[0]; a.m1 = r.mean[1]; a.m2 = r.mean[2];
+  return a;
+}
 __device__ __forceinline__ void pre_pixel(const PreArgs& a, int x, int y, float* f3) {
   f3[0] = f3[1] = f3[2] = 0.f;
   if (x >= 0 && x < a.dw && y >= 0 && y < a.dh) {
@@ -75,13 +87,20 @@ __device__ __forceinline__ void pre_pixel(const PreArgs& a, int x, int y, float*
   }
 }
 
-// Space-to-depth layout of the 7x7/2 stem: out [H/2+3, W/2+4, 16] fp16, element (Y, X, (dy*2+dx)*4 + c) = padded pixel
-// (2Y+dy, 2X+dx) = image pixel (2Y+dy-3, 2X+dx-3), channel c (c == 3: zero).  One thread = one 32-byte (Y, X) cell.
-__global__ void preprocess_u8_s2d_kernel(PreArgs a, __half* __restrict__ out, int H, int W) {
+// Space-to-depth layout of the 7x7/2 stem: out [N, H/2+3, W/2+4, 16] fp16, element (n, Y, X, (dy*2+dx)*4 + c) = padded
+// pixel (2Y+dy, 2X+dx) = pixel (2Y+dy-3, 2X+dx-3) of image n, channel c (c == 3: zero).  One thread = one 32-byte
+// (n, Y, X) cell; image n's source row is rows[n] (device memory, rewritten between graph replays) or, with rows == nullptr
+// (N == 1), row0 by value.  Write indices come from the canvas alone, so no row can make a thread write outside image n's
+// canvas; reads stay inside the row's source image because pre_pixel clamps every source row / column index.
+__global__ void preprocess_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows, smb_raw_src_t row0,
+                                         __half* __restrict__ out, int N, int H, int W) {
   const int Hq = H / 2 + 3, Wq = W / 2 + 4;
-  const long long total = (long long)Hq * Wq;
+  const long long cells = (long long)Hq * Wq, total = cells * N;
   for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)blockDim.x * gridDim.x) {
-    const int X = (int)(t % Wq), Y = (int)(t / Wq);
+    const int n = (int)(t / cells);
+    const long long c = t - n * cells;
+    const int X = (int)(c % Wq), Y = (int)(c / Wq);
+    const PreArgs a = rows ? pre_args(rows[n]) : pre_args(row0);
     float f[16];
 #pragma unroll
     for (int d = 0; d < 4; ++d) {
@@ -94,6 +113,16 @@ __global__ void preprocess_u8_s2d_kernel(PreArgs a, __half* __restrict__ out, in
   }
 }
 
+static int launch_preprocess(const smb_raw_src_t* rows, const smb_raw_src_t& row0, void* out, int N, int H, int W,
+                             smb_stream_t stream) {
+  const long long total = (long long)N * (H / 2 + 3) * (W / 2 + 4);
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  preprocess_u8_s2d_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(rows, row0, (__half*)out, N, H, W);
+  SMB_LAUNCH_OK("preprocess_u8_s2d_kernel");
+  return SMB_OK;
+}
+
 }  // namespace smb
 
 using namespace smb;
@@ -104,14 +133,17 @@ extern "C" int smb_preprocess_u8_s2d(const uint8_t* src, int src_h, int src_w, i
   SMB_CHECK_ARG(src_h > 0 && src_w > 0 && src_pitch_bytes >= 3 * src_w && dst_h > 0 && dst_w > 0 && dst_h <= H && dst_w <= W,
                 "smb_preprocess_u8_s2d: bad shape (src %dx%d -> %dx%d inside %dx%d)", src_h, src_w, dst_h, dst_w, H, W);
   SMB_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "smb_preprocess_u8_s2d: H, W must be even");
-  PreArgs a;
-  a.src = src; a.sh = src_h; a.sw = src_w; a.pitch = src_pitch_bytes; a.dh = dst_h; a.dw = dst_w;
-  a.scale_y = 1.0 / ((double)dst_h / src_h); a.scale_x = 1.0 / ((double)dst_w / src_w);
-  a.m0 = host_mean3[0]; a.m1 = host_mean3[1]; a.m2 = host_mean3[2];
-  const long long total = (long long)(H / 2 + 3) * (W / 2 + 4);
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  preprocess_u8_s2d_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, (__half*)out, H, W);
-  SMB_LAUNCH_OK("preprocess_u8_s2d_kernel");
-  return SMB_OK;
+  smb_raw_src_t r;
+  r.src = src; r.src_h = src_h; r.src_w = src_w; r.src_pitch_bytes = src_pitch_bytes; r.dst_h = dst_h; r.dst_w = dst_w;
+  r.mean[0] = host_mean3[0]; r.mean[1] = host_mean3[1]; r.mean[2] = host_mean3[2];
+  return launch_preprocess(nullptr, r, out, 1, H, W, stream);
+}
+
+extern "C" int smb_preprocess_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out, int H, int W, smb_stream_t stream) {
+  SMB_CHECK_ARG(rows && out, "smb_preprocess_u8_s2d_dev: null pointer");
+  SMB_CHECK_ARG(N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0,
+                "smb_preprocess_u8_s2d_dev: bad canvas (N %d, %dx%d; H, W must be even)", N, H, W);
+  smb_raw_src_t r;
+  memset(&r, 0, sizeof(r));
+  return launch_preprocess(rows, r, out, N, H, W, stream);
 }

@@ -737,27 +737,55 @@ class SipMaskEngine(object):
             r['mask_scores'] = self.mask_scores        # [N,max] fp32 SipMask++ mask scores (zeros after count)
         return r
 
-    def forward_raw(self, img_u8, mean=(102.9801, 115.9465, 122.7717)):
-        """img_u8: uint8 BGR HWC CUDA image straight from the decoder.  Resize (keep ratio, mmcv.imrescale rule towards this
-        engine's img_shape, or the one set_image_meta set) + mean subtraction + padding + layout run in ONE kernel that writes
-        the stem's input (SURVEY.md 8f-3); the rest of the step is the CUDA graph without its `image_to_s2d16` node; batch 1."""
-        assert self.N == 1, 'forward_raw preprocesses one image'
+    def forward_raw(self, imgs, mean=(102.9801, 115.9465, 122.7717)):
+        """imgs: N uint8 BGR HWC CUDA images straight from the decoder (a list; one tensor when N == 1).  Image n is resized
+        to its own img_shape (the constructor's, or the one set_image_meta set; cv2 INTER_LINEAR, bit-exact), mean-subtracted,
+        zero-padded and written in the stem's layout by ONE kernel for the whole batch (SURVEY.md 8f-3), captured in
+        `graph_raw` in place of the `image_to_s2d16` node.  A None entry is a filler image: an all-zero canvas, for a
+        partial batch.  Per call: the source rows are written with a stream-ordered H2D copy on the current stream, then
+        one graph replay.  The images must stay alive and unchanged until the forward has consumed them."""
+        rows = self._raw_src_rows(imgs, mean)        # host validation: ValueError before anything is enqueued
         if torch.cuda.current_device() != self.dev.index:
             with torch.cuda.device(self.dev):
-                return self.forward_raw(img_u8, mean)
-        C.preprocess_u8(img_u8, self.image_metas[0][0][:2], self.img8, mean)
+                return self._forward_raw_rows(rows)
+        return self._forward_raw_rows(rows)
+
+    def _raw_src_rows(self, imgs, mean):
+        srcs = [imgs] if isinstance(imgs, torch.Tensor) else list(imgs)
+        if len(srcs) != self.N:
+            raise ValueError('forward_raw: %d images for a batch of %d' % (len(srcs), self.N))
+        return (L.RawSrc * self.N)(*[C.raw_src_row(s, m[0][:2], (self.H, self.W), mean, self.dev)
+                                     for s, m in zip(srcs, self.image_metas)])
+
+    def _forward_raw_rows(self, rows):
+        """Writes the source rows the way set_image_meta writes the geometry (pinned staging -> one H2D copy on the current
+        stream, the staging reused only after that copy has run), then replays graph_raw.  The rows live outside the
+        arena: they persist between forwards."""
+        nbytes = ctypes.sizeof(rows)
+        if getattr(self, '_raw_rows', None) is None:
+            self._raw_rows = torch.empty(nbytes, dtype=torch.uint8, device=self.dev)
+            self._raw_host = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
+            self._raw_copied = torch.cuda.Event()
+        else:
+            self._raw_copied.synchronize()           # the previous copy has left the pinned staging rows
+        ctypes.memmove(self._raw_host.data_ptr(), ctypes.addressof(rows), nbytes)
+        self._raw_rows.copy_(self._raw_host, non_blocking=True)
+        self._raw_copied.record(torch.cuda.current_stream(self.dev))
+        names = set(self.op_names) - {'image_to_s2d16', 'fork', 'join'}
         if self.use_graph:
             if getattr(self, 'graph_raw', None) is None:
-                names = set(self.op_names) - {'image_to_s2d16', 'fork', 'join'}
+                C.preprocess_u8_rows(self._raw_rows, self.img8)
                 self._run_ops(only=names)
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
+                    C.preprocess_u8_rows(self._raw_rows, self.img8)
                     self._run_ops(only=names)
                 self.graph_raw = g
             self.graph_raw.replay()
         else:
-            self._run_ops(only=set(self.op_names) - {'image_to_s2d16', 'fork', 'join'})
+            C.preprocess_u8_rows(self._raw_rows, self.img8)
+            self._run_ops(only=names)
         return self._result()
 
     # head outputs in the reference's layout (for parity tests / the drop-in head)

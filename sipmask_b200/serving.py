@@ -310,16 +310,30 @@ class StreamRunner(object):
     submit(img): a uint8 BGR HWC image of any size up to max_src_hw (raw mode; the resize runs on the GPU), or for
     SipMask-benchmark checkpoints (benchmark=True, whose resize rule is not restated here) a preprocessed fp32 NCHW image
     padded to a multiple of 32 together with its meta = (img_shape, ori_shape, scale_factor).  result(slot) returns the
-    record with mask_bits cropped to the image's [max, ori_h, ceil(ori_w / 32)]."""
+    record with mask_bits cropped to the image's [max, ori_h, ceil(ori_w / 32)].
+
+    batch=B > 1 (raw mode only): every forward runs B images of ONE padded shape through batch-B bucket engines (the
+    throughput mode of the 544x544 configs).  Each image is uploaded into its slot's staging as soon as it is submitted;
+    the open batch is dispatched when it holds B images, when the next image has a different padded shape, or on flush().
+    Dispatch = geometry rows + source rows + one graph replay + one download of the real images' records.  A partial
+    batch is completed with filler images (all-zero canvases with the last real image's geometry) that are computed but
+    never returned.  submit() returns a ticket (the image's index in the stream) and result(ticket) that image's record.
+    The mask record of a batch-B engine holds B * max * max_ori_h * ceil(max_ori_w / 32) words and is cleared every
+    forward: set max_ori_hw to the largest original size expected, not the 2048 x 2048 default."""
 
     def __init__(self, state_dict, in_flight=1, resize=(1333, 800), keep_ratio=True, max_src_hw=(2048, 2048),
-                 max_ori_hw=None, min_mask_up=0.5, mean=(102.9801, 115.9465, 122.7717), device='cuda', **engine_kw):
-        self.sd, self.n = state_dict, int(in_flight)
+                 max_ori_hw=None, min_mask_up=0.5, mean=(102.9801, 115.9465, 122.7717), device='cuda', batch=1,
+                 **engine_kw):
+        self.sd, self.n, self.B = state_dict, int(in_flight), int(batch)
         self.resize, self.keep_ratio, self.mean = tuple(resize), keep_ratio, mean
         self.max_src_hw = tuple(int(v) for v in max_src_hw)
         self.max_ori_hw = tuple(int(v) for v in (max_ori_hw or max_src_hw))
         self.min_mask_up = float(min_mask_up)
         self.benchmark = bool(engine_kw.get('benchmark', False))
+        if self.B < 1:
+            raise ValueError('batch must be at least 1, got %d' % self.B)
+        if self.benchmark and self.B > 1:
+            raise ValueError('benchmark=True runners take one preprocessed image per forward (batch=1)')
         self.dev = torch.device(device)
         if self.dev.index is None:
             self.dev = torch.device('cuda', torch.cuda.current_device())
@@ -343,21 +357,29 @@ class StreamRunner(object):
         self.s_d2h = torch.cuda.Stream(device=self.dev)
         if self.benchmark:
             ph, pw = max(largest_pad_shapes(self.resize, self.keep_ratio), key=lambda s: s[0] * s[1])
-            in_elems = 3 * max(ph, pw) ** 2
-            self.in_dev = [torch.empty(in_elems, dtype=torch.float32, device=self.dev) for _ in range(self.n)]
+            self.src_elems = 3 * max(ph, pw) ** 2
+            self.in_dev = [torch.empty(self.src_elems, dtype=torch.float32, device=self.dev) for _ in range(self.n)]
         else:
-            in_elems = self.max_src_hw[0] * self.max_src_hw[1] * 3
-            self.in_dev = [torch.empty(in_elems, dtype=torch.uint8, device=self.dev) for _ in range(self.n)]
+            # B source images per slot, image j at [j * src_elems, (j + 1) * src_elems)
+            self.src_elems = self.max_src_hw[0] * self.max_src_hw[1] * 3
+            self.in_dev = [torch.empty(self.B * self.src_elems, dtype=torch.uint8, device=self.dev) for _ in range(self.n)]
         self.out_dev, self.out_host = [], []
         self.ev_in_ready, self.ev_in_free, self.ev_out_ready, self.ev_out_free = ([torch.cuda.Event() for _ in range(self.n)]
                                                                                   for _ in range(4))
         self.ev_hold = [None] * self.n
-        self.meta = [None] * self.n
-        self.i = 0
-        self.pending = []
+        self._init_queue()
         cur = torch.cuda.current_stream(self.dev)
         for e in self.ev_in_free + self.ev_out_free:
             e.record(cur)
+
+    def _init_queue(self):
+        """Host bookkeeping of the batches: tickets, the open batch, what each slot holds."""
+        self.i = 0                                    # next ticket
+        self.dispatched = 0                           # batches dispatched so far; batch b runs in slot b % in_flight
+        self._open = None                             # dict(slot, pad, images) of the batch being filled
+        self.slot_images = [[] for _ in range(self.n)]    # per slot: the image dicts of the batch it holds, in order
+        self.meta = [None] * self.n                   # per slot: its batch's last image dict (its only one at batch 1)
+        self.pending = []
 
     def _new_engine(self, hw, arena):
         from .engine import SipMaskEngine
@@ -367,7 +389,7 @@ class StreamRunner(object):
         prev = C.set_min_tiles(self.kw.get('min_tiles', self.tune['min_tiles']))
         try:
             kw = {k: v for k, v in self.kw.items() if k != 'min_tiles'}
-            return SipMaskEngine(self.sd, (H, W), img_shape=(H, W, 3), ori_shape=ori, scale_factor=1.0,
+            return SipMaskEngine(self.sd, (H, W), batch=self.B, img_shape=(H, W, 3), ori_shape=ori, scale_factor=1.0,
                                  share_weights=self._wcache, arena=arena, device=self.dev, **kw)
         finally:
             C.set_min_tiles(prev)
@@ -384,7 +406,7 @@ class StreamRunner(object):
                 if self.benchmark:
                     eng.forward(None)                  # warm-up + capture
                 else:
-                    eng.forward_raw(torch.zeros((32, 32, 3), dtype=torch.uint8, device=self.dev), self.mean)
+                    eng.forward_raw([torch.zeros((32, 32, 3), dtype=torch.uint8, device=self.dev)] * self.B, self.mean)
             torch.cuda.synchronize(self.dev)
             self.build_seconds.setdefault(hw, []).append(time.perf_counter() - t0)
             self.engines[k][hw] = eng
@@ -424,32 +446,43 @@ class StreamRunner(object):
                              % (g.ry, g.rx, ori[0], ori[1], self.min_mask_up))
         return tuple(img_shape), tuple(pad), sf, tuple(ori)
 
-    def _out(self, k, eng, oh, wq):
-        """Slot k's device / pinned host record for an image with an oh x wq-word mask region."""
-        spec = dict(det=(eng.det.shape[1:], torch.float32), lab=(eng.labels.shape[1:], torch.long),
-                    cnt=((1,), torch.int32), idx=(eng.idx.shape[1:], torch.long),
-                    bits=((eng.max_num, oh, wq), torch.int32))
+    def _out(self, k, eng, oris):
+        """Slot k's device / pinned host record for the images of a batch with these ori_shapes: per image a dict of
+        views, and per field the number of elements the images use (a prefix of the slot's flat buffers)."""
+        mx = eng.max_num
+        spec = dict(det=((mx, 5), torch.float32), lab=((mx,), torch.long), cnt=((1,), torch.int32), idx=((mx,), torch.long),
+                    bits=(None, torch.int32))
         if eng.vis:
-            spec['trk'] = (eng.det_track.shape[1:], torch.float32)
+            spec['trk'] = ((mx, 512), torch.float32)
         if eng.rescoring:
-            spec['msc'] = (eng.mask_scores.shape[1:], torch.float32)
+            spec['msc'] = ((mx,), torch.float32)
         if k >= len(self.out_dev):
             self.out_dev += [None] * (k + 1 - len(self.out_dev))
             self.out_host += [None] * (k + 1 - len(self.out_host))
-        cap = eng.max_num * self.max_ori_hw[0] * ((self.max_ori_hw[1] + 31) // 32)
         if self.out_dev[k] is None:
-            self.out_dev[k] = {n: torch.empty(cap if n == 'bits' else int(np.prod(s)), dtype=d, device=self.dev)
+            cap = dict(bits=mx * self.max_ori_hw[0] * ((self.max_ori_hw[1] + 31) // 32))
+            self.out_dev[k] = {n: torch.empty(self.B * cap.get(n, int(np.prod(s or ()))), dtype=d, device=self.dev)
                                for n, (s, d) in spec.items()}
             self.out_host[k] = {n: torch.empty(v.numel(), dtype=v.dtype).pin_memory() for n, v in self.out_dev[k].items()}
-        numel = {n: int(np.prod(s)) for n, (s, d) in spec.items()}
-        dev = {n: self.out_dev[k][n][:numel[n]].view(spec[n][0]) for n in spec}
-        host = {n: self.out_host[k][n][:numel[n]].view(spec[n][0]) for n in spec}
-        return dev, host
+        used = {n: 0 for n in spec}
+        dev, host = [], []
+        for oh, ow in oris:
+            shape = dict((n, s) for n, (s, d) in spec.items())
+            shape['bits'] = (mx, oh, (ow + 31) // 32)
+            dev.append({})
+            host.append({})
+            for n, sh in shape.items():
+                o, ne = used[n], int(np.prod(sh))
+                dev[-1][n] = self.out_dev[k][n][o:o + ne].view(sh)
+                host[-1][n] = self.out_host[k][n][o:o + ne].view(sh)
+                used[n] = o + ne
+        return dev, host, used
 
     def submit(self, img, meta=None):
         """img: uint8 BGR HWC host image (pinned for an asynchronous upload), or with meta = (img_shape, ori_shape,
-        scale_factor) an fp32 NCHW [1, 3, H, W] preprocessed image (benchmark=True).  Validates, then enqueues upload ->
-        preprocessing -> geometry rows -> graph replay -> download of the meaningful record; returns the slot."""
+        scale_factor) an fp32 NCHW [1, 3, H, W] preprocessed image (benchmark=True).  Validates, uploads the image into
+        the open batch's staging and dispatches the batch when it is due (see the class docstring).  Returns the slot
+        (batch=1) or the image's ticket (batch > 1)."""
         if self.benchmark != (meta is not None):
             raise ValueError('benchmark=True runners take preprocessed fp32 images with their meta; others raw uint8 images')
         if meta is None:
@@ -460,57 +493,97 @@ class StreamRunner(object):
             if img.dtype != torch.float32 or img.dim() != 4 or img.shape[:2] != (1, 3):
                 raise ValueError('preprocessed input is an fp32 [1, 3, H, W] image')
             img_shape, pad, sf, ori = self.check(img.shape[2:], meta)
-        k = self.i % self.n
-        eng = self._engine(k, pad[:2])
-        cs = self.streams[k]
-        src = self.in_dev[k][:img.numel()].view(img.shape)
+        if self._open is not None and self._open['pad'] != pad[:2]:
+            self._dispatch()                          # a new padded shape closes the open batch before it is staged
+        if self._open is None:
+            self._open = dict(slot=self.dispatched % self.n, pad=pad[:2], images=[])
+            self._begin(self._open['slot'], pad[:2])
+        ob = self._open
+        m = dict(ticket=self.i, img_shape=img_shape, pad_shape=pad, scale_factor=sf, ori_shape=ori)
+        m['src'] = self._stage(ob['slot'], len(ob['images']), img)
+        ob['images'].append(m)
+        self.i += 1
+        if len(ob['images']) == self.B:
+            self._dispatch()
+        return ob['slot'] if self.B == 1 else m['ticket']
+
+    def _begin(self, k, hw):
+        """A batch opens in slot k: its engine exists, and the uploads wait until the slot's previous batch consumed its
+        input."""
+        self._engine(k, hw)
+        self.s_h2d.wait_event(self.ev_in_free[k])
+
+    def _stage(self, k, j, img):
+        """Upload image j of slot k's open batch into its staging on the H2D stream; returns the device view."""
+        src = self.in_dev[k][j * self.src_elems:j * self.src_elems + img.numel()].view(img.shape)
         with torch.cuda.stream(self.s_h2d):
-            self.s_h2d.wait_event(self.ev_in_free[k])
             src.copy_(img, non_blocking=True)
-            self.ev_in_ready[k].record(self.s_h2d)
-        oh, wq = ori[0], (ori[1] + 31) // 32
+        return src
+
+    def _dispatch(self):
+        """Close the open batch: run it in its slot and enqueue the download of its real images' records."""
+        ob, self._open = self._open, None
+        k, images = ob['slot'], ob['images']
+        self._launch(k, ob['pad'], images)
+        for m in images:
+            m.pop('src', None)
+        self.slot_images[k] = images
+        self.meta[k] = images[-1]
+        self.dispatched += 1
+        return k
+
+    def _launch(self, k, pad, images):
+        eng = self._engine(k, pad)
+        cs = self.streams[k]
+        self.ev_in_ready[k].record(self.s_h2d)
+        nr = len(images)
+        metas = [(m['img_shape'], m['ori_shape'], m['scale_factor']) for m in images]
         with torch.cuda.stream(cs):
             cs.wait_event(self.ev_in_ready[k])
-            eng.set_image_meta([(img_shape, ori, sf)])
-            if meta is None:
-                eng.forward_raw(src, self.mean)
-            else:
-                eng.img.copy_(src, non_blocking=True)
+            eng.set_image_meta(metas + [metas[-1]] * (self.B - nr))      # fillers: the last real image's geometry
+            if self.benchmark:
+                eng.img.copy_(images[0]['src'], non_blocking=True)
                 eng.forward(None)
+            else:
+                eng.forward_raw([m['src'] for m in images] + [None] * (self.B - nr), self.mean)
             self.ev_in_free[k].record(cs)
             cs.wait_event(self.ev_out_free[k])
             if self.ev_hold[k] is not None:
                 cs.wait_event(self.ev_hold[k])
-            o, h = self._out(k, eng, oh, wq)
-            o['det'].copy_(eng.det[0])
-            o['lab'].copy_(eng.labels[0])
-            o['cnt'].copy_(eng.count)
-            o['idx'].copy_(eng.idx[0])
-            o['bits'].copy_(eng.mask_bits[0, :, :oh, :wq])
-            if 'trk' in o:
-                o['trk'].copy_(eng.det_track[0])
-            if 'msc' in o:
-                o['msc'].copy_(eng.mask_scores[0])
+            dev, host, used = self._out(k, eng, [m['ori_shape'][:2] for m in images])
+            flat = self.out_dev[k]
+            mx = eng.max_num
+            flat['det'][:used['det']].view(nr, mx, 5).copy_(eng.det[:nr])
+            flat['lab'][:used['lab']].view(nr, mx).copy_(eng.labels[:nr])
+            flat['cnt'][:nr].copy_(eng.count[:nr])
+            flat['idx'][:used['idx']].view(nr, mx).copy_(eng.idx[:nr])
+            if 'trk' in flat:
+                flat['trk'][:used['trk']].view(nr, mx, 512).copy_(eng.det_track[:nr])
+            if 'msc' in flat:
+                flat['msc'][:used['msc']].view(nr, mx).copy_(eng.mask_scores[:nr])
+            for j, (m, o) in enumerate(zip(images, dev)):
+                oh, wq = o['bits'].shape[1:]
+                o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
             self.ev_out_ready[k].record(cs)
         with torch.cuda.stream(self.s_d2h):
             self.s_d2h.wait_event(self.ev_out_ready[k])
-            for name in o:
-                h[name].copy_(o[name], non_blocking=True)
+            for name, n in used.items():
+                self.out_host[k][name][:n].copy_(flat[name][:n], non_blocking=True)
             self.ev_out_free[k].record(self.s_d2h)
-        self.meta[k] = dict(img_shape=img_shape, pad_shape=pad, scale_factor=sf, ori_shape=ori, dev=o, host=h)
-        self.i += 1
-        return k
+        for m, o, h in zip(images, dev, host):
+            m['dev'], m['host'] = o, h
 
     def consume(self, slot, fn):
-        """Run fn(slot's device record) on the CURRENT stream once it is ready; the slot is not overwritten before fn's
-        work has finished."""
+        """Run fn(record on the device) on the CURRENT stream for every image of the slot's batch, in submission order,
+        once the batch is done; the slot is not overwritten before fn's work has finished.  Returns fn's result (batch=1)
+        or the list of them."""
         cur = torch.cuda.current_stream(self.dev)
         cur.wait_event(self.ev_out_ready[slot])
-        r = fn(self._record(self.meta[slot]['dev']))
+        rs = [fn(self._record(m['dev'])) for m in self.slot_images[slot]]
         if self.ev_hold[slot] is None:
             self.ev_hold[slot] = torch.cuda.Event()
         self.ev_hold[slot].record(cur)
-        return r
+        return rs[0] if self.B == 1 else rs
 
     @staticmethod
     def _record(o):
@@ -522,28 +595,48 @@ class StreamRunner(object):
         return rec
 
     def step(self, img, fn=None, meta=None):
-        """submit() + hand the OLDEST slot in flight to fn (see EnginePool.step).  Returns the submitted slot."""
-        k = self.submit(img, meta)
-        self.pending.append(k)
-        if fn is not None and len(self.pending) >= self.n:
-            self.consume(self.pending.pop(0), fn)
-        elif fn is None:
+        """submit() + hand the images of the OLDEST batch in flight to fn once in_flight batches are dispatched (see
+        EnginePool.step).  Returns what submit() returned."""
+        before = self.dispatched
+        r = self.submit(img, meta)
+        self.pending += [b % self.n for b in range(before, self.dispatched)]
+        if fn is not None:
+            while len(self.pending) >= self.n:
+                self.consume(self.pending.pop(0), fn)
+        else:
             self.pending.clear()
-        return k
+        return r
 
     def flush(self, fn=None):
+        """Dispatch the open batch, hand every batch still pending to fn, and make the current stream wait for the
+        downloads."""
+        if self._open is not None:
+            self.pending.append(self._dispatch())
         while self.pending:
             k = self.pending.pop(0)
             if fn is not None:
                 self.consume(k, fn)
+        self._join()
+
+    def _join(self):
         torch.cuda.current_stream(self.dev).wait_stream(self.s_d2h)
 
-    def result(self, slot):
-        """Blocks until the slot's download finished; returns the pinned host record (det_bboxes, det_labels, count,
-        idxs_keep, mask_bits [max, ori_h, ceil(ori_w / 32)], track_feats / mask_scores when enabled) and the image's
-        meta.  Valid until the slot is reused."""
-        self.ev_out_free[slot].synchronize()
-        m = self.meta[slot]
+    def _locate(self, ticket):
+        if self._open is not None and any(m['ticket'] == ticket for m in self._open['images']):
+            raise ValueError('ticket %d is in the open batch: flush() dispatches it' % ticket)
+        for k, images in enumerate(self.slot_images):
+            for j, m in enumerate(images):
+                if m['ticket'] == ticket:
+                    return k, j
+        raise ValueError('ticket %d is not held by any slot (never submitted, or its slot was reused)' % ticket)
+
+    def result(self, key):
+        """key: the slot submit() returned (batch=1) or the image's ticket (batch > 1).  Blocks until the download
+        finished; returns the pinned host record (det_bboxes, det_labels, count, idxs_keep, mask_bits [max, ori_h,
+        ceil(ori_w / 32)], track_feats / mask_scores when enabled) and the image's meta.  Valid until the slot is reused."""
+        k, j = (key, 0) if self.B == 1 else self._locate(key)
+        self.ev_out_free[k].synchronize()
+        m = self.slot_images[k][j]
         rec = self._record(m['host'])
         rec['meta'] = dict(img_shape=m['img_shape'], pad_shape=m['pad_shape'], ori_shape=m['ori_shape'],
                            scale_factor=m['scale_factor'])
