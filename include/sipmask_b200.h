@@ -446,6 +446,16 @@ typedef struct {
  * every canvas is bit-identical to the single-image entry point.  Reads sum(src bytes), writes N*(H/2+3)*(W/2+4)*32 bytes. */
 int smb_preprocess_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out_s2d16, int H, int W, smb_stream_t stream);
 
+/* SipMask-benchmark's test transform for a batch (SipMask-benchmark/fcos_core/data/transforms/build.py:17-36,
+ * transforms.py:27-95: PIL Image.resize(BILINEAR) -> to_tensor -> to_bgr255 -> normalize(std = 1) -> pad), restated
+ * bit-exactly (Pillow's separable antialiased 22-bit fixed-point filter, horizontal pass clipped to uint8 first):
+ *   rows[n].src   : RGB HWC uint8, as PIL decodes it (the other fields as for smb_preprocess_u8_s2d_dev)
+ *   rows[n].mean  : in output (BGR) order; output channel c = float(src[2 - c]) - mean[c], rounded once to fp16
+ * Same [N, H/2+3, W/2+4, 16] canvas, halo / padding zeros and filler rows as smb_preprocess_u8_s2d_dev.  A downscale of
+ * more than 8x on either axis is not supported (the caller rejects it).  Reads sum(src bytes), writes
+ * N*(H/2+3)*(W/2+4)*32 bytes. */
+int smb_preprocess_pil_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out_s2d16, int H, int W, smb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -66,7 +66,7 @@ SYMBOLS = [
     'smb_groupnorm_relu_apply', 'smb_groupnorm_stats', 'smb_deform_im2col', 'smb_offset_conv1x1', 'smb_groupnorm_relu_apply_multi', 'smb_offset_conv1x1_multi', 'smb_offset_conv1x1_relu_multi', 'smb_deform_im2col_multi', 'smb_maxpool3x3s2',
     'smb_upsample_bilinear', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
     'smb_mask_assemble_dev', 'smb_mask_assemble_pack_dev', 'smb_decode_topk_dev', 'smb_pair_decode_topk_dev',
-    'smb_gather_track_feats_dev', 'smb_preprocess_u8_s2d_dev',
+    'smb_gather_track_feats_dev', 'smb_preprocess_u8_s2d_dev', 'smb_preprocess_pil_u8_s2d_dev',
 ]
 
 

@@ -219,16 +219,35 @@ def preprocess_u8_rows(rows, out):
     return out
 
 
-def raw_src_row(src, resized_hw, canvas_hw, mean, device):
-    """The smb_raw_src_t row of one uint8 BGR HWC image on `device` resized to resized_hw inside a canvas_hw canvas, or a
-    filler row (all-zero canvas, nothing read) for src=None.  Raises ValueError for anything the kernel could not read
-    safely."""
+@L.device_guard
+def preprocess_pil_rows(rows, out):
+    """SipMask-benchmark's test transform for a batch in one launch: canvas n of `out` [N, H/2+3, W/2+4, 16] from the
+    smb_raw_src_t row n of `rows` (a device tensor of N rows; src is an RGB image, mean in BGR order), PIL bilinear resize
+    bit-exact, BGR, mean-subtracted, zero-padded (smb_preprocess_pil_u8_s2d_dev).  The rows are not checked on the
+    device: write only rows that raw_src_row validated with max_downscale=PIL_MAX_DOWNSCALE."""
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.dim() == 4 and out.shape[3] == 16
+    assert rows.is_cuda and rows.dtype == torch.uint8 and rows.numel() == out.shape[0] * ctypes.sizeof(L.RawSrc)
+    H, W = 2 * (out.shape[1] - 3), 2 * (out.shape[2] - 4)
+    L.check(L.lib().smb_preprocess_pil_u8_s2d_dev(L.ptr(rows), int(out.shape[0]), L.ptr(out), H, W, L.stream_ptr()),
+            'smb_preprocess_pil_u8_s2d_dev')
+    return out
+
+
+# the steepest downscale per axis smb_preprocess_pil_u8_s2d_dev supports (its filter has at most 17 taps)
+PIL_MAX_DOWNSCALE = 8
+
+
+def raw_src_row(src, resized_hw, canvas_hw, mean, device, order='BGR', max_downscale=None):
+    """The smb_raw_src_t row of one uint8 HWC image (channel `order`: BGR for the cv2 pipeline, RGB for the PIL one) on
+    `device` resized to resized_hw inside a canvas_hw canvas, or a filler row (all-zero canvas, nothing read) for
+    src=None.  max_downscale: the steepest shrink per axis the kernel supports (None: no limit).  Raises ValueError for
+    anything the kernel could not read safely."""
     r = L.RawSrc()
     r.mean[:] = [float(v) for v in mean]
     if src is None:
         return r
     if not isinstance(src, torch.Tensor) or src.dtype != torch.uint8 or src.dim() != 3 or src.shape[2] != 3:
-        raise ValueError('raw input is a uint8 HWC BGR image')
+        raise ValueError('raw input is a uint8 HWC %s image' % order)
     h, w = int(src.shape[0]), int(src.shape[1])
     if src.stride(2) != 1 or src.stride(1) != 3 or not 3 * w <= src.stride(0) < 2 ** 31:
         raise ValueError('raw input must have HWC strides (row pitch, 3, 1), got %s' % (tuple(src.stride()),))
@@ -238,6 +257,8 @@ def raw_src_row(src, resized_hw, canvas_hw, mean, device):
     if h <= 0 or w <= 0 or not (0 < dh <= canvas_hw[0] and 0 < dw <= canvas_hw[1]):
         raise ValueError('image %dx%d resized to %dx%d does not fit the %dx%d canvas' % (h, w, dh, dw, canvas_hw[0],
                                                                                         canvas_hw[1]))
+    if max_downscale is not None and (h > max_downscale * dh or w > max_downscale * dw):
+        raise ValueError('image %dx%d resized to %dx%d shrinks more than %gx on an axis' % (h, w, dh, dw, max_downscale))
     r.src, r.src_h, r.src_w, r.src_pitch_bytes, r.dst_h, r.dst_w = src.data_ptr(), h, w, int(src.stride(0)), dh, dw
     return r
 

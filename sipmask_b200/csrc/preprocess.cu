@@ -5,7 +5,8 @@
 // (SipMask-mmdetection/mmdet/datasets/pipelines/transforms.py:97-110, 274-300, 335-363), i.e. mmcv -> cv2.resize(INTER_LINEAR),
 // followed by a 12.9 MB fp32 upload.  Here the upload is the raw uint8 image (<= 4 MB) and the arithmetic is OpenCV's
 // 8-bit fixed-point bilinear restated exactly (11-bit coefficients, int32 horizontal pass, the two truncating shifts of
-// the vertical pass), so the stem sees bit-identical input.
+// the vertical pass), so the stem sees bit-identical input.  SipMask-benchmark checkpoints get their own kernel below
+// (PIL bilinear on an RGB source).
 #include <stdint.h>
 
 #include <cuda_fp16.h>
@@ -88,10 +89,18 @@ __device__ __forceinline__ void pre_pixel(const PreArgs& a, int x, int y, float*
 }
 
 // Space-to-depth layout of the 7x7/2 stem: out [N, H/2+3, W/2+4, 16] fp16, element (n, Y, X, (dy*2+dx)*4 + c) = padded
-// pixel (2Y+dy, 2X+dx) = pixel (2Y+dy-3, 2X+dx-3) of image n, channel c (c == 3: zero).  One thread = one 32-byte
-// (n, Y, X) cell; image n's source row is rows[n] (device memory, rewritten between graph replays) or, with rows == nullptr
-// (N == 1), row0 by value.  Write indices come from the canvas alone, so no row can make a thread write outside image n's
-// canvas; reads stay inside the row's source image because pre_pixel clamps every source row / column index.
+// pixel (2Y+dy, 2X+dx) = pixel (2Y+dy-3, 2X+dx-3) of image n, channel c (c == 3: zero).  store_cell writes cell number
+// `cell` (= (n * (H/2+3) + Y) * (W/2+4) + X) from its 16 floats f[(dy*2+dx)*4 + c] as two 16-byte stores.
+__device__ __forceinline__ void store_cell(__half* __restrict__ out, long long cell, const float* f) {
+  uint4* o = reinterpret_cast<uint4*>(out + cell * 16);
+  o[0] = pack8h(f);
+  o[1] = pack8h(f + 8);
+}
+
+// One thread = one 32-byte (n, Y, X) cell; image n's source row is rows[n] (device memory, rewritten between graph
+// replays) or, with rows == nullptr (N == 1), row0 by value.  Write indices come from the canvas alone, so no row can make
+// a thread write outside image n's canvas; reads stay inside the row's source image because pre_pixel clamps every source
+// row / column index.
 __global__ void preprocess_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows, smb_raw_src_t row0,
                                          __half* __restrict__ out, int N, int H, int W) {
   const int Hq = H / 2 + 3, Wq = W / 2 + 4;
@@ -107,10 +116,130 @@ __global__ void preprocess_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows,
       pre_pixel(a, 2 * X + (d & 1) - 3, 2 * Y + (d >> 1) - 3, f + 4 * d);
       f[4 * d + 3] = 0.f;
     }
-    uint4* o = reinterpret_cast<uint4*>(out + t * 16);
-    o[0] = pack8h(f);
-    o[1] = pack8h(f + 8);
+    store_cell(out, t, f);
   }
+}
+
+// ------------------------------------------------------------------------------------------------------------------------
+// SipMask-benchmark's test transform (SipMask-benchmark/fcos_core/data/transforms/build.py:17-36, transforms.py:27-95):
+// PIL RGB image -> torchvision F.resize = PIL Image.resize(BILINEAR) -> to_tensor -> to_bgr255 -> normalize(std = 1) ->
+// zero pad to 32.  fl(fl(v / 255) * 255) == v for every uint8 v, so the network input is exactly float(v) - mean on the
+// BGR channel, which this kernel computes from the RGB source.
+//
+// Pillow's resize (libImaging/Resample.c) is separable and antialiased, in 22-bit fixed point: per output index xx of an
+// in -> out axis, scale = in / out, fs = max(scale, 1) (= the bilinear support), center = (xx + 0.5) * scale, taps
+// [xmin, xmin + n) with xmin = max((int)(center - fs + 0.5), 0), xmin + n = min((int)(center + fs + 0.5), in), weights
+// tri(((x + xmin) - center + 0.5) * (1 / fs)) summed in order in double, divided by the sum and stored as
+// (int)(0.5 + k * 2^22).  The horizontal pass runs first and clips to uint8; each pass is clamp((2^21 + sum v * k) >> 22,
+// 0, 255).  An axis whose size does not change gets the taps {2^22, 0}, which copy it exactly (Pillow skips that pass).
+// Every double operation is an explicit _rn intrinsic: the reference (x86-64 Pillow) does not contract to FMA, nvcc would.
+constexpr int PIL_TY = 8, PIL_TX = 32;                        // cells per CTA: 8 x 32 -> 16 output rows x 64 columns
+constexpr int PIL_OY = 2 * PIL_TY, PIL_OX = 2 * PIL_TX;
+constexpr int PIL_MAX_SCALE = 8;                              // steepest downscale per axis (validated by the host)
+constexpr int PIL_KMAX = 2 * PIL_MAX_SCALE + 1;               // taps per output index at that scale (< 2 * fs + 1)
+constexpr int PIL_RMAX = (PIL_OY - 1) * PIL_MAX_SCALE + PIL_KMAX;   // source rows the 16 output rows of a tile read
+
+// Taps of output index xx of an in -> out axis: first source index, count, fixed-point weights.
+__device__ void pil_taps(int xx, int in, int out, int* lo, int* cnt, int* w) {
+  const double scale = __ddiv_rn((double)in, (double)out);
+  const double fs = scale < 1.0 ? 1.0 : scale;
+  const double ss = __ddiv_rn(1.0, fs);
+  const double center = __dmul_rn(__dadd_rn((double)xx, 0.5), scale);
+  int xmin = __double2int_rz(__dadd_rn(__dsub_rn(center, fs), 0.5));
+  int xmax = __double2int_rz(__dadd_rn(__dadd_rn(center, fs), 0.5));
+  xmin = max(xmin, 0);
+  xmax = min(min(xmax, in) - xmin, PIL_KMAX);
+  double ww = 0.0;
+  for (int x = 0; x < xmax; ++x) {
+    const double t = fabs(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss));
+    ww = __dadd_rn(ww, t < 1.0 ? __dsub_rn(1.0, t) : 0.0);
+  }
+  for (int x = 0; x < xmax; ++x) {                            // the same weights again, normalised
+    const double t = fabs(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss));
+    double k = t < 1.0 ? __dsub_rn(1.0, t) : 0.0;
+    if (ww != 0.0) k = __ddiv_rn(k, ww);
+    w[x] = __double2int_rz(__dadd_rn(0.5, __dmul_rn(k, 4194304.0)));
+  }
+  *lo = xmin;
+  *cnt = xmax;
+}
+
+__device__ __forceinline__ int pil_clip8(int v) { return min(max(v >> 22, 0), 255); }
+
+// One CTA = a tile of PIL_TY x PIL_TX cells of canvas blockIdx.z.  It computes the taps of the tile's output columns and
+// rows once, runs the horizontal pass over the source rows those output rows need into shared memory (uint8, as Pillow's
+// intermediate image), then each thread runs the vertical pass for its cell's four pixels and writes the cell.  Write
+// indices come from the canvas alone; source indices are clamped inside the row's image and shared-memory rows inside
+// the tile's buffer, so an unvalidated row cannot make the kernel touch memory outside them.
+__global__ void __launch_bounds__(PIL_TY * PIL_TX) preprocess_pil_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows,
+                                                                               __half* __restrict__ out, int H, int W) {
+  __shared__ int cx_lo[PIL_OX], cx_n[PIL_OX], cx_w[PIL_OX][PIL_KMAX];
+  __shared__ int cy_lo[PIL_OY], cy_n[PIL_OY], cy_w[PIL_OY][PIL_KMAX];
+  __shared__ uint8_t hpass[PIL_RMAX][PIL_OX * 3];
+  const int Hq = H / 2 + 3, Wq = W / 2 + 4;
+  const int n = blockIdx.z, Y0 = blockIdx.y * PIL_TY, X0 = blockIdx.x * PIL_TX, t = threadIdx.x;
+  const smb_raw_src_t r = rows[n];
+  const bool fill = r.dst_h <= 0 || r.dst_w <= 0;
+  const int dh = fill ? 0 : r.dst_h, dw = fill ? 0 : r.dst_w;
+  const int py0 = 2 * Y0 - 3, px0 = 2 * X0 - 3;               // output pixel of the tile's local (0, 0)
+  // the tile's output pixels inside the resized image (everything else is halo / padding: zero)
+  const int ya = max(py0, 0), yb = min(py0 + PIL_OY, dh), xa = max(px0, 0), xb = min(px0 + PIL_OX, dw);
+  const bool any = ya < yb && xa < xb;                        // uniform over the CTA
+  int ybase = 0;
+  if (any) {
+    if (t < PIL_OX) {
+      const int x = px0 + t;
+      if (x >= xa && x < xb) pil_taps(x, r.src_w, dw, &cx_lo[t], &cx_n[t], cx_w[t]);
+    } else if (t < PIL_OX + PIL_OY) {
+      const int ly = t - PIL_OX, y = py0 + ly;
+      if (y >= ya && y < yb) pil_taps(y, r.src_h, dh, &cy_lo[ly], &cy_n[ly], cy_w[ly]);
+    }
+    __syncthreads();
+    ybase = cy_lo[ya - py0];
+    const int nrows = min(cy_lo[yb - 1 - py0] + cy_n[yb - 1 - py0] - ybase, PIL_RMAX);
+    const int nx = xb - xa, lx0 = xa - px0;
+    for (int i = t; i < nrows * nx; i += PIL_TY * PIL_TX) {
+      const int rr = i / nx, lx = lx0 + i % nx;
+      const uint8_t* p = r.src + (size_t)min(ybase + rr, r.src_h - 1) * r.src_pitch_bytes;
+      const int lo = cx_lo[lx], cnt = cx_n[lx];
+      int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+      for (int k = 0; k < cnt; ++k) {
+        const uint8_t* q = p + 3 * min(lo + k, r.src_w - 1);
+        const int w = cx_w[lx][k];
+        a0 += (int)q[0] * w;
+        a1 += (int)q[1] * w;
+        a2 += (int)q[2] * w;
+      }
+      hpass[rr][lx * 3 + 0] = (uint8_t)pil_clip8(a0);
+      hpass[rr][lx * 3 + 1] = (uint8_t)pil_clip8(a1);
+      hpass[rr][lx * 3 + 2] = (uint8_t)pil_clip8(a2);
+    }
+    __syncthreads();
+  }
+  const int ty = t / PIL_TX, tx = t % PIL_TX, Y = Y0 + ty, X = X0 + tx;
+  if (Y >= Hq || X >= Wq) return;
+  float f[16];
+#pragma unroll
+  for (int d = 0; d < 4; ++d) {
+    const int ly = 2 * ty + (d >> 1), lx = 2 * tx + (d & 1), y = py0 + ly, x = px0 + lx;
+    f[4 * d + 0] = f[4 * d + 1] = f[4 * d + 2] = f[4 * d + 3] = 0.f;
+    if (any && y >= ya && y < yb && x >= xa && x < xb) {
+      const int lo = cy_lo[ly] - ybase, cnt = cy_n[ly];
+      int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+      for (int k = 0; k < cnt; ++k) {
+        const uint8_t* q = &hpass[min(lo + k, PIL_RMAX - 1)][lx * 3];
+        const int w = cy_w[ly][k];
+        a0 += (int)q[0] * w;
+        a1 += (int)q[1] * w;
+        a2 += (int)q[2] * w;
+      }
+      // RGB source -> BGR network input
+      f[4 * d + 0] = __fsub_rn((float)pil_clip8(a2), r.mean[0]);
+      f[4 * d + 1] = __fsub_rn((float)pil_clip8(a1), r.mean[1]);
+      f[4 * d + 2] = __fsub_rn((float)pil_clip8(a0), r.mean[2]);
+    }
+  }
+  store_cell(out, ((long long)n * Hq + Y) * Wq + X, f);
 }
 
 static int launch_preprocess(const smb_raw_src_t* rows, const smb_raw_src_t& row0, void* out, int N, int H, int W,
@@ -146,4 +275,15 @@ extern "C" int smb_preprocess_u8_s2d_dev(const smb_raw_src_t* rows, int N, void*
   smb_raw_src_t r;
   memset(&r, 0, sizeof(r));
   return launch_preprocess(rows, r, out, N, H, W, stream);
+}
+
+extern "C" int smb_preprocess_pil_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out, int H, int W,
+                                             smb_stream_t stream) {
+  SMB_CHECK_ARG(rows && out, "smb_preprocess_pil_u8_s2d_dev: null pointer");
+  SMB_CHECK_ARG(N > 0 && N <= 65535 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0,
+                "smb_preprocess_pil_u8_s2d_dev: bad canvas (N %d, %dx%d; H, W must be even)", N, H, W);
+  const dim3 grid(cdiv(W / 2 + 4, PIL_TX), cdiv(H / 2 + 3, PIL_TY), N);
+  preprocess_pil_u8_s2d_kernel<<<grid, PIL_TY * PIL_TX, 0, (cudaStream_t)stream>>>(rows, (__half*)out, H, W);
+  SMB_LAUNCH_OK("preprocess_pil_u8_s2d_kernel");
+  return SMB_OK;
 }

@@ -737,30 +737,39 @@ class SipMaskEngine(object):
             r['mask_scores'] = self.mask_scores        # [N,max] fp32 SipMask++ mask scores (zeros after count)
         return r
 
-    def forward_raw(self, imgs, mean=(102.9801, 115.9465, 122.7717)):
-        """imgs: N uint8 BGR HWC CUDA images straight from the decoder (a list; one tensor when N == 1).  Image n is resized
-        to its own img_shape (the constructor's, or the one set_image_meta set; cv2 INTER_LINEAR, bit-exact), mean-subtracted,
-        zero-padded and written in the stem's layout by ONE kernel for the whole batch (SURVEY.md 8f-3), captured in
-        `graph_raw` in place of the `image_to_s2d16` node.  A None entry is a filler image: an all-zero canvas, for a
-        partial batch.  Per call: the source rows are written with a stream-ordered H2D copy on the current stream, then
-        one graph replay.  The images must stay alive and unchanged until the forward has consumed them."""
-        rows = self._raw_src_rows(imgs, mean)        # host validation: ValueError before anything is enqueued
+    def forward_raw(self, imgs, mean=(102.9801, 115.9465, 122.7717), pipeline='mmdet'):
+        """imgs: N uint8 HWC CUDA images straight from the decoder (a list; one tensor when N == 1).  Image n is resized
+        to its own img_shape (the constructor's, or the one set_image_meta set), mean-subtracted, zero-padded and written
+        in the stem's layout by ONE kernel for the whole batch (SURVEY.md 8f-3), captured in place of the
+        `image_to_s2d16` node.  A None entry is a filler image: an all-zero canvas, for a partial batch.  Per call: the
+        source rows are written with a stream-ordered H2D copy on the current stream, then one graph replay.  The images
+        must stay alive and unchanged until the forward has consumed them.
+        pipeline='mmdet': BGR images, cv2 INTER_LINEAR (bit-exact), graph `graph_raw`.
+        pipeline='benchmark' (benchmark=True engines only): RGB images as PIL decodes them, SipMask-benchmark's test
+        transform (PIL bilinear, bit-exact; BGR x 255 - mean), graph `graph_raw_bm`; a downscale steeper than
+        conv.PIL_MAX_DOWNSCALE on either axis raises ValueError.  mean is in BGR order for both."""
+        if pipeline not in ('mmdet', 'benchmark'):
+            raise ValueError("forward_raw: pipeline is 'mmdet' or 'benchmark', got %r" % (pipeline,))
+        if pipeline == 'benchmark' and not self.benchmark:
+            raise ValueError("forward_raw: pipeline='benchmark' needs a benchmark=True engine")
+        rows = self._raw_src_rows(imgs, mean, pipeline)   # host validation: ValueError before anything is enqueued
         if torch.cuda.current_device() != self.dev.index:
             with torch.cuda.device(self.dev):
-                return self._forward_raw_rows(rows)
-        return self._forward_raw_rows(rows)
+                return self._forward_raw_rows(rows, pipeline)
+        return self._forward_raw_rows(rows, pipeline)
 
-    def _raw_src_rows(self, imgs, mean):
+    def _raw_src_rows(self, imgs, mean, pipeline='mmdet'):
         srcs = [imgs] if isinstance(imgs, torch.Tensor) else list(imgs)
         if len(srcs) != self.N:
             raise ValueError('forward_raw: %d images for a batch of %d' % (len(srcs), self.N))
-        return (L.RawSrc * self.N)(*[C.raw_src_row(s, m[0][:2], (self.H, self.W), mean, self.dev)
+        kw = dict(order='RGB', max_downscale=C.PIL_MAX_DOWNSCALE) if pipeline == 'benchmark' else {}
+        return (L.RawSrc * self.N)(*[C.raw_src_row(s, m[0][:2], (self.H, self.W), mean, self.dev, **kw)
                                      for s, m in zip(srcs, self.image_metas)])
 
-    def _forward_raw_rows(self, rows):
+    def _forward_raw_rows(self, rows, pipeline='mmdet'):
         """Writes the source rows the way set_image_meta writes the geometry (pinned staging -> one H2D copy on the current
-        stream, the staging reused only after that copy has run), then replays graph_raw.  The rows live outside the
-        arena: they persist between forwards."""
+        stream, the staging reused only after that copy has run), then replays the pipeline's graph.  The rows live
+        outside the arena: they persist between forwards, and both pipelines' graphs read the same rows."""
         nbytes = ctypes.sizeof(rows)
         if getattr(self, '_raw_rows', None) is None:
             self._raw_rows = torch.empty(nbytes, dtype=torch.uint8, device=self.dev)
@@ -772,19 +781,21 @@ class SipMaskEngine(object):
         self._raw_rows.copy_(self._raw_host, non_blocking=True)
         self._raw_copied.record(torch.cuda.current_stream(self.dev))
         names = set(self.op_names) - {'image_to_s2d16', 'fork', 'join'}
+        pre = C.preprocess_pil_rows if pipeline == 'benchmark' else C.preprocess_u8_rows
+        attr = 'graph_raw_bm' if pipeline == 'benchmark' else 'graph_raw'
         if self.use_graph:
-            if getattr(self, 'graph_raw', None) is None:
-                C.preprocess_u8_rows(self._raw_rows, self.img8)
+            if getattr(self, attr, None) is None:
+                pre(self._raw_rows, self.img8)
                 self._run_ops(only=names)
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    C.preprocess_u8_rows(self._raw_rows, self.img8)
+                    pre(self._raw_rows, self.img8)
                     self._run_ops(only=names)
-                self.graph_raw = g
-            self.graph_raw.replay()
+                setattr(self, attr, g)
+            getattr(self, attr).replay()
         else:
-            C.preprocess_u8_rows(self._raw_rows, self.img8)
+            pre(self._raw_rows, self.img8)
             self._run_ops(only=names)
         return self._result()
 

@@ -297,6 +297,34 @@ def largest_pad_shapes(resize=(1333, 800), keep_ratio=True, size_divisor=32):
     return [(s, l), (l, s)] if s != l else [(s, l)]
 
 
+def bm_resize_size(h, w, min_size=800, max_size=1333):
+    """SipMask-benchmark's test size rule (fcos_core/data/transforms/transforms.py:36-55, Resize.get_size) for an h x w
+    image -> (oh, ow), in Python float arithmetic: the short side becomes min_size unless the long side would exceed
+    max_size, in which case the short side becomes int(round(max_size * short / long)); an image whose short side already
+    has that size is not resized; otherwise long = int(size * long / short).  The long side is not bounded: extreme
+    aspect ratios (1 x 2048) keep their size."""
+    size = min_size
+    if max_size is not None:
+        mn, mx = float(min((w, h))), float(max((w, h)))
+        if mx / mn * size > max_size:
+            size = int(round(max_size * mn / mx))
+    if (w <= h and w == size) or (h <= w and h == size):
+        return h, w
+    if w < h:
+        return int(size * h / w), size
+    return size, int(size * w / h)
+
+
+def bm_image_meta(h, w, min_size=800, max_size=1333, size_divisor=32):
+    """(img_shape, pad_shape, scale_factor) of an h x w image under SipMask-benchmark's test transform (bm_resize_size,
+    then to_image_list(size_divisible=32)).  The benchmark post-processing reads only img_shape and ori_shape
+    (postproc.image_geometry(benchmark=True)); scale_factor = min(oh / h, ow / w) is the ratio its mask resize uses."""
+    nh, nw = bm_resize_size(h, w, min_size, max_size)
+    ph = (nh + size_divisor - 1) // size_divisor * size_divisor
+    pw = (nw + size_divisor - 1) // size_divisor * size_divisor
+    return (nh, nw, 3), (ph, pw, 3), min(nh / h, nw / w)
+
+
 class StreamRunner(object):
     """Serves a stream of images of ANY size.  Every image runs the network on the canvas of its own padded shape (one
     engine per padded shape, a "bucket", built and captured on first use); only the post-processing geometry
@@ -307,12 +335,16 @@ class StreamRunner(object):
     rule produces) from which every bucket engine of the slot carves its activations: a second bucket costs its graph
     and bookkeeping, not another activation set.  Packed weights are shared by all engines.
 
-    submit(img): a uint8 BGR HWC image of any size up to max_src_hw (raw mode; the resize runs on the GPU), or for
-    SipMask-benchmark checkpoints (benchmark=True, whose resize rule is not restated here) a preprocessed fp32 NCHW image
-    padded to a multiple of 32 together with its meta = (img_shape, ori_shape, scale_factor).  result(slot) returns the
-    record with mask_bits cropped to the image's [max, ori_h, ceil(ori_w / 32)].
+    submit(img): a uint8 BGR HWC image of any size up to max_src_hw (raw mode; the resize runs on the GPU).  For
+    SipMask-benchmark checkpoints (benchmark=True) either a uint8 RGB HWC image as PIL decodes it (raw=True: the
+    benchmark's own test transform, PIL bilinear resize under bm_resize_size with min(resize) / max(resize) as min / max
+    size, runs on the GPU), or a preprocessed fp32 NCHW image padded to a multiple of 32 together with its meta =
+    (img_shape, ori_shape, scale_factor).  result(slot) returns the record with mask_bits cropped to the image's
+    [max, ori_h, ceil(ori_w / 32)].  raw=True rejects, before anything is enqueued, images whose padded shape falls
+    outside the arena's shapes (800x1344 / 1344x800 for the default rule: aspect ratios beyond about 24:1) and resizes
+    that shrink more than conv.PIL_MAX_DOWNSCALE times on an axis.
 
-    batch=B > 1 (raw mode only): every forward runs B images of ONE padded shape through batch-B bucket engines (the
+    batch=B > 1 (raw images only): every forward runs B images of ONE padded shape through batch-B bucket engines (the
     throughput mode of the 544x544 configs).  Each image is uploaded into its slot's staging as soon as it is submitted;
     the open batch is dispatched when it holds B images, when the next image has a different padded shape, or on flush().
     Dispatch = geometry rows + source rows + one graph replay + one download of the real images' records.  A partial
@@ -321,9 +353,11 @@ class StreamRunner(object):
     The mask record of a batch-B engine holds B * max * max_ori_h * ceil(max_ori_w / 32) words and is cleared every
     forward: set max_ori_hw to the largest original size expected, not the 2048 x 2048 default."""
 
+    bm_raw = False                                    # benchmark=True, raw=True: raw RGB images, PIL resize on the GPU
+
     def __init__(self, state_dict, in_flight=1, resize=(1333, 800), keep_ratio=True, max_src_hw=(2048, 2048),
                  max_ori_hw=None, min_mask_up=0.5, mean=(102.9801, 115.9465, 122.7717), device='cuda', batch=1,
-                 **engine_kw):
+                 raw=False, **engine_kw):
         self.sd, self.n, self.B = state_dict, int(in_flight), int(batch)
         self.resize, self.keep_ratio, self.mean = tuple(resize), keep_ratio, mean
         self.max_src_hw = tuple(int(v) for v in max_src_hw)
@@ -332,8 +366,15 @@ class StreamRunner(object):
         self.benchmark = bool(engine_kw.get('benchmark', False))
         if self.B < 1:
             raise ValueError('batch must be at least 1, got %d' % self.B)
-        if self.benchmark and self.B > 1:
-            raise ValueError('benchmark=True runners take one preprocessed image per forward (batch=1)')
+        self.bm_raw = bool(raw)
+        if self.bm_raw and not self.benchmark:
+            raise ValueError('raw=True selects raw RGB images for benchmark=True runners; other runners always take raw '
+                             'BGR images')
+        if self.benchmark and self.B > 1 and not self.bm_raw:
+            raise ValueError('benchmark=True runners take one preprocessed image per forward (batch=1); raw=True batches '
+                             'raw images')
+        if self.bm_raw and not keep_ratio:
+            raise ValueError('SipMask-benchmark resizes keep the aspect ratio: keep_ratio=False is not supported')
         self.dev = torch.device(device)
         if self.dev.index is None:
             self.dev = torch.device('cuda', torch.cuda.current_device())
@@ -355,7 +396,7 @@ class StreamRunner(object):
         self.streams = [torch.cuda.Stream(device=self.dev) for _ in range(self.n)]
         self.s_h2d = torch.cuda.Stream(device=self.dev)
         self.s_d2h = torch.cuda.Stream(device=self.dev)
-        if self.benchmark:
+        if self.benchmark and not self.bm_raw:
             ph, pw = max(largest_pad_shapes(self.resize, self.keep_ratio), key=lambda s: s[0] * s[1])
             self.src_elems = 3 * max(ph, pw) ** 2
             self.in_dev = [torch.empty(self.src_elems, dtype=torch.float32, device=self.dev) for _ in range(self.n)]
@@ -403,14 +444,19 @@ class StreamRunner(object):
             t0 = time.perf_counter()
             eng = self._new_engine(hw, self.arenas[k])
             with torch.cuda.stream(self.streams[k]):
-                if self.benchmark:
+                if self.benchmark and not self.bm_raw:
                     eng.forward(None)                  # warm-up + capture
                 else:
-                    eng.forward_raw([torch.zeros((32, 32, 3), dtype=torch.uint8, device=self.dev)] * self.B, self.mean)
+                    eng.forward_raw([torch.zeros((32, 32, 3), dtype=torch.uint8, device=self.dev)] * self.B, self.mean,
+                                    self._pipeline)
             torch.cuda.synchronize(self.dev)
             self.build_seconds.setdefault(hw, []).append(time.perf_counter() - t0)
             self.engines[k][hw] = eng
         return eng
+
+    @property
+    def _pipeline(self):
+        return 'benchmark' if self.bm_raw else 'mmdet'
 
     @property
     def buckets(self):
@@ -424,7 +470,10 @@ class StreamRunner(object):
             h, w = int(src_hw[0]), int(src_hw[1])
             if not (0 < h <= self.max_src_hw[0] and 0 < w <= self.max_src_hw[1]):
                 raise ValueError('image %dx%d exceeds max_src_hw %dx%d' % (h, w, self.max_src_hw[0], self.max_src_hw[1]))
-            img_shape, pad, sf = image_meta(h, w, self.resize, self.keep_ratio)
+            if self.bm_raw:
+                img_shape, pad, sf = self._bm_meta(h, w)
+            else:
+                img_shape, pad, sf = image_meta(h, w, self.resize, self.keep_ratio)
             ori = (h, w, 3)
         else:
             img_shape, ori, sf = meta
@@ -445,6 +494,20 @@ class StreamRunner(object):
             raise ValueError('mask resize step (%g, %g) of the %dx%d image is steeper than min_mask_up=%g allows'
                              % (g.ry, g.rx, ori[0], ori[1], self.min_mask_up))
         return tuple(img_shape), tuple(pad), sf, tuple(ori)
+
+    def _bm_meta(self, h, w):
+        """bm_image_meta of an h x w raw RGB image, or ValueError if the runner cannot serve it."""
+        img_shape, pad, sf = bm_image_meta(h, w, min(self.resize), max(self.resize))
+        if not any(pad[0] <= a and pad[1] <= b for a, b in largest_pad_shapes(self.resize, True)):
+            raise ValueError('image %dx%d: the SipMask-benchmark size rule (short side %d, long side at most %d, aspect kept, '
+                             'padded to 32) gives %dx%d, outside the padded shapes %s the runner serves'
+                             % (h, w, min(self.resize), max(self.resize), pad[0], pad[1],
+                                ' / '.join('%dx%d' % s for s in largest_pad_shapes(self.resize, True))))
+        f = C.PIL_MAX_DOWNSCALE
+        if not (0 < img_shape[0] and 0 < img_shape[1]) or h > f * img_shape[0] or w > f * img_shape[1]:
+            raise ValueError('image %dx%d resized to %dx%d by the SipMask-benchmark size rule shrinks more than %dx on an '
+                             'axis' % (h, w, img_shape[0], img_shape[1], f))
+        return img_shape, pad, sf
 
     def _out(self, k, eng, oris):
         """Slot k's device / pinned host record for the images of a batch with these ori_shapes: per image a dict of
@@ -479,15 +542,16 @@ class StreamRunner(object):
         return dev, host, used
 
     def submit(self, img, meta=None):
-        """img: uint8 BGR HWC host image (pinned for an asynchronous upload), or with meta = (img_shape, ori_shape,
-        scale_factor) an fp32 NCHW [1, 3, H, W] preprocessed image (benchmark=True).  Validates, uploads the image into
-        the open batch's staging and dispatches the batch when it is due (see the class docstring).  Returns the slot
-        (batch=1) or the image's ticket (batch > 1)."""
-        if self.benchmark != (meta is not None):
-            raise ValueError('benchmark=True runners take preprocessed fp32 images with their meta; others raw uint8 images')
+        """img: uint8 BGR HWC host image (pinned for an asynchronous upload; RGB for benchmark=True, raw=True), or with
+        meta = (img_shape, ori_shape, scale_factor) an fp32 NCHW [1, 3, H, W] preprocessed image (benchmark=True without
+        raw).  Validates, uploads the image into the open batch's staging and dispatches the batch when it is due (see the
+        class docstring).  Returns the slot (batch=1) or the image's ticket (batch > 1)."""
+        if (self.benchmark and not self.bm_raw) != (meta is not None):
+            raise ValueError('benchmark=True runners take preprocessed fp32 images with their meta (raw=True: raw uint8 '
+                             'RGB images); others raw uint8 images')
         if meta is None:
             if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
-                raise ValueError('raw input is a uint8 HWC BGR image')
+                raise ValueError('raw input is a uint8 HWC %s image' % ('RGB' if self.bm_raw else 'BGR'))
             img_shape, pad, sf, ori = self.check(img.shape[:2])
         else:
             if img.dtype != torch.float32 or img.dim() != 4 or img.shape[:2] != (1, 3):
@@ -541,11 +605,11 @@ class StreamRunner(object):
         with torch.cuda.stream(cs):
             cs.wait_event(self.ev_in_ready[k])
             eng.set_image_meta(metas + [metas[-1]] * (self.B - nr))      # fillers: the last real image's geometry
-            if self.benchmark:
+            if self.benchmark and not self.bm_raw:
                 eng.img.copy_(images[0]['src'], non_blocking=True)
                 eng.forward(None)
             else:
-                eng.forward_raw([m['src'] for m in images] + [None] * (self.B - nr), self.mean)
+                eng.forward_raw([m['src'] for m in images] + [None] * (self.B - nr), self.mean, self._pipeline)
             self.ev_in_free[k].record(cs)
             cs.wait_event(self.ev_out_free[k])
             if self.ev_hold[k] is not None:
