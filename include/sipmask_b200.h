@@ -137,7 +137,8 @@ int smb_mask_rescore_f16(const void* pos_masks, int n_img, int max_rows, int H, 
 
 /* COCO RLE of bit-packed masks on the device (replaces the per-detection `masks[i].cpu().numpy()` + pycocotools
  * `mask_util.encode(order='F')` tail, sipmask_head.py:645-657; SURVEY.md 8f-1).
- *   mask_bits : [N, mask_h, words] uint32 (pixel x = bit x&31 of word x>>5), cropped to the top-left H x W (= ori_shape)
+ *   mask_bits : [N, mask_h, words] uint32 (pixel x = bit x&31 of word x>>5), cropped to the top-left H x W (= ori_shape),
+ *               any width
  *   n_valid   : device int (number of valid detections, may be NULL = N)
  *   counts    : [N, cap] uint32 run lengths in COLUMN-major order, starting with the zeros run
  *   n_counts  : [N] int32: number of runs, 0 for det >= *n_valid, or -(boundaries+1) if cap was too small */
@@ -146,6 +147,27 @@ int smb_mask_rle_counts(const uint32_t* mask_bits, int N, int mask_h, int words,
 /* HOST helper (plain C, no CUDA): pycocotools' rleToString of `n` run lengths; returns the length written, -1 if cap is
  * too small.  counts is a host pointer. */
 int smb_rle_to_string(const uint32_t* host_counts, int n, char* host_out, int cap);
+
+/* The pycocotools strings of a whole batch of engine records, encoded on the device (two launches, graph-capturable):
+ *   mask_bits : [N, max_num, cap_h, words] uint32 (the engine's record), count: device int [N] (clamped to [0, max_num]),
+ *   geom      : device rows [N]; image n's canvas is (out_h, out_w) of its row (clamped to cap_h x 32*words)
+ *   dst       : DEVICE word holding the address (as the device sees it, see smb_host_device_pointer) of an arena of
+ *               N * img_bytes bytes, read when the kernel runs (0: nothing is written).  Image n's region starts at
+ *               n * img_bytes: int32 header {status, n, off[max_num + 1]} (4 * (max_num + 3) bytes), then the strings of
+ *               its n detections back to back, string i = bytes [off[i], off[i+1]) after the header.
+ *   status    : 0, or SMB_RLE_RUNS_OVERFLOW (a mask has more than run_cap runs) | SMB_RLE_BYTES_OVERFLOW (the strings exceed
+ *               img_bytes - header).  With a non-zero status the strings are not written; nothing is ever written outside
+ *               the image's region.
+ * Every pointer is read when the kernels run, so the rows, counts and destination may change between graph replays.
+ * max_num <= 1024, img_bytes a multiple of 16, workspace >= smb_rle_encode_workspace_bytes(N, max_num, run_cap). */
+#define SMB_RLE_RUNS_OVERFLOW 1
+#define SMB_RLE_BYTES_OVERFLOW 2
+size_t smb_rle_encode_workspace_bytes(int N, int max_num, int run_cap);
+int smb_rle_encode_dev(const uint32_t* mask_bits, int N, int max_num, int cap_h, int words, const int* count,
+                       const smb_img_geom_t* geom, int run_cap, const uint64_t* dst, int img_bytes, void* workspace,
+                       size_t workspace_bytes, smb_stream_t stream);
+/* The device address of page-locked host memory (cudaHostGetDevicePointer), for the dst word above. */
+int smb_host_device_pointer(void* host_ptr, void** dev_ptr_out);
 
 /* Fully fused mask path (sipmask_head.py:609-633,648-654): prototypes -> selected sub-region dot product -> sigmoid ->
  * crop -> bilinear resize to (full_h, full_w) -> `> thr` -> bit-pack into [N,out_h,ceil(out_w/32)] (a memset node zero-fills

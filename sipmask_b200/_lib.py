@@ -67,6 +67,7 @@ SYMBOLS = [
     'smb_upsample_bilinear', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
     'smb_mask_assemble_dev', 'smb_mask_assemble_pack_dev', 'smb_decode_topk_dev', 'smb_pair_decode_topk_dev',
     'smb_gather_track_feats_dev', 'smb_preprocess_u8_s2d_dev', 'smb_preprocess_pil_u8_s2d_dev',
+    'smb_rle_encode_workspace_bytes', 'smb_rle_encode_dev', 'smb_host_device_pointer',
 ]
 
 
@@ -79,7 +80,8 @@ def lib():
         L = ctypes.CDLL(LIB_PATH)
         L.smb_last_error.restype = ctypes.c_char_p
         for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes',
-                  'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes'):
+                  'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes',
+                  'smb_rle_encode_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

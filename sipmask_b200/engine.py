@@ -29,7 +29,8 @@ class SipMaskEngine(object):
                  mask_thr=0.4, use_graph=True, head_only=False, feat_sizes=None, in_channels=256,
                  fcos=False, prefix_head='bbox_head.', build_postproc=True, share_weights=None,
                  max_ctas=None, head_max_ctas=None, backbone_dcn=False, ori_shape=None, legacy_interp=False, vis=False,
-                 rescoring_flag=False, benchmark=False, max_ori_hw=None, min_mask_up=None, arena=None):
+                 rescoring_flag=False, benchmark=False, max_ori_hw=None, min_mask_up=None, arena=None, rle_bytes=0,
+                 rle_runs=None):
         # SipMask-benchmark checkpoints (keys from sipmask_b200.benchmark.convert_state_dict): FrozenBatchNorm without eps,
         # tower / DCN convs with bias before GN, relu'd regression, pair candidates, label-aware NMS, k-th-value cut
         self.benchmark = benchmark
@@ -68,6 +69,14 @@ class SipMaskEngine(object):
         self.mask_cap = tuple(int(v) for v in (max_ori_hw if max_ori_hw is not None else self.ori_shape[:2]))
         # the steepest mask resize the fused mask kernel's tile is sized for (None: this engine's own scale_factor)
         self.min_mask_up = min_mask_up
+        # COCO RLE strings of every detection, encoded on the device at the end of each forward (rle_bytes > 0: the string
+        # bytes per image of the destination region; rle_runs: the runs one mask may have, default 4 * max width + 2)
+        self.rle_bytes = int(rle_bytes)
+        self.rle_runs = None if rle_runs is None else int(rle_runs)
+        if self.rle_bytes < 0 or (self.rle_runs is not None and self.rle_runs < 1):
+            raise ValueError('rle_bytes must be >= 0 and rle_runs >= 1')
+        if self.rle_bytes and (fcos or not build_postproc):
+            raise ValueError('rle_bytes > 0 encodes the post-processing record: it needs build_postproc=True')
         # activations, workspaces and outputs carved from a caller-owned uint8 device tensor (engines that share one never
         # run concurrently); arena_bytes is what this engine needs of it (counted without an arena too)
         self._arena = arena
@@ -568,6 +577,63 @@ class SipMaskEngine(object):
         if self.rescoring:
             self._add(lambda: ops.mask_rescore_f16(self.pos_masks, self.count, self._rescore_w, self.labels, self.det,
                                                    workspace=self._rescore_ws, out=self.mask_scores), 5, name='rescore')
+        if self.rle_bytes:
+            self._build_rle(cap_h, cap_w)
+
+    def _build_rle(self, cap_h, cap_w):
+        """The encoder node after the per-image chains: every detection's pycocotools string, written per image into the
+        region the destination word points at (smb_rle_encode_dev).  The workspace lives in the arena (rewritten each
+        forward before it is read); the destination word and the default region persist between forwards, outside it."""
+        from . import rle as R
+        N, mx = self.N, self.max_num
+        if mx > 1024:
+            raise ValueError('rle_bytes > 0 supports at most 1024 detections per image, got max_per_img=%d' % mx)
+        if self.rle_runs is None:
+            self.rle_runs = 4 * cap_w + 2
+        self.rle_img_bytes = R.image_bytes(mx, self.rle_bytes)
+        ws = self._t(ops.rle_encode_workspace_bytes(N, mx, self.rle_runs), dtype=torch.uint8)
+        self._rle_dst = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self._rle_stage = {}                         # region address -> (pinned word holding its device address, region)
+        self.rle_region = torch.zeros(N * self.rle_img_bytes, dtype=torch.uint8).pin_memory()
+        self.set_rle_dest(self.rle_region)
+        torch.cuda.current_stream(self.dev).synchronize()
+        geom = self.geom
+
+        def encode():
+            ops.rle_encode_dev(self.mask_bits, self.count, geom, self._rle_dst, self.rle_img_bytes, self.rle_runs, ws)
+        self._add(encode, 2, name='rle_encode')
+
+    def set_rle_dest(self, region):
+        """Points the next forwards on the current stream at `region`, a pinned uint8 host tensor of at least
+        N * rle_img_bytes bytes (image n's region at n * rle_img_bytes).  Stream-ordered like set_image_meta: the device
+        word the encoder reads is written by an H2D copy on the current stream, from a pinned word that holds the region's
+        device address and never changes, so no host wait is needed and the region stays referenced by the engine."""
+        if not self.rle_bytes:
+            raise ValueError('set_rle_dest: this engine was built without rle_bytes')
+        if (region.dtype != torch.uint8 or region.dim() != 1 or region.is_cuda or not region.is_pinned()
+                or region.numel() < self.N * self.rle_img_bytes or region.data_ptr() % 16):
+            raise ValueError('set_rle_dest: need a 16-byte aligned, pinned 1-D uint8 host tensor of at least %d bytes'
+                             % (self.N * self.rle_img_bytes))
+        key = region.data_ptr()
+        if key not in self._rle_stage:
+            with torch.cuda.device(self.dev):
+                addr = ops.host_device_pointer(region)
+            self._rle_stage[key] = (torch.tensor([addr], dtype=torch.int64).pin_memory(), region)
+        self._rle_dst.copy_(self._rle_stage[key][0], non_blocking=True)
+        self._rle_region_cur = region
+
+    def rle_results(self):
+        """Per image, the list of its count RLE dicts {'size': [ori_h, ori_w], 'counts': bytes} in detection order (the
+        layout pycocotools.mask.encode returns), read from the region the last forward wrote.  Valid once the stream has
+        passed that forward.  An image whose strings did not fit (rle_runs / rle_bytes) is encoded on the host from this
+        engine's mask_bits instead."""
+        from . import rle as R
+        ib, out = self.rle_img_bytes, []
+        region = self._rle_region_cur.numpy()
+        for n, (_, ori, _) in enumerate(self.image_metas):
+            out.append(R.image_segms(region[n * ib:(n + 1) * ib], self.max_num, ori[:2],
+                                     lambda k, n=n: self.mask_bits[n, :k].cpu().numpy()))
+        return out
 
     def _geometry(self, img_shape, ori_shape, scale_factor):
         from .postproc import image_geometry

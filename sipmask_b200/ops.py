@@ -517,6 +517,33 @@ def masks_to_rle(mask_bits, H, W, k, cap=8192):
     return [{'size': [int(H), int(W)], 'counts': rle_to_string(c_host[j, :n_host[j]])} for j in range(k)]
 
 
+def rle_encode_workspace_bytes(N, max_num, run_cap):
+    return int(L.lib().smb_rle_encode_workspace_bytes(int(N), int(max_num), int(run_cap)))
+
+
+@L.device_guard
+def rle_encode_dev(mask_bits, count, geom, dst_word, img_bytes, run_cap, workspace):
+    """smb_rle_encode_dev: the pycocotools strings of every detection of a batch of records, packed per image into the
+    arena whose device address the int64 device word dst_word holds (see rle.read_region for the layout).
+    mask_bits int32 [N, max_num, cap_h, words], count int32 [N], geom the engine's geometry rows [N, words of a row]."""
+    _need_cuda(mask_bits, count, geom, dst_word, workspace)
+    assert mask_bits.dtype == torch.int32 and mask_bits.is_contiguous() and mask_bits.dim() == 4
+    assert count.dtype == torch.int32 and dst_word.dtype == torch.int64 and workspace.dtype == torch.uint8
+    N, mx, cap_h, words = mask_bits.shape
+    L.check(L.lib().smb_rle_encode_dev(L.ptr(mask_bits), N, mx, cap_h, words, L.ptr(count), L.ptr(geom), int(run_cap),
+                                       L.ptr(dst_word), int(img_bytes), L.ptr(workspace), ctypes.c_size_t(workspace.numel()),
+                                       L.stream_ptr()), 'smb_rle_encode_dev')
+
+
+def host_device_pointer(pinned):
+    """The device address of a page-locked host tensor (cudaHostGetDevicePointer), for the current device."""
+    if not pinned.is_pinned():
+        raise ValueError('host_device_pointer: the tensor is not in page-locked memory')
+    out = ctypes.c_void_p(0)
+    L.check(L.lib().smb_host_device_pointer(ctypes.c_void_p(pinned.data_ptr()), ctypes.byref(out)), 'smb_host_device_pointer')
+    return int(out.value)
+
+
 @L.device_guard
 def conv3x3s2_relu(x, weight, bias):
     """One `convs_scoring` ConvModule (sipmask_head.py:200-214): NCHW fp32 conv3x3 stride 2 pad 0 + bias + ReLU."""

@@ -31,6 +31,17 @@ def _tuning(n):
     return dict(max_ctas=cap, head_max_ctas=cap, min_tiles=16)
 
 
+def _masks_mode(masks):
+    """True for masks='rle' (COCO RLE strings encoded on the device), False for masks='bits' (bit planes)."""
+    if masks not in ('bits', 'rle'):
+        raise ValueError("masks is 'bits' or 'rle', got %r" % (masks,))
+    return masks == 'rle'
+
+
+# string bytes per image of a masks='rle' runner's regions unless rle_bytes is given
+DEFAULT_RLE_BYTES = 1 << 16
+
+
 def make_engines(state_dict, img_hw, in_flight=1, **kw):
     """n engines for n images in flight (weights shared, activations private)."""
     tune = _tuning(in_flight)
@@ -115,12 +126,21 @@ class EnginePool(object):
 
 class PipelinedRunner(object):
     """raw_hw=(h, w): the host hands over the decoder's uint8 BGR HWC image (h*w*3 bytes H2D instead of 4*3*H*W) and the
-    step starts with the fused resize / normalise / pad kernel (engine.forward_raw, SURVEY 8f-3)."""
+    step starts with the fused resize / normalise / pad kernel (engine.forward_raw, SURVEY 8f-3).
 
-    def __init__(self, engines, depth=2, raw_hw=None):
+    masks='rle' (engines built with rle_bytes > 0): every slot owns a pinned region the engine's encoder writes the COCO RLE
+    strings into during the forward (set_rle_dest before each replay, so slots that share one engine and graph still own
+    their region); the bit planes are not downloaded.  result() then carries 'segms' (per image of the forward, the list of
+    RLE dicts) in place of 'bits'.  The bit planes stay in the slot's device record, from which an image whose strings
+    overflowed the encoder's capacities is encoded on the host."""
+
+    def __init__(self, engines, depth=2, raw_hw=None, masks='bits'):
         self.engs = list(engines) if isinstance(engines, (list, tuple)) else [engines]
         self.n = len(self.engs)
         self.eng = engine = self.engs[0]
+        self.rle = _masks_mode(masks)
+        if self.rle and not all(e.rle_bytes for e in self.engs):
+            raise ValueError("masks='rle' needs engines built with rle_bytes > 0")
         # one staging slot per engine when several images are in flight, `depth` slots for a single engine
         self.nslots = self.n if self.n > 1 else depth
         ns = self.nslots
@@ -143,7 +163,12 @@ class PipelinedRunner(object):
         if engine.rescoring:                      # SipMask++: the mask scores travel with the record
             for o in self.out_dev:
                 o['msc'] = torch.empty_like(engine.mask_scores)
-        self.out_host = [{k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in o.items()} for o in self.out_dev]
+        # rle: the planes stay on the device (the overflow fallback's copy), the strings arrive in the slot's region
+        self.out_host = [{k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in o.items()
+                          if not (self.rle and k == 'bits')} for o in self.out_dev]
+        if self.rle:
+            self.rle_regions = [torch.zeros(engine.N * engine.rle_img_bytes, dtype=torch.uint8).pin_memory() for _ in range(ns)]
+            self.slot_oris = [None] * ns
         self.ev_in_ready = [torch.cuda.Event() for _ in range(ns)]      # H2D of slot finished
         self.ev_in_free = [torch.cuda.Event() for _ in range(ns)]       # compute consumed the slot's input
         self.ev_out_ready = [torch.cuda.Event() for _ in range(ns)]     # compute wrote the slot's output
@@ -152,7 +177,8 @@ class PipelinedRunner(object):
         self.i = 0
         self.pending = []
         self.h2d_bytes = self.in_dev[0].numel() * self.in_dev[0].element_size()
-        self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.out_dev[0].values())
+        # fixed-size downloads per forward (rle: plus the strings and headers the encoder writes, which vary per image)
+        self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.out_host[0].values())
         cur = torch.cuda.current_stream(dev)
         if self.n > 1:
             for st, eng in zip(self.s_comp, self.engs):
@@ -188,6 +214,9 @@ class PipelinedRunner(object):
             self.ev_in_ready[k].record(self.s_h2d)
         with torch.cuda.stream(cs):
             cs.wait_event(self.ev_in_ready[k])
+            if self.rle:
+                eng.set_rle_dest(self.rle_regions[k])      # this slot's strings go to this slot's region
+                self.slot_oris[k] = [m[1][:2] for m in eng.image_metas]
             if self.raw:
                 eng.forward_raw(self.in_dev[k])            # preprocess kernel reads the staged uint8 image, then the graph
                 self.ev_in_free[k].record(cs)
@@ -210,7 +239,7 @@ class PipelinedRunner(object):
             self.ev_out_ready[k].record(cs)
         with torch.cuda.stream(self.s_d2h):
             self.s_d2h.wait_event(self.ev_out_ready[k])
-            for name in o:
+            for name in self.out_host[k]:
                 self.out_host[k][name].copy_(o[name], non_blocking=True)
             self.ev_out_free[k].record(self.s_d2h)
         self.i += 1
@@ -251,9 +280,19 @@ class PipelinedRunner(object):
         self.join()
 
     def result(self, slot):
-        """Blocks until the slot's download finished; returns pinned host tensors (valid until the slot is reused)."""
+        """Blocks until the slot's download finished; returns pinned host tensors (valid until the slot is reused).
+        masks='rle': a dict of them with 'segms' (one list of RLE dicts per image of the forward) in place of 'bits'."""
         self.ev_out_free[slot].synchronize()
-        return self.out_host[slot]
+        if not self.rle:
+            return self.out_host[slot]
+        from . import rle as R
+        eng = self.engs[slot % self.n]
+        ib, bits = eng.rle_img_bytes, self.out_dev[slot]['bits']
+        region = self.rle_regions[slot].numpy()
+        rec = dict(self.out_host[slot])
+        rec['segms'] = [R.image_segms(region[i * ib:(i + 1) * ib], eng.max_num, ori, lambda k, i=i: bits[i, :k].cpu().numpy())
+                        for i, ori in enumerate(self.slot_oris[slot])]
+        return rec
 
     def join(self):
         """Make the current stream wait for the downloads (and so for every image in flight)."""
@@ -351,13 +390,25 @@ class StreamRunner(object):
     batch is completed with filler images (all-zero canvases with the last real image's geometry) that are computed but
     never returned.  submit() returns a ticket (the image's index in the stream) and result(ticket) that image's record.
     The mask record of a batch-B engine holds B * max * max_ori_h * ceil(max_ori_w / 32) words and is cleared every
-    forward: set max_ori_hw to the largest original size expected, not the 2048 x 2048 default."""
+    forward: set max_ori_hw to the largest original size expected, not the 2048 x 2048 default.
+
+    masks='rle': the engines encode every detection's COCO RLE string on the device (rle_bytes string bytes per image,
+    default DEFAULT_RLE_BYTES) into a pinned region each slot owns, shared by the slot's bucket engines; the bit planes are
+    neither copied nor downloaded.  result() returns 'segms' (the image's list of RLE dicts {'size': [ori_h, ori_w],
+    'counts': bytes}) in place of mask_bits; an image whose strings overflowed the encoder's capacities is encoded on the
+    host from the bucket engine's planes, which stay valid until the slot is reused.  consume() hands fn the device record
+    without mask_bits."""
 
     bm_raw = False                                    # benchmark=True, raw=True: raw RGB images, PIL resize on the GPU
 
     def __init__(self, state_dict, in_flight=1, resize=(1333, 800), keep_ratio=True, max_src_hw=(2048, 2048),
                  max_ori_hw=None, min_mask_up=0.5, mean=(102.9801, 115.9465, 122.7717), device='cuda', batch=1,
-                 raw=False, **engine_kw):
+                 raw=False, masks='bits', **engine_kw):
+        self.rle = _masks_mode(masks)
+        if self.rle:
+            engine_kw.setdefault('rle_bytes', DEFAULT_RLE_BYTES)
+            if int(engine_kw['rle_bytes']) <= 0:
+                raise ValueError("masks='rle' needs rle_bytes > 0")
         self.sd, self.n, self.B = state_dict, int(in_flight), int(batch)
         self.resize, self.keep_ratio, self.mean = tuple(resize), keep_ratio, mean
         self.max_src_hw = tuple(int(v) for v in max_src_hw)
@@ -405,6 +456,7 @@ class StreamRunner(object):
             self.src_elems = self.max_src_hw[0] * self.max_src_hw[1] * 3
             self.in_dev = [torch.empty(self.B * self.src_elems, dtype=torch.uint8, device=self.dev) for _ in range(self.n)]
         self.out_dev, self.out_host = [], []
+        self.rle_regions = [None] * self.n                # masks='rle': per slot, the pinned region of its batch's strings
         self.ev_in_ready, self.ev_in_free, self.ev_out_ready, self.ev_out_free = ([torch.cuda.Event() for _ in range(self.n)]
                                                                                   for _ in range(4))
         self.ev_hold = [None] * self.n
@@ -513,8 +565,9 @@ class StreamRunner(object):
         """Slot k's device / pinned host record for the images of a batch with these ori_shapes: per image a dict of
         views, and per field the number of elements the images use (a prefix of the slot's flat buffers)."""
         mx = eng.max_num
-        spec = dict(det=((mx, 5), torch.float32), lab=((mx,), torch.long), cnt=((1,), torch.int32), idx=((mx,), torch.long),
-                    bits=(None, torch.int32))
+        spec = dict(det=((mx, 5), torch.float32), lab=((mx,), torch.long), cnt=((1,), torch.int32), idx=((mx,), torch.long))
+        if not self.rle:
+            spec['bits'] = (None, torch.int32)
         if eng.vis:
             spec['trk'] = ((mx, 512), torch.float32)
         if eng.rescoring:
@@ -531,7 +584,8 @@ class StreamRunner(object):
         dev, host = [], []
         for oh, ow in oris:
             shape = dict((n, s) for n, (s, d) in spec.items())
-            shape['bits'] = (mx, oh, (ow + 31) // 32)
+            if 'bits' in shape:
+                shape['bits'] = (mx, oh, (ow + 31) // 32)
             dev.append({})
             host.append({})
             for n, sh in shape.items():
@@ -605,6 +659,10 @@ class StreamRunner(object):
         with torch.cuda.stream(cs):
             cs.wait_event(self.ev_in_ready[k])
             eng.set_image_meta(metas + [metas[-1]] * (self.B - nr))      # fillers: the last real image's geometry
+            if self.rle:
+                if self.rle_regions[k] is None:
+                    self.rle_regions[k] = torch.zeros(self.B * eng.rle_img_bytes, dtype=torch.uint8).pin_memory()
+                eng.set_rle_dest(self.rle_regions[k])
             if self.benchmark and not self.bm_raw:
                 eng.img.copy_(images[0]['src'], non_blocking=True)
                 eng.forward(None)
@@ -626,8 +684,9 @@ class StreamRunner(object):
             if 'msc' in flat:
                 flat['msc'][:used['msc']].view(nr, mx).copy_(eng.mask_scores[:nr])
             for j, (m, o) in enumerate(zip(images, dev)):
-                oh, wq = o['bits'].shape[1:]
-                o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
+                if 'bits' in o:
+                    oh, wq = o['bits'].shape[1:]
+                    o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
             self.ev_out_ready[k].record(cs)
         with torch.cuda.stream(self.s_d2h):
             self.s_d2h.wait_event(self.ev_out_ready[k])
@@ -651,7 +710,9 @@ class StreamRunner(object):
 
     @staticmethod
     def _record(o):
-        rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'], idxs_keep=o['idx'], mask_bits=o['bits'])
+        rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'], idxs_keep=o['idx'])
+        if 'bits' in o:
+            rec['mask_bits'] = o['bits']
         if 'trk' in o:
             rec['track_feats'] = o['trk']
         if 'msc' in o:
@@ -697,11 +758,18 @@ class StreamRunner(object):
     def result(self, key):
         """key: the slot submit() returned (batch=1) or the image's ticket (batch > 1).  Blocks until the download
         finished; returns the pinned host record (det_bboxes, det_labels, count, idxs_keep, mask_bits [max, ori_h,
-        ceil(ori_w / 32)], track_feats / mask_scores when enabled) and the image's meta.  Valid until the slot is reused."""
+        ceil(ori_w / 32)], track_feats / mask_scores when enabled) and the image's meta.  Valid until the slot is reused.
+        masks='rle': segms (the image's RLE dicts, in detection order) in place of mask_bits."""
         k, j = (key, 0) if self.B == 1 else self._locate(key)
         self.ev_out_free[k].synchronize()
         m = self.slot_images[k][j]
         rec = self._record(m['host'])
+        if self.rle:
+            from . import rle as R
+            eng = self.engines[k][m['pad_shape'][:2]]
+            ib = eng.rle_img_bytes
+            rec['segms'] = R.image_segms(self.rle_regions[k].numpy()[j * ib:(j + 1) * ib], eng.max_num, m['ori_shape'][:2],
+                                         lambda n: eng.mask_bits[j, :n].cpu().numpy())
         rec['meta'] = dict(img_shape=m['img_shape'], pad_shape=m['pad_shape'], ori_shape=m['ori_shape'],
                            scale_factor=m['scale_factor'])
         return rec
