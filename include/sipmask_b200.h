@@ -327,6 +327,32 @@ int smb_track_step(const float* host_det, const int64_t* host_labels, const floa
                    float* host_prev_det, int64_t* host_prev_labels, float* host_prev_feats, int n_prev, int capacity,
                    const float* host_match_coeff3, int32_t* host_ids_out);
 
+/* The same association on the DEVICE for every frame of a batch, one launch (graph-capturable).  Each video runs on a lane
+ * whose tracker state is caller-owned device memory:
+ *   state_boxes [lanes, capacity, 5] f32, state_labels [lanes, capacity] i64, state_feats [lanes, capacity, 512] f32,
+ *   n_obj [lanes] i32 (the number of tracked objects; -1: no state yet), status [lanes] i32 (bits are OR-ed in).
+ * Frame r of the batch is frames[r] (device rows); its record is det [N, max_num, 5], labels [N, max_num],
+ * count [N] (clamped to [0, max_num]), track_feats [N, max_num, 512]; ids [N, max_num] receives its object ids.
+ * The rows of one lane are associated in batch order, each exactly as smb_track_step associates a frame:
+ *   - count 0: ids -1, state unchanged (even with is_first: the reference returns before the tracker);
+ *   - is_first, or n_obj < 0: the state becomes the frame's detections, ids 0..n-1;
+ *   - otherwise the comp matrix against the n_obj tracked objects, first maximum per row, appends and best claims.
+ * An object appended beyond capacity is not stored: its detection gets id -1 and status[lane] |= SMB_TRACK_CAPACITY.
+ * Rows whose lane is outside [0, lanes) (lane < 0: a filler) touch no state and get ids -1.  ids past a row's count are -1.
+ * Every pointer is read when the kernel runs; n_obj is clamped to [-1, capacity].  Feature arrays 16-byte aligned,
+ * max_num <= 1024, workspace >= smb_track_assoc_workspace_bytes(lanes, max_num, capacity). */
+#define SMB_TRACK_FEAT_DIM 512
+#define SMB_TRACK_CAPACITY 1
+typedef struct {
+  int32_t lane;      /* the video's lane, < 0: filler row */
+  int32_t is_first;  /* non-zero: the video's first frame (the reference's img_meta['is_first']) */
+} smb_track_frame_t;
+size_t smb_track_assoc_workspace_bytes(int lanes, int max_num, int capacity);
+int smb_track_assoc_dev(const smb_track_frame_t* frames, int N, const float* det, const int64_t* labels, const int* count,
+                        const float* track_feats, int max_num, float* state_boxes, int64_t* state_labels, float* state_feats,
+                        int* n_obj, int* status, int lanes, int capacity, const float* host_match_coeff3, int32_t* ids,
+                        void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
 /* gather rows: dst[i,:] = src[idx[i],:] for i < *count (device count), zero otherwise. */
 int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev,
                         int max_rows, int row_elems, float* dst, smb_stream_t stream);

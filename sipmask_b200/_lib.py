@@ -48,6 +48,14 @@ class RawSrc(ctypes.Structure):
                 ('dst_h', ctypes.c_int), ('dst_w', ctypes.c_int), ('mean', ctypes.c_float * 3)]
 
 
+class TrackFrame(ctypes.Structure):
+    """smb_track_frame_t: one frame row of a device tracker association (include/sipmask_b200.h)."""
+    _fields_ = [('lane', ctypes.c_int32), ('is_first', ctypes.c_int32)]
+
+
+TRACK_CAPACITY = 1                   # SMB_TRACK_CAPACITY: a lane had more tracked objects than its capacity
+
+
 class RescoreWeights(ctypes.Structure):
     _fields_ = [('conv_w', ctypes.c_void_p * 6), ('conv_b', ctypes.c_void_p * 6), ('score_w', ctypes.c_void_p),
                 ('score_b', ctypes.c_void_p), ('num_classes', ctypes.c_int)]
@@ -68,6 +76,7 @@ SYMBOLS = [
     'smb_mask_assemble_dev', 'smb_mask_assemble_pack_dev', 'smb_decode_topk_dev', 'smb_pair_decode_topk_dev',
     'smb_gather_track_feats_dev', 'smb_preprocess_u8_s2d_dev', 'smb_preprocess_pil_u8_s2d_dev',
     'smb_rle_encode_workspace_bytes', 'smb_rle_encode_dev', 'smb_host_device_pointer',
+    'smb_track_assoc_workspace_bytes', 'smb_track_assoc_dev',
 ]
 
 
@@ -81,7 +90,7 @@ def lib():
         L.smb_last_error.restype = ctypes.c_char_p
         for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes',
                   'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes',
-                  'smb_rle_encode_workspace_bytes'):
+                  'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

@@ -535,6 +535,53 @@ def rle_encode_dev(mask_bits, count, geom, dst_word, img_bytes, run_cap, workspa
                                        L.stream_ptr()), 'smb_rle_encode_dev')
 
 
+def track_assoc_workspace_bytes(lanes, max_num, capacity):
+    return int(L.lib().smb_track_assoc_workspace_bytes(int(lanes), int(max_num), int(capacity)))
+
+
+@L.device_guard
+def track_assoc(frames, det, labels, count, track_feats, state, match_coeff=(1.0, 2.0, 10.0), ids=None, workspace=None):
+    """smb_track_assoc_dev: the tracker association of a batch of frame records on the device, in one launch.
+    frames int32 [N, 2] device rows (lane, is_first); det [N, max, 5] f32, labels [N, max] int64, count int32 [N],
+    track_feats [N, max, 512] f32; state = dict(boxes [lanes, cap, 5] f32, labels [lanes, cap] int64,
+    feats [lanes, cap, 512] f32, n_obj int32 [lanes], status int32 [lanes]), updated in place.  Returns ids int32 [N, max]."""
+    _need_cuda(frames, det, labels, count, track_feats)
+    N, mx = det.shape[0], det.shape[1]
+    lanes, cap = state['boxes'].shape[0], state['boxes'].shape[1]
+    assert frames.dtype == torch.int32 and tuple(frames.shape) == (N, 2) and frames.is_contiguous()
+    assert det.dtype == torch.float32 and tuple(det.shape) == (N, mx, 5) and det.is_contiguous()
+    assert labels.dtype == torch.int64 and tuple(labels.shape) == (N, mx) and labels.is_contiguous()
+    assert count.dtype == torch.int32 and count.numel() == N and count.is_contiguous()
+    assert track_feats.dtype == torch.float32 and tuple(track_feats.shape) == (N, mx, 512) and track_feats.is_contiguous()
+    want = dict(boxes=((lanes, cap, 5), torch.float32), labels=((lanes, cap), torch.int64),
+                feats=((lanes, cap, 512), torch.float32), n_obj=((lanes,), torch.int32), status=((lanes,), torch.int32))
+    for name, (shape, dtype) in want.items():
+        t = state[name]
+        if t.device != det.device or t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError('track_assoc: state[%r] must be a contiguous %s %s tensor on %s, got %s %s on %s'
+                             % (name, dtype, list(shape), det.device, t.dtype, list(t.shape), t.device))
+    for name, t in (('frames', frames), ('labels', labels), ('count', count), ('track_feats', track_feats)):
+        if t.device != det.device:
+            raise ValueError('track_assoc: %s is on %s, det on %s' % (name, t.device, det.device))
+    if ids is None:
+        ids = torch.empty((N, mx), dtype=torch.int32, device=det.device)
+    if ids.device != det.device or ids.dtype != torch.int32 or tuple(ids.shape) != (N, mx) or not ids.is_contiguous():
+        raise ValueError('track_assoc: ids must be a contiguous int32 [%d, %d] tensor on %s' % (N, mx, det.device))
+    need = track_assoc_workspace_bytes(lanes, mx, cap)
+    if workspace is None:
+        workspace = torch.empty(need, dtype=torch.uint8, device=det.device)
+    if (workspace.device != det.device or workspace.dtype != torch.uint8 or not workspace.is_contiguous()
+            or workspace.numel() < need):
+        raise ValueError('track_assoc: workspace must be a contiguous uint8 tensor of >= %d bytes on %s' % (need, det.device))
+    coef = (ctypes.c_float * 3)(*[float(np.float32(c)) for c in match_coeff])
+    L.check(L.lib().smb_track_assoc_dev(L.ptr(frames), N, L.ptr(det), L.ptr(labels), L.ptr(count), L.ptr(track_feats), mx,
+                                        L.ptr(state['boxes']), L.ptr(state['labels']), L.ptr(state['feats']),
+                                        L.ptr(state['n_obj']), L.ptr(state['status']), lanes, cap, coef, L.ptr(ids),
+                                        L.ptr(workspace), ctypes.c_size_t(workspace.numel()), L.stream_ptr()),
+            'smb_track_assoc_dev')
+    return ids
+
+
 def host_device_pointer(pinned):
     """The device address of a page-locked host tensor (cudaHostGetDevicePointer), for the current device."""
     if not pinned.is_pinned():

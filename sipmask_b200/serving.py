@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import conv as C
+from ._lib import TRACK_CAPACITY, SmbError
 from .engine import SipMaskEngine
 
 # grid cap / planner min_tiles per number of images in flight
@@ -688,13 +689,18 @@ class StreamRunner(object):
                     oh, wq = o['bits'].shape[1:]
                     o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
             self.ev_out_ready[k].record(cs)
+        self._download(k, used, images)
+        for m, o, h in zip(images, dev, host):
+            m['dev'], m['host'] = o, h
+
+    def _download(self, k, used, images):
+        """Enqueue the download of slot k's record (the first used[name] elements of every field) once its batch is done."""
+        flat = self.out_dev[k]
         with torch.cuda.stream(self.s_d2h):
             self.s_d2h.wait_event(self.ev_out_ready[k])
             for name, n in used.items():
                 self.out_host[k][name][:n].copy_(flat[name][:n], non_blocking=True)
             self.ev_out_free[k].record(self.s_d2h)
-        for m, o, h in zip(images, dev, host):
-            m['dev'], m['host'] = o, h
 
     def consume(self, slot, fn):
         """Run fn(record on the device) on the CURRENT stream for every image of the slot's batch, in submission order,
@@ -773,3 +779,180 @@ class StreamRunner(object):
         rec['meta'] = dict(img_shape=m['img_shape'], pad_shape=m['pad_shape'], ori_shape=m['ori_shape'],
                            scale_factor=m['scale_factor'])
         return rec
+
+
+# SipMask-VIS test configuration (SipMask-VIS/configs/sipmask/sipmask_r50_caffe_fpn_gn_1x.py)
+VIS_ENGINE_KW = dict(vis=True, stacked_convs=3, num_classes=41,
+                     test_cfg=dict(nms_pre=200, score_thr=0.03, nms=dict(type='nms', iou_thr=0.5), max_per_img=10))
+
+
+class VideoRunner(StreamRunner):
+    """Serves videos from a SipMask-VIS checkpoint: StreamRunner's frames (any size, batches, resize on the GPU) plus the
+    tracker association on the device after every batch, and YouTube-VIS results (tools/test_video.py ->
+    results2json_videoseg).
+
+    submit(frame, video_id, frame_id) -> ticket.  A new video starts at frame 0 and takes the lowest free lane of the
+    device tracker (tracker.LaneTracker, one tracker state per lane); every later frame must follow the previous one.
+    end_video(video_id) frees the lane; its tracker state stays, so that, as in the reference's single tracker, the next
+    video on the lane carries it over when its first frame has no detections.  With lanes=1 and the videos submitted in
+    dataset order the runner therefore reproduces test_video.py's sequential state.  A new video that takes over a lane
+    whose previous video still has frames in the open batch dispatches that batch first, so each lane belongs to one
+    video per launch.  Otherwise frames of any videos share batches as in StreamRunner.
+
+    Streams.  Once a batch's record is in the slot's device buffers (ev_out_ready), one tracker stream, shared by all
+    slots, associates the batch's frames (one smb_track_assoc_dev launch) and writes their object ids; batches are
+    dispatched in submission order, so this stream runs every video's frames in order whatever slot they ran in.  The
+    slot's download waits for the association, so the slot is not reused before the association has read its record.
+    The tracking features stay on the device: the download is the record without them, the ids and the lanes' status.
+
+    result(ticket) -> the frame's record (without track_feats) plus obj_ids [count] int32, segms (masks='rle') or
+    mask_bits ('bits'), and frame, the reference's per-frame pair (ytvis.frame_result).  Valid until the next batch opens
+    in the frame's slot.
+    An association that overflowed max_objects on the frame's lane raises SmbError naming the video.
+    video_json(video_id) -> the video's results2json_videoseg entries (ytvis.video_json), once the video has ended and
+    its frames are dispatched.  The runner keeps every frame's pair until then (before a slot takes a new batch, the
+    frames it holds are read into their videos) and forgets the video afterwards, so its video_id may be served again.
+    For a video whose lane overflowed max_objects, video_json forgets the video and raises SmbError."""
+
+    def __init__(self, state_dict, lanes=8, batch=1, in_flight=6, resize=(640, 360), keep_ratio=True,
+                 max_src_hw=(1920, 1920), max_ori_hw=None, masks='rle', max_objects=4096, match_coeff=(1.0, 2.0, 10.0),
+                 **engine_kw):
+        from .tracker import LaneTracker
+        from .ytvis import VideoBook
+        for k, v in VIS_ENGINE_KW.items():
+            engine_kw.setdefault(k, v)
+        if not engine_kw['vis']:
+            raise ValueError('VideoRunner serves SipMask-VIS checkpoints: vis=False is not supported')
+        super(VideoRunner, self).__init__(state_dict, in_flight=in_flight, resize=resize, keep_ratio=keep_ratio,
+                                          max_src_hw=max_src_hw, max_ori_hw=max_ori_hw, batch=batch, masks=masks, **engine_kw)
+        self.num_classes = int(engine_kw['num_classes'])
+        self.tracker = LaneTracker(lanes, max_objects, match_coeff, self.dev, max_rows=self.B, depth=2 * self.n + 2)
+        self.book = VideoBook(lanes)
+        self.s_trk = torch.cuda.Stream(device=self.dev)
+        self.s_trk.wait_stream(torch.cuda.current_stream(self.dev))        # the lanes' initial state
+        self.ev_assoc = [torch.cuda.Event() for _ in range(self.n)]
+        self.ids_dev, self.ids_host = [None] * self.n, [None] * self.n
+        self.status_dev = [torch.zeros(self.tracker.lanes, dtype=torch.int32, device=self.dev) for _ in range(self.n)]
+        self.status_host = [torch.zeros(self.tracker.lanes, dtype=torch.int32).pin_memory() for _ in range(self.n)]
+        self.rows = {}                      # ticket -> (lane, is_first, video_id, frame_id)
+        self.frames = {}                    # video_id -> {frame_id: the frame's (det, seg) pair}
+        self.overflowed = set()             # videos with an association beyond max_objects
+        self._unread = set()                # dispatched tickets whose pair is not in self.frames yet
+
+    def submit(self, img, video_id, frame_id):
+        """img: uint8 BGR HWC host frame of video_id (pinned for an asynchronous upload).  Raises ValueError before
+        anything is enqueued for a frame out of order, a new video when every lane is busy, or an image the runner cannot
+        serve.  Returns the frame's ticket."""
+        lane, first = self.book.check(video_id, frame_id)
+        if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
+            raise ValueError('raw input is a uint8 HWC BGR image')
+        self.check(img.shape[:2])
+        if first and self._open is not None and any(self.rows[m['ticket']][0] == lane for m in self._open['images']):
+            self._dispatch()                                # the lane's previous video still has frames in the open batch
+        t = self.i
+        self.rows[t] = (lane, first, video_id, int(frame_id))
+        try:
+            super(VideoRunner, self).submit(img)
+        except Exception:
+            del self.rows[t]
+            raise
+        self.book.commit(video_id, frame_id, t)
+        return t
+
+    def step(self, *args, **kwargs):
+        raise TypeError('VideoRunner: use submit(frame, video_id, frame_id) and result(ticket)')
+
+    def end_video(self, video_id):
+        """The video has no more frames: its lane is free for the next new video (the lane's state stays)."""
+        self.book.end(video_id)
+
+    def _begin(self, k, hw):
+        # a batch opens in slot k: read the frames the slot still holds first (an RLE overflow falls back to the bucket
+        # engine's planes, and building a new padded-shape engine runs a warm-up forward in the slot's arena); from here on
+        # the slot no longer holds them
+        self._read_slot(k)
+        for m in self.slot_images[k]:
+            del self.rows[m['ticket']]
+        self.slot_images[k] = []
+        super(VideoRunner, self)._begin(k, hw)
+
+    def _launch(self, k, pad, images):
+        super(VideoRunner, self)._launch(k, pad, images)
+        self._unread.update(m['ticket'] for m in images)
+
+    def _download(self, k, used, images):
+        nr = len(images)
+        mx = used['lab'] // nr
+        if self.ids_dev[k] is None:
+            self.ids_dev[k] = torch.empty((self.B, mx), dtype=torch.int32, device=self.dev)
+            self.ids_host[k] = torch.empty((self.B, mx), dtype=torch.int32).pin_memory()
+        flat, st, trk = self.out_dev[k], self.s_trk, self.tracker
+        with torch.cuda.stream(st):
+            st.wait_event(self.ev_out_ready[k])
+            trk.associate([self.rows[m['ticket']][:2] for m in images], flat['det'][:nr * mx * 5].view(nr, mx, 5),
+                          flat['lab'][:nr * mx].view(nr, mx), flat['cnt'][:nr], flat['trk'][:nr * mx * 512].view(nr, mx, 512),
+                          ids=self.ids_dev[k][:nr])
+            self.status_dev[k].copy_(trk.status)            # this launch's status bits, then clear them for the next
+            trk.status.zero_()
+            self.ev_assoc[k].record(st)
+        with torch.cuda.stream(self.s_d2h):
+            self.s_d2h.wait_event(self.ev_assoc[k])
+            for name, n in used.items():
+                if name != 'trk':                           # the tracking features stay on the device
+                    self.out_host[k][name][:n].copy_(flat[name][:n], non_blocking=True)
+            self.ids_host[k][:nr].copy_(self.ids_dev[k][:nr], non_blocking=True)
+            self.status_host[k].copy_(self.status_dev[k], non_blocking=True)
+            self.ev_out_free[k].record(self.s_d2h)
+
+    def _read(self, k, j):
+        """Frame j of slot k's batch (downloaded): its record with obj_ids, segms / mask_bits and frame; records the
+        frame's pair for its video."""
+        from . import rle as R
+        from .ytvis import frame_result
+        m = self.slot_images[k][j]
+        rec = StreamRunner.result(self, k if self.B == 1 else m['ticket'])
+        rec.pop('track_feats', None)
+        lane, _, video_id, frame_id = self.rows[m['ticket']]
+        cnt = int(rec['count'].reshape(-1)[0])
+        rec['obj_ids'] = self.ids_host[k][j, :cnt]
+        segms = rec['segms'] if self.rle else R.encode_planes(rec['mask_bits'][:cnt].numpy(), m['ori_shape'][:2])
+        rec['frame'] = frame_result(rec['det_bboxes'][:cnt].numpy(), rec['det_labels'][:cnt].numpy(),
+                                    rec['obj_ids'].numpy(), segms, self.num_classes)
+        if int(self.status_host[k][lane]) & TRACK_CAPACITY:
+            self.overflowed.add(video_id)
+        if m['ticket'] in self._unread:
+            self._unread.discard(m['ticket'])
+            self.frames.setdefault(video_id, {})[frame_id] = rec['frame']
+        return rec, video_id
+
+    def _read_slot(self, k):
+        for j, m in enumerate(self.slot_images[k]):
+            if m['ticket'] in self._unread:
+                self._read(k, j)
+
+    def result(self, ticket):
+        k, j = self._locate(ticket)
+        rec, video_id = self._read(k, j)
+        if video_id in self.overflowed:
+            self._raise_overflow(video_id)
+        return rec
+
+    def _raise_overflow(self, video_id):
+        raise SmbError('video %r: more than max_objects=%d tracked objects on its lane' % (video_id, self.tracker.capacity))
+
+    def video_json(self, video_id):
+        """The video's YouTube-VIS result entries (results2json_videoseg), with video_id as given to submit."""
+        from .ytvis import video_json
+        v = self.book.videos.get(video_id)
+        if v is None or not v['ended']:
+            raise ValueError('video %r has not ended: end_video() first' % (video_id,))
+        if self._open is not None and any(m['ticket'] in v['frames'] for m in self._open['images']):
+            raise ValueError('video %r has frames in the open batch: flush() dispatches them' % (video_id,))
+        for k in range(self.n):
+            self._read_slot(k)
+        got = self.frames.pop(video_id, {})            # the runner forgets the video, also when it overflowed
+        del self.book.videos[video_id]
+        if video_id in self.overflowed:
+            self.overflowed.discard(video_id)
+            self._raise_overflow(video_id)
+        return video_json(video_id, [got[f] for f in range(len(v['frames']))])

@@ -118,3 +118,65 @@ class Tracker(object):
                     self.prev_roi_feats[obj] = feats[i]
                     self.prev_bboxes[obj] = det[i]
         return ids
+
+
+class LaneTracker(object):
+    """The association on the DEVICE (smb_track_assoc_dev): `lanes` videos, each with its tracker state in device memory
+    (boxes [lanes, capacity, 5], labels [lanes, capacity], features [lanes, capacity, 512], n_obj [lanes] (-1: no state
+    yet), status [lanes]).  associate() enqueues one launch for a batch of frame records on the current stream; the frame
+    rows go through pinned staging (a ring of `depth` buffers, each reused only after the event of its last launch) and one
+    stream-ordered H2D copy, as the engine's geometry rows do.  Nothing here waits for the device except that reuse."""
+
+    def __init__(self, lanes, capacity=4096, match_coeff=(1.0, 2.0, 10.0), device='cuda', max_rows=64, depth=16):
+        import torch
+        self.lanes, self.capacity, self.max_rows = int(lanes), int(capacity), int(max_rows)
+        if self.lanes < 1 or self.capacity < 1 or self.max_rows < 1:
+            raise ValueError('LaneTracker: lanes, capacity and max_rows must be positive')
+        self.match_coeff = tuple(float(np.float32(c)) for c in match_coeff)
+        self.dev = torch.device(device)
+        if self.dev.index is None:
+            self.dev = torch.device('cuda', torch.cuda.current_device())
+        L, C = self.lanes, self.capacity
+        self.boxes = torch.zeros((L, C, 5), dtype=torch.float32, device=self.dev)
+        self.labels = torch.zeros((L, C), dtype=torch.int64, device=self.dev)
+        self.feats = torch.zeros((L, C, 512), dtype=torch.float32, device=self.dev)
+        self.n_obj = torch.full((L,), -1, dtype=torch.int32, device=self.dev)
+        self.status = torch.zeros((L,), dtype=torch.int32, device=self.dev)
+        self.state = dict(boxes=self.boxes, labels=self.labels, feats=self.feats, n_obj=self.n_obj, status=self.status)
+        self._host = [torch.empty((self.max_rows, 2), dtype=torch.int32).pin_memory() for _ in range(depth)]
+        self._rows = [torch.empty((self.max_rows, 2), dtype=torch.int32, device=self.dev) for _ in range(depth)]
+        self._ev = [None] * depth
+        self._i = 0
+        self._ws = {}                                  # max_num -> workspace
+
+    def associate(self, rows, det, labels, count, track_feats, ids=None):
+        """rows: one (lane, is_first) per frame of the batch (lane < 0: a filler, skipped); det [N, max, 5], labels
+        [N, max] int64, count int32 [N], track_feats [N, max, 512] on the device.  Enqueues the association on the current
+        stream and returns ids int32 [N, max] (written when it runs)."""
+        import torch
+        from . import ops
+        n = len(rows)
+        if n > self.max_rows:
+            raise ValueError('LaneTracker: %d frame rows, max_rows is %d' % (n, self.max_rows))
+        for lane, _ in rows:
+            if int(lane) >= self.lanes:
+                raise ValueError('LaneTracker: lane %d of %d' % (int(lane), self.lanes))
+        s = self._i % len(self._host)
+        self._i += 1
+        if self._ev[s] is not None:
+            self._ev[s].synchronize()                  # the launch that last read this staging has run
+        host, dev = self._host[s], self._rows[s]
+        h = host.numpy()
+        for r, (lane, first) in enumerate(rows):
+            h[r, 0], h[r, 1] = int(lane), int(bool(first))
+        dev[:n].copy_(host[:n], non_blocking=True)
+        mx = det.shape[1]
+        ws = self._ws.get(mx)
+        if ws is None:
+            ws = self._ws[mx] = torch.empty(ops.track_assoc_workspace_bytes(self.lanes, mx, self.capacity),
+                                            dtype=torch.uint8, device=self.dev)
+        ids = ops.track_assoc(dev[:n], det, labels, count, track_feats, self.state, self.match_coeff, ids=ids, workspace=ws)
+        if self._ev[s] is None:
+            self._ev[s] = torch.cuda.Event()
+        self._ev[s].record(torch.cuda.current_stream(self.dev))
+        return ids
