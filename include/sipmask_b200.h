@@ -353,6 +353,106 @@ int smb_track_assoc_dev(const smb_track_frame_t* frames, int N, const float* det
                         int* n_obj, int* status, int lanes, int capacity, const float* host_match_coeff3, int32_t* ids,
                         void* workspace, size_t workspace_bytes, smb_stream_t stream);
 
+/* ------------------------------------------------------------------ COCO box / mask AP (pycocotools 2.0 COCOeval)
+ * bbox and segm evaluation with the default parameters: 10 IoU thresholds, 101 recall thresholds, 4 area ranges,
+ * maxDets 1 / 10 / 100.  Masks are bit planes in the image's h x w canvas (pixel x = bit x&31 of word x>>5).
+ *
+ * Detection row, as the result json carries it: xywh box, score[0] = bbox score, score[1] = segm score, area_box = w * h
+ * (loadRes), the plane's word offset in the detection planes, its pixel count (maskUtils.area), the category index
+ * (-1: none) and ext = {row0, row1, word0, word1} (half-open) of its set bits. */
+typedef struct {
+  double box[4];
+  double score[2];
+  double area_box;
+  int64_t plane;
+  int32_t area_mask;
+  int32_t cat;
+  int32_t ext[4];
+  int32_t order;   /* the detection's position in the result json (ties of equal scores keep this order) */
+  int32_t pad;
+} smb_coco_det_t;
+/* Ground-truth row: bbox, the annotation's own area, plane offset, annotation id, iscrowd, pixel count, extents. */
+typedef struct {
+  double box[4];
+  double area;
+  int64_t plane;
+  int64_t id;
+  int32_t crowd;
+  int32_t area_mask;
+  int32_t ext[4];
+} smb_coco_gt_t;
+/* One image of a match launch: canvas, row pitches (words) of its detection and ground-truth planes, number of detection
+ * rows (the record path writes it), image id, and its first output row. */
+typedef struct {
+  int32_t h, w;
+  int32_t det_pitch, gt_pitch;
+  int32_t n_det, pad;
+  int64_t image_id;
+  int64_t out_off;
+} smb_coco_img_t;
+/* Per detection and metric: score, image, matched / ignored bits (bit t*4 + a), category index (K: not evaluated) and its
+ * rank by score inside its (image, category) (-1: not evaluated). */
+typedef struct {
+  double score;
+  int64_t image_id;
+  uint64_t matched;
+  uint64_t ignored;
+  int32_t cat;
+  int32_t rank;
+} smb_coco_out_t;
+#define SMB_COCO_T 10
+#define SMB_COCO_R 101
+#define SMB_COCO_A 4
+#define SMB_COCO_MAX_DET 100
+#define SMB_COCO_DET_CAP 4096
+#define SMB_COCO_MAX_CATS 2048
+#define SMB_COCO_LABEL_RANGE 1   /* status: a record label outside [0, num_labels) */
+#define SMB_COCO_CAPACITY 2      /* status: an output row outside [0, n_out) */
+
+/* HOST helpers (plain C++, no CUDA), pycocotools maskApi.c restated:
+ *   smb_coco_poly_counts     : rleFrPoly's run lengths of one polygon of k vertices (*host_n = their number; written
+ *                              when it is <= cap)
+ *   smb_coco_poly_to_bits    : the same polygon OR-ed into a bit plane (merge of several polygons = union)
+ *   smb_coco_rle_to_bits     : column-major run lengths (zeros first) OR-ed into a bit plane; SMB_EINVAL unless they
+ *                              cover h * w pixels exactly
+ *   smb_coco_rle_from_string : rleFrString of a compressed counts string (*host_n = the number of counts, at most len;
+ *                              written when it is <= cap; SMB_EINVAL on a malformed string)
+ *   smb_coco_plane_stats     : {pixel count, row0, row1, word0, word1} of an h x w plane */
+int smb_coco_poly_counts(const double* host_xy, int k, int h, int w, uint32_t* host_counts, int cap, int* host_n);
+int smb_coco_poly_to_bits(const double* host_xy, int k, int h, int w, uint32_t* host_plane, int pitch);
+int smb_coco_rle_to_bits(const uint32_t* host_counts, int n, int h, int w, uint32_t* host_plane, int pitch);
+int smb_coco_rle_from_string(const char* host_s, int len, uint32_t* host_counts, int cap, int* host_n);
+int smb_coco_plane_stats(const uint32_t* host_plane, int h, int w, int pitch, int32_t* host_stats5);
+
+/* Detection rows [N, max_num] of a batch of engine records, identical to what coco.coco_json writes: MM boxes
+ * (x2 - x1) + 1 in float64, BM boxes resized by the float32 ratio out / img of the geometry row with TO_REMOVE = 1 in
+ * float32; segm score = mask_scores (MM only, may be NULL); category = label_cat[label] (a label outside [0, num_labels)
+ * gives -1 and sets SMB_COCO_LABEL_RANGE in *status).  The planes are mask_bits' [cap_h, words] planes cropped to the
+ * geometry row's (out_h, out_w).  imgs[n].n_det = clamp(count[n], 0, max_num). */
+int smb_coco_det_from_record_dev(const float* det, const int64_t* labels, const int* count, const float* mask_scores,
+                                 const uint32_t* mask_bits, int N, int max_num, int cap_h, int words,
+                                 const smb_img_geom_t* geom, const int32_t* label_cat, int num_labels, int benchmark,
+                                 smb_coco_det_t* rows, smb_coco_img_t* imgs, int* status, smb_stream_t stream);
+/* computeIoU + evaluateImg (maxDet 100) of every (image, category) with a ground truth or a detection, one CTA per image:
+ *   dets [n_img, det_cap] (image b's rows b*det_cap + [0, n_det)), gts: rows of image b's category k are
+ *   [gt_cat_off[b*(K+1)+k], gt_cat_off[b*(K+1)+k+1]) in annotation order; metric 0 = bbox, 1 = segm.
+ *   host_iou_thr[10], host_area_rng[4][2] (float64, as COCOeval's Params hold them).
+ *   out: row imgs[b].out_off + j for detection j of image b (every row [0, n_det) of the image is written);
+ *   npig [K, 4]: non-ignored ground truths are added (int atomics).
+ * det_cap <= SMB_COCO_DET_CAP, K <= SMB_COCO_MAX_CATS, workspace >= smb_coco_match_workspace_bytes(n_gt). */
+size_t smb_coco_match_workspace_bytes(int n_gt);
+int smb_coco_match_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                       const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt,
+                       const uint32_t* gt_planes, int64_t gt_plane_words, const int32_t* gt_cat_off, int K, int metric,
+                       const double* host_iou_thr, const double* host_area_rng, smb_coco_out_t* out, int64_t n_out,
+                       int* npig, int* status, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+/* accumulate: rows sorted by (category, score descending, image id, rank), category k's rows [cat_off[k], cat_off[k+1]);
+ * rec_thr[101] device float64; precision / scores [10, 101, K, 4, 3], recall [10, K, 4, 3] float64 (pycocotools layout),
+ * -1 where a (category, area range) has no non-ignored ground truth. */
+int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K, const int* npig,
+                            const double* rec_thr, const int* host_max_dets3, double* precision, double* recall,
+                            double* scores, smb_stream_t stream);
+
 /* gather rows: dst[i,:] = src[idx[i],:] for i < *count (device count), zero otherwise. */
 int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev,
                         int max_rows, int row_elems, float* dst, smb_stream_t stream);

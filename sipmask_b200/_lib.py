@@ -77,6 +77,9 @@ SYMBOLS = [
     'smb_gather_track_feats_dev', 'smb_preprocess_u8_s2d_dev', 'smb_preprocess_pil_u8_s2d_dev',
     'smb_rle_encode_workspace_bytes', 'smb_rle_encode_dev', 'smb_host_device_pointer',
     'smb_track_assoc_workspace_bytes', 'smb_track_assoc_dev',
+    'smb_coco_poly_counts', 'smb_coco_poly_to_bits', 'smb_coco_rle_to_bits', 'smb_coco_rle_from_string',
+    'smb_coco_plane_stats', 'smb_coco_det_from_record_dev', 'smb_coco_match_workspace_bytes', 'smb_coco_match_dev',
+    'smb_coco_accumulate_dev',
 ]
 
 
@@ -90,7 +93,7 @@ def lib():
         L.smb_last_error.restype = ctypes.c_char_p
         for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes',
                   'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes',
-                  'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes'):
+                  'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes', 'smb_coco_match_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

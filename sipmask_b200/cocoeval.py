@@ -1,0 +1,513 @@
+"""COCO box and mask AP on the device: pycocotools 2.0 COCOeval (iouType 'bbox' / 'segm', default Params) as MM's
+CocoDataset.evaluate (SipMask-mmdetection/mmdet/datasets/coco.py:290-392) and SipMask-benchmark's coco_eval.py run it.
+
+Host: the ground truth (CocoGroundTruth: pycocotools COCO's indexing, annToRLE through the library's C restatement of
+rleFrPoly / rleFrString) and summarize (numpy, the code of COCOeval.summarize).  Device (csrc/cocoeval.cu): the result
+json's values from the engine record, computeIoU + evaluateImg for every (image, category) after every batch, and
+accumulate's precision / recall / scores arrays at evaluate().
+
+Restated only: pycocotools is neither vendored in the reference nor installed where this was written, so the semantics
+are pycocotools 2.0's as read from its source, not pinned by running it.
+"""
+import ctypes
+
+import numpy as np
+import torch
+
+from . import _lib as L
+
+DET_DTYPE = np.dtype([('box', '<f8', (4,)), ('score', '<f8', (2,)), ('area_box', '<f8'), ('plane', '<i8'),
+                      ('area_mask', '<i4'), ('cat', '<i4'), ('ext', '<i4', (4,)), ('order', '<i4'), ('pad', '<i4')])
+GT_DTYPE = np.dtype([('box', '<f8', (4,)), ('area', '<f8'), ('plane', '<i8'), ('id', '<i8'), ('crowd', '<i4'),
+                     ('area_mask', '<i4'), ('ext', '<i4', (4,))])
+IMG_DTYPE = np.dtype([('h', '<i4'), ('w', '<i4'), ('det_pitch', '<i4'), ('gt_pitch', '<i4'), ('n_det', '<i4'),
+                      ('pad', '<i4'), ('image_id', '<i8'), ('out_off', '<i8')])
+OUT_DTYPE = np.dtype([('score', '<f8'), ('image_id', '<i8'), ('matched', '<u8'), ('ignored', '<u8'), ('cat', '<i4'),
+                      ('rank', '<i4')])
+assert (DET_DTYPE.itemsize, GT_DTYPE.itemsize, IMG_DTYPE.itemsize, OUT_DTYPE.itemsize) == (96, 80, 40, 40)
+
+# COCOeval Params (iouType 'segm' / 'bbox'), as float64 data
+IOU_THRS = np.linspace(.5, 0.95, int(np.round((0.95 - .5) / .05)) + 1, endpoint=True)
+REC_THRS = np.linspace(.0, 1.00, int(np.round((1.00 - .0) / .01)) + 1, endpoint=True)
+MAX_DETS = [1, 10, 100]
+AREA_RNG = [[0 ** 2, 1e5 ** 2], [0 ** 2, 32 ** 2], [32 ** 2, 96 ** 2], [96 ** 2, 1e5 ** 2]]
+AREA_RNG_LBL = ['all', 'small', 'medium', 'large']
+METRIC_ITEMS = ['mAP', 'mAP_50', 'mAP_75', 'mAP_s', 'mAP_m', 'mAP_l']
+DET_CAP = 4096                       # SMB_COCO_DET_CAP: detections of one image in one launch
+MAX_CATS = 2048                      # SMB_COCO_MAX_CATS
+LABEL_RANGE, CAPACITY = 1, 2         # status bits
+
+
+def _ptr(a):
+    return a.ctypes.data_as(ctypes.c_void_p)
+
+
+# ---------------------------------------------------------------------------------------------------- host RLE / masks
+def string_to_counts(s):
+    """pycocotools rleFrString: a compressed counts string (str or bytes) -> uint32 run lengths."""
+    b = s.encode() if isinstance(s, str) else bytes(s)
+    out = np.zeros(len(b) + 1, np.uint32)                   # every count takes at least one character
+    n = ctypes.c_int(0)
+    if L.lib().smb_coco_rle_from_string(b, len(b), _ptr(out), out.size, ctypes.byref(n)) != 0:
+        raise ValueError('malformed RLE string: %s' % L.lib().smb_last_error().decode())
+    return out[:n.value]
+
+
+def poly_counts(xy, h, w):
+    """rleFrPoly's run lengths of one polygon [x0, y0, x1, y1, ...] in an h x w canvas (the C restatement)."""
+    xy = np.asarray(xy, dtype=np.float64).reshape(-1)
+    xy = np.ascontiguousarray(xy[:xy.size // 2 * 2])
+    k, n = xy.size // 2, ctypes.c_int(0)
+    L.check(L.lib().smb_coco_poly_counts(_ptr(xy), k, int(h), int(w), None, 0, ctypes.byref(n)), 'smb_coco_poly_counts')
+    out = np.zeros(max(n.value, 1), np.uint32)
+    L.check(L.lib().smb_coco_poly_counts(_ptr(xy), k, int(h), int(w), _ptr(out), out.size, ctypes.byref(n)),
+            'smb_coco_poly_counts')
+    return out[:n.value]
+
+
+def _check_size(rle, h, w, what):
+    size = rle.get('size')
+    if not isinstance(size, (list, tuple)) or len(size) != 2 or [int(size[0]), int(size[1])] != [h, w]:
+        raise ValueError('%s: RLE size %r differs from the image canvas %dx%d' % (what, size, h, w))
+
+
+def _or_counts(plane, cnts, h, w, what):
+    cnts = np.ascontiguousarray(np.asarray(cnts, dtype=np.int64))
+    if cnts.ndim != 1 or (cnts.size and (cnts.min() < 0 or cnts.max() > 0xffffffff)):
+        raise ValueError('%s: run lengths must be a list of non-negative integers' % what)
+    c = cnts.astype(np.uint32)
+    if L.lib().smb_coco_rle_to_bits(_ptr(c), c.size, h, w, _ptr(plane), plane.shape[1]) != 0:
+        raise ValueError('%s: %s' % (what, L.lib().smb_last_error().decode()))
+
+
+def segm_plane(segm, h, w, what='segmentation'):
+    """COCO.annToRLE of a ground-truth segmentation, as a bit plane [h, ceil(w / 32)] uint32: polygons (frPyObjects + merge,
+    a first element of exactly 4 numbers makes every element a box, frBbox), an uncompressed RLE, or a compressed one."""
+    pitch = (w + 31) // 32
+    plane = np.zeros((h, pitch), np.uint32)
+    lib = L.lib()
+    if isinstance(segm, list):
+        if len(segm) == 0 or not isinstance(segm[0], (list, tuple)):
+            raise ValueError('%s: a polygon list needs lists of coordinates' % what)
+        n0 = len(segm[0])
+        if n0 == 4:                                           # frBbox: [x, y, x, y+h, x+w, y+h, x+w, y]
+            polys = []
+            for bb in segm:
+                if len(bb) != 4:
+                    raise ValueError('%s: boxes must have 4 numbers' % what)
+                x, y, bw, bh = [float(v) for v in bb]
+                xe, ye = x + bw, y + bh
+                polys.append([x, y, x, ye, xe, ye, xe, y])
+        elif n0 > 4:
+            polys = [[float(v) for v in p] for p in segm]
+        else:
+            raise ValueError('%s: input type is not supported (a polygon of %d numbers)' % (what, n0))
+        for p in polys:
+            xy = np.ascontiguousarray(np.asarray(p, dtype=np.float64)[:len(p) // 2 * 2])
+            L.check(lib.smb_coco_poly_to_bits(_ptr(xy), xy.size // 2, h, w, _ptr(plane), pitch), 'smb_coco_poly_to_bits')
+        return plane
+    if not isinstance(segm, dict) or 'counts' not in segm or 'size' not in segm:
+        raise ValueError('%s: not a polygon list or an RLE dict' % what)
+    _check_size(segm, h, w, what)
+    counts = segm['counts']
+    if isinstance(counts, list):
+        _or_counts(plane, counts, h, w, what)
+    elif isinstance(counts, (str, bytes)):
+        _or_counts(plane, string_to_counts(counts), h, w, what)
+    else:
+        raise ValueError('%s: counts must be a list or a string' % what)
+    return plane
+
+
+def plane_stats(plane, w):
+    s = np.zeros(5, np.int32)
+    p = np.ascontiguousarray(plane, dtype=np.uint32)
+    L.check(L.lib().smb_coco_plane_stats(_ptr(p), p.shape[0], int(w), p.shape[1], _ptr(s)), 'smb_coco_plane_stats')
+    return int(s[0]), s[1:].copy()
+
+
+# ---------------------------------------------------------------------------------------------------- ground truth
+class CocoGroundTruth:
+    """A loaded COCO annotation json, indexed as pycocotools' COCO and COCOeval._prepare see it.
+      img_ids : sorted unique image ids (COCOeval.evaluate: np.unique(p.imgIds))
+      cat_ids : sorted category ids (p.catIds = sorted(getCatIds()))
+    Per image, its annotations of those categories in annotation-file order (imgToAnns)."""
+
+    def __init__(self, ann_dict):
+        try:
+            images, cats, anns = ann_dict['images'], ann_dict['categories'], ann_dict['annotations']
+            self.hw = {int(im['id']): (int(im['height']), int(im['width'])) for im in images}
+            self.cat_ids = sorted(int(c['id']) for c in cats)
+        except (KeyError, TypeError, ValueError) as e:
+            raise ValueError('CocoGroundTruth: malformed images / categories: %r' % (e,))
+        if len(set(self.cat_ids)) != len(self.cat_ids) or not 0 < len(self.cat_ids) <= MAX_CATS:
+            raise ValueError('CocoGroundTruth: need 1..%d distinct category ids' % MAX_CATS)
+        self.img_ids = sorted(self.hw)
+        self.cat_index = {c: i for i, c in enumerate(self.cat_ids)}
+        self.anns = {i: [] for i in self.img_ids}
+        for a in anns:
+            try:
+                img, cat = int(a['image_id']), int(a['category_id'])
+                bbox = [float(v) for v in a['bbox']]
+                row = dict(id=int(a['id']), cat=cat, bbox=bbox, area=float(a['area']), iscrowd=int(a['iscrowd']),
+                           segmentation=a.get('segmentation'))
+            except (KeyError, TypeError, ValueError) as e:
+                raise ValueError('CocoGroundTruth: malformed annotation %r: %r' % (a.get('id') if isinstance(a, dict) else a, e))
+            if len(bbox) != 4:
+                raise ValueError('CocoGroundTruth: annotation %d: bbox needs 4 numbers' % row['id'])
+            if img in self.anns and cat in self.cat_index:        # getAnnIds(imgIds=p.imgIds, catIds=p.catIds)
+                self.anns[img].append(row)
+
+    def image(self, img_id, masks=True):
+        """One image's ground truth for a match launch: (rows GT_DTYPE, per-category offsets [K+1], planes [G, h, pitch]
+        or None).  Rows are grouped by category index, annotation order inside a category."""
+        h, w = self.hw[img_id]
+        anns = self.anns[img_id]
+        K = len(self.cat_ids)
+        order = sorted(range(len(anns)), key=lambda i: self.cat_index[anns[i]['cat']])      # stable
+        rows = np.zeros(len(anns), GT_DTYPE)
+        pitch = (w + 31) // 32
+        planes = np.zeros((len(anns), h, pitch), np.uint32) if masks else None
+        cnt = np.zeros(K + 1, np.int32)
+        for r, i in enumerate(order):
+            a = anns[i]
+            rows[r]['box'] = a['bbox']
+            rows[r]['area'] = a['area']
+            rows[r]['id'] = a['id']
+            rows[r]['crowd'] = a['iscrowd']
+            cnt[self.cat_index[a['cat']] + 1] += 1
+            if masks:
+                if a['segmentation'] is None:
+                    raise ValueError('CocoGroundTruth: annotation %d has no segmentation' % a['id'])
+                planes[r] = segm_plane(a['segmentation'], h, w, 'annotation %d' % a['id'])
+                area, ext = plane_stats(planes[r], w)
+                rows[r]['area_mask'] = area
+                rows[r]['ext'] = ext
+        return rows, np.cumsum(cnt).astype(np.int32), planes
+
+
+# ---------------------------------------------------------------------------------------------------- summarize (host)
+def summarize(precision, recall):
+    """COCOeval.summarize's 12 stats of the accumulated arrays (its _summarize / _summarizeDets code)."""
+    iouThrs, maxDets, areaRngLbl = IOU_THRS, MAX_DETS, AREA_RNG_LBL
+
+    def _summarize(ap=1, iouThr=None, areaRng='all', maxDets=100):
+        aind = [i for i, aRng in enumerate(areaRngLbl) if aRng == areaRng]
+        mind = [i for i, mDet in enumerate(MAX_DETS) if mDet == maxDets]
+        if ap == 1:
+            s = precision
+            if iouThr is not None:
+                t = np.where(iouThr == iouThrs)[0]
+                s = s[t]
+            s = s[:, :, :, aind, mind]
+        else:
+            s = recall
+            if iouThr is not None:
+                t = np.where(iouThr == iouThrs)[0]
+                s = s[t]
+            s = s[:, :, aind, mind]
+        if len(s[s > -1]) == 0:
+            mean_s = -1
+        else:
+            mean_s = np.mean(s[s > -1])
+        return mean_s
+
+    stats = np.zeros((12,))
+    stats[0] = _summarize(1)
+    stats[1] = _summarize(1, iouThr=.5, maxDets=maxDets[2])
+    stats[2] = _summarize(1, iouThr=.75, maxDets=maxDets[2])
+    stats[3] = _summarize(1, areaRng='small', maxDets=maxDets[2])
+    stats[4] = _summarize(1, areaRng='medium', maxDets=maxDets[2])
+    stats[5] = _summarize(1, areaRng='large', maxDets=maxDets[2])
+    stats[6] = _summarize(0, maxDets=maxDets[0])
+    stats[7] = _summarize(0, maxDets=maxDets[1])
+    stats[8] = _summarize(0, maxDets=maxDets[2])
+    stats[9] = _summarize(0, areaRng='small', maxDets=maxDets[2])
+    stats[10] = _summarize(0, areaRng='medium', maxDets=maxDets[2])
+    stats[11] = _summarize(0, areaRng='large', maxDets=maxDets[2])
+    return stats
+
+
+def mm_results(metric, stats):
+    """CocoDataset.evaluate's entries of one metric: rounded stats[:6] and the copypaste string."""
+    out = {}
+    for i, item in enumerate(METRIC_ITEMS):
+        out['{}_{}'.format(metric, item)] = float('{:.3f}'.format(stats[i]))
+    out['{}_mAP_copypaste'.format(metric)] = ('{ap[0]:.3f} {ap[1]:.3f} {ap[2]:.3f} {ap[3]:.3f} '
+                                             '{ap[4]:.3f} {ap[5]:.3f}').format(ap=stats[:6])
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------- evaluator
+def _dev_bytes(arr, dev):
+    return torch.from_numpy(np.ascontiguousarray(arr).view(np.uint8).reshape(-1)).to(dev)
+
+
+class CocoEvaluator:
+    """Device state of one COCO evaluation: per evaluated image, its detections' matched / ignored flags (per metric),
+    and npig per (category, area range).  Images are added as engine records (add_records) or result lists
+    (add_results); evaluate() accumulates and summarizes.
+      gt      : CocoGroundTruth
+      cat_ids : COCO category id per 0-based record label (as coco.coco_json takes it)
+      benchmark: SipMask-benchmark records (BoxList.resize boxes, box scores for segm)."""
+
+    def __init__(self, gt, cat_ids, metrics=('bbox', 'segm'), benchmark=False, device=None):
+        metrics = [metrics] if isinstance(metrics, str) else list(metrics)
+        for m in metrics:
+            if m not in ('bbox', 'segm'):
+                raise KeyError('metric {} is not supported'.format(m))
+        self.gt, self.metrics, self.benchmark = gt, metrics, bool(benchmark)
+        self.dev = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
+        self.K = len(gt.cat_ids)
+        self.label_cat_host = np.array([gt.cat_index.get(int(c), -1) for c in cat_ids], np.int32)
+        self.label_cat = torch.from_numpy(self.label_cat_host).to(self.dev)
+        self.npig = {m: torch.zeros(self.K * 4, dtype=torch.int32, device=self.dev) for m in metrics}
+        self.rows = {m: [] for m in metrics}
+        self.status = torch.zeros(1, dtype=torch.int32, device=self.dev)
+        self.n_results = {m: torch.zeros((), dtype=torch.int64, device=self.dev) for m in metrics}
+        self.image_ids = []
+        self._seen = set()
+        self._iou_thr = np.ascontiguousarray(IOU_THRS, dtype=np.float64)
+        self._area_rng = np.ascontiguousarray(np.array(AREA_RNG, dtype=np.float64).reshape(-1))
+
+    # ---- bookkeeping
+    def _claim(self, image_ids, ori_hws=None):
+        ids = [int(i) for i in image_ids]
+        for n, i in enumerate(ids):
+            if i not in self.gt.hw:
+                raise ValueError('image id %d is not in the ground truth' % i)
+            if i in self._seen or ids.count(i) > 1:
+                raise ValueError('image id %d is evaluated twice' % i)
+            if ori_hws is not None and tuple(int(v) for v in ori_hws[n][:2]) != self.gt.hw[i]:
+                raise ValueError('image %d: ori_shape %r differs from the annotation %dx%d'
+                                 % (i, tuple(ori_hws[n][:2]), self.gt.hw[i][0], self.gt.hw[i][1]))
+        return ids
+
+    def stage_gt(self, image_id, stream=None):
+        """Rasterize one image's ground truth on the host and upload it from pinned memory on `stream` (default: the
+        current stream).  Returns its device tensors, for add_records(..., gts=[...]) on a stream that is ordered after
+        `stream`."""
+        rows, off, planes = self.gt.image(int(image_id), 'segm' in self.metrics)
+        if planes is not None and len(rows):
+            rows['plane'] = np.arange(len(rows), dtype=np.int64) * planes[0].size
+        n_gt = len(rows)
+        host = dict(rows=torch.from_numpy(np.ascontiguousarray(rows).view(np.uint8).reshape(-1) if n_gt
+                                          else np.zeros(GT_DTYPE.itemsize, np.uint8)),
+                    off=torch.from_numpy(off),
+                    planes=torch.from_numpy(planes.reshape(-1).view(np.int32) if planes is not None and planes.size
+                                            else np.zeros(1, np.int32)))
+        stream = stream or torch.cuda.current_stream(self.dev)
+        with torch.cuda.device(self.dev), torch.cuda.stream(stream):
+            dev = {k: v.pin_memory().to(self.dev, non_blocking=True) for k, v in host.items()}
+        dev['n_gt'] = n_gt
+        dev['plane_words'] = int(planes.size) if planes is not None else 0
+        dev['stream'] = stream
+        return dev
+
+    def _match(self, metric, imgs, n, dets, det_cap, det_planes, det_plane_words, gt, out_rows):
+        """The match launch of image n of a batch (imgs / dets: the batch's device rows) on the current stream."""
+        lib = L.lib()
+        cur = torch.cuda.current_stream(self.dev)
+        if gt['stream'] != cur:                          # uploaded on another stream: keep it until this stream is done
+            for key in ('rows', 'off', 'planes'):
+                gt[key].record_stream(cur)
+        ws_bytes = lib.smb_coco_match_workspace_bytes(gt['n_gt'])
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+        n_out = out_rows.numel() // OUT_DTYPE.itemsize
+        L.check(lib.smb_coco_match_dev(ctypes.c_void_p(imgs.data_ptr() + n * IMG_DTYPE.itemsize), 1,
+                                       ctypes.c_void_p(dets.data_ptr() + n * det_cap * DET_DTYPE.itemsize), det_cap,
+                                       L.ptr(det_planes), ctypes.c_int64(det_plane_words), L.ptr(gt['rows']), gt['n_gt'],
+                                       L.ptr(gt['planes']), ctypes.c_int64(gt['plane_words']), L.ptr(gt['off']), self.K,
+                                       0 if metric == 'bbox' else 1, _ptr(self._iou_thr), _ptr(self._area_rng),
+                                       L.ptr(out_rows), ctypes.c_int64(n_out), L.ptr(self.npig[metric]), L.ptr(self.status),
+                                       L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_coco_match_dev')
+
+    def _img_rows(self, ids, det_pitch, det_cap, n_det=None):
+        imgs = np.zeros(len(ids), IMG_DTYPE)
+        for n, i in enumerate(ids):
+            h, w = self.gt.hw[i]
+            imgs[n]['h'], imgs[n]['w'] = h, w
+            imgs[n]['det_pitch'] = det_pitch[n] if hasattr(det_pitch, '__len__') else det_pitch
+            imgs[n]['gt_pitch'] = (w + 31) // 32
+            imgs[n]['n_det'] = 0 if n_det is None else n_det[n]
+            imgs[n]['image_id'] = i
+            imgs[n]['out_off'] = n * det_cap
+        return imgs
+
+    # ---- engine records
+    def check_image(self, image_id, ori_shape):
+        """Raises ValueError unless image_id can be evaluated next with this ori_shape (in the ground truth, not evaluated
+        yet, ori_shape equal to the annotation's height x width)."""
+        self._claim([image_id], [ori_shape])
+
+    def add_records(self, rec, geom, image_ids, ori_shapes, gts=None):
+        """Evaluate the first len(image_ids) images of a batch of engine records (det_bboxes, det_labels, count,
+        mask_bits, mask_scores when present; device tensors of the engine's last forward) on the current stream.
+        geom: the engine's device geometry rows of that forward; ori_shapes: each image's ori_shape (checked against the
+        annotation's height x width); gts: each image's stage_gt (default: staged here on the current stream).  The record
+        may be overwritten once the stream has passed these launches."""
+        with torch.cuda.device(self.dev):
+            ids = self._claim(image_ids, ori_shapes)
+            B = len(ids)
+            if B == 0:
+                return
+            det, labels, count, bits = rec['det_bboxes'], rec['det_labels'], rec['count'], rec['mask_bits']
+            ms = rec.get('mask_scores') if not self.benchmark else None
+            N, max_num, cap_h, words = bits.shape
+            if B > N or det.shape[:2] != (N, max_num) or labels.shape[:2] != (N, max_num) or max_num > DET_CAP:
+                raise ValueError('add_records: %d image ids for a record of %d images x %d detections' % (B, N, max_num))
+            for t, dt in ((det, torch.float32), (labels, torch.int64), (count, torch.int32), (bits, torch.int32),
+                          (geom, torch.int32)):
+                if t.device != self.dev or t.dtype != dt or not t.is_contiguous():
+                    raise ValueError('add_records: record tensors must be contiguous on %s' % self.dev)
+            if ms is not None and (ms.dtype != torch.float32 or ms.shape[:2] != (N, max_num) or not ms.is_contiguous()):
+                raise ValueError('add_records: mask_scores must be a contiguous float32 [N, max_num] tensor')
+            if gts is None:
+                gts = [self.stage_gt(i) for i in ids]
+            lib = L.lib()
+            imgs = _dev_bytes(self._img_rows(ids, words, max_num), self.dev)
+            dets = torch.empty(B * max_num * DET_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+            L.check(lib.smb_coco_det_from_record_dev(L.ptr(det), L.ptr(labels), L.ptr(count), L.ptr(ms), L.ptr(bits), B,
+                                                     max_num, cap_h, words, L.ptr(geom), L.ptr(self.label_cat),
+                                                     len(self.label_cat_host), int(self.benchmark), L.ptr(dets), L.ptr(imgs),
+                                                     L.ptr(self.status), L.stream_ptr()), 'smb_coco_det_from_record_dev')
+            n_json = count[:B].clamp(0, max_num).sum()
+            for m in self.metrics:
+                out = torch.empty(B * max_num * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+                for n in range(B):
+                    self._match(m, imgs, n, dets, max_num, bits, bits.numel(), gts[n], out)
+                self.rows[m].append(out)
+                self.n_results[m] += n_json
+            self.image_ids += ids
+            self._seen.update(ids)
+
+    # ---- result lists
+    def add_results(self, per_image, metric):
+        """Evaluate `metric` of images from result-json entries (dicts with image_id, category_id, score, and bbox or
+        segmentation).  per_image: [(image_id, its entries in list order)].  Used by evaluate_json, one metric at a time,
+        for images it has claimed."""
+        with torch.cuda.device(self.dev):
+            ids = [int(i) for i, _ in per_image]
+            det_cap = max([1] + [len(v) for _, v in per_image])
+            if det_cap > DET_CAP:
+                raise ValueError('add_results: %d results for one image (at most %d)' % (det_cap, DET_CAP))
+            B = len(ids)
+            dets = np.zeros(B * det_cap, DET_DTYPE)
+            dets['cat'] = -1
+            planes, pbase, pitches = [], 0, []
+            n_det = []
+            for n, (i, res) in enumerate(zip(ids, (v for _, v in per_image))):
+                h, w = self.gt.hw[i]
+                pitch = (w + 31) // 32
+                pitches.append(pitch)
+                n_det.append(len(res))
+                for j, r in enumerate(res):
+                    d = dets[n * det_cap + j]
+                    d['order'] = j
+                    try:
+                        score = float(r['score'])
+                        cat = int(r['category_id'])
+                        if metric == 'bbox':
+                            bb = [float(v) for v in r['bbox']]
+                            if len(bb) != 4:
+                                raise ValueError('bbox needs 4 numbers')
+                            d['box'] = bb
+                            d['area_box'] = bb[2] * bb[3]
+                        else:
+                            seg = r['segmentation']
+                            if not isinstance(seg, dict):
+                                raise ValueError('result of image %d: segmentation must be an RLE dict' % i)
+                            p = segm_plane(seg, h, w, 'result of image %d' % i)
+                            area, ext = plane_stats(p, w)
+                            d['area_mask'], d['ext'], d['plane'] = area, ext, pbase
+                            planes.append(p.reshape(-1))
+                            pbase += p.size
+                    except (KeyError, TypeError) as e:
+                        raise ValueError('add_results: malformed result %r: %r' % (r, e))
+                    d['score'][0 if metric == 'bbox' else 1] = score
+                    d['cat'] = self.gt.cat_index.get(cat, -1)
+            imgs = _dev_bytes(self._img_rows(ids, pitches, det_cap, n_det), self.dev)
+            dd = _dev_bytes(dets, self.dev)
+            planes = np.concatenate(planes) if planes else np.zeros(1, np.uint32)
+            pd = torch.from_numpy(planes).to(self.dev)
+            out = torch.empty(B * det_cap * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+            for n, i in enumerate(ids):
+                self._match(metric, imgs, n, dd, det_cap, pd, planes.size, self.stage_gt(i), out)
+            self.rows[metric].append(out)
+
+    # ---- accumulate + summarize
+    def _accumulate(self, metric):
+        K, dev = self.K, self.dev
+        parts = [r.view(torch.int64).view(-1, 5) for r in self.rows[metric]]
+        rows = torch.cat(parts) if parts else torch.zeros((0, 5), dtype=torch.int64, device=dev)
+        score = rows[:, 0].contiguous().view(torch.float64)
+        img = rows[:, 1].contiguous()
+        cat = (rows[:, 4] & 0xffffffff).to(torch.int32)      # little-endian {cat, rank} in the last word
+        rank = (rows[:, 4] >> 32).to(torch.int32)
+        # global order: category, score descending, image id, rank (stable sorts from the last key to the first)
+        o = torch.argsort(rank, stable=True)
+        o = o[torch.argsort(img[o], stable=True)]
+        o = o[torch.argsort(-score[o], stable=True)]
+        o = o[torch.argsort(cat[o], stable=True)]
+        srt = rows[o].contiguous()
+        cat_off = torch.searchsorted(cat[o].contiguous(), torch.arange(K + 1, dtype=torch.int32, device=dev)).to(torch.int32)
+        T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
+        precision = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
+        scores = torch.empty_like(precision)
+        recall = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
+        rec_thr = torch.from_numpy(np.ascontiguousarray(REC_THRS)).to(dev)
+        md = (ctypes.c_int * 3)(*MAX_DETS)
+        L.check(L.lib().smb_coco_accumulate_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K,
+                                                L.ptr(self.npig[metric]), L.ptr(rec_thr), md, L.ptr(precision),
+                                                L.ptr(recall), L.ptr(scores), L.stream_ptr()), 'smb_coco_accumulate_dev')
+        return precision.cpu().numpy(), recall.cpu().numpy(), scores.cpu().numpy()
+
+    def evaluate(self):
+        """Accumulate and summarize every metric.  Returns MM's dict (bbox_mAP, ..., segm_mAP_copypaste) plus
+        'stats' and 'arrays' ({metric: {'precision', 'recall', 'scores'}}) with COCOeval's eval arrays."""
+        with torch.cuda.device(self.dev):
+            status = int(self.status.item())
+            if status & LABEL_RANGE:
+                raise ValueError('a record label is outside the %d labels of cat_ids' % len(self.label_cat_host))
+            if status:
+                raise L.SmbError('COCO evaluation status %d' % status)
+            out, stats, arrays = {}, {}, {}
+            for m in self.metrics:
+                if int(self.n_results[m].item()) == 0:
+                    raise ValueError('%s: the results of the evaluated images are empty' % m)
+                p, r, s = self._accumulate(m)
+                stats[m] = summarize(p, r)
+                arrays[m] = dict(precision=p, recall=r, scores=s)
+                out.update(mm_results(m, stats[m]))
+            out['stats'] = stats
+            out['arrays'] = arrays
+            return out
+
+
+def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None):
+    """COCOeval of result lists (coco.coco_json output or a loaded results file) against `gt` on the device: the same
+    kernels as CocoEvaluator, with the detections' RLE strings decoded on the host.  img_ids: the evaluated images
+    (p.imgIds; default every ground-truth image).  As in pycocotools, a result whose image is not in the ground truth
+    raises (loadRes), and results of ground-truth images outside img_ids are not evaluated (_prepare).  Returns
+    CocoEvaluator.evaluate()'s dict for the metrics given."""
+    metrics = [m for m, j in (('bbox', bbox_json), ('segm', segm_json)) if j is not None]
+    ev = CocoEvaluator(gt, cat_ids, metrics=metrics, device=device)
+    ids = ev._claim(gt.img_ids if img_ids is None else sorted(set(int(i) for i in img_ids)))
+    for m, res in (('bbox', bbox_json), ('segm', segm_json)):
+        if res is None:
+            continue
+        per = {i: [] for i in ids}
+        for r in res:
+            if not isinstance(r, dict) or 'image_id' not in r:
+                raise ValueError('%s results: malformed entry %r' % (m, r))
+            i = int(r['image_id'])
+            if i not in gt.hw:                       # loadRes: 'Results do not correspond to current coco set'
+                raise ValueError('%s results: image %r is not in the ground truth' % (m, r['image_id']))
+            if i in per:
+                per[i].append(r)
+        for c in range(0, len(ids), chunk):
+            ev.add_results([(i, per[i]) for i in ids[c:c + chunk]], m)
+        ev.n_results[m] += len(res)                   # loadRes fails on an empty list
+    ev.image_ids = list(ids)
+    ev._seen.update(ids)
+    return ev.evaluate()

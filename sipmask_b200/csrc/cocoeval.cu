@@ -1,0 +1,627 @@
+// COCO box and mask AP (pycocotools 2.0 COCOeval, iouType 'bbox' / 'segm', default parameters) on the device, plus the
+// host rasterizer of the ground truth (pycocotools maskApi.c rleFrPoly / rleFrString restated).
+//
+//   smb_coco_det_from_record_dev : engine record -> detection rows as the result json carries them (coco.coco_json)
+//   smb_coco_match_dev           : computeIoU + evaluateImg for every (image, category) of a batch of images
+//   smb_coco_accumulate_dev      : accumulate's precision / recall / scores arrays from the globally sorted rows
+//
+// Every float64 operation whose result is compared with pycocotools is an explicit _rn intrinsic, so nvcc cannot
+// contract it into an FMA (x86-64 pycocotools has none).
+#include <math.h>
+#include <limits.h>
+#include <algorithm>
+#include <vector>
+
+#include "common.cuh"
+
+namespace {
+
+constexpr int kT = SMB_COCO_T, kA = SMB_COCO_A, kR = SMB_COCO_R, kMaxDet = SMB_COCO_MAX_DET;
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+
+// ------------------------------------------------------------------------------------------------ 2a: record -> rows
+__global__ void __launch_bounds__(kThreads) det_from_record_kernel(
+    const float* __restrict__ det, const int64_t* __restrict__ labels, const int* __restrict__ count,
+    const float* __restrict__ mask_scores, const uint32_t* __restrict__ mask_bits, int max_num, int cap_h, int words,
+    const smb_img_geom_t* __restrict__ geom, const int32_t* __restrict__ label_cat, int num_labels, int benchmark,
+    smb_coco_det_t* __restrict__ rows, smb_coco_img_t* __restrict__ imgs, int* __restrict__ status) {
+  const int n = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lid = tid & 31;
+  const int cnt = min(max(count[n], 0), max_num);
+  const smb_img_geom_t g = geom[n];
+  const int oh = min(max(g.out_h, 0), cap_h), ow = min(max(g.out_w, 0), words * 32);
+  const int ow_words = (ow + 31) >> 5;
+  const uint32_t last_mask = (ow & 31) ? ((1u << (ow & 31)) - 1u) : 0xffffffffu;
+  if (tid == 0) imgs[n].n_det = cnt;
+  for (int j = warp; j < max_num; j += kWarps) {
+    smb_coco_det_t r;
+    const size_t rj = (size_t)n * max_num + j;
+    const int64_t plane = (int64_t)rj * cap_h * words;
+    // ---- area and extents by popcount over the ori_shape canvas (maskUtils.area)
+    int area = 0, r0 = INT_MAX, r1 = -1, w0 = INT_MAX, w1 = -1;
+    if (j < cnt) {
+      const uint32_t* p = mask_bits + plane;
+      for (int y = 0; y < oh; ++y) {
+        for (int x = lid; x < ow_words; x += 32) {
+          uint32_t v = p[(size_t)y * words + x];
+          if (x == ow_words - 1) v &= last_mask;
+          if (v) { area += __popc(v); r0 = min(r0, y); r1 = max(r1, y); w0 = min(w0, x); w1 = max(w1, x); }
+        }
+      }
+      for (int o = 16; o > 0; o >>= 1) {
+        area += __shfl_xor_sync(0xffffffffu, area, o);
+        r0 = min(r0, __shfl_xor_sync(0xffffffffu, r0, o));
+        r1 = max(r1, __shfl_xor_sync(0xffffffffu, r1, o));
+        w0 = min(w0, __shfl_xor_sync(0xffffffffu, w0, o));
+        w1 = max(w1, __shfl_xor_sync(0xffffffffu, w1, o));
+      }
+    }
+    if (lid != 0) continue;
+    if (j >= cnt) {
+      memset(&r, 0, sizeof(r));
+      r.cat = -1;
+      rows[rj] = r;
+      continue;
+    }
+    const float* d = det + rj * 5;
+    if (benchmark) {
+      // BoxList.resize to the ori_shape canvas: float32 boxes times the float32 ratio (torch scalar arithmetic), then
+      // TO_REMOVE = 1 in float32 (coco_eval.py prepare_for_coco_detection)
+      const float rw = __double2float_rn(__ddiv_rn((double)g.out_w, (double)g.img_w));
+      const float rh = __double2float_rn(__ddiv_rn((double)g.out_h, (double)g.img_h));
+      const float x1 = __fmul_rn(d[0], rw), y1 = __fmul_rn(d[1], rh), x2 = __fmul_rn(d[2], rw), y2 = __fmul_rn(d[3], rh);
+      r.box[0] = x1;
+      r.box[1] = y1;
+      r.box[2] = __fadd_rn(__fsub_rn(x2, x1), 1.0f);
+      r.box[3] = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
+    } else {
+      // MM xyxy2xywh on python floats of the float32 boxes: (x2 - x1) + 1 in float64
+      r.box[0] = d[0];
+      r.box[1] = d[1];
+      r.box[2] = __dadd_rn(__dsub_rn((double)d[2], (double)d[0]), 1.0);
+      r.box[3] = __dadd_rn(__dsub_rn((double)d[3], (double)d[1]), 1.0);
+    }
+    r.score[0] = d[4];
+    r.score[1] = (!benchmark && mask_scores) ? (double)mask_scores[rj] : (double)d[4];
+    r.area_box = __dmul_rn(r.box[2], r.box[3]);              // loadRes: bb[2] * bb[3]
+    r.plane = plane;
+    r.area_mask = area;
+    if (area > 0) {
+      r.ext[0] = r0; r.ext[1] = r1 + 1; r.ext[2] = w0; r.ext[3] = w1 + 1;
+    } else {
+      r.ext[0] = r.ext[1] = r.ext[2] = r.ext[3] = 0;
+    }
+    const int64_t lab = labels[rj];
+    // json order: MM writes label-major (ascending labels), record order inside a label; BM record order
+    r.order = benchmark ? j : (int)min(max(lab, (int64_t)0), (int64_t)num_labels) * max_num + j;
+    r.pad = 0;
+    if (lab < 0 || lab >= num_labels) {
+      r.cat = -1;
+      atomicOr(status, SMB_COCO_LABEL_RANGE);
+    } else {
+      r.cat = label_cat[lab];
+    }
+    rows[rj] = r;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ block scans
+template <typename T, typename Op>
+__device__ __forceinline__ T block_inclusive_scan(T v, Op op, T* s_warp, T& total) {
+  const int tid = threadIdx.x, lid = tid & 31, warp = tid >> 5;
+  for (int o = 1; o < 32; o <<= 1) {
+    const T u = __shfl_up_sync(0xffffffffu, v, o);
+    if (lid >= o) v = op(u, v);
+  }
+  if (lid == 31) s_warp[warp] = v;
+  __syncthreads();
+  if (warp == 0) {
+    T w = lid < kWarps ? s_warp[lid] : s_warp[0];
+    for (int o = 1; o < kWarps; o <<= 1) {
+      const T u = __shfl_up_sync(0xffffffffu, w, o);
+      if (lid >= o) w = op(u, w);
+    }
+    if (lid < kWarps) s_warp[lid] = w;
+  }
+  __syncthreads();
+  if (warp > 0) v = op(s_warp[warp - 1], v);
+  total = s_warp[kWarps - 1];
+  __syncthreads();
+  return v;
+}
+
+struct Add { __device__ int operator()(int a, int b) const { return a + b; } };
+struct Max { __device__ double operator()(double a, double b) const { return a > b ? a : b; } };
+
+// ------------------------------------------------------------------------------------------------ 2b + 2c: IoU, matching
+struct MatchParams {
+  double iou_thr[kT];
+  double area_rng[kA][2];
+};
+
+__device__ __forceinline__ double box_iou(const double* d, const double* g, int crowd) {
+  // maskApi.c bbIou, operation by operation
+  const double da = __dmul_rn(d[2], d[3]), ga = __dmul_rn(g[2], g[3]);
+  const double w = __dsub_rn(fmin(__dadd_rn(d[2], d[0]), __dadd_rn(g[2], g[0])), fmax(d[0], g[0]));
+  if (w <= 0) return 0.0;
+  const double h = __dsub_rn(fmin(__dadd_rn(d[3], d[1]), __dadd_rn(g[3], g[1])), fmax(d[1], g[1]));
+  if (h <= 0) return 0.0;
+  const double i = __dmul_rn(w, h);
+  const double u = crowd ? da : __dsub_rn(__dadd_rn(da, ga), i);
+  return __ddiv_rn(i, u);
+}
+
+__global__ void __launch_bounds__(kThreads) match_kernel(
+    const smb_coco_img_t* __restrict__ imgs, const smb_coco_det_t* __restrict__ dets, int det_cap,
+    const uint32_t* __restrict__ det_planes, int64_t det_plane_words, const smb_coco_gt_t* __restrict__ gts, int n_gt,
+    const uint32_t* __restrict__ gt_planes, int64_t gt_plane_words, const int32_t* __restrict__ gt_cat_off, int K,
+    int metric, MatchParams P, smb_coco_out_t* __restrict__ out, int64_t n_out, int* __restrict__ npig,
+    double* __restrict__ iou_ws, uint8_t* __restrict__ gtm_ws, int* __restrict__ status) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  uint64_t* s_m = (uint64_t*)smem;                 // [kMaxDet] matched bits (t * kA + a) of the sorted detections
+  uint64_t* s_ig = s_m + kMaxDet;                  // [kMaxDet] ignore bits
+  int* s_sorted = (int*)(s_ig + kMaxDet);          // [kMaxDet] detection row of rank r
+  int* s_start = s_sorted + kMaxDet;               // [K + 1] per category: first entry of s_list
+  int* s_list = s_start + K + 1;                   // [det_cap] detections grouped by category, record order inside
+  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lid = tid & 31;
+  const smb_coco_img_t im = imgs[b];
+  const int nd = min(max(im.n_det, 0), det_cap);
+  const smb_coco_det_t* drow = dets + (size_t)b * det_cap;
+  const int32_t* goff = gt_cat_off + (size_t)b * (K + 1);
+  const int H = max(im.h, 0), gpitch = max(im.gt_pitch, 0), dpitch = max(im.det_pitch, 0);
+  auto out_row = [&](int j) -> smb_coco_out_t* {
+    const int64_t o = im.out_off + j;
+    return (o >= 0 && o < n_out) ? out + o : nullptr;
+  };
+  // every row of the image starts excluded (cat = K sorts after every category); its category's pass overwrites it
+  for (int j = tid; j < det_cap; j += kThreads) {
+    smb_coco_out_t* o = out_row(j);
+    if (o) { o->score = 0; o->image_id = im.image_id; o->matched = 0; o->ignored = 0; o->cat = K; o->rank = -1; }
+  }
+  // counting sort of the detections by category, stable (thread 0: at most det_cap steps)
+  if (tid == 0) {
+    for (int k = 0; k <= K; ++k) s_start[k] = 0;
+    for (int j = 0; j < nd; ++j) {
+      const int c = drow[j].cat;
+      if (c >= 0 && c < K) s_start[c + 1]++;
+    }
+    for (int k = 0; k < K; ++k) s_start[k + 1] += s_start[k];
+    for (int j = 0; j < nd; ++j) {
+      const int c = drow[j].cat;
+      if (c >= 0 && c < K) s_list[s_start[c]++] = j;
+    }
+    for (int k = K; k > 0; --k) s_start[k] = s_start[k - 1];
+    s_start[0] = 0;
+  }
+  __syncthreads();
+  for (int k = 0; k < K; ++k) {
+    const int l0 = s_start[k], n = s_start[k + 1] - l0;
+    const int g0 = min(max(goff[k], 0), n_gt), g1 = min(max(goff[k + 1], g0), n_gt), G = g1 - g0;
+    if (n == 0 && G == 0) continue;                // evaluateImg returns None
+    const int D = min(n, kMaxDet);
+    // ---- rank inside (image, category): score descending, stable over the json order
+    for (int i = tid; i < n; i += kThreads) {
+      const int j = s_list[l0 + i];
+      const double s = drow[j].score[metric];
+      const int oj = drow[j].order;
+      int r = 0;
+      for (int q = 0; q < n; ++q) {
+        const int jq = s_list[l0 + q];
+        const double sq = drow[jq].score[metric];
+        const int oq = drow[jq].order;
+        r += (sq > s) || (sq == s && (oq < oj || (oq == oj && jq < j)));
+      }
+      if (r < kMaxDet) s_sorted[r] = j;            // computeIoU keeps the first maxDets[-1]
+    }
+    for (int i = tid; i < D; i += kThreads) { s_m[i] = 0; s_ig[i] = 0; }
+    __syncthreads();
+    // ---- IoU [D, G] (ground truths in annotation order)
+    double* ious = iou_ws + (size_t)kMaxDet * g0;
+    if (metric == 0) {
+      for (int p = tid; p < D * G; p += kThreads) {
+        const int d = p / G, g = p - d * G;
+        ious[p] = box_iou(drow[s_sorted[d]].box, gts[g0 + g].box, gts[g0 + g].crowd);
+      }
+    } else {
+      for (int p = warp; p < D * G; p += kWarps) {
+        const int d = p / G, g = p - d * G;
+        const smb_coco_det_t& dr = drow[s_sorted[d]];
+        const smb_coco_gt_t& gr = gts[g0 + g];
+        const int y0 = max(max(dr.ext[0], gr.ext[0]), 0), y1 = min(min(dr.ext[1], gr.ext[1]), H);
+        const int x0 = max(max(dr.ext[2], gr.ext[2]), 0), x1 = min(min(min(dr.ext[3], gr.ext[3]), dpitch), gpitch);
+        const int nx = x1 - x0;
+        int inter = 0;
+        const bool dok = dr.plane >= 0 && dr.plane + (int64_t)H * dpitch <= det_plane_words;
+        const bool gok = gr.plane >= 0 && gr.plane + (int64_t)H * gpitch <= gt_plane_words;
+        if (dok && gok && nx > 0 && y1 > y0) {
+          const uint32_t* pd = det_planes + dr.plane;
+          const uint32_t* pg = gt_planes + gr.plane;
+          for (int e = lid; e < (y1 - y0) * nx; e += 32) {
+            const int y = y0 + e / nx, x = x0 + e % nx;
+            inter += __popc(pd[(size_t)y * dpitch + x] & pg[(size_t)y * gpitch + x]);
+          }
+        }
+        for (int o = 16; o > 0; o >>= 1) inter += __shfl_xor_sync(0xffffffffu, inter, o);
+        if (lid == 0) {
+          double v = 0.0;                          // rleIou: i == 0 -> 0
+          if (inter > 0) {
+            const long long u = gr.crowd ? (long long)dr.area_mask : (long long)dr.area_mask + gr.area_mask - inter;
+            v = __ddiv_rn((double)inter, (double)u);
+          }
+          ious[p] = v;
+        }
+      }
+    }
+    __syncthreads();
+    // ---- evaluateImg's greedy matching, one thread per (threshold, area range)
+    if (tid < kT * kA) {
+      const int t = tid / kA, a = tid - t * kA;
+      const double lo = P.area_rng[a][0], hi = P.area_rng[a][1];
+      uint8_t* gtm = gtm_ws + (size_t)kT * kA * g0 + (size_t)tid * G;
+      for (int g = 0; g < G; ++g) gtm[g] = 0;
+      auto gt_ig = [&](int g) {
+        const smb_coco_gt_t& gr = gts[g0 + g];
+        return gr.crowd || gr.area < lo || gr.area > hi;
+      };
+      if (t == 0) {
+        int np = 0;
+        for (int g = 0; g < G; ++g) np += !gt_ig(g);
+        if (np) atomicAdd(npig + k * kA + a, np);
+      }
+      const double thr = P.iou_thr[t] < 1.0 - 1e-10 ? P.iou_thr[t] : 1.0 - 1e-10;
+      const uint64_t bit = 1ull << tid;
+      for (int d = 0; d < D; ++d) {
+        double iou = thr;
+        int m = -1, mig = 0;
+        // ground truths stably reordered: not ignored first
+        for (int pass = 0; pass < 2 && !(pass == 1 && m > -1 && mig == 0); ++pass) {
+          for (int g = 0; g < G; ++g) {
+            const int ig = gt_ig(g);
+            if (ig != pass) continue;
+            if (gtm[g] && !gts[g0 + g].crowd) continue;
+            if (m > -1 && mig == 0 && ig == 1) break;
+            const double v = ious[(size_t)d * G + g];
+            if (v < iou) continue;
+            iou = v;
+            m = g;
+            mig = ig;
+          }
+        }
+        const smb_coco_det_t& dr = drow[s_sorted[d]];
+        const double area = metric == 0 ? dr.area_box : (double)dr.area_mask;
+        bool matched = false, ignored = false;
+        if (m > -1) {
+          gtm[m] = 1;
+          matched = gts[g0 + m].id != 0;           // pycocotools tests dtm != 0 with dtm the ground truth's id
+          ignored = mig;
+        }
+        if (!matched && (area < lo || area > hi)) ignored = true;
+        if (matched) atomicOr((unsigned long long*)&s_m[d], (unsigned long long)bit);
+        if (ignored) atomicOr((unsigned long long*)&s_ig[d], (unsigned long long)bit);
+      }
+    }
+    __syncthreads();
+    for (int r = tid; r < D; r += kThreads) {
+      const int j = s_sorted[r];
+      smb_coco_out_t* o = out_row(j);
+      if (o) {
+        o->score = drow[j].score[metric];
+        o->matched = s_m[r];
+        o->ignored = s_ig[r];
+        o->cat = k;
+        o->rank = r;
+      } else {
+        atomicOr(status, SMB_COCO_CAPACITY);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ 2d: accumulate
+__global__ void __launch_bounds__(kThreads) accumulate_kernel(
+    const smb_coco_out_t* __restrict__ rows, const int32_t* __restrict__ cat_off, int64_t n_rows, int K,
+    const int* __restrict__ npig_in, const double* __restrict__ rec_thr, int3 max_dets, double* __restrict__ precision,
+    double* __restrict__ recall, double* __restrict__ scores) {
+  __shared__ int s_wi[kWarps];
+  __shared__ double s_wd[kWarps];
+  __shared__ double s_q[kR], s_ss[kR];
+  const int k = blockIdx.x, a = blockIdx.y / 3, mi = blockIdx.y % 3, t = blockIdx.z, tid = threadIdx.x;
+  const int M = 3;
+  const int max_det = mi == 0 ? max_dets.x : (mi == 1 ? max_dets.y : max_dets.z);
+  const int64_t s0 = min(max((int64_t)cat_off[k], (int64_t)0), n_rows);
+  const int64_t s1 = min(max((int64_t)cat_off[k + 1], s0), n_rows);
+  const uint64_t bit = 1ull << (t * kA + a);
+  const int npig = npig_in[k * kA + a];
+  auto p_idx = [&](int r) { return ((((size_t)t * kR + r) * K + k) * kA + a) * M + mi; };
+  const size_t r_idx = (((size_t)t * K + k) * kA + a) * M + mi;
+  if (npig <= 0) {                                 // no ground truth to recall: every entry stays -1
+    for (int r = tid; r < kR; r += kThreads) { precision[p_idx(r)] = -1.0; scores[p_idx(r)] = -1.0; }
+    if (tid == 0) recall[r_idx] = -1.0;
+    return;
+  }
+  for (int r = tid; r < kR; r += kThreads) { s_q[r] = 0.0; s_ss[r] = 0.0; }
+  // ---- totals: included detections (rank < maxDet), tp, fp
+  int nd = 0, tp_tot = 0, fp_tot = 0;
+  for (int64_t base = s0; base < s1; base += kThreads) {
+    const int64_t e = base + tid;
+    int inc = 0, tpf = 0, fpf = 0;
+    if (e < s1) {
+      const smb_coco_out_t& o = rows[e];
+      inc = o.rank >= 0 && o.rank < max_det;
+      const bool ig = o.ignored & bit, m = o.matched & bit;
+      tpf = inc && m && !ig;
+      fpf = inc && !m && !ig;
+    }
+    int tot;
+    block_inclusive_scan(inc, Add(), s_wi, tot); nd += tot;
+    block_inclusive_scan(tpf, Add(), s_wi, tot); tp_tot += tot;
+    block_inclusive_scan(fpf, Add(), s_wi, tot); fp_tot += tot;
+  }
+  const double dn = (double)npig;
+  if (tid == 0) recall[r_idx] = nd ? __ddiv_rn((double)tp_tot, dn) : 0.0;
+  // ---- right to left: cumulative counts from the suffix sums, the precision envelope as a suffix maximum, and for
+  // every recall threshold the first detection whose recall reaches it (searchsorted 'left')
+  int c_inc = 0, c_tp = 0, c_fp = 0;               // counts strictly after the current chunk
+  double c_max = -1.0;
+  for (int64_t base = 0; base < s1 - s0; base += kThreads) {
+    const int64_t e = s1 - 1 - (base + tid);
+    int inc = 0, tpf = 0, fpf = 0;
+    double score = 0.0;
+    if (e >= s0) {
+      const smb_coco_out_t& o = rows[e];
+      inc = o.rank >= 0 && o.rank < max_det;
+      const bool ig = o.ignored & bit, m = o.matched & bit;
+      tpf = inc && m && !ig;
+      fpf = inc && !m && !ig;
+      score = o.score;
+    }
+    int ti, tt, tf;
+    const int si = block_inclusive_scan(inc, Add(), s_wi, ti) + c_inc;
+    const int st = block_inclusive_scan(tpf, Add(), s_wi, tt) + c_tp;
+    const int sf = block_inclusive_scan(fpf, Add(), s_wi, tf) + c_fp;
+    const int tp = tp_tot - (st - tpf), fp = fp_tot - (sf - fpf);   // cumulative counts up to and including e
+    double pr = -1.0;
+    if (inc) pr = __ddiv_rn((double)tp, __dadd_rn((double)(fp + tp), 2.220446049250313e-16));   // + np.spacing(1)
+    double tm;
+    double env = block_inclusive_scan(pr, Max(), s_wd, tm);
+    env = env > c_max ? env : c_max;
+    if (inc) {
+      const bool first = (nd - si) == 0;
+      const double rc = __ddiv_rn((double)tp, dn);
+      const double rc_prev = first ? -INFINITY : __ddiv_rn((double)(tp - tpf), dn);
+      if (rc > rc_prev) {
+        for (int r = 0; r < kR; ++r) {
+          const double x = rec_thr[r];
+          if (rc_prev < x && x <= rc) { s_q[r] = env; s_ss[r] = score; }
+        }
+      }
+    }
+    c_inc += ti; c_tp += tt; c_fp += tf;
+    c_max = c_max > tm ? c_max : tm;
+  }
+  __syncthreads();
+  for (int r = tid; r < kR; r += kThreads) { precision[p_idx(r)] = s_q[r]; scores[p_idx(r)] = s_ss[r]; }
+}
+
+// ------------------------------------------------------------------------------------------------ host rasterizer
+// pycocotools maskApi.c rleFrPoly: the run lengths of one polygon (k vertices) in an h x w canvas.
+std::vector<uint32_t> poly_counts(const double* xy, int k, int h, int w) {
+  const double scale = 5;
+  std::vector<int> x(k + 1), y(k + 1);
+  for (int j = 0; j < k; ++j) x[j] = (int)(scale * xy[j * 2 + 0] + .5);
+  for (int j = 0; j < k; ++j) y[j] = (int)(scale * xy[j * 2 + 1] + .5);
+  if (k > 0) { x[k] = x[0]; y[k] = y[0]; }
+  std::vector<int> u, v;
+  for (int j = 0; j < k; ++j) {
+    int xs = x[j], xe = x[j + 1], ys = y[j], ye = y[j + 1];
+    const int dx = abs(xe - xs), dy = abs(ys - ye);
+    const bool flip = (dx >= dy && xs > xe) || (dx < dy && ys > ye);
+    if (flip) { std::swap(xs, xe); std::swap(ys, ye); }
+    if (dx == 0 && dy == 0) {                      // s = 0/0 = NaN: pycocotools stores (int)NaN, INT_MIN on x86-64
+      u.push_back(xs);
+      v.push_back(INT_MIN);
+      continue;
+    }
+    const double s = dx >= dy ? (double)(ye - ys) / dx : (double)(xe - xs) / dy;
+    if (dx >= dy) {
+      for (int d = 0; d <= dx; ++d) {
+        const int t = flip ? dx - d : d;
+        u.push_back(t + xs);
+        v.push_back((int)(ys + s * t + .5));
+      }
+    } else {
+      for (int d = 0; d <= dy; ++d) {
+        const int t = flip ? dy - d : d;
+        v.push_back(t + ys);
+        u.push_back((int)(xs + s * t + .5));
+      }
+    }
+  }
+  std::vector<uint32_t> a;
+  for (size_t j = 1; j < u.size(); ++j) {
+    if (u[j] == u[j - 1]) continue;
+    double xd = (double)(u[j] < u[j - 1] ? u[j] : u[j] - 1);
+    xd = (xd + .5) / scale - .5;
+    if (floor(xd) != xd || xd < 0 || xd > (double)(w - 1)) continue;
+    double yd = (double)(v[j] < v[j - 1] ? v[j] : v[j - 1]);
+    yd = (yd + .5) / scale - .5;
+    if (yd < 0) yd = 0; else if (yd > h) yd = h;
+    yd = ceil(yd);
+    a.push_back((uint32_t)((int)xd * h + (int)yd));
+  }
+  a.push_back((uint32_t)h * (uint32_t)w);
+  std::sort(a.begin(), a.end());
+  uint32_t p = 0;
+  for (auto& e : a) { const uint32_t t = e; e -= p; p = t; }
+  std::vector<uint32_t> b;
+  size_t j = 0;
+  b.push_back(a[j++]);
+  while (j < a.size()) {
+    if (a[j] > 0) {
+      b.push_back(a[j++]);
+    } else {
+      ++j;
+      if (j < a.size()) b.back() += a[j++];
+    }
+  }
+  return b;
+}
+
+// OR the mask of column-major run lengths into a bit plane; -1 if the runs do not cover exactly h * w pixels.
+int or_runs(const uint32_t* cnts, int n, int h, int w, uint32_t* plane, int pitch) {
+  uint64_t pos = 0;
+  const uint64_t total = (uint64_t)h * w;
+  for (int i = 0; i < n; ++i) {
+    const uint64_t end = pos + cnts[i];
+    if (end > total) return -1;
+    if (i & 1) {
+      for (uint64_t q = pos; q < end; ++q) {
+        const int x = (int)(q / h), y = (int)(q % h);
+        plane[(size_t)y * pitch + (x >> 5)] |= 1u << (x & 31);
+      }
+    }
+    pos = end;
+  }
+  return pos == total ? 0 : -1;
+}
+
+}  // namespace
+
+extern "C" int smb_coco_poly_counts(const double* host_xy, int k, int h, int w, uint32_t* host_counts, int cap, int* host_n) {
+  SMB_CHECK_ARG(k >= 0 && h >= 0 && w >= 0 && (k == 0 || host_xy) && host_n, "smb_coco_poly_counts: bad arguments");
+  const std::vector<uint32_t> c = poly_counts(host_xy, k, h, w);
+  *host_n = (int)c.size();
+  if ((int)c.size() <= cap && host_counts) memcpy(host_counts, c.data(), c.size() * sizeof(uint32_t));
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_poly_to_bits(const double* host_xy, int k, int h, int w, uint32_t* host_plane, int pitch) {
+  SMB_CHECK_ARG(k >= 0 && h >= 0 && w >= 0 && (k == 0 || host_xy) && host_plane && pitch >= (w + 31) / 32,
+                "smb_coco_poly_to_bits: bad arguments");
+  const std::vector<uint32_t> c = poly_counts(host_xy, k, h, w);
+  return or_runs(c.data(), (int)c.size(), h, w, host_plane, pitch) == 0 ? SMB_OK : SMB_EINVAL;
+}
+
+extern "C" int smb_coco_rle_to_bits(const uint32_t* host_counts, int n, int h, int w, uint32_t* host_plane, int pitch) {
+  SMB_CHECK_ARG(n >= 0 && h >= 0 && w >= 0 && (n == 0 || host_counts) && host_plane && pitch >= (w + 31) / 32,
+                "smb_coco_rle_to_bits: bad arguments");
+  SMB_CHECK_ARG(or_runs(host_counts, n, h, w, host_plane, pitch) == 0,
+                "smb_coco_rle_to_bits: the runs do not cover the %d x %d canvas", h, w);
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_rle_from_string(const char* host_s, int len, uint32_t* host_counts, int cap, int* host_n) {
+  SMB_CHECK_ARG(len >= 0 && (len == 0 || host_s) && host_n, "smb_coco_rle_from_string: bad arguments");
+  // maskApi.c rleFrString: 5 bits per character, continuation bit 0x20, sign bit 0x10 on the last, deltas from m > 2
+  int m = 0, p = 0;
+  std::vector<uint32_t> cnts;
+  while (p < len) {
+    long long x = 0;
+    int k = 0, more = 1;
+    while (more) {
+      SMB_CHECK_ARG(p < len && k < 7, "smb_coco_rle_from_string: truncated or overlong value at byte %d", p);
+      const int c = host_s[p] - 48;
+      SMB_CHECK_ARG(c >= 0 && c < 64, "smb_coco_rle_from_string: byte %d is not an RLE character", p);
+      x |= (long long)(c & 0x1f) << (5 * k);
+      more = c & 0x20;
+      ++p;
+      ++k;
+      if (!more && (c & 0x10)) x |= -1LL << (5 * k);
+    }
+    if (m > 2) x += (long long)cnts[m - 2];
+    SMB_CHECK_ARG(x >= 0 && x <= 0xffffffffLL, "smb_coco_rle_from_string: count %lld out of range", x);
+    cnts.push_back((uint32_t)x);
+    ++m;
+  }
+  *host_n = m;
+  if (m <= cap && host_counts && m) memcpy(host_counts, cnts.data(), m * sizeof(uint32_t));
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_plane_stats(const uint32_t* host_plane, int h, int w, int pitch, int32_t* host_stats5) {
+  SMB_CHECK_ARG(host_plane && host_stats5 && h >= 0 && w >= 0 && pitch >= (w + 31) / 32, "smb_coco_plane_stats: bad arguments");
+  const int words = (w + 31) / 32;
+  const uint32_t last = (w & 31) ? ((1u << (w & 31)) - 1u) : 0xffffffffu;
+  int area = 0, r0 = INT_MAX, r1 = -1, w0 = INT_MAX, w1 = -1;
+  for (int y = 0; y < h; ++y)
+    for (int x = 0; x < words; ++x) {
+      uint32_t v = host_plane[(size_t)y * pitch + x];
+      if (x == words - 1) v &= last;
+      if (v) {
+        area += __builtin_popcount(v);
+        r0 = std::min(r0, y); r1 = std::max(r1, y); w0 = std::min(w0, x); w1 = std::max(w1, x);
+      }
+    }
+  host_stats5[0] = area;
+  if (area) { host_stats5[1] = r0; host_stats5[2] = r1 + 1; host_stats5[3] = w0; host_stats5[4] = w1 + 1; }
+  else host_stats5[1] = host_stats5[2] = host_stats5[3] = host_stats5[4] = 0;
+  return SMB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ device entry points
+extern "C" int smb_coco_det_from_record_dev(const float* det, const int64_t* labels, const int* count, const float* mask_scores,
+                                            const uint32_t* mask_bits, int N, int max_num, int cap_h, int words,
+                                            const smb_img_geom_t* geom, const int32_t* label_cat, int num_labels,
+                                            int benchmark, smb_coco_det_t* rows, smb_coco_img_t* imgs, int* status,
+                                            smb_stream_t stream) {
+  SMB_CHECK_ARG(N >= 0 && max_num >= 1 && cap_h >= 0 && words >= 0 && num_labels >= 0,
+                "smb_coco_det_from_record_dev: bad sizes (N %d, max_num %d, cap_h %d, words %d)", N, max_num, cap_h, words);
+  if (N == 0) return SMB_OK;
+  SMB_CHECK_ARG(det && labels && count && mask_bits && geom && (label_cat || num_labels == 0) && rows && imgs && status,
+                "smb_coco_det_from_record_dev: null pointer");
+  det_from_record_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(det, labels, count, mask_scores, mask_bits, max_num, cap_h,
+                                                                   words, geom, label_cat, num_labels, benchmark, rows, imgs,
+                                                                   status);
+  SMB_LAUNCH_OK("det_from_record_kernel");
+  return SMB_OK;
+}
+
+extern "C" size_t smb_coco_match_workspace_bytes(int n_gt) {
+  if (n_gt < 0) return 0;
+  return smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256) + smb::align_up((size_t)n_gt * kT * kA, 256) + 256;
+}
+
+extern "C" int smb_coco_match_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                                  const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt,
+                                  const uint32_t* gt_planes, int64_t gt_plane_words, const int32_t* gt_cat_off, int K,
+                                  int metric, const double* host_iou_thr, const double* host_area_rng,
+                                  smb_coco_out_t* out, int64_t n_out, int* npig, int* status, void* workspace,
+                                  size_t workspace_bytes, smb_stream_t stream) {
+  SMB_CHECK_ARG(n_img >= 0 && det_cap >= 1 && det_cap <= SMB_COCO_DET_CAP && K >= 1 && K <= SMB_COCO_MAX_CATS && n_gt >= 0 &&
+                    (metric == 0 || metric == 1) && n_out >= 0 && det_plane_words >= 0 && gt_plane_words >= 0,
+                "smb_coco_match_dev: bad sizes (n_img %d, det_cap %d, K %d, n_gt %d, metric %d)", n_img, det_cap, K, n_gt,
+                metric);
+  SMB_CHECK_ARG(host_iou_thr && host_area_rng, "smb_coco_match_dev: null thresholds");
+  if (n_img == 0) return SMB_OK;
+  SMB_CHECK_ARG(imgs && dets && gt_cat_off && out && npig && status && (gts || n_gt == 0) && workspace,
+                "smb_coco_match_dev: null pointer");
+  SMB_CHECK_ARG(metric == 0 || (det_planes && (gt_planes || n_gt == 0)), "smb_coco_match_dev: segm needs the planes");
+  SMB_CHECK_ARG(workspace_bytes >= smb_coco_match_workspace_bytes(n_gt), "smb_coco_match_dev: workspace of %zu bytes, %zu needed",
+                workspace_bytes, smb_coco_match_workspace_bytes(n_gt));
+  MatchParams P;
+  for (int t = 0; t < kT; ++t) P.iou_thr[t] = host_iou_thr[t];
+  for (int a = 0; a < kA; ++a) { P.area_rng[a][0] = host_area_rng[2 * a]; P.area_rng[a][1] = host_area_rng[2 * a + 1]; }
+  double* iou_ws = (double*)workspace;
+  uint8_t* gtm_ws = (uint8_t*)workspace + smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256);
+  const size_t smem = 2 * kMaxDet * sizeof(uint64_t) + (size_t)(kMaxDet + K + 1 + det_cap) * sizeof(int);
+  match_kernel<<<n_img, kThreads, smem, (cudaStream_t)stream>>>(imgs, dets, det_cap, det_planes, det_plane_words, gts, n_gt,
+                                                               gt_planes, gt_plane_words, gt_cat_off, K, metric, P, out, n_out,
+                                                               npig, iou_ws, gtm_ws, status);
+  SMB_LAUNCH_OK("match_kernel");
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
+                                       const int* npig, const double* rec_thr, const int* host_max_dets3, double* precision,
+                                       double* recall, double* scores, smb_stream_t stream) {
+  SMB_CHECK_ARG(n_rows >= 0 && K >= 1 && K <= SMB_COCO_MAX_CATS, "smb_coco_accumulate_dev: bad sizes (n_rows %lld, K %d)",
+                (long long)n_rows, K);
+  SMB_CHECK_ARG(cat_off && npig && rec_thr && host_max_dets3 && precision && recall && scores && (rows || n_rows == 0),
+                "smb_coco_accumulate_dev: null pointer");
+  const int3 md = make_int3(host_max_dets3[0], host_max_dets3[1], host_max_dets3[2]);
+  accumulate_kernel<<<dim3(K, kA * 3, kT), kThreads, 0, (cudaStream_t)stream>>>(rows, cat_off, n_rows, K, npig, rec_thr, md,
+                                                                               precision, recall, scores);
+  SMB_LAUNCH_OK("accumulate_kernel");
+  return SMB_OK;
+}

@@ -689,9 +689,15 @@ class StreamRunner(object):
                     oh, wq = o['bits'].shape[1:]
                     o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
             self.ev_out_ready[k].record(cs)
+            self._after_forward(k, eng, images)
         self._download(k, used, images)
         for m, o, h in zip(images, dev, host):
             m['dev'], m['host'] = o, h
+
+    def _after_forward(self, k, eng, images):
+        """Work on slot k's stream right after the batch's forward and record copies, while the bucket engine still holds
+        the batch's full record (mask_bits included, also with masks='rle'); the slot's next forward is ordered after it
+        and the download does not wait for it.  Nothing here; CocoEvalRunner evaluates the batch."""
 
     def _download(self, k, used, images):
         """Enqueue the download of slot k's record (the first used[name] elements of every field) once its batch is done."""
@@ -956,3 +962,63 @@ class VideoRunner(StreamRunner):
             self.overflowed.discard(video_id)
             self._raise_overflow(video_id)
         return video_json(video_id, [got[f] for f in range(len(v['frames']))])
+
+
+class CocoEvalRunner(StreamRunner):
+    """StreamRunner plus COCO box and mask AP (pycocotools COCOeval, as CocoDataset.evaluate runs it) from the stream.
+
+    submit(img, image_id[, meta]) checks the image against the ground truth (known id, not submitted before, ori_shape
+    equal to the annotation's height x width) before anything is enqueued, then rasterizes the image's ground truth on the
+    host and uploads it from pinned memory on the H2D stream with the image.  Right after each batch's forward, on the
+    slot's stream, the batch's real images are evaluated from the bucket engine's record (cocoeval.CocoEvaluator
+    .add_records: the result json's values, IoU and matching on the device).  flush() dispatches the open batch;
+    evaluate() accumulates and summarizes every image submitted so far and returns MM's evaluate() dict plus the raw
+    stats and arrays.  result(ticket) still returns each record, so the result json can be written as well.
+      gt      : cocoeval.CocoGroundTruth; cat_ids: COCO category id per 0-based label (as coco.coco_json takes it)
+      metrics : 'bbox' and / or 'segm'
+    Every other argument is StreamRunner's; SipMask-VIS (vis=True) is not supported."""
+
+    def __init__(self, state_dict, gt, cat_ids, metrics=('bbox', 'segm'), **kw):
+        from .cocoeval import CocoEvaluator
+        if kw.get('vis'):
+            raise ValueError('CocoEvalRunner: YouTube-VIS evaluation (vis=True) is not supported')
+        super(CocoEvalRunner, self).__init__(state_dict, **kw)
+        self.evaluator = CocoEvaluator(gt, cat_ids, metrics=metrics, benchmark=self.benchmark, device=self.dev)
+        torch.cuda.current_stream(self.dev).synchronize()   # the evaluator's zeroed state, before the slots use it
+        self._eval_rows = {}                # ticket -> (image id, its staged ground truth) until its batch is evaluated
+        self._submitted = set()
+
+    def submit(self, img, image_id, meta=None):
+        """img / meta as StreamRunner.submit; image_id: the image's COCO id.  Returns what StreamRunner.submit returns."""
+        image_id = int(image_id)
+        ori = tuple(meta[1][:2]) if meta is not None else tuple(img.shape[:2])
+        if image_id in self._submitted:
+            raise ValueError('image id %d is evaluated twice' % image_id)
+        self.evaluator.check_image(image_id, ori)
+        t = self.i
+        self._eval_rows[t] = (image_id, self.evaluator.stage_gt(image_id, self.s_h2d))
+        try:
+            r = super(CocoEvalRunner, self).submit(img, meta)
+        except Exception:
+            self._eval_rows.pop(t, None)
+            raise
+        self._submitted.add(image_id)
+        return r
+
+    def step(self, *args, **kwargs):
+        raise TypeError('CocoEvalRunner: use submit(img, image_id), flush() and evaluate()')
+
+    def _after_forward(self, k, eng, images):
+        rec = dict(det_bboxes=eng.det, det_labels=eng.labels, count=eng.count, mask_bits=eng.mask_bits)
+        if eng.rescoring:
+            rec['mask_scores'] = eng.mask_scores
+        ids, gts = zip(*[self._eval_rows.pop(m['ticket']) for m in images])
+        self.evaluator.add_records(rec, eng.geom, list(ids), [m['ori_shape'] for m in images], gts=list(gts))
+
+    def evaluate(self):
+        """Dispatch the open batch, wait for every slot's evaluation and return CocoEvaluator.evaluate()'s dict."""
+        self.flush()
+        cur = torch.cuda.current_stream(self.dev)
+        for s in self.streams:
+            cur.wait_stream(s)
+        return self.evaluator.evaluate()
