@@ -453,6 +453,77 @@ int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_rows, const in
                             const double* rec_thr, const int* host_max_dets3, double* precision, double* recall,
                             double* scores, smb_stream_t stream);
 
+/* ------------------------------------------------------------------ YouTube-VIS mask AP (YTVOSeval, iouType 'segm')
+ * The sequence IoU of a result entry d and a ground-truth object g over a video is sum_f I_f / U with
+ *   U = sum A_d (frames where d is present) + sum A_g (frames where g is present) - sum I (frames where both are),
+ * all integer pixel counts, so it is accumulated frame by frame in int64 and divided once in float64.
+ *
+ * One frame row of an overlap / scatter launch: its detection planes (absolute device pointer of detection 0, words from
+ * one detection plane to the next, words per row), its number of detections when no count array is given, its h x w
+ * canvas, the row pitch of its ground-truth planes, its ground-truth rows [g0, g0 + n_gt) and its accumulator slot
+ * (< 0: the row accumulates nothing). */
+typedef struct {
+  const uint32_t* det;
+  int64_t det_stride;
+  int32_t det_pitch;
+  int32_t n_det;
+  int32_t h, w;
+  int32_t gt_pitch;
+  int32_t n_gt, g0;
+  int32_t slot;
+} smb_ytvis_frame_t;
+/* A ground-truth object present in a frame: its plane (absolute device pointer, h x gt_pitch words), its index in the
+ * video's ground truth (the accumulator column) and ext = {row0, row1, word0, word1} (half-open) of its set bits. */
+typedef struct {
+  const uint32_t* plane;
+  int32_t g;
+  int32_t ext[4];
+  int32_t pad;
+} smb_ytvis_gt_frame_t;
+/* A ground-truth object of a video at its sequence match: avg_area (mean of its non-zero annotation areas), the sum of
+ * its pixel counts over the frames it is present in, its annotation id, iscrowd and accumulator column. */
+typedef struct {
+  double avg_area;
+  int64_t sum_area;
+  int64_t id;
+  int32_t crowd;
+  int32_t g;
+} smb_ytvis_gt_t;
+/* A result entry of a video, in json order: its score, object id (accumulator row) and category index (-1: none). */
+typedef struct {
+  double score;
+  int32_t obj;
+  int32_t cat;
+} smb_ytvis_entry_t;
+#define SMB_YTVIS_OBJECTS 1   /* status: an object id at or beyond the accumulators' object capacity */
+#define SMB_YTVIS_GTS 2       /* status: a ground-truth column at or beyond g_max */
+#define SMB_YTVIS_RANGE 4     /* status: a slot, ground-truth row or output row outside its buffer */
+
+/* Per-frame overlaps, one CTA per (frame row, detection): area[n, j] = pixel count of detection j (j < count[n], or < frames[n].n_det
+ * when count is NULL, clamped to max_num) over the h x w canvas, inter[n, j, g] = |detection j AND ground truth g| for
+ * every ground truth g present in the frame; every other entry of inter [N, max_num, g_max] and area [N, max_num] is 0. */
+int smb_ytvis_overlap_dev(const smb_ytvis_frame_t* frames, int N, const int* count, int max_num,
+                          const smb_ytvis_gt_frame_t* gts, int n_gts, int g_max, int32_t* inter, int32_t* area, int* status,
+                          smb_stream_t stream);
+/* Adds every frame row's overlaps into its slot's accumulators, keyed by object id: for each object id >= 0 among the
+ * row's detections (count / n_det as above, ids [N, max_num]) only its LAST detection counts (a frame's result keeps the
+ * last detection of a duplicate id).  acc_inter [slots, objects, g_max] += inter, acc_area [slots, objects] += area,
+ * acc_nz [slots, objects] += (area > 0); int64 / int32 atomics. */
+int smb_ytvis_scatter_dev(const smb_ytvis_frame_t* frames, int N, const int* count, const int32_t* ids, int max_num,
+                          const int32_t* inter, const int32_t* area, int g_max, int64_t* acc_inter, int64_t* acc_area,
+                          int32_t* acc_nz, int slots, int objects, int* status, smb_stream_t stream);
+/* evaluateVid of one video (slot's accumulators) for every category, one CTA: the sequence IoU, ranks by score
+ * (descending, stable over json order, the first SMB_COCO_MAX_DET kept), evaluateImg's greedy matching for the 10 x 4
+ * (threshold, area range) pairs with avg_area as the area.  gts of category k are [gt_cat_off[k], gt_cat_off[k + 1])
+ * in annotation order; out row e (< n_out) receives entry e with image_id = video_id (smb_coco_accumulate_dev's input);
+ * npig [K, 4] is added to.  n_ent <= SMB_COCO_DET_CAP, workspace >= smb_ytvis_match_workspace_bytes(n_gt). */
+size_t smb_ytvis_match_workspace_bytes(int n_gt);
+int smb_ytvis_match_dev(const smb_ytvis_entry_t* ents, int n_ent, const smb_ytvis_gt_t* gts, int n_gt,
+                        const int32_t* gt_cat_off, int K, int slot, const int64_t* acc_inter, const int64_t* acc_area,
+                        const int32_t* acc_nz, int slots, int objects, int g_max, int64_t video_id,
+                        const double* host_iou_thr, const double* host_area_rng, smb_coco_out_t* out, int64_t n_out,
+                        int* npig, int* status, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
 /* gather rows: dst[i,:] = src[idx[i],:] for i < *count (device count), zero otherwise. */
 int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev,
                         int max_rows, int row_elems, float* dst, smb_stream_t stream);

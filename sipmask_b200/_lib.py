@@ -80,6 +80,7 @@ SYMBOLS = [
     'smb_coco_poly_counts', 'smb_coco_poly_to_bits', 'smb_coco_rle_to_bits', 'smb_coco_rle_from_string',
     'smb_coco_plane_stats', 'smb_coco_det_from_record_dev', 'smb_coco_match_workspace_bytes', 'smb_coco_match_dev',
     'smb_coco_accumulate_dev',
+    'smb_ytvis_overlap_dev', 'smb_ytvis_scatter_dev', 'smb_ytvis_match_workspace_bytes', 'smb_ytvis_match_dev',
 ]
 
 
@@ -93,7 +94,8 @@ def lib():
         L.smb_last_error.restype = ctypes.c_char_p
         for n in ('smb_decode_workspace_bytes', 'smb_multiclass_nms_workspace_bytes', 'smb_fast_nms_workspace_bytes',
                   'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes',
-                  'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes', 'smb_coco_match_workspace_bytes'):
+                  'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes', 'smb_coco_match_workspace_bytes',
+                  'smb_ytvis_match_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

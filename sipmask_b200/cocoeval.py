@@ -187,13 +187,14 @@ class CocoGroundTruth:
 
 
 # ---------------------------------------------------------------------------------------------------- summarize (host)
-def summarize(precision, recall):
-    """COCOeval.summarize's 12 stats of the accumulated arrays (its _summarize / _summarizeDets code)."""
-    iouThrs, maxDets, areaRngLbl = IOU_THRS, MAX_DETS, AREA_RNG_LBL
+def summarize(precision, recall, area_rng_lbl=AREA_RNG_LBL, max_dets=MAX_DETS):
+    """COCOeval.summarize's 12 stats of the accumulated arrays (its _summarize / _summarizeDets code).  area_rng_lbl /
+    max_dets: the Params' areaRngLbl and maxDets (YTVOSeval keeps COCO's labels for its own ranges)."""
+    iouThrs, maxDets, areaRngLbl = IOU_THRS, list(max_dets), list(area_rng_lbl)
 
-    def _summarize(ap=1, iouThr=None, areaRng='all', maxDets=100):
+    def _summarize(ap=1, iouThr=None, areaRng='all', maxDets_=100):
         aind = [i for i, aRng in enumerate(areaRngLbl) if aRng == areaRng]
-        mind = [i for i, mDet in enumerate(MAX_DETS) if mDet == maxDets]
+        mind = [i for i, mDet in enumerate(maxDets) if mDet == maxDets_]
         if ap == 1:
             s = precision
             if iouThr is not None:
@@ -214,17 +215,17 @@ def summarize(precision, recall):
 
     stats = np.zeros((12,))
     stats[0] = _summarize(1)
-    stats[1] = _summarize(1, iouThr=.5, maxDets=maxDets[2])
-    stats[2] = _summarize(1, iouThr=.75, maxDets=maxDets[2])
-    stats[3] = _summarize(1, areaRng='small', maxDets=maxDets[2])
-    stats[4] = _summarize(1, areaRng='medium', maxDets=maxDets[2])
-    stats[5] = _summarize(1, areaRng='large', maxDets=maxDets[2])
-    stats[6] = _summarize(0, maxDets=maxDets[0])
-    stats[7] = _summarize(0, maxDets=maxDets[1])
-    stats[8] = _summarize(0, maxDets=maxDets[2])
-    stats[9] = _summarize(0, areaRng='small', maxDets=maxDets[2])
-    stats[10] = _summarize(0, areaRng='medium', maxDets=maxDets[2])
-    stats[11] = _summarize(0, areaRng='large', maxDets=maxDets[2])
+    stats[1] = _summarize(1, iouThr=.5, maxDets_=maxDets[2])
+    stats[2] = _summarize(1, iouThr=.75, maxDets_=maxDets[2])
+    stats[3] = _summarize(1, areaRng='small', maxDets_=maxDets[2])
+    stats[4] = _summarize(1, areaRng='medium', maxDets_=maxDets[2])
+    stats[5] = _summarize(1, areaRng='large', maxDets_=maxDets[2])
+    stats[6] = _summarize(0, maxDets_=maxDets[0])
+    stats[7] = _summarize(0, maxDets_=maxDets[1])
+    stats[8] = _summarize(0, maxDets_=maxDets[2])
+    stats[9] = _summarize(0, areaRng='small', maxDets_=maxDets[2])
+    stats[10] = _summarize(0, areaRng='medium', maxDets_=maxDets[2])
+    stats[11] = _summarize(0, areaRng='large', maxDets_=maxDets[2])
     return stats
 
 
@@ -236,6 +237,35 @@ def mm_results(metric, stats):
     out['{}_mAP_copypaste'.format(metric)] = ('{ap[0]:.3f} {ap[1]:.3f} {ap[2]:.3f} {ap[3]:.3f} '
                                              '{ap[4]:.3f} {ap[5]:.3f}').format(ap=stats[:6])
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- accumulate
+def accumulate(row_parts, npig, K, dev):
+    """COCOeval.accumulate on the device: the precision / recall / scores arrays (numpy) of the OUT_DTYPE rows (a list
+    of uint8 device tensors) and npig [K, 4], on the current stream."""
+    parts = [r.view(torch.int64).view(-1, 5) for r in row_parts]
+    rows = torch.cat(parts) if parts else torch.zeros((0, 5), dtype=torch.int64, device=dev)
+    score = rows[:, 0].contiguous().view(torch.float64)
+    img = rows[:, 1].contiguous()
+    cat = (rows[:, 4] & 0xffffffff).to(torch.int32)      # little-endian {cat, rank} in the last word
+    rank = (rows[:, 4] >> 32).to(torch.int32)
+    # global order: category, score descending, image id, rank (stable sorts from the last key to the first)
+    o = torch.argsort(rank, stable=True)
+    o = o[torch.argsort(img[o], stable=True)]
+    o = o[torch.argsort(-score[o], stable=True)]
+    o = o[torch.argsort(cat[o], stable=True)]
+    srt = rows[o].contiguous()
+    cat_off = torch.searchsorted(cat[o].contiguous(), torch.arange(K + 1, dtype=torch.int32, device=dev)).to(torch.int32)
+    T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
+    precision = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
+    scores = torch.empty_like(precision)
+    recall = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
+    rec_thr = torch.from_numpy(np.ascontiguousarray(REC_THRS)).to(dev)
+    md = (ctypes.c_int * 3)(*MAX_DETS)
+    L.check(L.lib().smb_coco_accumulate_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K, L.ptr(npig),
+                                            L.ptr(rec_thr), md, L.ptr(precision), L.ptr(recall), L.ptr(scores),
+                                            L.stream_ptr()), 'smb_coco_accumulate_dev')
+    return precision.cpu().numpy(), recall.cpu().numpy(), scores.cpu().numpy()
 
 
 # ---------------------------------------------------------------------------------------------------- evaluator
@@ -437,30 +467,7 @@ class CocoEvaluator:
 
     # ---- accumulate + summarize
     def _accumulate(self, metric):
-        K, dev = self.K, self.dev
-        parts = [r.view(torch.int64).view(-1, 5) for r in self.rows[metric]]
-        rows = torch.cat(parts) if parts else torch.zeros((0, 5), dtype=torch.int64, device=dev)
-        score = rows[:, 0].contiguous().view(torch.float64)
-        img = rows[:, 1].contiguous()
-        cat = (rows[:, 4] & 0xffffffff).to(torch.int32)      # little-endian {cat, rank} in the last word
-        rank = (rows[:, 4] >> 32).to(torch.int32)
-        # global order: category, score descending, image id, rank (stable sorts from the last key to the first)
-        o = torch.argsort(rank, stable=True)
-        o = o[torch.argsort(img[o], stable=True)]
-        o = o[torch.argsort(-score[o], stable=True)]
-        o = o[torch.argsort(cat[o], stable=True)]
-        srt = rows[o].contiguous()
-        cat_off = torch.searchsorted(cat[o].contiguous(), torch.arange(K + 1, dtype=torch.int32, device=dev)).to(torch.int32)
-        T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
-        precision = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
-        scores = torch.empty_like(precision)
-        recall = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
-        rec_thr = torch.from_numpy(np.ascontiguousarray(REC_THRS)).to(dev)
-        md = (ctypes.c_int * 3)(*MAX_DETS)
-        L.check(L.lib().smb_coco_accumulate_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K,
-                                                L.ptr(self.npig[metric]), L.ptr(rec_thr), md, L.ptr(precision),
-                                                L.ptr(recall), L.ptr(scores), L.stream_ptr()), 'smb_coco_accumulate_dev')
-        return precision.cpu().numpy(), recall.cpu().numpy(), scores.cpu().numpy()
+        return accumulate(self.rows[metric], self.npig[metric], self.K, self.dev)
 
     def evaluate(self):
         """Accumulate and summarize every metric.  Returns MM's dict (bbox_mAP, ..., segm_mAP_copypaste) plus

@@ -12,11 +12,15 @@
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "coco_match.cuh"
 
 namespace {
 
-constexpr int kT = SMB_COCO_T, kA = SMB_COCO_A, kR = SMB_COCO_R, kMaxDet = SMB_COCO_MAX_DET;
+using smb_match::kT;
+using smb_match::kA;
+using smb_match::kMaxDet;
+using smb_match::MatchParams;
+constexpr int kR = SMB_COCO_R;
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
@@ -134,11 +138,6 @@ struct Add { __device__ int operator()(int a, int b) const { return a + b; } };
 struct Max { __device__ double operator()(double a, double b) const { return a > b ? a : b; } };
 
 // ------------------------------------------------------------------------------------------------ 2b + 2c: IoU, matching
-struct MatchParams {
-  double iou_thr[kT];
-  double area_rng[kA][2];
-};
-
 __device__ __forceinline__ double box_iou(const double* d, const double* g, int crowd) {
   // maskApi.c bbIou, operation by operation
   const double da = __dmul_rn(d[2], d[3]), ga = __dmul_rn(g[2], g[3]);
@@ -254,52 +253,17 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
     }
     __syncthreads();
     // ---- evaluateImg's greedy matching, one thread per (threshold, area range)
-    if (tid < kT * kA) {
-      const int t = tid / kA, a = tid - t * kA;
-      const double lo = P.area_rng[a][0], hi = P.area_rng[a][1];
-      uint8_t* gtm = gtm_ws + (size_t)kT * kA * g0 + (size_t)tid * G;
-      for (int g = 0; g < G; ++g) gtm[g] = 0;
-      auto gt_ig = [&](int g) {
-        const smb_coco_gt_t& gr = gts[g0 + g];
-        return gr.crowd || gr.area < lo || gr.area > hi;
-      };
-      if (t == 0) {
-        int np = 0;
-        for (int g = 0; g < G; ++g) np += !gt_ig(g);
-        if (np) atomicAdd(npig + k * kA + a, np);
-      }
-      const double thr = P.iou_thr[t] < 1.0 - 1e-10 ? P.iou_thr[t] : 1.0 - 1e-10;
-      const uint64_t bit = 1ull << tid;
-      for (int d = 0; d < D; ++d) {
-        double iou = thr;
-        int m = -1, mig = 0;
-        // ground truths stably reordered: not ignored first
-        for (int pass = 0; pass < 2 && !(pass == 1 && m > -1 && mig == 0); ++pass) {
-          for (int g = 0; g < G; ++g) {
-            const int ig = gt_ig(g);
-            if (ig != pass) continue;
-            if (gtm[g] && !gts[g0 + g].crowd) continue;
-            if (m > -1 && mig == 0 && ig == 1) break;
-            const double v = ious[(size_t)d * G + g];
-            if (v < iou) continue;
-            iou = v;
-            m = g;
-            mig = ig;
-          }
-        }
-        const smb_coco_det_t& dr = drow[s_sorted[d]];
-        const double area = metric == 0 ? dr.area_box : (double)dr.area_mask;
-        bool matched = false, ignored = false;
-        if (m > -1) {
-          gtm[m] = 1;
-          matched = gts[g0 + m].id != 0;           // pycocotools tests dtm != 0 with dtm the ground truth's id
-          ignored = mig;
-        }
-        if (!matched && (area < lo || area > hi)) ignored = true;
-        if (matched) atomicOr((unsigned long long*)&s_m[d], (unsigned long long)bit);
-        if (ignored) atomicOr((unsigned long long*)&s_ig[d], (unsigned long long)bit);
-      }
-    }
+    smb_match::greedy_match(
+        tid, D, G, ious, gtm_ws + (size_t)kT * kA * g0, P,
+        [&](int g) {
+          const smb_coco_gt_t& gr = gts[g0 + g];
+          return smb_match::MatchGt{gr.area, gr.id, gr.crowd};
+        },
+        [&](int d) {
+          const smb_coco_det_t& dr = drow[s_sorted[d]];
+          return metric == 0 ? dr.area_box : (double)dr.area_mask;
+        },
+        npig + k * kA, s_m, s_ig);
     __syncthreads();
     for (int r = tid; r < D; r += kThreads) {
       const int j = s_sorted[r];
@@ -577,10 +541,7 @@ extern "C" int smb_coco_det_from_record_dev(const float* det, const int64_t* lab
   return SMB_OK;
 }
 
-extern "C" size_t smb_coco_match_workspace_bytes(int n_gt) {
-  if (n_gt < 0) return 0;
-  return smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256) + smb::align_up((size_t)n_gt * kT * kA, 256) + 256;
-}
+extern "C" size_t smb_coco_match_workspace_bytes(int n_gt) { return smb_match::match_workspace_bytes(n_gt); }
 
 extern "C" int smb_coco_match_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
                                   const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt,

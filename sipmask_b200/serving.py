@@ -900,6 +900,7 @@ class VideoRunner(StreamRunner):
                           ids=self.ids_dev[k][:nr])
             self.status_dev[k].copy_(trk.status)            # this launch's status bits, then clear them for the next
             trk.status.zero_()
+            self._after_associate(k, images)
             self.ev_assoc[k].record(st)
         with torch.cuda.stream(self.s_d2h):
             self.s_d2h.wait_event(self.ev_assoc[k])
@@ -909,6 +910,10 @@ class VideoRunner(StreamRunner):
             self.ids_host[k][:nr].copy_(self.ids_dev[k][:nr], non_blocking=True)
             self.status_host[k].copy_(self.status_dev[k], non_blocking=True)
             self.ev_out_free[k].record(self.s_d2h)
+
+    def _after_associate(self, k, images):
+        """Work on the tracker stream right after slot k's batch is associated (its object ids are in ids_dev[k]); the
+        slot's download waits for it.  Nothing here; VideoEvalRunner accumulates the batch's overlaps by object id."""
 
     def _read(self, k, j):
         """Frame j of slot k's batch (downloaded): its record with obj_ids, segms / mask_bits and frame; records the
@@ -1020,5 +1025,150 @@ class CocoEvalRunner(StreamRunner):
         self.flush()
         cur = torch.cuda.current_stream(self.dev)
         for s in self.streams:
+            cur.wait_stream(s)
+        return self.evaluator.evaluate()
+
+
+class VideoEvalRunner(VideoRunner):
+    """VideoRunner plus YouTube-VIS mask AP (YTVOSeval, as SipMask-VIS's ytvos_eval runs it) from the stream.
+
+    submit(frame, video_id, frame_id) takes the video's YouTube-VIS id and checks the frame against the ground truth
+    (known video, its height x width, a frame inside its length, a video not evaluated before) before anything is
+    enqueued; it then rasterizes the frame's ground truth on the host and uploads it on the H2D stream with the frame.
+      - Right after each batch's forward, on the slot's stream: every detection's pixel count and its intersections with
+        the frame's ground-truth objects (ytviseval kernel a), from the bucket engine's planes.
+      - Right after the association, on the tracker stream: the last detection of each object id is added into its
+        video's accumulators (kernel b).  Each video being evaluated holds one of `eval_slots` accumulator slots (default
+        2 x lanes) from its frame 0 until its sequence match; when none is free, the ended videos are matched first.
+      - Once a video has ended and its frames are read, its result json (VideoRunner.video_json) gives every object's
+        score and category, and one launch on the tracker stream matches it (kernel c).
+    end_video(video_id) raises ValueError unless the video got exactly its annotated number of frames.  evaluate()
+    dispatches the open batch, matches every ended video and returns YtvisEvaluator.evaluate()'s dict; every video
+    submitted must have ended.  video_json(video_id) returns what VideoRunner returns, also for a video already matched
+    (the runner keeps the entries of matched videos until they are asked for).
+      gt        : ytviseval.YtvisGroundTruth
+      cat_ids   : the category ids the results carry (default 1 .. num_classes - 1, label + 1 as video_json writes)
+      max_gts   : ground-truth objects per video the accumulators hold
+    A video whose lane overflowed max_objects raises SmbError from video_json and evaluate(), as in VideoRunner.  Every
+    other argument is VideoRunner's."""
+
+    def __init__(self, state_dict, gt, cat_ids=None, eval_slots=None, max_gts=64, **kw):
+        from .ytviseval import YtvisEvaluator
+        super(VideoEvalRunner, self).__init__(state_dict, **kw)
+        slots = int(eval_slots) if eval_slots is not None else 2 * self.tracker.lanes
+        if slots < self.tracker.lanes:
+            raise ValueError('eval_slots=%d: at least one accumulator slot per lane (%d)' % (slots, self.tracker.lanes))
+        cats = range(1, self.num_classes) if cat_ids is None else cat_ids
+        with torch.cuda.stream(self.s_trk):
+            self.evaluator = YtvisEvaluator(gt, cats, slots=slots, objects=self.tracker.capacity, max_gts=max_gts,
+                                            device=self.dev)
+        self.s_trk.synchronize()            # the evaluator's zeroed state, before the slots use it
+        self._free = list(range(slots))     # accumulator slots not held by a video
+        self._vslot = {}                    # video id -> its accumulator slot until its sequence match
+        self._staged = {}                   # ticket -> its frame's staged ground truth until the batch's overlaps
+        self._ovl = [None] * self.n         # per slot: its batch's overlaps, until the association adds them up
+        self.ev_ovl = [torch.cuda.Event() for _ in range(self.n)]
+        self._json = {}                     # matched video -> its result entries, until video_json asks for them
+
+    def submit(self, img, video_id, frame_id):
+        frame_id = int(frame_id)
+        if img.dim() != 3:
+            raise ValueError('raw input is a uint8 HWC BGR image')
+        self.evaluator.check_frame(video_id, frame_id, tuple(img.shape[:2]))
+        _, first = self.book.check(video_id, frame_id)
+        if first:
+            slot = self._acquire()
+            self._vslot[video_id] = slot
+            with torch.cuda.stream(self.s_trk):     # after the previous holder's sequence match
+                self.evaluator.begin_video(video_id, slot)
+        t = self.i
+        try:
+            staged = self._staged[t] = self.evaluator.stage_frame(video_id, frame_id, self.s_h2d)
+            super(VideoEvalRunner, self).submit(img, video_id, frame_id)
+        except Exception:
+            self._staged.pop(t, None)
+            if first:
+                self.evaluator.abort_video(video_id)
+                self._free.append(self._vslot.pop(video_id))
+            raise
+        self.evaluator.commit_frame(staged)
+        return t
+
+    def _acquire(self):
+        if not self._free:
+            ended = [v for v in self._vslot if self.book.videos[v]['ended']]
+            if ended and self._open is not None:
+                self._dispatch()
+            for v in ended:
+                self._finish(v)
+        if not self._free:
+            raise ValueError('all %d accumulator slots hold videos that have not ended' % self.evaluator.slots)
+        return self._free.pop(0)
+
+    def end_video(self, video_id):
+        v = self.book.videos.get(video_id)
+        if v is not None and not v['ended'] and video_id in self._vslot:
+            n = self.evaluator.gt.videos[video_id]['length']
+            if len(v['frames']) != n:
+                raise ValueError('video %r ends after %d frames, the annotation has %d' % (video_id, len(v['frames']), n))
+        super(VideoEvalRunner, self).end_video(video_id)
+
+    def _after_forward(self, k, eng, images):
+        nr, mx = len(images), eng.max_num
+        cap_h, words = eng.mask_bits.shape[2:]
+        plane = cap_h * words
+        base = eng.mask_bits.data_ptr()
+        staged = [self._staged.pop(m['ticket']) for m in images]
+        self._ovl[k] = self.evaluator.overlap(staged, [base + 4 * j * mx * plane for j in range(nr)], plane, words, mx,
+                                              count=eng.count)
+        self.ev_ovl[k].record(torch.cuda.current_stream(self.dev))
+
+    def _after_associate(self, k, images):
+        ovl, self._ovl[k] = self._ovl[k], None
+        self.s_trk.wait_event(self.ev_ovl[k])
+        nr = len(images)
+        self.evaluator.scatter(ovl, self.ids_dev[k][:nr], count=self.out_dev[k]['cnt'][:nr])
+
+    def _finish(self, video_id):
+        """Read the ended video's result entries and enqueue its sequence match on the tracker stream."""
+        for k in range(self.n):
+            self._read_slot(k)
+        fr = self.frames.get(video_id, {})
+        obj_ids = list(dict.fromkeys(oid for f in sorted(fr) for oid in fr[f][0]))     # video_json's entry order
+        try:
+            entries = VideoRunner.video_json(self, video_id)
+        except SmbError:
+            self.evaluator.abort_video(video_id)
+            self._free.append(self._vslot.pop(video_id))
+            raise
+        slot = self._vslot.pop(video_id)
+        self._json[video_id] = entries
+        try:
+            with torch.cuda.stream(self.s_trk):
+                self.evaluator.end_video(video_id, entries, obj_ids)
+        except ValueError:
+            self.evaluator.abort_video(video_id)
+            raise
+        finally:
+            self._free.append(slot)
+
+    def video_json(self, video_id):
+        if video_id not in self._json:
+            if video_id not in self._vslot:
+                return super(VideoEvalRunner, self).video_json(video_id)
+            self._finish(video_id)
+        return self._json.pop(video_id)
+
+    def evaluate(self):
+        """Dispatch the open batch, match every ended video, wait for the slot and tracker streams and return
+        YtvisEvaluator.evaluate()'s dict."""
+        self.flush()
+        open_videos = [v for v in self._vslot if not self.book.videos[v]['ended']]
+        if open_videos:
+            raise ValueError('video %r has not ended: end_video() first' % (open_videos[0],))
+        for v in list(self._vslot):
+            self._finish(v)
+        cur = torch.cuda.current_stream(self.dev)
+        for s in self.streams + [self.s_trk]:
             cur.wait_stream(s)
         return self.evaluator.evaluate()
