@@ -41,6 +41,7 @@ by `conv_patch` exactly as the planner does) and its 64-channel N block.
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -301,3 +302,341 @@ def check_rescore_chain(pos, count, conv_w, conv_b, score_w, score_b, labels, de
     tight = float((bound / old).max()) if float(old.max()) > 0 else 0.0
     res['score bound / 1e-2 bound'] = tight
     return res
+
+
+# ------------------------------------------------------------------------------------------------------------ masks
+# Mask chain model (mask_assemble.cu).  Per detection the kernels evaluate, at every prototype pixel inside the roi, the
+# sigmoid of ONE 32-term dot product (the CropSplit cell of the pixel), bilinearly resize those values and threshold them.
+#   crop geometry: exact float32 arithmetic (rois = boxes * roi_scale, roi_w = float32((float64(x2 - x1) + 0.1) / 2),
+#                  inside on integer pixel coordinates, cell = trunc(float32(float32(w - x1) / roi_w)), clamped to [0, 3]);
+#   logit z:       float64 dot product of the prototypes as the kernel reads them with the fp32 coefficients;
+#     scalar family (sequential fmaf): |z_dev - z| <= gamma_32 sum|p c|;
+#     tensor family (fp16 hi + lo coefficients, four m16n8k16 fp32 accumulations): the split costs 2^-22 sum|p c| +
+#                  2^-25 sum|p| (lo is an fp16 subnormal below 2^-14), each of the four MMA steps at most 2^-22 of the
+#                  running magnitude: |z_dev - z| <= 2^-20 sum|p c| + 2^-24 sum|p|.  Pixels the kernels send to their
+#                  scalar cold path (a cell quotient >= 2, or a detection with a coefficient beyond the fp16 range) are
+#                  bounded by the larger of the two models;
+#   value:         sigmoid over [z - dz, z + dz], plus the sigmoid's own fp32 error (< 3e-7 for __expf + IEEE division
+#                  and for ex2.approx + rcp.approx);
+#   resize:        source index and lambda by torch's float32 rule s = r * (d + 0.5) - 0.5 (r = float32(1 / up), or
+#                  in / out in float32 for recompute_scale_factor=True), evaluated both as written and FMA-contracted; where
+#                  the two forms disagree the value is their midpoint and the bound grows by half the difference.  The
+#                  bilinear value is float64 with the fp32 weights; its bound is the weights applied to the tap bounds plus
+#                  4 * 2^-24 of the weighted tap magnitudes (three roundings deep in fp32).
+# A pixel is ambiguous when |v - thr| <= bound: the kernel may decide it either way.  Every other bit is determined.
+# Measured on an H100 (80 GB): at most 1.7e-6 of the in-frame pixels are ambiguous over the kernel matrix of
+# tests/test_gpu_mask_bits.py and the engine configurations of the layer audit; the cap is 1e-4.
+# The float64 work is restricted to each roi's extent (prototype pixels) and the output pixels whose taps reach it.
+U32 = 2.0 ** -24
+GAMMA32 = 32 * U32 / (1 - 32 * U32)
+SIGMOID_ERR = 3e-7
+COF_FP16_LIMIT = 65000.0            # the tensor family's fp16 hi part holds coefficients up to this magnitude
+BILINEAR_ERR = 4 * U32
+MASK_AMBIGUOUS_CAP = 1e-4
+
+
+def _sigmoid(z):
+    return 0.5 * (1.0 + np.tanh(0.5 * z))
+
+
+class MaskVals(object):
+    """One detection's prototype-resolution values: window [y0, y1) x [x0, x1) of the map (the roi's pixels), value v
+    and bound b (0 outside the crop), inside mask, cell, roi (float32 x1, y1, x2, y2)."""
+
+    def __init__(self, win, v, b, inside=None, cell=None, roi=None):
+        self.win, self.v, self.b, self.inside, self.cell, self.roi = win, v, b, inside, cell, roi
+
+
+def crop_rois(boxes, roi_scale4):
+    """float32 rois [N, 4] = boxes * roi_scale and cell sizes roi_w, roi_h [N] exactly as the kernels compute them."""
+    b = np.asarray(boxes, np.float32).reshape(-1, 4)
+    s = np.atleast_1d(np.asarray(roi_scale4, np.float32))
+    s = s if s.size == 4 else np.repeat(s[:1], 4)
+    roi = (b * s[None, :]).astype(np.float32)
+    rw = (((roi[:, 2] - roi[:, 0]).astype(np.float64) + 0.1) / 2).astype(np.float32)
+    rh = (((roi[:, 3] - roi[:, 1]).astype(np.float64) + 0.1) / 2).astype(np.float32)
+    return roi, rw, rh
+
+
+def _crop_axis(lo, hi, cell, n):
+    """Pixels p of [0, n) with lo <= p < hi (float32 compare on integers) and trunc(float32(float32(p - lo) / cell))."""
+    lo, hi, cell = np.float32(lo), np.float32(hi), np.float32(cell)
+    if not (np.isfinite(lo) and np.isfinite(hi)) or not hi > lo:
+        return 0, 0, np.zeros(0, np.int64)
+    p0 = int(min(max(np.ceil(np.float64(lo)), 0), n))
+    p1 = int(min(max(np.ceil(np.float64(hi)), 0), n))
+    p = np.arange(p0, max(p0, p1), dtype=np.float32)
+    with np.errstate(divide='ignore', invalid='ignore', over='ignore'):
+        q = ((p - lo).astype(np.float32) / cell).astype(np.float32)
+    return p0, max(p0, p1), np.minimum(q, np.float32(64.0)).astype(np.int64)
+
+
+def crop_geometry(boxes, roi_scale4, H, W):
+    """Per detection: (window (y0, y1, x0, x1), idx_h [h], idx_w [w]) of the CropSplit crop on an H x W map; every pixel
+    of the window is inside the roi, cell = clip(2 idx_h + idx_w, 0, 3)."""
+    roi, rw, rh = crop_rois(boxes, roi_scale4)
+    out = []
+    for n in range(roi.shape[0]):
+        y0, y1, ih = _crop_axis(roi[n, 1], roi[n, 3], rh[n], H)
+        x0, x1, iw = _crop_axis(roi[n, 0], roi[n, 2], rw[n], W)
+        if y1 == y0 or x1 == x0:
+            y0 = y1 = x0 = x1 = 0
+            ih, iw = ih[:0], iw[:0]
+        out.append(((y0, y1, x0, x1), ih, iw))
+    return out, roi
+
+
+def mask_values(protos, cofs, boxes, roi_scale4, family='scalar'):
+    """Float64 values and bounds of the cropped sigmoid masks (module comment above), one MaskVals per detection.
+    protos [32, H, W] as the kernel receives them (numpy or torch, fp16 or fp32), cofs [N, 128] fp32, boxes [N, 4]
+    image space, family 'scalar' (sequential fmaf) or 'tensor' (mma.sync, fp16 prototypes)."""
+    assert family in ('scalar', 'tensor'), family
+    P = protos.detach().cpu().numpy() if hasattr(protos, 'detach') else np.asarray(protos)
+    C = cofs.detach().cpu().numpy() if hasattr(cofs, 'detach') else np.asarray(cofs)
+    C = C.astype(np.float32).astype(np.float64).reshape(-1, 4, 32)
+    _, H, W = P.shape
+    geo, roi = crop_geometry(boxes.detach().cpu().numpy() if hasattr(boxes, 'detach') else boxes, roi_scale4, H, W)
+    res = []
+    for n, ((y0, y1, x0, x1), ih, iw) in enumerate(geo):
+        h, w = y1 - y0, x1 - x0
+        if h == 0:
+            res.append(MaskVals((0, 0, 0, 0), np.zeros((0, 0)), np.zeros((0, 0)), np.zeros((0, 0), bool),
+                                np.zeros((0, 0), np.int64), roi[n]))
+            continue
+        win = P[:, y0:y1, x0:x1].astype(np.float64).reshape(32, -1)
+        cell = np.clip(2 * ih[:, None] + iw[None, :], 0, 3)
+        sel = cell.reshape(1, -1)
+        z = np.take_along_axis(C[n] @ win, sel, 0)[0]
+        m = np.take_along_axis(np.abs(C[n]) @ np.abs(win), sel, 0)[0]
+        if family == 'scalar':
+            dz = GAMMA32 * m
+        else:
+            dz = 2.0 ** -20 * m + 2.0 ** -24 * np.abs(win).sum(0)
+            cold = ((ih[:, None] >= 2) | (iw[None, :] >= 2)).reshape(-1)
+            if np.abs(C[n]).max() > COF_FP16_LIMIT:
+                cold[:] = True
+            dz = np.where(cold, np.maximum(dz, GAMMA32 * m), dz)
+        v = _sigmoid(z)
+        b = np.maximum(_sigmoid(z + dz) - v, v - _sigmoid(z - dz)) + SIGMOID_ERR
+        res.append(MaskVals((y0, y1, x0, x1), v.reshape(h, w), b.reshape(h, w), np.ones((h, w), bool), cell, roi[n]))
+    return res
+
+
+def dense_values(pos):
+    """MaskVals of given [N, H, W] values (a kernel's pos_masks), exact: the window is each plane's non-zero extent."""
+    a = pos.detach().cpu().numpy() if hasattr(pos, 'detach') else np.asarray(pos)
+    res = []
+    for n in range(a.shape[0]):
+        nz = np.nonzero(a[n])
+        if nz[0].size == 0:
+            res.append(MaskVals((0, 0, 0, 0), np.zeros((0, 0)), np.zeros((0, 0))))
+            continue
+        y0, y1, x0, x1 = int(nz[0].min()), int(nz[0].max()) + 1, int(nz[1].min()), int(nz[1].max()) + 1
+        v = a[n, y0:y1, x0:x1].astype(np.float64)
+        res.append(MaskVals((y0, y1, x0, x1), v, np.zeros_like(v), v != 0))
+    return res
+
+
+def src_index(r, n_out, n_in):
+    """[(i0, i1, lam) as written, (i0, i1, lam) FMA-contracted] of the float32 rule s = r * (d + 0.5) - 0.5, clamped at 0,
+    i0 = min(trunc(s), n_in - 1), i1 = i0 + (i0 < n_in - 1), lam = float32(s - i0), for d = 0 .. n_out - 1."""
+    r = np.float32(r)
+    d = np.arange(n_out, dtype=np.float32) + np.float32(0.5)
+    plain = (r * d).astype(np.float32) - np.float32(0.5)
+    fma = (np.float64(r) * d.astype(np.float64) - 0.5).astype(np.float32)
+    out = []
+    for s in (plain, fma):
+        s = np.maximum(s.astype(np.float32), np.float32(0.0))
+        i0 = np.minimum(s.astype(np.int64), n_in - 1)
+        i1 = i0 + (i0 < n_in - 1)
+        lam = (s - i0.astype(np.float32)).astype(np.float32)
+        out.append((i0, i1, lam))
+    return out
+
+
+def resize_step(n_in, full, r):
+    """The source step the kernels use: r when positive, else float32(n_in) / float32(full) (recompute_scale_factor)."""
+    return float(np.float32(r)) if r > 0 else float(np.float32(n_in) / np.float32(full))
+
+
+class MaskRef(object):
+    """Bilinear-resized reference of every detection (resize_reference)."""
+
+    def __init__(self, dets, vals, H, W, full_hw, r_yx, out_hw, thr, proto_bytes):
+        self.dets, self.vals, self.H, self.W = dets, vals, H, W
+        self.full_hw, self.r_yx, self.out_hw = tuple(full_hw), tuple(r_yx), tuple(out_hw)
+        self.thr = float(np.float32(thr))
+        self.frame = (min(out_hw[0], full_hw[0]), min(out_hw[1], full_hw[1]))
+        self.proto_bytes = proto_bytes
+
+
+def _axis_range(forms, w0, w1):
+    """Output indices whose taps (either form) reach source window [w0, w1): (o0, o1), empty as (0, 0)."""
+    hit = np.zeros(forms[0][0].size, bool)
+    for i0, i1, _ in forms:
+        hit |= ((i0 >= w0) & (i0 < w1)) | ((i1 >= w0) & (i1 < w1))
+    idx = np.nonzero(hit)[0]
+    return (int(idx[0]), int(idx[-1]) + 1) if idx.size else (0, 0)
+
+
+def resize_reference(vals, H, W, full_hw, r_yx, out_hw, thr, proto_bytes=64):
+    """Per detection, the float64 bilinear values and bounds over the output pixels its window reaches, inside the valid
+    frame min(out, full); all other output pixels are exactly 0.  r_yx: source steps (<= 0: in / out)."""
+    fh, fw = int(full_hw[0]), int(full_hw[1])
+    ry, rx = resize_step(H, fh, r_yx[0]), resize_step(W, fw, r_yx[1])
+    vh, vw = min(int(out_hw[0]), fh), min(int(out_hw[1]), fw)
+    fy, fx = src_index(ry, vh, H), src_index(rx, vw, W)
+    same = all(np.array_equal(a, b) for f in (fy, fx) for a, b in zip(f[0], f[1]))     # FMA contraction changes nothing
+    dets = []
+    for d in vals:
+        y0, y1, x0, x1 = d.win
+        oy = _axis_range(fy, y0, y1) if y1 > y0 else (0, 0)
+        ox = _axis_range(fx, x0, x1) if x1 > x0 else (0, 0)
+        if oy[1] == oy[0] or ox[1] == ox[0]:
+            dets.append(((0, 0), (0, 0), np.zeros((0, 0)), np.zeros((0, 0))))
+            continue
+        res = []
+        for k, ((yi0, yi1, ly), (xi0, xi1, lx)) in enumerate(zip(fy, fx)):
+            if k == 1 and same:
+                res.append(res[0])
+                break
+            yi0, yi1, ly = yi0[oy[0]:oy[1]], yi1[oy[0]:oy[1]], ly[oy[0]:oy[1]]
+            xi0, xi1, lx = xi0[ox[0]:ox[1]], xi1[ox[0]:ox[1]], lx[ox[0]:ox[1]]
+            hy, hx = (np.float32(1) - ly).astype(np.float64), (np.float32(1) - lx).astype(np.float64)
+            ly, lx = ly.astype(np.float64), lx.astype(np.float64)
+
+            def tap(a, iy, ix):
+                oky = ((iy >= y0) & (iy < y1)).astype(np.float64)
+                okx = ((ix >= x0) & (ix < x1)).astype(np.float64)
+                t = a[np.clip(iy - y0, 0, y1 - y0 - 1)][:, np.clip(ix - x0, 0, x1 - x0 - 1)]
+                return t * oky[:, None] * okx[None, :]
+            wts = ((hy[:, None] * hx[None, :], yi0, xi0), (hy[:, None] * lx[None, :], yi0, xi1),
+                   (ly[:, None] * hx[None, :], yi1, xi0), (ly[:, None] * lx[None, :], yi1, xi1))
+            v = np.zeros((oy[1] - oy[0], ox[1] - ox[0]))
+            b = np.zeros_like(v)
+            mag = np.zeros_like(v)
+            for wt, iy, ix in wts:
+                tv, tb = tap(d.v, iy, ix), tap(d.b, iy, ix)
+                v += wt * tv
+                b += np.abs(wt) * tb
+                mag += np.abs(wt) * (np.abs(tv) + tb)
+            res.append((v, b + BILINEAR_ERR * mag))
+        (va, ba), (vb, bb) = res
+        dets.append((oy, ox, 0.5 * (va + vb), np.maximum(ba, bb) + 0.5 * np.abs(va - vb)))
+    return MaskRef(dets, vals, H, W, (fh, fw), (ry, rx), out_hw, thr, proto_bytes)
+
+
+def mask_reference(protos, cofs, boxes, roi_scale4, full_hw, r_yx, out_hw, thr, family='scalar'):
+    """The whole mask chain of the fused kernel (mask_values, then resize_reference)."""
+    P = protos.detach().cpu() if hasattr(protos, 'detach') else protos
+    vals = mask_values(P, cofs, boxes, roi_scale4, family)
+    pb = 64 if str(getattr(P, 'dtype', '')).endswith('float16') else 128
+    return resize_reference(vals, P.shape[1], P.shape[2], full_hw, r_yx, out_hw, thr, proto_bytes=pb)
+
+
+def reference_bits(ref, n_planes, plane_h, words):
+    """int32 bit planes [n_planes, plane_h, words] holding the reference's decision v > thr (ambiguous pixels included):
+    what a correct kernel writes up to the ambiguous pixels."""
+    px = np.zeros((n_planes, plane_h, words * 32), bool)
+    for n, (oy, ox, v, _) in enumerate(ref.dets[:n_planes]):
+        if oy[1] > oy[0]:
+            px[n, oy[0]:oy[1], ox[0]:ox[1]] = v > ref.thr
+    return np.packbits(px, axis=-1, bitorder='little').view(np.int32).reshape(n_planes, plane_h, words)
+
+
+def _tile_of(ref, y, x, tile_r):
+    from sipmask_b200.postproc import fused_mask_tile
+    TY, TW, _ = fused_mask_tile(*(tile_r or ref.r_yx), proto_bytes=ref.proto_bytes)
+    sy = int(src_index(ref.r_yx[0], y + 1, ref.H)[0][0][y])
+    sx = int(src_index(ref.r_yx[1], x + 1, ref.W)[0][0][x])
+    return 'fused tile (%d,%d) of %dx%d words, source pixel (%d,%d) in 8x64 dense tile (%d,%d)' % (
+        y // TY, x // (32 * TW), TY, TW, sy, sx, sy // 8, sx // 64)
+
+
+def check_mask_bits(bits, ref, count, cap=MASK_AMBIGUOUS_CAP, what='masks', tile_r=None):
+    """Bit planes int32 [N, plane_h, words] (pixel x = bit x & 31 of word x >> 5) against a MaskRef of (at least) the first
+    `count` detections: every non-ambiguous bit equals the reference, the ambiguous fraction of in-frame pixels stays
+    below `cap`, everything outside the frame min(out, full) (bits past out_w of the last word included) and every plane
+    at or past `count` is 0.  Returns dict(ambiguous=fraction, margin=smallest |v - thr| / bound of a decided pixel,
+    pixels=in-frame pixels checked); raises BoundError naming the first wrong bit."""
+    a = bits.detach().cpu().numpy() if hasattr(bits, 'detach') else np.asarray(bits)
+    a = np.ascontiguousarray(a).view(np.uint32)
+    Np, ph, words = a.shape
+    count = min(max(int(count), 0), Np)
+    if a[count:].any():
+        n, y, wq = (int(i[0]) for i in np.nonzero(a[count:]))
+        raise BoundError('%s: plane %d at or past the count %d is not zero (row %d, word %d = %#x)' % (
+            what, count + n, count, y, wq, int(a[count + n, y, wq])))
+    vh, vw = ref.frame
+    assert vh <= ph and vw <= 32 * words, (ref.frame, a.shape)
+    thr = ref.thr
+    amb_total, margin = 0, float('inf')
+    for n in range(count):
+        px = np.unpackbits(a[n].view(np.uint8), axis=-1, bitorder='little').reshape(ph, 32 * words).astype(bool)
+        outside = px.copy()
+        outside[:vh, :vw] = False
+        if outside.any():
+            y, x = (int(i[0]) for i in np.nonzero(outside))
+            raise BoundError('%s: detection %d has a set bit outside the %dx%d frame at (y %d, x %d)' % (what, n, vh, vw, y, x))
+        oy, ox, v, b = ref.dets[n]
+        got = px[:vh, :vw]
+        bad = got.copy()
+        if oy[1] > oy[0]:
+            bad[oy[0]:oy[1], ox[0]:ox[1]] = False
+            g = got[oy[0]:oy[1], ox[0]:ox[1]]
+            d = np.abs(v - thr)
+            amb = d <= b
+            wrong = (g != (v > thr)) & ~amb
+            amb_total += int(amb.sum())
+            dec = ~amb & (b > 0)
+            if dec.any():
+                margin = min(margin, float((d[dec] / b[dec]).min()))
+            if wrong.any():
+                i, j = (int(t[0]) for t in np.nonzero(wrong))
+                raise BoundError('%s: detection %d, y %d, x %d: bit %d, reference %.9g %s thr %.9g with bound %.3g '
+                                 '(%.3g bounds away); %s' % (
+                                     what, n, oy[0] + i, ox[0] + j, int(g[i, j]), v[i, j], '>' if v[i, j] > thr else '<=', thr,
+                                     b[i, j], d[i, j] / b[i, j] if b[i, j] > 0 else float('inf'),
+                                     _tile_of(ref, oy[0] + i, ox[0] + j, tile_r)))
+        if bad.any():
+            y, x = (int(i[0]) for i in np.nonzero(bad))
+            raise BoundError('%s: detection %d, y %d, x %d: bit set where the reference is exactly 0; %s' % (
+                what, n, y, x, _tile_of(ref, y, x, tile_r)))
+    pixels = count * vh * vw
+    frac = amb_total / pixels if pixels else 0.0
+    if frac > cap:
+        raise BoundError('%s: %.3g of the in-frame pixels are ambiguous (cap %.3g): the bound is too loose' % (what, frac, cap))
+    return dict(ambiguous=frac, margin=margin, pixels=pixels)
+
+
+def check_mask_values(out, vals, what='pos_masks'):
+    """Dense cropped masks [N, H, W] (fp32 or fp16) against mask_values: |out - v| <= bound (plus half an fp16 spacing for
+    fp16 outputs) inside the crop, exactly 0 outside it.  Returns the worst |out - v| / bound."""
+    o = out.detach().cpu() if hasattr(out, 'detach') else out
+    fp16 = str(o.dtype).endswith('float16')
+    a = np.asarray(o.float().numpy() if hasattr(o, 'numpy') else o, np.float64)
+    assert a.shape[0] >= len(vals), (a.shape, len(vals))
+    worst = 0.0
+    for n, d in enumerate(vals):
+        y0, y1, x0, x1 = d.win
+        rest = a[n].copy()
+        rest[y0:y1, x0:x1] = 0.0
+        if rest.any():
+            y, x = (int(i[0]) for i in np.nonzero(rest))
+            raise BoundError('%s: detection %d, y %d, x %d: %r outside the crop (must be 0)' % (what, n, y, x, a[n, y, x]))
+        if y1 == y0:
+            continue
+        g = a[n, y0:y1, x0:x1]
+        bound = d.b.copy()
+        if fp16:
+            bound += 0.5 * fp16_spacing(torch.from_numpy(d.v + d.b)).numpy()
+        err = np.abs(g - d.v)
+        ratio = np.where(err == 0, 0.0, err / np.where(bound > 0, bound, 1e-300))
+        i = int(np.argmax(ratio))
+        r = float(ratio.reshape(-1)[i])
+        if not r <= 1.0:
+            y, x = divmod(i, x1 - x0)
+            raise BoundError('%s: detection %d, y %d, x %d (8x64 tile %d,%d): out %r, ref %r, bound %.3g' % (
+                what, n, y0 + y, x0 + x, (y0 + y) // 8, (x0 + x) // 64, g[y, x], d.v[y, x], bound[y, x]))
+        worst = max(worst, r)
+    return worst

@@ -518,15 +518,19 @@ __device__ __forceinline__ void load_a_frag(uint32_t addr, int sw, uint32_t (&a)
 }
 
 // B fragments of column n = g: cof32 = the 32 fp32 coefficients of (detection, cell); b0 = (k 2t..2t+1, n), b1 = (k 2t+8..2t+9, n).
-// hi = fp16(c), lo = fp16(c - hi); |c| is clamped to the fp16 range first (a coefficient beyond 6e4 saturates the sigmoid
-// through any non-zero prototype anyway).
-__device__ __forceinline__ void load_b_frag(const float* __restrict__ cof32, int t, bool valid, uint32_t (&bh)[2][2], uint32_t (&bl)[2][2]) {
+// hi = fp16(c), lo = fp16(c - hi).  fp16 holds |c| <= 65504 only: the MMA operands are clamped to +-65000 (no inf, so the
+// other columns stay finite) and the return value flags a coefficient of this lane beyond that.  The callers send every
+// pixel of such a detection to the scalar cold path, which reads the fp32 coefficients as they are: with small prototypes
+// a coefficient of 1e5 gives an ordinary logit, and the clamped one would give a different mask.
+__device__ __forceinline__ bool load_b_frag(const float* __restrict__ cof32, int t, bool valid, uint32_t (&bh)[2][2], uint32_t (&bl)[2][2]) {
+  bool beyond = false;
 #pragma unroll
   for (int ks = 0; ks < 2; ++ks) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float2 v = make_float2(0.f, 0.f);
       if (valid) v = __ldg(reinterpret_cast<const float2*>(cof32 + ks * 16 + h * 8 + 2 * t));
+      beyond |= fmaxf(fabsf(v.x), fabsf(v.y)) > 65000.f;
       v.x = fminf(fmaxf(v.x, -65000.f), 65000.f);
       v.y = fminf(fmaxf(v.y, -65000.f), 65000.f);
       const __half2 hi = __floats2half2_rn(v.x, v.y);
@@ -536,6 +540,13 @@ __device__ __forceinline__ void load_b_frag(const float* __restrict__ cof32, int
       bl[ks][h] = *reinterpret_cast<const uint32_t*>(&lo);
     }
   }
+  return beyond;
+}
+
+// Detection slot t (accumulator columns 2t, 2t + 1) has a coefficient beyond the fp16 range in the B columns loaded by
+// load_b_frag: those columns belong to lanes 8t .. 8t + 7 (g = 2t, 2t + 1).  All 32 lanes must call it.
+__device__ __forceinline__ bool slot_beyond_fp16(bool lane_beyond, int t) {
+  return ((__ballot_sync(0xffffffffu, lane_beyond) >> (8 * t)) & 0xffu) != 0u;
 }
 
 // sigmoid for the tensor-core kernels: ex2.approx + rcp.approx (4 instructions, |error| < 3e-7; the IEEE division of
@@ -669,13 +680,15 @@ __global__ void __launch_bounds__(MA_THREADS2, 4) mask_assemble_mma_kernel(
     for (int j0 = 0; j0 < cnt; j0 += 4) {
       // B side: this lane feeds column n = g: detection slot g >> 1, idx_w = g & 1, row half of THIS row in that roi
       uint32_t bh[2][2], bl[2][2];
+      bool beyond;
       {
         const int jb = j0 + (g >> 1);
         const bool vb = jb < cnt;
         const int js = vb ? jb : j0;
         const int hb = (hf - s_box[js].y1 >= s_box[js].roi_h) ? 1 : 0;          // min(idx_h, 1)
-        load_b_frag(cofs + (size_t)s_det[js] * 128 + (hb * 2 + (g & 1)) * 32, t, vb, bh, bl);
+        beyond = load_b_frag(cofs + (size_t)s_det[js] * 128 + (hb * 2 + (g & 1)) * 32, t, vb, bh, bl);
       }
+      beyond = slot_beyond_fp16(beyond, t);
       // C side: accumulator columns 2t, 2t+1 = detection slot t, idx_w 0 / 1
       const int jc = j0 + t;
       const bool vc = jc < cnt;
@@ -684,7 +697,7 @@ __global__ void __launch_bounds__(MA_THREADS2, 4) mask_assemble_mma_kernel(
       const int n = s_det[js];
       RowSel rsel;
       rsel.row_in = vc & (hf >= b.y1) & (hf < b.y2);
-      rsel.rare = rsel.row_in & (hf - b.y1 >= b.roi_h + b.roi_h);
+      rsel.rare = rsel.row_in & ((hf - b.y1 >= b.roi_h + b.roi_h) | beyond);
       rsel.x0f = seg_x0;
       OT* dst = out + ((size_t)n * H + h) * W + x0t + wseg + g;
 #pragma unroll 1
@@ -816,11 +829,13 @@ __global__ void __launch_bounds__(MF_THREADS, 4) mask_fused_pack_mma_kernel(
         const bool vb = jb < cnt;
         const int jsb = vb ? jb : j0;
         const float bb_y1 = s_box[jsb].y1, bb_roi_h = s_box[jsb].roi_h;
+        bool beyond;
         {
           const float* cb = cofs + (size_t)s_det[jsb] * 128 + (g & 1) * 32;
-          load_b_frag(cb, t, vb, bh0, bl0);
-          load_b_frag(cb + 64, t, vb, bh1, bl1);
+          beyond = load_b_frag(cb, t, vb, bh0, bl0);
+          beyond |= load_b_frag(cb + 64, t, vb, bh1, bl1);
         }
+        beyond = slot_beyond_fp16(beyond, t);
         // C side: detection slot t
         const int jc = j0 + t;
         const bool vc = jc < cnt;
@@ -833,7 +848,7 @@ __global__ void __launch_bounds__(MF_THREADS, 4) mask_fused_pack_mma_kernel(
           const float hf = win_y0 + (float)r;
           RowSel rsel;
           rsel.row_in = vc & (hf >= b.y1) & (hf < b.y2);
-          rsel.rare = rsel.row_in & (hf - b.y1 >= roi_h2);
+          rsel.rare = rsel.row_in & ((hf - b.y1 >= roi_h2) | beyond);
           rsel.x0f = win_x0;
           const float run_x0 = win_x0 + (float)(m * 16), run_x1 = run_x0 + 15.f;
           const bool any_in = __any_sync(0xffffffffu, rsel.row_in & (run_x1 >= b.x1) & (run_x0 < b.x2));

@@ -464,6 +464,35 @@ def mask_assemble_pack(protos, cofs, boxes, box_scale, out_hw, thr=0.4, layout='
     return out
 
 
+@L.device_guard
+def mask_assemble_pack_dev(protos, cofs, boxes, geom, tile_r, cap_hw, thr=0.4, layout='hwc', out=None):
+    """The engine's fused mask call (smb_mask_assemble_pack_dev): roi scale, resize and canvas read from the device row
+    `geom` (int32 words of an smb_img_geom_t, see geom_row) when the kernel runs; the tile is sized for the source steps
+    tile_r = (max_ry, max_rx), which must be at least the row's.  Bit planes int32 [N, cap_h, ceil(cap_w / 32)]."""
+    _need_cuda(protos, cofs, boxes, geom)
+    protos = protos.contiguous()
+    if layout == 'chw':
+        _, H, W = protos.shape
+    else:
+        H, W, _ = protos.shape
+    N = cofs.shape[0]
+    cofs = cofs.float().contiguous()
+    boxes = boxes.float().contiguous()
+    cap_h, cap_w = int(cap_hw[0]), int(cap_hw[1])
+    if out is None:
+        out = torch.empty((N, cap_h, (cap_w + 31) // 32), dtype=torch.int32, device=protos.device)
+    L.check(L.lib().smb_mask_assemble_pack_dev(L.ptr(protos), _dt(protos), 1 if layout == 'hwc' else 0, L.ptr(cofs),
+                                               L.ptr(boxes), L.ptr(geom), ctypes.c_float(tile_r[0]), ctypes.c_float(tile_r[1]),
+                                               L.ptr(out), H, W, N, cap_h, cap_w, ctypes.c_float(thr), L.stream_ptr()),
+            'smb_mask_assemble_pack_dev')
+    return out
+
+
+def geom_row(g, device):
+    """An smb_img_geom_t (postproc.image_geometry) as the device row of int32 words the *_dev entry points read."""
+    return torch.from_numpy(np.frombuffer(bytes(g), dtype=np.int32).copy()).to(device)
+
+
 def unpack_mask_bits(bits, out_w):
     """int32 [N,h,words] -> uint8 [N,h,out_w] (host or device tensor); used by tests and result conversion."""
     b = bits.view(torch.uint8) if bits.dtype == torch.int32 else bits

@@ -14,7 +14,8 @@ from oracle import numerics as NU
 
 pytestmark = pytest.mark.gpu
 
-POSTPROC = {'gather_cofs', 'mask_fused', 'mask_dense', 'gather_track', 'decode_topk', 'nms'}      # bit-exact elsewhere
+POSTPROC = {'gather_cofs', 'gather_track', 'decode_topk', 'nms'}      # bit-exact elsewhere
+MASKS = ('mask_fused', 'mask_dense')
 PATCHED = ('image_to_s2d16', 'maxpool3x3s2', 'upsample_bilinear', 'groupnorm_relu_apply_multi', 'offset_conv1x1_multi',
            'deform_im2col', 'deform_im2col_multi')
 
@@ -247,6 +248,32 @@ def _check_rescore(eng, pos, count, labels, det, out):
                 tight=res['score bound / 1e-2 bound'])
 
 
+def _mask_inputs(eng, n):
+    """Image n's mask operands as the engine holds them: fp16 prototypes [32, H, W], coefficients, rois, geometry row,
+    count, and the kernel family the fp16 prototypes run on."""
+    from sipmask_b200 import _lib as L, ops
+    gm = L.ImgGeom.from_buffer_copy(eng.geom[n].cpu().numpy().tobytes())
+    k = min(max(int(eng.count[n]), 0), eng.max_num)
+    family = 'tensor' if ops.set_mask_tensor_dot(None) else 'scalar'
+    return eng.protos[n].permute(2, 0, 1).cpu(), eng.det_cofs[n].cpu(), eng.det_boxes4[n].cpu(), gm, k, family
+
+
+def _check_mask_fused(eng, n):
+    """mask_bits[n] against the float64 reference of the engine's own operands (oracle/numerics.py check_mask_bits)."""
+    protos, cofs, boxes, gm, k, family = _mask_inputs(eng, n)
+    ref = NU.mask_reference(protos, cofs[:k], boxes[:k], list(gm.roi_scale), (gm.full_h, gm.full_w), (gm.ry, gm.rx),
+                            (gm.out_h, gm.out_w), eng.mask_thr, family)
+    st = NU.check_mask_bits(eng.mask_bits[n], ref, k, what='mask_fused image %d' % n, tile_r=eng.mask_tile_r)
+    return dict(ratio=0.0, ambiguous=st['ambiguous'], margin=st['margin'], count=k)
+
+
+def _check_mask_dense(eng, n):
+    """pos_masks[n] (fp16, every row: rows past the count have empty rois) within the bounds of the float64 values."""
+    protos, cofs, boxes, gm, k, family = _mask_inputs(eng, n)
+    vals = NU.mask_values(protos, cofs, boxes, list(gm.roi_scale), family)
+    return dict(ratio=NU.check_mask_values(eng.pos_masks[n], vals, what='mask_dense image %d' % n), count=k)
+
+
 # ------------------------------------------------------------------------------------------------------- the audit
 def audit(eng, log=print):
     """Steps through eng.ops; returns {kind: [ratio, misrounded, count]} and checks the graph replay afterwards."""
@@ -317,6 +344,21 @@ def audit(eng, log=print):
                 continue
             if name in POSTPROC:
                 f()
+                continue
+            if name in MASKS:
+                n = f.__defaults__[0]                     # the image the per-image closure was built for
+                out = eng.mask_bits[n] if name == 'mask_fused' else eng.pos_masks[n]
+                if out.dtype == torch.int32:
+                    out.fill_(-1)                         # poison: the memset node and the kernel must rewrite every word
+                guard.prepare([out])
+                f()
+                torch.cuda.synchronize()
+                guard.verify('op %d %s image %d' % (i, name, n))
+                st = _check_mask_fused(eng, n) if name == 'mask_fused' else _check_mask_dense(eng, n)
+                if 'ambiguous' in st:
+                    log('     %s image %d: %d masks, ambiguous %.2e, margin %.3g' % (name, n, st['count'], st['ambiguous'],
+                                                                                 st['margin']))
+                note(name, i, '%s image %d' % (name, n), tuple(out.shape), None, st)
                 continue
             if name == 'conv':
                 plan = f.__self__

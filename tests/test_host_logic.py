@@ -85,11 +85,14 @@ def test_fp16_hi_lo_coefficient_split_keeps_fp32_logits():
     hi = fp16(c), lo = fp16(c - hi): 22 mantissa bits for |c| >= 0.125; below that lo is an fp16 subnormal and the error is
     absolute, <= 2^-25 per coefficient.  A numpy model of that split with fp32 accumulation stays within
     2^-21 * sum|p c| + 2^-24 * sum|p| of the float64 dot product - the same order as the sequential fp32 fmaf of the scalar
-    kernels - including tiny coefficients and coefficients clamped at the fp16 range."""
+    kernels - including tiny coefficients and coefficients up to the fp16 range.  A row with a coefficient beyond +-65000
+    (which fp16 cannot hold) is evaluated by the kernels' scalar cold path on the fp32 coefficients as they are: the
+    sequential model holds it against the unclamped dot product."""
     rng = np.random.RandomState(1)
     p = np.maximum(rng.randn(4096, 32), 0).astype(np.float16)                  # prototypes: fp16 storage
     for scale in (1.0, 1e-3, 40.0, 3e4):
         c = (rng.randn(4096, 32) * scale).astype(np.float32)
+        beyond = np.abs(c).max(1) > 65000.0                                     # rows the kernels send to the cold path
         cc = np.clip(c, -65000.0, 65000.0)
         hi = cc.astype(np.float16)
         lo = (cc - hi.astype(np.float32)).astype(np.float16)
@@ -101,11 +104,15 @@ def test_fp16_hi_lo_coefficient_split_keeps_fp32_logits():
             acc = acc + p[:, k].astype(np.float32) * lo[:, k].astype(np.float32)
         bound = (np.abs(p.astype(np.float64) * cc.astype(np.float64))).sum(1) * 2.0 ** -21 + \
             np.abs(p.astype(np.float64)).sum(1) * 2.0 ** -24 + 1e-9
-        assert (np.abs(acc.astype(np.float64) - exact) <= bound).all(), scale
+        assert (np.abs(acc.astype(np.float64) - exact) <= bound)[~beyond].all(), scale
+        exact = (p.astype(np.float64) * c.astype(np.float64)).sum(1)
+        bound = (np.abs(p.astype(np.float64) * c.astype(np.float64))).sum(1) * 2.0 ** -21 + \
+            np.abs(p.astype(np.float64)).sum(1) * 2.0 ** -24 + 1e-9
         seq = np.zeros(4096, np.float32)
         for k in range(32):                                                    # the scalar kernels' arithmetic
-            seq = seq + p[:, k].astype(np.float32) * cc[:, k]
+            seq = seq + p[:, k].astype(np.float32) * c[:, k]
         assert (np.abs(seq.astype(np.float64) - exact) <= bound).all(), scale
+    assert beyond.any()
 
 
 
