@@ -524,6 +524,37 @@ int smb_ytvis_match_dev(const smb_ytvis_entry_t* ents, int n_ent, const smb_ytvi
                         const double* host_iou_thr, const double* host_area_rng, smb_coco_out_t* out, int64_t n_out,
                         int* npig, int* status, void* workspace, size_t workspace_bytes, smb_stream_t stream);
 
+/* ------------------------------------------------------------------ segmentations to bit planes on the device
+ * What pycocotools' rleFrPoly / rleFrBbox / rleFrString followed by rleDecode compute, as the bit planes the evaluators
+ * read (row-major [h, pitch] uint32, pixel x = bit x&31 of word x>>5, bits past w zero), without a sort: a column-major
+ * mask is the parity of the number of run boundaries at or before each pixel, so every boundary toggles one bit of a
+ * column-major scratch bitmap and a prefix XOR fills it.
+ *
+ * One item: a polygon (kind 0: n vertices, float64 x,y pairs from vertex `off` of the vertex pool; an frBbox box is its
+ * four-vertex polygon) or column-major run lengths (kind 1: n uint32 counts from `off` of the count pool, zeros first),
+ * in an h x w canvas, OR-ed into plane `plane` of the launch.  Items of one plane are adjacent (annToRLE's merge of an
+ * annotation's polygons).  The caller guarantees 5 * |coordinate| < 2^29 and that run lengths sum to h * w. */
+typedef struct {
+  int32_t kind;
+  int32_t plane;
+  int64_t off, n;
+  int32_t h, w;
+} smb_segm_item_t;
+#define SMB_SEGM_RANGE 1   /* status: an item's pool range, plane index or canvas is outside what the launch owns */
+
+/* Zeroes planes [n_planes, plane_stride_words] and rasterizes the items into them on `stream` (memsets and three
+ * launches, no allocation or synchronisation; graph-capturable).  n_xy: vertices in xy_pool; max_hw / max_w: the largest
+ * h * w (< 2^31) and w of any item, which size the workspace (>= smb_segm_raster_workspace_bytes).  area / ext (either may
+ * be NULL): plane p's pixel count goes to area[p * area_stride] and its {row0, row1, word0, word1} (half-open, zeros for
+ * an empty plane) to ext[p * ext_stride ...], strides in int32 units, so both can land inside the caller's rows.  An item
+ * that fails a bound writes nothing and sets SMB_SEGM_RANGE in *status. */
+size_t smb_segm_raster_workspace_bytes(int n_items, int64_t max_hw, int max_w);
+int smb_segm_raster_dev(const smb_segm_item_t* items, int n_items, const double* xy_pool, int64_t n_xy,
+                        const uint32_t* count_pool, int64_t n_counts, int64_t max_hw, int max_w, uint32_t* planes,
+                        int n_planes, int64_t plane_stride_words, int pitch, int32_t* area, int64_t area_stride,
+                        int32_t* ext, int64_t ext_stride, int* status, void* workspace, size_t workspace_bytes,
+                        smb_stream_t stream);
+
 /* gather rows: dst[i,:] = src[idx[i],:] for i < *count (device count), zero otherwise. */
 int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev,
                         int max_rows, int row_elems, float* dst, smb_stream_t stream);

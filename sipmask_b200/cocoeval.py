@@ -1,10 +1,11 @@
 """COCO box and mask AP on the device: pycocotools 2.0 COCOeval (iouType 'bbox' / 'segm', default Params) as MM's
 CocoDataset.evaluate (SipMask-mmdetection/mmdet/datasets/coco.py:290-392) and SipMask-benchmark's coco_eval.py run it.
 
-Host: the ground truth (CocoGroundTruth: pycocotools COCO's indexing, annToRLE through the library's C restatement of
-rleFrPoly / rleFrString) and summarize (numpy, the code of COCOeval.summarize).  Device (csrc/cocoeval.cu): the result
+Host: the ground truth (CocoGroundTruth: pycocotools COCO's indexing; annToRLE through the library's C restatement of
+rleFrPoly / rleFrString as the public host rasterizer, segm_plane) and summarize (numpy, the code of COCOeval.summarize).
+Device: the masks of ground truth and result files (csrc/segm_raster.cu, from packed vertices and run lengths), the result
 json's values from the engine record, computeIoU + evaluateImg for every (image, category) after every batch, and
-accumulate's precision / recall / scores arrays at evaluate().
+accumulate's precision / recall / scores arrays at evaluate() (csrc/cocoeval.cu).
 
 Restated only: pycocotools is neither vendored in the reference nor installed where this was written, so the semantics
 are pycocotools 2.0's as read from its source, not pinned by running it.
@@ -185,6 +186,22 @@ class CocoGroundTruth:
                 rows[r]['ext'] = ext
         return rows, np.cumsum(cnt).astype(np.int32), planes
 
+    def packed(self, img_id):
+        """image()'s rows and offsets with the segmentations packed for the device rasterizer instead of rasterized:
+        (rows with area_mask / ext left zero, per-category offsets [K+1], segm_raster.SegmPack with row r's
+        segmentation in plane r).  Raises what image() raises, from the numbers alone."""
+        from .segm_raster import SegmPack
+        rows, off, _ = self.image(img_id, masks=False)
+        h, w = self.hw[img_id]
+        anns = self.anns[img_id]
+        pack = SegmPack()
+        for r, i in enumerate(sorted(range(len(anns)), key=lambda i: self.cat_index[anns[i]['cat']])):
+            a = anns[i]
+            if a['segmentation'] is None:
+                raise ValueError('CocoGroundTruth: annotation %d has no segmentation' % a['id'])
+            pack.add(a['segmentation'], h, w, r, 'annotation %d' % a['id'])
+        return rows, off, pack
+
 
 # ---------------------------------------------------------------------------------------------------- summarize (host)
 def summarize(precision, recall, area_rng_lbl=AREA_RNG_LBL, max_dets=MAX_DETS):
@@ -294,6 +311,7 @@ class CocoEvaluator:
         self.npig = {m: torch.zeros(self.K * 4, dtype=torch.int32, device=self.dev) for m in metrics}
         self.rows = {m: [] for m in metrics}
         self.status = torch.zeros(1, dtype=torch.int32, device=self.dev)
+        self.raster_status = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.n_results = {m: torch.zeros((), dtype=torch.int64, device=self.dev) for m in metrics}
         self.image_ids = []
         self._seen = set()
@@ -313,26 +331,37 @@ class CocoEvaluator:
                                  % (i, tuple(ori_hws[n][:2]), self.gt.hw[i][0], self.gt.hw[i][1]))
         return ids
 
-    def stage_gt(self, image_id, stream=None):
-        """Rasterize one image's ground truth on the host and upload it from pinned memory on `stream` (default: the
-        current stream).  Returns its device tensors, for add_records(..., gts=[...]) on a stream that is ordered after
-        `stream`."""
-        rows, off, planes = self.gt.image(int(image_id), 'segm' in self.metrics)
-        if planes is not None and len(rows):
-            rows['plane'] = np.arange(len(rows), dtype=np.int64) * planes[0].size
+    def stage_gt(self, image_id, stream=None, masks=None):
+        """Pack one image's ground truth (rows, per-category offsets and, for 'segm', what describes its masks: polygon
+        vertices and run lengths) and upload it from pinned memory on `stream` (default: the current stream); its planes
+        are reserved on the device and rasterized there right before the image's first segm match.  Returns its device
+        tensors, for add_records(..., gts=[...]) on a stream that is ordered after `stream`.  masks: whether the masks
+        are needed (default: when 'segm' is evaluated)."""
+        from . import segm_raster as SR
+        image_id = int(image_id)
+        segm = 'segm' in self.metrics if masks is None else bool(masks)
+        rows, off, pack = self.gt.packed(image_id) if segm else self.gt.image(image_id, False)[:2] + (None,)
+        h, w = self.gt.hw[image_id]
+        pitch = (w + 31) // 32
         n_gt = len(rows)
-        host = dict(rows=torch.from_numpy(np.ascontiguousarray(rows).view(np.uint8).reshape(-1) if n_gt
-                                          else np.zeros(GT_DTYPE.itemsize, np.uint8)),
-                    off=torch.from_numpy(off),
-                    planes=torch.from_numpy(planes.reshape(-1).view(np.int32) if planes is not None and planes.size
-                                            else np.zeros(1, np.int32)))
+        if segm:
+            rows['plane'] = np.arange(n_gt, dtype=np.int64) * (h * pitch)
         stream = stream or torch.cuda.current_stream(self.dev)
         with torch.cuda.device(self.dev), torch.cuda.stream(stream):
-            dev = {k: v.pin_memory().to(self.dev, non_blocking=True) for k, v in host.items()}
-        dev['n_gt'] = n_gt
-        dev['plane_words'] = int(planes.size) if planes is not None else 0
-        dev['stream'] = stream
-        return dev
+            st, (rows_dev, off_dev) = SR.staged(pack if segm else SR.SegmPack(), self.dev, (rows, off))
+            planes = torch.empty(max(n_gt * h * pitch, 1) if segm else 1, dtype=torch.int32, device=self.dev)
+        return dict(rows=rows_dev, off=off_dev.view(torch.int32), planes=planes, n_gt=n_gt,
+                    plane_words=n_gt * h * pitch if segm else 0, stream=stream,
+                    raster=dict(st, stride=h * pitch, pitch=pitch) if segm and n_gt else None)
+
+    def _raster_gt(self, gt):
+        """Rasterize a staged ground truth into its planes on the current stream, with each plane's pixel count and
+        extents written into its row."""
+        from . import segm_raster as SR
+        r, gt['raster'] = gt['raster'], None
+        rows = gt['rows'].view(torch.int32)              # smb_coco_gt_t: area_mask is int32 15, ext 16..19 of 20
+        SR.raster(r, gt['planes'], gt['n_gt'], r['stride'], r['pitch'], self.raster_status, area=rows[15:],
+                  area_stride=GT_DTYPE.itemsize // 4, ext=rows[16:], ext_stride=GT_DTYPE.itemsize // 4)
 
     def _match(self, metric, imgs, n, dets, det_cap, det_planes, det_plane_words, gt, out_rows):
         """The match launch of image n of a batch (imgs / dets: the batch's device rows) on the current stream."""
@@ -341,6 +370,8 @@ class CocoEvaluator:
         if gt['stream'] != cur:                          # uploaded on another stream: keep it until this stream is done
             for key in ('rows', 'off', 'planes'):
                 gt[key].record_stream(cur)
+        if metric == 'segm' and gt['raster'] is not None:
+            self._raster_gt(gt)
         ws_bytes = lib.smb_coco_match_workspace_bytes(gt['n_gt'])
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
         n_out = out_rows.numel() // OUT_DTYPE.itemsize
@@ -424,12 +455,14 @@ class CocoEvaluator:
             B = len(ids)
             dets = np.zeros(B * det_cap, DET_DTYPE)
             dets['cat'] = -1
-            planes, pbase, pitches = [], 0, []
+            from . import segm_raster as SR
+            # segm: every result's counts go into one launch; the chunk's planes share the largest canvas' stride and pitch
+            pack, rows_of_plane = SR.SegmPack(), []
+            pitch = max([1] + [(self.gt.hw[i][1] + 31) // 32 for i in ids])
+            stride = max([1] + [self.gt.hw[i][0] for i in ids]) * pitch
             n_det = []
             for n, (i, res) in enumerate(zip(ids, (v for _, v in per_image))):
                 h, w = self.gt.hw[i]
-                pitch = (w + 31) // 32
-                pitches.append(pitch)
                 n_det.append(len(res))
                 for j, r in enumerate(res):
                     d = dets[n * det_cap + j]
@@ -447,22 +480,30 @@ class CocoEvaluator:
                             seg = r['segmentation']
                             if not isinstance(seg, dict):
                                 raise ValueError('result of image %d: segmentation must be an RLE dict' % i)
-                            p = segm_plane(seg, h, w, 'result of image %d' % i)
-                            area, ext = plane_stats(p, w)
-                            d['area_mask'], d['ext'], d['plane'] = area, ext, pbase
-                            planes.append(p.reshape(-1))
-                            pbase += p.size
+                            pack.add(seg, h, w, len(rows_of_plane), 'result of image %d' % i)
+                            d['plane'] = len(rows_of_plane) * stride
+                            rows_of_plane.append(n * det_cap + j)
                     except (KeyError, TypeError) as e:
                         raise ValueError('add_results: malformed result %r: %r' % (r, e))
                     d['score'][0 if metric == 'bbox' else 1] = score
                     d['cat'] = self.gt.cat_index.get(cat, -1)
-            imgs = _dev_bytes(self._img_rows(ids, pitches, det_cap, n_det), self.dev)
-            dd = _dev_bytes(dets, self.dev)
-            planes = np.concatenate(planes) if planes else np.zeros(1, np.uint32)
-            pd = torch.from_numpy(planes).to(self.dev)
+            imgs = _dev_bytes(self._img_rows(ids, pitch, det_cap, n_det), self.dev)
+            P = len(rows_of_plane)
+            st, (dd, at) = SR.staged(pack, self.dev, (dets, np.array(rows_of_plane, np.int64)))
+            pd = torch.empty(max(P * stride, 1), dtype=torch.int32, device=self.dev)
+            if P:
+                # pixel counts and extents of the planes, scattered into their rows (smb_coco_det_t: area_mask is
+                # int32 16, ext 18..21 of 24)
+                stats = torch.zeros((P, 5), dtype=torch.int32, device=self.dev)
+                SR.raster(st, pd, P, stride, pitch, self.raster_status, area=stats, area_stride=5, ext=stats[:, 1:],
+                          ext_stride=5)
+                at = at.view(torch.int64)[:P]
+                rows32 = dd.view(torch.int32)[:B * det_cap * 24].view(B * det_cap, 24)
+                rows32[at, 16] = stats[:, 0]
+                rows32[at[:, None], torch.arange(18, 22, device=self.dev)[None]] = stats[:, 1:]
             out = torch.empty(B * det_cap * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
             for n, i in enumerate(ids):
-                self._match(metric, imgs, n, dd, det_cap, pd, planes.size, self.stage_gt(i), out)
+                self._match(metric, imgs, n, dd, det_cap, pd, pd.numel(), self.stage_gt(i, masks=metric == 'segm'), out)
             self.rows[metric].append(out)
 
     # ---- accumulate + summarize
@@ -478,6 +519,8 @@ class CocoEvaluator:
                 raise ValueError('a record label is outside the %d labels of cat_ids' % len(self.label_cat_host))
             if status:
                 raise L.SmbError('COCO evaluation status %d' % status)
+            from .segm_raster import check_status
+            check_status(self.raster_status)
             out, stats, arrays = {}, {}, {}
             for m in self.metrics:
                 if int(self.n_results[m].item()) == 0:
@@ -493,7 +536,8 @@ class CocoEvaluator:
 
 def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None):
     """COCOeval of result lists (coco.coco_json output or a loaded results file) against `gt` on the device: the same
-    kernels as CocoEvaluator, with the detections' RLE strings decoded on the host.  img_ids: the evaluated images
+    kernels as CocoEvaluator, with the detections' RLE strings parsed to run lengths on the host and rasterized on the
+    device.  img_ids: the evaluated images
     (p.imgIds; default every ground-truth image).  As in pycocotools, a result whose image is not in the ground truth
     raises (loadRes), and results of ground-truth images outside img_ids are not evaluated (_prepare).  Returns
     CocoEvaluator.evaluate()'s dict for the metrics given."""

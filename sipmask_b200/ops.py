@@ -611,6 +611,38 @@ def track_assoc(frames, det, labels, count, track_feats, state, match_coeff=(1.0
     return ids
 
 
+def segm_raster_workspace_bytes(n_items, max_hw, max_w):
+    return int(L.lib().smb_segm_raster_workspace_bytes(int(n_items), ctypes.c_int64(int(max_hw)), int(max_w)))
+
+
+@L.device_guard
+def segm_raster(items, n_items, xy, n_xy, counts, n_counts, max_hw, max_w, planes, n_planes, plane_stride, pitch, status,
+                area=None, area_stride=1, ext=None, ext_stride=4, workspace=None):
+    """smb_segm_raster_dev: zero planes [n_planes, plane_stride words] (int32, rows of `pitch` words) and rasterize
+    n_items segmentations into them on the current stream.  items: smb_segm_item_t rows, xy: the float64 vertex pool
+    (n_xy vertices), counts: the uint32 run-length pool, all device tensors (segm_raster.SegmPack builds them); max_hw /
+    max_w: the largest canvas of any item.  area / ext: device int32 tensors whose element p * stride (.. + 3) receives
+    plane p's pixel count / extents.  status: int32 [1], SMB_SEGM_RANGE is OR-ed into it."""
+    _need_cuda(items, planes, status)
+    assert planes.dtype == torch.int32 and planes.is_contiguous() and status.dtype == torch.int32
+    if planes.numel() < int(n_planes) * int(plane_stride):
+        raise ValueError('segm_raster: %d planes of %d words in a tensor of %d' % (n_planes, plane_stride, planes.numel()))
+    for t in (area, ext):                          # views into the caller's rows: only the caller knows their extent
+        if t is not None and (t.dtype != torch.int32 or t.device != planes.device):
+            raise ValueError('segm_raster: area / ext must be int32 tensors on %s' % planes.device)
+    need = segm_raster_workspace_bytes(n_items, max_hw, max_w)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=planes.device)
+    if workspace.device != planes.device or workspace.dtype != torch.uint8 or workspace.numel() < need:
+        raise ValueError('segm_raster: workspace must be a uint8 tensor of >= %d bytes on %s' % (need, planes.device))
+    L.check(L.lib().smb_segm_raster_dev(L.ptr(items), int(n_items), L.ptr(xy), ctypes.c_int64(int(n_xy)), L.ptr(counts),
+                                        ctypes.c_int64(int(n_counts)), ctypes.c_int64(int(max_hw)), int(max_w),
+                                        L.ptr(planes), int(n_planes), ctypes.c_int64(int(plane_stride)), int(pitch),
+                                        L.ptr(area), ctypes.c_int64(int(area_stride)), L.ptr(ext),
+                                        ctypes.c_int64(int(ext_stride)), L.ptr(status), L.ptr(workspace),
+                                        ctypes.c_size_t(workspace.numel()), L.stream_ptr()), 'smb_segm_raster_dev')
+
+
 def host_device_pointer(pinned):
     """The device address of a page-locked host tensor (cudaHostGetDevicePointer), for the current device."""
     if not pinned.is_pinned():

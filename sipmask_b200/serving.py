@@ -973,8 +973,9 @@ class CocoEvalRunner(StreamRunner):
     """StreamRunner plus COCO box and mask AP (pycocotools COCOeval, as CocoDataset.evaluate runs it) from the stream.
 
     submit(img, image_id[, meta]) checks the image against the ground truth (known id, not submitted before, ori_shape
-    equal to the annotation's height x width) before anything is enqueued, then rasterizes the image's ground truth on the
-    host and uploads it from pinned memory on the H2D stream with the image.  Right after each batch's forward, on the
+    equal to the annotation's height x width) before anything is enqueued, then packs the image's ground truth (a
+    malformed segmentation raises here) and uploads it from pinned memory on the H2D stream with the image; its planes are
+    rasterized on the device.  Right after each batch's forward, on the
     slot's stream, the batch's real images are evaluated from the bucket engine's record (cocoeval.CocoEvaluator
     .add_records: the result json's values, IoU and matching on the device).  flush() dispatches the open batch;
     evaluate() accumulates and summarizes every image submitted so far and returns MM's evaluate() dict plus the raw
@@ -1034,7 +1035,8 @@ class VideoEvalRunner(VideoRunner):
 
     submit(frame, video_id, frame_id) takes the video's YouTube-VIS id and checks the frame against the ground truth
     (known video, its height x width, a frame inside its length, a video not evaluated before) before anything is
-    enqueued; it then rasterizes the frame's ground truth on the host and uploads it on the H2D stream with the frame.
+    enqueued; it then packs the frame's ground truth and uploads it on the H2D stream with the frame (the planes are
+    rasterized on the device, with the frame's overlaps).
       - Right after each batch's forward, on the slot's stream: every detection's pixel count and its intersections with
         the frame's ground-truth objects (ytviseval kernel a), from the bucket engine's planes.
       - Right after the association, on the tracker stream: the last detection of each object id is added into its

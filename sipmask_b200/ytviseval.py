@@ -125,6 +125,20 @@ class YtvisGroundTruth:
             rows[r]['g'] = g
         return rows, planes, areas
 
+    def packed_frame(self, video_id, frame_id):
+        """frame()'s rows with the segmentations packed for the device rasterizer instead of rasterized: (rows GTF_DTYPE
+        without plane pointers and extents, segm_raster.SegmPack with row r's segmentation in plane r).  Raises what
+        frame() raises, from the numbers alone."""
+        from .segm_raster import SegmPack
+        v = self.videos[video_id]
+        present = [(g, a) for g, a in enumerate(self.anns[video_id]) if a['segmentations'][frame_id] is not None]
+        rows = np.zeros(len(present), GTF_DTYPE)
+        pack = SegmPack()
+        for r, (g, a) in enumerate(present):
+            pack.add(a['segmentations'][frame_id], v['h'], v['w'], r, 'annotation %d frame %d' % (a['id'], frame_id))
+            rows[r]['g'] = g
+        return rows, pack
+
     def video(self, video_id):
         """The video's ground truth for its sequence match: (rows VGT_DTYPE without sum_area, grouped by category
         index with annotation order inside, per-category offsets [K+1])."""
@@ -145,7 +159,8 @@ class YtvisGroundTruth:
 # ---------------------------------------------------------------------------------------------------- evaluator
 class YtvisEvaluator:
     """Device state of one YouTube-VIS evaluation: a pool of `slots` accumulator slots (one per video being evaluated;
-    objects x max_gts int64 intersections, objects int64 areas and int32 non-zero frame counts each), the evaluated
+    objects x max_gts int64 intersections, objects int64 areas and int32 non-zero frame counts, max_gts int64 ground-truth
+    pixel sums each), the evaluated
     entries' matched / ignored rows and npig per (category, area range).
       gt       : YtvisGroundTruth
       cat_ids  : the category ids result entries may carry (default the ground truth's); any other raises ValueError.
@@ -166,12 +181,14 @@ class YtvisEvaluator:
             self.acc_inter = torch.zeros((S, O, G), dtype=torch.int64, device=self.dev)
             self.acc_area = torch.zeros((S, O), dtype=torch.int64, device=self.dev)
             self.acc_nz = torch.zeros((S, O), dtype=torch.int32, device=self.dev)
+            self.gt_area = torch.zeros((S, G), dtype=torch.int64, device=self.dev)     # per ground truth: sum of its frames' pixels
+            self.raster_status = torch.zeros(1, dtype=torch.int32, device=self.dev)
             self.status = torch.zeros(1, dtype=torch.int32, device=self.dev)
             self.npig = torch.zeros(self.K * 4, dtype=torch.int32, device=self.dev)
         self.rows = []
         self.n_results = 0
         self.video_ids = []                  # ended videos, in end order
-        self._vids = {}                      # video id -> dict(slot, frames, sum_area) while being evaluated
+        self._vids = {}                      # video id -> dict(slot, frames) while being evaluated
         self._iou_thr = np.ascontiguousarray(IOU_THRS, dtype=np.float64)
         self._area_rng = np.ascontiguousarray(np.array(AREA_RNG, dtype=np.float64).reshape(-1))
 
@@ -190,34 +207,38 @@ class YtvisEvaluator:
         self.acc_inter[slot].zero_()
         self.acc_area[slot].zero_()
         self.acc_nz[slot].zero_()
-        self._vids[video_id] = dict(slot=int(slot), frames=0, sum_area=np.zeros(len(self.gt.anns[video_id]), np.int64))
+        self.gt_area[slot].zero_()
+        self._vids[video_id] = dict(slot=int(slot), frames=0)
 
     def abort_video(self, video_id):
         self._vids.pop(video_id, None)
 
     def stage_frame(self, video_id, frame_id, stream=None):
-        """Rasterize one frame's ground truth on the host and upload its planes from pinned memory on `stream` (default:
-        the current stream).  commit_frame() then counts it."""
-        rows, planes, areas = self.gt.frame(video_id, int(frame_id))
+        """Pack what describes one frame's ground-truth masks (polygon vertices, run lengths) and upload it from pinned
+        memory on `stream` (default: the current stream); its planes are reserved on the device and rasterized there by
+        overlap().  commit_frame() then counts the frame."""
+        from . import segm_raster as SR
+        rows, pack = self.gt.packed_frame(video_id, int(frame_id))
         v = self.gt.videos[video_id]
+        pitch = (v['w'] + 31) // 32
+        words = v['h'] * pitch
         stream = stream or torch.cuda.current_stream(self.dev)
         with torch.cuda.device(self.dev), torch.cuda.stream(stream):
-            dev = torch.from_numpy(planes.reshape(-1).view(np.int32) if planes.size else np.zeros(1, np.int32))
-            dev = dev.pin_memory().to(self.dev, non_blocking=True)
+            st, _ = SR.staged(pack, self.dev)
+            planes = torch.empty(max(len(rows) * words, 1), dtype=torch.int32, device=self.dev)
         if len(rows):
-            rows['plane'] = np.uint64(dev.data_ptr()) + np.arange(len(rows), dtype=np.uint64) * np.uint64(planes[0].size * 4)
-        return dict(video_id=video_id, rows=rows, planes=dev, areas=areas, stream=stream, h=v['h'], w=v['w'],
-                    pitch=(v['w'] + 31) // 32)
+            rows['plane'] = np.uint64(planes.data_ptr()) + np.arange(len(rows), dtype=np.uint64) * np.uint64(words * 4)
+        return dict(video_id=video_id, rows=rows, planes=planes, raster=st, stream=stream, h=v['h'], w=v['w'], pitch=pitch)
 
     def commit_frame(self, staged):
-        st = self._vids[staged['video_id']]
-        np.add.at(st['sum_area'], staged['rows']['g'], staged['areas'])
-        st['frames'] += 1
+        self._vids[staged['video_id']]['frames'] += 1
 
     def overlap(self, staged, dets, det_stride, det_pitch, max_num, count=None, n_det=None):
         """Kernel a on the current stream for a batch of frames: staged[n] = frame n's stage_frame, dets[n] = the
         device address of its first detection plane (det_stride / det_pitch words); count: int32 device tensor [N], or
-        n_det: host numbers.  Returns dict(frames, inter, area, max_num) of device tensors for scatter()."""
+        n_det: host numbers.  The frames' ground truth is rasterized first, on the same stream.  Returns dict(frames, inter,
+        area, max_num, ...) of device tensors for scatter()."""
+        from . import segm_raster as SR
         N = len(staged)
         cur = torch.cuda.current_stream(self.dev)
         fr = np.zeros(N, FRAME_DTYPE)
@@ -233,24 +254,44 @@ class YtvisEvaluator:
             g0 += len(s['rows'])
             if s['stream'] != cur:                   # uploaded on another stream: keep it until this stream is done
                 s['planes'].record_stream(cur)
+                s['raster']['items'].record_stream(cur)
         gts = np.concatenate([s['rows'] for s in staged]) if N else np.zeros(0, GTF_DTYPE)
+        # where scatter() adds each ground truth's pixel count: its slot's row of gt_area (columns the overlap kernel
+        # reports as out of range are left out)
+        slots = np.repeat([self._vids[s['video_id']]['slot'] for s in staged], [len(s['rows']) for s in staged])
+        ok = (gts['g'] >= 0) & (gts['g'] < self.max_gts)
+        cells = (slots.astype(np.int64) * self.max_gts + gts['g'])[ok]
         with torch.cuda.device(self.dev):
             frames = _pinned_to(fr, self.dev)
             gts_dev = _pinned_to(gts, self.dev)
+            gt_area = torch.zeros(max(len(gts), 1), dtype=torch.int32, device=self.dev)
+            gt_sel = _pinned_to(np.concatenate([cells, np.nonzero(ok)[0].astype(np.int64)]), self.dev)
+            g0, rows32 = 0, gts_dev.view(torch.int32)    # smb_ytvis_gt_frame_t: ext is int32 3..6 of 8
+            for s in staged:
+                n = len(s['rows'])
+                if n:
+                    SR.raster(s['raster'], s['planes'], n, s['h'] * s['pitch'], s['pitch'], self.raster_status,
+                              area=gt_area[g0:], area_stride=1, ext=rows32[g0 * 8 + 3:], ext_stride=8)
+                g0 += n
             inter = torch.empty(max(N, 1) * max_num * self.max_gts, dtype=torch.int32, device=self.dev)
             area = torch.empty(max(N, 1) * max_num, dtype=torch.int32, device=self.dev)
             L.check(L.lib().smb_ytvis_overlap_dev(L.ptr(frames), N, L.ptr(count), max_num, L.ptr(gts_dev), len(gts),
                                                   self.max_gts, L.ptr(inter), L.ptr(area), L.ptr(self.status),
                                                   L.stream_ptr()), 'smb_ytvis_overlap_dev')
-        return dict(frames=frames, inter=inter, area=area, max_num=max_num, n=N, gts=gts_dev)
+        return dict(frames=frames, inter=inter, area=area, max_num=max_num, n=N, gts=gts_dev, gt_area=gt_area, gt_sel=gt_sel,
+                    n_sel=len(cells))
 
     def scatter(self, ovl, ids, count=None):
         """Kernel b on the current stream: ovl from overlap(), ids int32 device tensor [N, max_num] of object ids, count
-        as for overlap()."""
+        as for overlap().  The frames' ground-truth pixel counts are added into their videos' sums as well."""
         cur = torch.cuda.current_stream(self.dev)
-        for key in ('frames', 'inter', 'area'):
+        for key in ('frames', 'inter', 'area', 'gt_area', 'gt_sel'):
             ovl[key].record_stream(cur)
         with torch.cuda.device(self.dev):
+            if ovl['n_sel']:
+                sel = ovl['gt_sel'].view(torch.int64)
+                k = ovl['n_sel']
+                self.gt_area.view(-1).index_add_(0, sel[:k], ovl['gt_area'][sel[k:2 * k]].to(torch.int64))
             L.check(L.lib().smb_ytvis_scatter_dev(L.ptr(ovl['frames']), ovl['n'], L.ptr(count), L.ptr(ids), ovl['max_num'],
                                                   L.ptr(ovl['inter']), L.ptr(ovl['area']), self.max_gts,
                                                   L.ptr(self.acc_inter), L.ptr(self.acc_area), L.ptr(self.acc_nz),
@@ -271,6 +312,9 @@ class YtvisEvaluator:
             raise ValueError('video %d: %d entries and %d object ids' % (video_id, len(entries), len(obj_ids)))
         if len(entries) > DET_CAP:
             raise ValueError('video %d: %d result entries (at most %d)' % (video_id, len(entries), DET_CAP))
+        if len(self.gt.anns[video_id]) > self.max_gts:
+            raise ValueError('video %d has %d ground-truth objects, max_gts is %d' % (video_id, len(self.gt.anns[video_id]),
+                                                                                       self.max_gts))
         ents = np.zeros(len(entries), ENT_DTYPE)
         for e, (r, o) in enumerate(zip(entries, obj_ids)):
             try:
@@ -283,10 +327,13 @@ class YtvisEvaluator:
             ents[e]['cat'] = self.gt.cat_index.get(cat, -1)
             ents[e]['obj'] = int(o)
         gts, off = self.gt.video(video_id)
-        gts['sum_area'] = st['sum_area'][gts['g']]
         lib = L.lib()
         with torch.cuda.device(self.dev):
             ents_dev, gts_dev, off_dev = _pinned_to(ents, self.dev), _pinned_to(gts, self.dev), _pinned_to(off, self.dev)
+            if len(gts):                             # smb_ytvis_gt_t: sum_area is int64 1 of 4, from the slot's sums
+                rows64 = gts_dev.view(torch.int64)[:len(gts) * 4].view(len(gts), 4)
+                g = _pinned_to(gts['g'].astype(np.int64), self.dev).view(torch.int64)[:len(gts)]
+                rows64[:, 1] = self.gt_area[st['slot']][g]
             ws_bytes = lib.smb_ytvis_match_workspace_bytes(len(gts))
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
             out = torch.empty(max(len(ents), 1) * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
@@ -317,6 +364,8 @@ class YtvisEvaluator:
                 raise L.SmbError('YouTube-VIS evaluation: a ground-truth column reached max_gts=%d' % self.max_gts)
             if status:
                 raise L.SmbError('YouTube-VIS evaluation status %d' % status)
+            from .segm_raster import check_status
+            check_status(self.raster_status)
             if self.n_results == 0:
                 raise ValueError('segm: the results of the evaluated videos are empty')
             p, r, s = accumulate(self.rows, self.npig, self.K, self.dev)
@@ -329,8 +378,8 @@ class YtvisEvaluator:
 
 def evaluate_json(gt, results, cat_ids=None, vid_ids=None, chunk=16, device=None):
     """YTVOSeval of a result list in the results2json_videoseg format (the reference's output, or VideoRunner.video_json
-    over all videos) against `gt` on the device: the same kernels, with each present frame's RLE decoded on the host and
-    each entry its own accumulator row.  vid_ids: the evaluated videos (p.vidIds; default every ground-truth video).  A
+    over all videos) against `gt` on the device: the same kernels, with each present frame's RLE string parsed to run
+    lengths on the host and rasterized on the device, and each entry its own accumulator row.  vid_ids: the evaluated videos (p.vidIds; default every ground-truth video).  A
     result whose video is not in the ground truth, whose segmentations do not cover the video's frames or whose
     category is not in cat_ids raises ValueError; results of other ground-truth videos are not evaluated."""
     vids = gt.vid_ids if vid_ids is None else sorted(set(int(v) for v in vid_ids))
@@ -357,6 +406,7 @@ def evaluate_json(gt, results, cat_ids=None, vid_ids=None, chunk=16, device=None
         raise ValueError('segm: the results are empty')
     objects = max([1] + [len(e) for e in per.values()])
     max_gts = max([1] + [len(gt.anns[v]) for v in vids])
+    from . import segm_raster as SR
     ev = YtvisEvaluator(gt, cat_ids, slots=1, objects=objects, max_gts=max_gts, device=device)
     dev = ev.dev
     with torch.cuda.device(dev):
@@ -370,22 +420,24 @@ def evaluate_json(gt, results, cat_ids=None, vid_ids=None, chunk=16, device=None
             max_num = max(1, len(ents))
             for f0 in range(0, n_f, chunk):
                 fs = list(range(f0, min(f0 + chunk, n_f)))
-                staged, planes, n_det = [], [], []
+                staged, pack, n_det = [], SR.SegmPack(), []
                 ids = np.full((len(fs), max_num), -1, np.int32)
                 for n, f in enumerate(fs):
                     s = ev.stage_frame(v, f)
                     staged.append(s)
                     present = [e for e, r in enumerate(ents) if r['segmentations'][f] is not None]
-                    for e in present:
+                    for j, e in enumerate(present):
                         seg = ents[e]['segmentations'][f]
                         if not isinstance(seg, dict):
                             raise ValueError('results: video %d frame %d: segmentation must be an RLE dict' % (v, f))
-                        planes.append(segm_plane(seg, h, w, 'result of video %d frame %d' % (v, f)))
+                        pack.add(seg, h, w, sum(n_det) + j, 'result of video %d frame %d' % (v, f))
                     ids[n, :len(present)] = present
                     n_det.append(len(present))
                 stride = h * pitch
-                pl = torch.from_numpy(np.stack(planes).reshape(-1).view(np.int32) if planes else np.zeros(1, np.int32))
-                pl = pl.to(dev)
+                P = sum(n_det)
+                pl = torch.empty(max(P * stride, 1), dtype=torch.int32, device=dev)
+                if P:
+                    SR.raster(SR.staged(pack, dev)[0], pl, P, stride, pitch, ev.raster_status)
                 base, offs = pl.data_ptr(), np.concatenate([[0], np.cumsum(n_det)[:-1]]).astype(np.int64)
                 ovl = ev.overlap(staged, [base + 4 * stride * int(o) for o in offs], stride, pitch, max_num, n_det=n_det)
                 ev.scatter(ovl, torch.from_numpy(ids).to(dev))
