@@ -408,6 +408,7 @@ typedef struct {
 #define SMB_COCO_MAX_CATS 2048
 #define SMB_COCO_LABEL_RANGE 1   /* status: a record label outside [0, num_labels) */
 #define SMB_COCO_CAPACITY 2      /* status: an output row outside [0, n_out) */
+#define SMB_COCO_ANALYSIS_RANGE 4 /* status: an annotation position or a supercategory index outside its table */
 
 /* HOST helpers (plain C++, no CUDA), pycocotools maskApi.c restated:
  *   smb_coco_poly_counts     : rleFrPoly's run lengths of one polygon of k vertices (*host_n = their number; written
@@ -452,6 +453,53 @@ int smb_coco_match_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det
 int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K, const int* npig,
                             const double* rec_thr, const int* host_max_dets3, double* precision, double* recall,
                             double* scores, smb_stream_t stream);
+
+/* COCOeval with user-given Params (p.iouThrs, p.recThrs, p.areaRng as float64 data, in any order; p.maxDets ascending, as
+ * COCOeval.evaluate() sorts them).
+ * Limits: 1 <= T, 1 <= A, T * A <= SMB_COCO_MAX_TA (the matched / ignored bits of a row are one uint64 each);
+ * 1 <= M <= SMB_COCO_MAX_M with every maxDet in [1, SMB_COCO_MAX_DET], in ascending order; 1 <= R <= SMB_COCO_R; no NaN.  A launch with
+ * Params outside them returns SMB_EINVAL.  The default Params make these entry points compute what the two above do. */
+#define SMB_COCO_MAX_TA 64
+#define SMB_COCO_MAX_M 3
+typedef struct {
+  int32_t T, A, M, R;
+  int32_t max_dets[SMB_COCO_MAX_M];
+  int32_t pad;
+  double iou_thr[SMB_COCO_MAX_TA];
+  double area_rng[SMB_COCO_MAX_TA][2];
+  double rec_thr[SMB_COCO_R];
+} smb_coco_params_t;
+/* SMB_OK when *host_params is within the limits, else SMB_EINVAL with the limit in smb_last_error(). */
+int smb_coco_params_check(const smb_coco_params_t* host_params);
+/* smb_coco_match_dev with Params: matched / ignored bit t*A + a, the first maxDets[M-1] detections of each (image,
+ * category) ranked, npig [K, A]; workspace >= smb_coco_match_params_workspace_bytes(n_gt, host_params). */
+size_t smb_coco_match_params_workspace_bytes(int n_gt, const smb_coco_params_t* host_params);
+int smb_coco_match_params_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                              const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt,
+                              const uint32_t* gt_planes, int64_t gt_plane_words, const int32_t* gt_cat_off, int K,
+                              int metric, const smb_coco_params_t* host_params, smb_coco_out_t* out, int64_t n_out,
+                              int* npig, int* status, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+/* smb_coco_accumulate_dev with Params: npig [K, A]; precision / scores [T, R, K, A, M], recall [T, K, A, M].  As in
+ * pycocotools, the recall thresholds after the first one the detections do not reach keep precision and score 0. */
+int smb_coco_accumulate_params_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
+                                   const int* npig, const smb_coco_params_t* host_params, double* precision,
+                                   double* recall, double* scores, smb_stream_t stream);
+
+/* coco_error_analysis.py's per-category evaluations with relabelled ground truth (iouThrs [.1], maxDets [100], the four
+ * area ranges host_area_rng[4][2]), for every (image, category) with detections: category k's detections against the
+ * image's ground truths in annotation order, where an annotation of another category counts as a crowd annotation of k
+ * when it is in k's supercategory (Sim, bit a of the row) or always (Oth, bit 4 + a).
+ *   gt_pos [n_gt]: position of each ground-truth row in its image's annotation order (a permutation of [0, G_img));
+ *   sup [K]: supercategory index of each category, in [0, n_sup).
+ * Rows as smb_coco_match_dev writes them; no npig (the plain evaluation's applies).  A position or supercategory index
+ * out of range sets SMB_COCO_ANALYSIS_RANGE.  workspace >= smb_coco_analysis_workspace_bytes(n_gt). */
+size_t smb_coco_analysis_workspace_bytes(int n_gt);
+int smb_coco_analysis_match_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                                const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt,
+                                const uint32_t* gt_planes, int64_t gt_plane_words, const int32_t* gt_cat_off,
+                                const int32_t* gt_pos, const int32_t* sup, int n_sup, int K, int metric,
+                                const double* host_area_rng, smb_coco_out_t* out, int64_t n_out, int* status,
+                                void* workspace, size_t workspace_bytes, smb_stream_t stream);
 
 /* ------------------------------------------------------------------ YouTube-VIS mask AP (YTVOSeval, iouType 'segm')
  * The sequence IoU of a result entry d and a ground-truth object g over a video is sum_f I_f / U with

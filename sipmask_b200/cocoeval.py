@@ -1,5 +1,6 @@
-"""COCO box and mask AP on the device: pycocotools 2.0 COCOeval (iouType 'bbox' / 'segm', default Params) as MM's
-CocoDataset.evaluate (SipMask-mmdetection/mmdet/datasets/coco.py:290-392) and SipMask-benchmark's coco_eval.py run it.
+"""COCO box and mask AP on the device: pycocotools 2.0 COCOeval (iouType 'bbox' / 'segm') as MM's CocoDataset.evaluate
+(SipMask-mmdetection/mmdet/datasets/coco.py:290-392) and SipMask-benchmark's coco_eval.py run it, with the default Params
+or user-given ones (CocoParams: IoU thresholds, recall thresholds, maxDets and area ranges as data).
 
 Host: the ground truth (CocoGroundTruth: pycocotools COCO's indexing; annToRLE through the library's C restatement of
 rleFrPoly / rleFrString as the public host rasterizer, segm_plane) and summarize (numpy, the code of COCOeval.summarize).
@@ -36,7 +37,81 @@ AREA_RNG_LBL = ['all', 'small', 'medium', 'large']
 METRIC_ITEMS = ['mAP', 'mAP_50', 'mAP_75', 'mAP_s', 'mAP_m', 'mAP_l']
 DET_CAP = 4096                       # SMB_COCO_DET_CAP: detections of one image in one launch
 MAX_CATS = 2048                      # SMB_COCO_MAX_CATS
-LABEL_RANGE, CAPACITY = 1, 2         # status bits
+LABEL_RANGE, CAPACITY, ANALYSIS_RANGE = 1, 2, 4   # status bits
+MAX_TA, MAX_M, MAX_DET = 64, 3, 100  # SMB_COCO_MAX_TA, SMB_COCO_MAX_M, SMB_COCO_MAX_DET
+
+
+class _ParamsC(ctypes.Structure):
+    """smb_coco_params_t (include/sipmask_b200.h)."""
+    _fields_ = [('T', ctypes.c_int32), ('A', ctypes.c_int32), ('M', ctypes.c_int32), ('R', ctypes.c_int32),
+                ('max_dets', ctypes.c_int32 * MAX_M), ('pad', ctypes.c_int32), ('iou_thr', ctypes.c_double * MAX_TA),
+                ('area_rng', ctypes.c_double * (2 * MAX_TA)), ('rec_thr', ctypes.c_double * 101)]
+
+
+class CocoParams:
+    """COCOeval's Params as data: iouThrs, recThrs, maxDets, areaRng and areaRngLbl (default: COCOeval's, iouType 'bbox'
+    / 'segm').  Thresholds and area ranges keep the order given, as pycocotools keeps them; maxDets are sorted, as
+    COCOeval.evaluate() sorts them (p.maxDets = sorted(p.maxDets)) before anything reads them.  Limits, each a ValueError
+    here:
+      1 <= T (IoU thresholds), 1 <= A (area ranges), T * A <= 64: a detection's matched / ignored bits are one uint64;
+      1 <= M <= 3 maxDets, each an integer in [1, 100]; 1 <= R <= 101 recall thresholds; no NaN;
+      one label per area range.
+    Not supported: useCats = 0 and catIds subsets (every category of the ground truth is evaluated)."""
+
+    def __init__(self, iou_thrs=None, rec_thrs=None, max_dets=None, area_rng=None, area_rng_lbl=None, use_cats=1,
+                 cat_ids=None):
+        if use_cats != 1:
+            raise ValueError('CocoParams: useCats = 0 is not supported (categories are always used)')
+        if cat_ids is not None:
+            raise ValueError('CocoParams: catIds subsets are not supported (every ground-truth category is evaluated)')
+        self.iou_thrs = self._floats(IOU_THRS if iou_thrs is None else iou_thrs, 'iou_thrs')
+        self.rec_thrs = self._floats(REC_THRS if rec_thrs is None else rec_thrs, 'rec_thrs')
+        self.area_rng = self._floats(AREA_RNG if area_rng is None else area_rng, 'area_rng', (-1, 2))
+        self.area_rng_lbl = list(AREA_RNG_LBL if area_rng_lbl is None else area_rng_lbl)
+        md = list(MAX_DETS if max_dets is None else max_dets)
+        if not all(isinstance(m, (int, np.integer)) and not isinstance(m, bool) for m in md):
+            raise ValueError('CocoParams: maxDets must be integers, got %r' % (md,))
+        self.max_dets = sorted(int(m) for m in md)
+        T, A, M, R = len(self.iou_thrs), len(self.area_rng), len(self.max_dets), len(self.rec_thrs)
+        if T < 1 or A < 1 or T * A > MAX_TA:
+            raise ValueError('CocoParams: %d IoU thresholds x %d area ranges; need 1 <= T, 1 <= A and T * A <= %d '
+                             '(the matched / ignored bits of a detection are one uint64)' % (T, A, MAX_TA))
+        if not 1 <= M <= MAX_M:
+            raise ValueError('CocoParams: %d maxDets; 1 to %d are supported' % (M, MAX_M))
+        if any(not 1 <= m <= MAX_DET for m in self.max_dets):
+            raise ValueError('CocoParams: maxDets %r; each must be in [1, %d]' % (self.max_dets, MAX_DET))
+        if not 1 <= R <= 101:
+            raise ValueError('CocoParams: %d recall thresholds; 1 to 101 are supported' % R)
+        if len(self.area_rng_lbl) != A:
+            raise ValueError('CocoParams: %d area range labels for %d area ranges' % (len(self.area_rng_lbl), A))
+
+    @staticmethod
+    def _floats(v, name, shape=(-1,)):
+        try:
+            a = np.array(v, dtype=np.float64).reshape(shape)
+        except (TypeError, ValueError) as e:
+            raise ValueError('CocoParams: %s: %s' % (name, e))
+        if np.isnan(a).any():
+            raise ValueError('CocoParams: %s has a NaN' % name)
+        return np.ascontiguousarray(a)
+
+    @property
+    def shape(self):
+        """(T, R, A, M): precision / scores are [T, R, K, A, M], recall [T, K, A, M]."""
+        return len(self.iou_thrs), len(self.rec_thrs), len(self.area_rng), len(self.max_dets)
+
+    def summarizable(self):
+        """Whether COCOeval.summarize runs on these Params: three maxDets and the labels all / small / medium / large."""
+        return len(self.max_dets) == 3 and all(l in self.area_rng_lbl for l in AREA_RNG_LBL)
+
+    def c_struct(self):
+        T, R, A, M = self.shape
+        p = _ParamsC(T=T, A=A, M=M, R=R)
+        p.max_dets[:M] = self.max_dets
+        p.iou_thr[:T] = self.iou_thrs.tolist()
+        p.area_rng[:2 * A] = self.area_rng.reshape(-1).tolist()
+        p.rec_thr[:R] = self.rec_thrs.tolist()
+        return p
 
 
 def _ptr(a):
@@ -132,6 +207,7 @@ class CocoGroundTruth:
     """A loaded COCO annotation json, indexed as pycocotools' COCO and COCOeval._prepare see it.
       img_ids : sorted unique image ids (COCOeval.evaluate: np.unique(p.imgIds))
       cat_ids : sorted category ids (p.catIds = sorted(getCatIds()))
+      names / supercategories: per sorted category, its 'name' and 'supercategory' (None where the file has none)
     Per image, its annotations of those categories in annotation-file order (imgToAnns)."""
 
     def __init__(self, ann_dict):
@@ -139,12 +215,15 @@ class CocoGroundTruth:
             images, cats, anns = ann_dict['images'], ann_dict['categories'], ann_dict['annotations']
             self.hw = {int(im['id']): (int(im['height']), int(im['width'])) for im in images}
             self.cat_ids = sorted(int(c['id']) for c in cats)
+            info = {int(c['id']): c for c in cats}
         except (KeyError, TypeError, ValueError) as e:
             raise ValueError('CocoGroundTruth: malformed images / categories: %r' % (e,))
         if len(set(self.cat_ids)) != len(self.cat_ids) or not 0 < len(self.cat_ids) <= MAX_CATS:
             raise ValueError('CocoGroundTruth: need 1..%d distinct category ids' % MAX_CATS)
         self.img_ids = sorted(self.hw)
         self.cat_index = {c: i for i, c in enumerate(self.cat_ids)}
+        self.names = [str(info[c].get('name', c)) for c in self.cat_ids]
+        self.supercategories = [info[c].get('supercategory') for c in self.cat_ids]
         self.anns = {i: [] for i in self.img_ids}
         for a in anns:
             try:
@@ -186,6 +265,22 @@ class CocoGroundTruth:
                 rows[r]['ext'] = ext
         return rows, np.cumsum(cnt).astype(np.int32), planes
 
+    def positions(self, img_id):
+        """[G] int32: the position of image()'s row r in the image's annotation order."""
+        anns = self.anns[img_id]
+        return np.array(sorted(range(len(anns)), key=lambda i: self.cat_index[anns[i]['cat']]), np.int32)
+
+    def supercategory_index(self):
+        """[K] int32 index of each category's supercategory (numbered by first appearance) and the number of them.
+        Raises ValueError when a category has none (the error analysis' Sim evaluation groups categories by it)."""
+        missing = [c for c, s in zip(self.cat_ids, self.supercategories) if s is None]
+        if missing:
+            raise ValueError('CocoGroundTruth: categories %r have no supercategory' % missing[:8])
+        index = {}
+        for s in self.supercategories:
+            index.setdefault(s, len(index))
+        return np.array([index[s] for s in self.supercategories], np.int32), len(index)
+
     def packed(self, img_id):
         """image()'s rows and offsets with the segmentations packed for the device rasterizer instead of rasterized:
         (rows with area_mask / ext left zero, per-category offsets [K+1], segm_raster.SegmPack with row r's
@@ -204,10 +299,11 @@ class CocoGroundTruth:
 
 
 # ---------------------------------------------------------------------------------------------------- summarize (host)
-def summarize(precision, recall, area_rng_lbl=AREA_RNG_LBL, max_dets=MAX_DETS):
+def summarize(precision, recall, area_rng_lbl=AREA_RNG_LBL, max_dets=MAX_DETS, iou_thrs=IOU_THRS):
     """COCOeval.summarize's 12 stats of the accumulated arrays (its _summarize / _summarizeDets code).  area_rng_lbl /
-    max_dets: the Params' areaRngLbl and maxDets (YTVOSeval keeps COCO's labels for its own ranges)."""
-    iouThrs, maxDets, areaRngLbl = IOU_THRS, list(max_dets), list(area_rng_lbl)
+    max_dets / iou_thrs: the Params' areaRngLbl, maxDets and iouThrs (YTVOSeval keeps COCO's labels for its own ranges);
+    a stat whose IoU threshold, range label or maxDet the Params lack is -1, as in pycocotools."""
+    iouThrs, maxDets, areaRngLbl = np.asarray(iou_thrs, dtype=np.float64), list(max_dets), list(area_rng_lbl)
 
     def _summarize(ap=1, iouThr=None, areaRng='all', maxDets_=100):
         aind = [i for i, aRng in enumerate(areaRngLbl) if aRng == areaRng]
@@ -257,9 +353,9 @@ def mm_results(metric, stats):
 
 
 # ---------------------------------------------------------------------------------------------------- accumulate
-def accumulate(row_parts, npig, K, dev):
+def accumulate(row_parts, npig, K, dev, params=None):
     """COCOeval.accumulate on the device: the precision / recall / scores arrays (numpy) of the OUT_DTYPE rows (a list
-    of uint8 device tensors) and npig [K, 4], on the current stream."""
+    of uint8 device tensors) and npig [K, A], on the current stream.  params: CocoParams (None: the default Params)."""
     parts = [r.view(torch.int64).view(-1, 5) for r in row_parts]
     rows = torch.cat(parts) if parts else torch.zeros((0, 5), dtype=torch.int64, device=dev)
     score = rows[:, 0].contiguous().view(torch.float64)
@@ -273,16 +369,62 @@ def accumulate(row_parts, npig, K, dev):
     o = o[torch.argsort(cat[o], stable=True)]
     srt = rows[o].contiguous()
     cat_off = torch.searchsorted(cat[o].contiguous(), torch.arange(K + 1, dtype=torch.int32, device=dev)).to(torch.int32)
-    T, R, A, M = len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)
+    T, R, A, M = (len(IOU_THRS), len(REC_THRS), len(AREA_RNG), len(MAX_DETS)) if params is None else params.shape
     precision = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
     scores = torch.empty_like(precision)
     recall = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
-    rec_thr = torch.from_numpy(np.ascontiguousarray(REC_THRS)).to(dev)
-    md = (ctypes.c_int * 3)(*MAX_DETS)
-    L.check(L.lib().smb_coco_accumulate_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K, L.ptr(npig),
-                                            L.ptr(rec_thr), md, L.ptr(precision), L.ptr(recall), L.ptr(scores),
-                                            L.stream_ptr()), 'smb_coco_accumulate_dev')
+    if params is None:
+        rec_thr = torch.from_numpy(np.ascontiguousarray(REC_THRS)).to(dev)
+        md = (ctypes.c_int * 3)(*MAX_DETS)
+        L.check(L.lib().smb_coco_accumulate_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K, L.ptr(npig),
+                                                L.ptr(rec_thr), md, L.ptr(precision), L.ptr(recall), L.ptr(scores),
+                                                L.stream_ptr()), 'smb_coco_accumulate_dev')
+    else:
+        pc = params.c_struct()
+        L.check(L.lib().smb_coco_accumulate_params_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K,
+                                                       L.ptr(npig), ctypes.byref(pc), L.ptr(precision), L.ptr(recall),
+                                                       L.ptr(scores), L.stream_ptr()), 'smb_coco_accumulate_params_dev')
     return precision.cpu().numpy(), recall.cpu().numpy(), scores.cpu().numpy()
+
+
+# ---------------------------------------------------------------------------------------------------- error analysis
+# SipMask-mmdetection's tools/coco_error_analysis.py: one COCOeval of every result with these Params (ps[0:3]), and per
+# category k two more of k's results against relabelled ground truth (Sim, Oth: iouThrs [.1], maxDets [100]).  On the
+# device the two per-category evaluations are one more match per image (smb_coco_analysis_match_dev) whose rows carry
+# Sim in bits 0..3 and Oth in bits 4..7, accumulated as two "thresholds".
+ANALYSIS_PARAMS = CocoParams(iou_thrs=[.75, .5, .1], max_dets=[100])
+_SIM_OTH_PARAMS = CocoParams(iou_thrs=[.1, .1], max_dets=[100])
+ANALYSIS_TYPES = ['C75', 'C50', 'Loc', 'Sim', 'Oth', 'BG', 'FN']
+ANALYSIS_AREAS = ['allarea', 'small', 'medium', 'large']
+
+
+def analysis_arrays(p3, p2):
+    """coco_error_analysis.py's ps [7, R, K, 4, 1] from the precision of the [.75, .5, .1] evaluation (p3) and of the
+    Sim / Oth rows (p2 [2, R, K, 4, 1]): C75, C50, Loc, Sim, Oth with -1 -> 0, then BG = Oth > 0 and FN = 1."""
+    ps = np.zeros((7,) + p3.shape[1:])
+    ps[0:3] = p3
+    ps[3:5] = p2
+    ps[ps == -1] = 0
+    ps[5] = ps[4] > 0
+    ps[6] = 1.0
+    return ps
+
+
+def analysis_table(ps, gt):
+    """The numbers the tool's plot legends show: per class k, type t and area a, ps[t, :, k, a, 0].mean(); for
+    'allclass', the mean over recall thresholds and classes.  Returns dict(types, areas, cat_ids, names,
+    classes [K, 7, 4], allclass [7, 4])."""
+    ps = np.asarray(ps)
+    return dict(types=list(ANALYSIS_TYPES), areas=list(ANALYSIS_AREAS), cat_ids=list(gt.cat_ids), names=list(gt.names),
+                classes=ps[..., 0].mean(axis=1).transpose(1, 0, 2), allclass=ps[..., 0].mean(axis=(1, 2)))
+
+
+def analyze_json(gt, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None):
+    """coco_error_analysis.py's arrays of result lists against `gt` on the device: {metric: ps [7, R, K, 4, 1]}, K in
+    the order of gt.cat_ids (sorted ids; the tool uses the file's order of categories, the same when the file lists
+    them sorted by id, as COCO's does).  Raises ValueError when a category has no supercategory."""
+    metrics = [m for m, j in (('bbox', bbox_json), ('segm', segm_json)) if j is not None]
+    return _run_json(gt, gt.cat_ids, bbox_json, segm_json, img_ids, chunk, device, None, True, metrics)['analysis']
 
 
 # ---------------------------------------------------------------------------------------------------- evaluator
@@ -296,19 +438,25 @@ class CocoEvaluator:
     (add_results); evaluate() accumulates and summarizes.
       gt      : CocoGroundTruth
       cat_ids : COCO category id per 0-based record label (as coco.coco_json takes it)
-      benchmark: SipMask-benchmark records (BoxList.resize boxes, box scores for segm)."""
+      benchmark: SipMask-benchmark records (BoxList.resize boxes, box scores for segm)
+      params  : CocoParams (None: COCOeval's default Params)
+      analyze : also run, for every image added, the matches of coco_error_analysis.py (see analysis_arrays), so that
+                evaluate() returns its precision arrays as well."""
 
-    def __init__(self, gt, cat_ids, metrics=('bbox', 'segm'), benchmark=False, device=None):
+    def __init__(self, gt, cat_ids, metrics=('bbox', 'segm'), benchmark=False, device=None, params=None, analyze=False):
         metrics = [metrics] if isinstance(metrics, str) else list(metrics)
         for m in metrics:
             if m not in ('bbox', 'segm'):
                 raise KeyError('metric {} is not supported'.format(m))
-        self.gt, self.metrics, self.benchmark = gt, metrics, bool(benchmark)
+        if params is not None and not isinstance(params, CocoParams):
+            raise ValueError('params must be a CocoParams')
+        self.gt, self.metrics, self.benchmark, self.params = gt, metrics, bool(benchmark), params
+        A = len(AREA_RNG) if params is None else params.shape[2]
         self.dev = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
         self.K = len(gt.cat_ids)
         self.label_cat_host = np.array([gt.cat_index.get(int(c), -1) for c in cat_ids], np.int32)
         self.label_cat = torch.from_numpy(self.label_cat_host).to(self.dev)
-        self.npig = {m: torch.zeros(self.K * 4, dtype=torch.int32, device=self.dev) for m in metrics}
+        self.npig = {m: torch.zeros(self.K * A, dtype=torch.int32, device=self.dev) for m in metrics}
         self.rows = {m: [] for m in metrics}
         self.status = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.raster_status = torch.zeros(1, dtype=torch.int32, device=self.dev)
@@ -317,6 +465,15 @@ class CocoEvaluator:
         self._seen = set()
         self._iou_thr = np.ascontiguousarray(IOU_THRS, dtype=np.float64)
         self._area_rng = np.ascontiguousarray(np.array(AREA_RNG, dtype=np.float64).reshape(-1))
+        self._params_c = params.c_struct() if params is not None else None
+        self.analyze = bool(analyze)
+        if self.analyze:
+            sup, self.n_sup = gt.supercategory_index()
+            self.sup = torch.from_numpy(sup).to(self.dev)
+            self._ana_c = ANALYSIS_PARAMS.c_struct()
+            self.npig_ana = {m: torch.zeros(self.K * len(AREA_RNG), dtype=torch.int32, device=self.dev) for m in metrics}
+            self.rows_c = {m: [] for m in metrics}         # ps[0:3]: iouThrs [.75, .5, .1], maxDets [100]
+            self.rows_so = {m: [] for m in metrics}        # ps[3:5]: Sim / Oth rows
 
     # ---- bookkeeping
     def _claim(self, image_ids, ori_hws=None):
@@ -347,10 +504,13 @@ class CocoEvaluator:
         if segm:
             rows['plane'] = np.arange(n_gt, dtype=np.int64) * (h * pitch)
         stream = stream or torch.cuda.current_stream(self.dev)
+        extra = (rows, off) + ((self.gt.positions(image_id),) if self.analyze else ())
         with torch.cuda.device(self.dev), torch.cuda.stream(stream):
-            st, (rows_dev, off_dev) = SR.staged(pack if segm else SR.SegmPack(), self.dev, (rows, off))
+            st, views = SR.staged(pack if segm else SR.SegmPack(), self.dev, extra)
             planes = torch.empty(max(n_gt * h * pitch, 1) if segm else 1, dtype=torch.int32, device=self.dev)
-        return dict(rows=rows_dev, off=off_dev.view(torch.int32), planes=planes, n_gt=n_gt,
+        rows_dev, off_dev = views[:2]
+        pos = views[2].view(torch.int32) if self.analyze else None
+        return dict(rows=rows_dev, off=off_dev.view(torch.int32), pos=pos, planes=planes, n_gt=n_gt,
                     plane_words=n_gt * h * pitch if segm else 0, stream=stream,
                     raster=dict(st, stride=h * pitch, pitch=pitch) if segm and n_gt else None)
 
@@ -363,25 +523,59 @@ class CocoEvaluator:
         SR.raster(r, gt['planes'], gt['n_gt'], r['stride'], r['pitch'], self.raster_status, area=rows[15:],
                   area_stride=GT_DTYPE.itemsize // 4, ext=rows[16:], ext_stride=GT_DTYPE.itemsize // 4)
 
-    def _match(self, metric, imgs, n, dets, det_cap, det_planes, det_plane_words, gt, out_rows):
-        """The match launch of image n of a batch (imgs / dets: the batch's device rows) on the current stream."""
+    def _outs(self, n_rows):
+        """Output rows of a batch: the plain match's and, when analyzing, those of the two analysis matches."""
+        return [torch.empty(n_rows * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+                for _ in range(3 if self.analyze else 1)]
+
+    def _keep(self, metric, outs):
+        self.rows[metric].append(outs[0])
+        if self.analyze:
+            self.rows_c[metric].append(outs[1])
+            self.rows_so[metric].append(outs[2])
+
+    def _match(self, metric, imgs, n, dets, det_cap, det_planes, det_plane_words, gt, outs):
+        """The match launches of image n of a batch (imgs / dets: the batch's device rows) on the current stream."""
         lib = L.lib()
         cur = torch.cuda.current_stream(self.dev)
         if gt['stream'] != cur:                          # uploaded on another stream: keep it until this stream is done
-            for key in ('rows', 'off', 'planes'):
-                gt[key].record_stream(cur)
+            for key in ('rows', 'off', 'planes', 'pos'):
+                if gt.get(key) is not None:
+                    gt[key].record_stream(cur)
         if metric == 'segm' and gt['raster'] is not None:
             self._raster_gt(gt)
-        ws_bytes = lib.smb_coco_match_workspace_bytes(gt['n_gt'])
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+        out_rows = outs[0]
         n_out = out_rows.numel() // OUT_DTYPE.itemsize
-        L.check(lib.smb_coco_match_dev(ctypes.c_void_p(imgs.data_ptr() + n * IMG_DTYPE.itemsize), 1,
-                                       ctypes.c_void_p(dets.data_ptr() + n * det_cap * DET_DTYPE.itemsize), det_cap,
-                                       L.ptr(det_planes), ctypes.c_int64(det_plane_words), L.ptr(gt['rows']), gt['n_gt'],
-                                       L.ptr(gt['planes']), ctypes.c_int64(gt['plane_words']), L.ptr(gt['off']), self.K,
-                                       0 if metric == 'bbox' else 1, _ptr(self._iou_thr), _ptr(self._area_rng),
-                                       L.ptr(out_rows), ctypes.c_int64(n_out), L.ptr(self.npig[metric]), L.ptr(self.status),
-                                       L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_coco_match_dev')
+        args = (ctypes.c_void_p(imgs.data_ptr() + n * IMG_DTYPE.itemsize), 1,
+                ctypes.c_void_p(dets.data_ptr() + n * det_cap * DET_DTYPE.itemsize), det_cap, L.ptr(det_planes),
+                ctypes.c_int64(det_plane_words), L.ptr(gt['rows']), gt['n_gt'], L.ptr(gt['planes']),
+                ctypes.c_int64(gt['plane_words']), L.ptr(gt['off']), self.K, 0 if metric == 'bbox' else 1)
+        tail = (L.ptr(out_rows), ctypes.c_int64(n_out), L.ptr(self.npig[metric]), L.ptr(self.status))
+        if self._params_c is None:
+            ws_bytes = lib.smb_coco_match_workspace_bytes(gt['n_gt'])
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+            L.check(lib.smb_coco_match_dev(*args, _ptr(self._iou_thr), _ptr(self._area_rng), *tail, L.ptr(ws),
+                                           ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_coco_match_dev')
+        else:
+            pc = ctypes.byref(self._params_c)
+            ws_bytes = lib.smb_coco_match_params_workspace_bytes(gt['n_gt'], pc)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+            L.check(lib.smb_coco_match_params_dev(*args, pc, *tail, L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
+                    'smb_coco_match_params_dev')
+        if not self.analyze:
+            return
+        pc = ctypes.byref(self._ana_c)
+        ws_bytes = lib.smb_coco_match_params_workspace_bytes(gt['n_gt'], pc)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+        L.check(lib.smb_coco_match_params_dev(*args, pc, L.ptr(outs[1]), ctypes.c_int64(n_out), L.ptr(self.npig_ana[metric]),
+                                              L.ptr(self.status), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
+                'smb_coco_match_params_dev')
+        ws_bytes = lib.smb_coco_analysis_workspace_bytes(gt['n_gt'])
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+        L.check(lib.smb_coco_analysis_match_dev(*args[:11], L.ptr(gt['pos']), L.ptr(self.sup), self.n_sup, *args[11:],
+                                                _ptr(self._area_rng), L.ptr(outs[2]), ctypes.c_int64(n_out),
+                                                L.ptr(self.status), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
+                'smb_coco_analysis_match_dev')
 
     def _img_rows(self, ids, det_pitch, det_cap, n_det=None):
         imgs = np.zeros(len(ids), IMG_DTYPE)
@@ -434,10 +628,10 @@ class CocoEvaluator:
                                                      L.ptr(self.status), L.stream_ptr()), 'smb_coco_det_from_record_dev')
             n_json = count[:B].clamp(0, max_num).sum()
             for m in self.metrics:
-                out = torch.empty(B * max_num * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+                outs = self._outs(B * max_num)
                 for n in range(B):
-                    self._match(m, imgs, n, dets, max_num, bits, bits.numel(), gts[n], out)
-                self.rows[m].append(out)
+                    self._match(m, imgs, n, dets, max_num, bits, bits.numel(), gts[n], outs)
+                self._keep(m, outs)
                 self.n_results[m] += n_json
             self.image_ids += ids
             self._seen.update(ids)
@@ -501,22 +695,26 @@ class CocoEvaluator:
                 rows32 = dd.view(torch.int32)[:B * det_cap * 24].view(B * det_cap, 24)
                 rows32[at, 16] = stats[:, 0]
                 rows32[at[:, None], torch.arange(18, 22, device=self.dev)[None]] = stats[:, 1:]
-            out = torch.empty(B * det_cap * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+            outs = self._outs(B * det_cap)
             for n, i in enumerate(ids):
-                self._match(metric, imgs, n, dd, det_cap, pd, pd.numel(), self.stage_gt(i, masks=metric == 'segm'), out)
-            self.rows[metric].append(out)
+                self._match(metric, imgs, n, dd, det_cap, pd, pd.numel(), self.stage_gt(i, masks=metric == 'segm'), outs)
+            self._keep(metric, outs)
 
     # ---- accumulate + summarize
     def _accumulate(self, metric):
-        return accumulate(self.rows[metric], self.npig[metric], self.K, self.dev)
+        return accumulate(self.rows[metric], self.npig[metric], self.K, self.dev, self.params)
 
     def evaluate(self):
-        """Accumulate and summarize every metric.  Returns MM's dict (bbox_mAP, ..., segm_mAP_copypaste) plus
-        'stats' and 'arrays' ({metric: {'precision', 'recall', 'scores'}}) with COCOeval's eval arrays."""
+        """Accumulate and summarize every metric.  Returns 'arrays' ({metric: {'precision', 'recall', 'scores'}}) with
+        COCOeval's eval arrays in the Params' shapes and, where COCOeval.summarize runs on the Params (three maxDets and
+        the labels all / small / medium / large), MM's dict (bbox_mAP, ..., segm_mAP_copypaste) and 'stats'.  With
+        analyze=True, also 'analysis' ({metric: ps}, see analysis_arrays)."""
         with torch.cuda.device(self.dev):
             status = int(self.status.item())
             if status & LABEL_RANGE:
                 raise ValueError('a record label is outside the %d labels of cat_ids' % len(self.label_cat_host))
+            if status & ANALYSIS_RANGE:
+                raise L.SmbError('COCO error analysis: an annotation position or supercategory index is out of range')
             if status:
                 raise L.SmbError('COCO evaluation status %d' % status)
             from .segm_raster import check_status
@@ -526,23 +724,40 @@ class CocoEvaluator:
                 if int(self.n_results[m].item()) == 0:
                     raise ValueError('%s: the results of the evaluated images are empty' % m)
                 p, r, s = self._accumulate(m)
-                stats[m] = summarize(p, r)
                 arrays[m] = dict(precision=p, recall=r, scores=s)
+                if self.params is None:
+                    stats[m] = summarize(p, r)
+                elif self.params.summarizable():
+                    stats[m] = summarize(p, r, self.params.area_rng_lbl, self.params.max_dets, self.params.iou_thrs)
+                else:
+                    continue
                 out.update(mm_results(m, stats[m]))
-            out['stats'] = stats
+            if stats:
+                out['stats'] = stats
             out['arrays'] = arrays
+            if self.analyze:
+                out['analysis'] = {m: self._analysis(m) for m in self.metrics}
             return out
 
+    def _analysis(self, m):
+        p3 = accumulate(self.rows_c[m], self.npig_ana[m], self.K, self.dev, ANALYSIS_PARAMS)[0]
+        p2 = accumulate(self.rows_so[m], self.npig_ana[m], self.K, self.dev, _SIM_OTH_PARAMS)[0]
+        return analysis_arrays(p3, p2)
 
-def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None):
+
+def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None, params=None):
     """COCOeval of result lists (coco.coco_json output or a loaded results file) against `gt` on the device: the same
     kernels as CocoEvaluator, with the detections' RLE strings parsed to run lengths on the host and rasterized on the
     device.  img_ids: the evaluated images
     (p.imgIds; default every ground-truth image).  As in pycocotools, a result whose image is not in the ground truth
-    raises (loadRes), and results of ground-truth images outside img_ids are not evaluated (_prepare).  Returns
-    CocoEvaluator.evaluate()'s dict for the metrics given."""
+    raises (loadRes), and results of ground-truth images outside img_ids are not evaluated (_prepare).  params:
+    CocoParams (None: the default Params).  Returns CocoEvaluator.evaluate()'s dict for the metrics given."""
     metrics = [m for m, j in (('bbox', bbox_json), ('segm', segm_json)) if j is not None]
-    ev = CocoEvaluator(gt, cat_ids, metrics=metrics, device=device)
+    return _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, False, metrics)
+
+
+def _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, analyze, metrics):
+    ev = CocoEvaluator(gt, cat_ids, metrics=metrics, device=device, params=params, analyze=analyze)
     ids = ev._claim(gt.img_ids if img_ids is None else sorted(set(int(i) for i in img_ids)))
     for m, res in (('bbox', bbox_json), ('segm', segm_json)):
         if res is None:

@@ -5,43 +5,60 @@
 
 namespace smb_match {
 
-constexpr int kT = SMB_COCO_T, kA = SMB_COCO_A, kMaxDet = SMB_COCO_MAX_DET;
+constexpr int kT = SMB_COCO_T, kA = SMB_COCO_A, kMaxDet = SMB_COCO_MAX_DET, kMaxTA = SMB_COCO_MAX_TA;
 
+// What the loop reads of COCOeval's Params: T IoU thresholds and A area ranges (T * A <= kMaxTA, any order), and
+// maxDets[-1], the detections kept per (image, category).
 struct MatchParams {
-  double iou_thr[kT];
-  double area_rng[kA][2];
+  int T, A, max_det;
+  double iou_thr[kMaxTA];
+  double area_rng[kMaxTA][2];
 };
 
+// The default Params' thresholds and ranges as COCOeval holds them (host_iou_thr[kT], host_area_rng[kA][2]).
+inline MatchParams default_params(const double* host_iou_thr, const double* host_area_rng) {
+  MatchParams P;
+  P.T = kT;
+  P.A = kA;
+  P.max_det = kMaxDet;
+  for (int t = 0; t < kT; ++t) P.iou_thr[t] = host_iou_thr[t];
+  for (int a = 0; a < kA; ++a) { P.area_rng[a][0] = host_area_rng[2 * a]; P.area_rng[a][1] = host_area_rng[2 * a + 1]; }
+  return P;
+}
+
 // What the loop reads of a ground truth: the area its range test uses, its annotation id (a match to id 0 does not count,
-// as pycocotools tests dtm != 0) and iscrowd.
+// as pycocotools tests dtm != 0), iscrowd, and skip: not part of this thread's ground-truth set (the error analysis runs
+// one set per thread over the same IoU matrix; every other caller leaves it 0).
 struct MatchGt {
   double area;
   int64_t id;
   int crowd;
+  int skip;
 };
 
-// One thread per (threshold t, area range a), tid = t * kA + a < kT * kA; the other threads return at once.
-//   ious    : [D, G] of the D score-sorted detections (at most kMaxDet) and the G ground truths in annotation order
-//   gtm     : kT * kA * G bytes of workspace
+// One thread per (threshold t, area range a), tid = t * P.A + a < P.T * P.A; the other threads return at once.
+//   ious    : [D, G] of the D score-sorted detections (at most P.max_det) and the G ground truths in annotation order
+//   gtm     : P.T * P.A * G bytes of workspace
 //   gt_at(g): MatchGt of ground truth g; det_area(d): the area of sorted detection d
-//   npig_k  : [kA] non-ignored ground truths of the category, added with integer atomics by the t == 0 threads
-//   s_m/s_ig: [D] matched / ignored bits (t * kA + a) of the sorted detections, zeroed by the caller
+//   npig_k  : [P.A] non-ignored ground truths of the category, added with integer atomics by the t == 0 threads (NULL:
+//             not counted)
+//   s_m/s_ig: [D] matched / ignored bits (t * P.A + a) of the sorted detections, zeroed by the caller
 template <typename GtAt, typename DetArea>
 __device__ __forceinline__ void greedy_match(int tid, int D, int G, const double* __restrict__ ious, uint8_t* __restrict__ gtm_ws,
                                              const MatchParams& P, GtAt gt_at, DetArea det_area, int* npig_k, uint64_t* s_m,
                                              uint64_t* s_ig) {
-  if (tid >= kT * kA) return;
-  const int t = tid / kA, a = tid - t * kA;
+  if (tid >= P.T * P.A) return;
+  const int t = tid / P.A, a = tid - t * P.A;
   const double lo = P.area_rng[a][0], hi = P.area_rng[a][1];
   uint8_t* gtm = gtm_ws + (size_t)tid * G;
   for (int g = 0; g < G; ++g) gtm[g] = 0;
-  auto gt_ig = [&](int g) {
+  auto gt_ig = [&](int g) {                        // 2: skipped, never equal to a pass
     const MatchGt gr = gt_at(g);
-    return gr.crowd || gr.area < lo || gr.area > hi;
+    return gr.skip ? 2 : (int)(gr.crowd || gr.area < lo || gr.area > hi);
   };
-  if (t == 0) {
+  if (t == 0 && npig_k) {
     int np = 0;
-    for (int g = 0; g < G; ++g) np += !gt_ig(g);
+    for (int g = 0; g < G; ++g) np += gt_ig(g) == 0;
     if (np) atomicAdd(npig_k + a, np);
   }
   const double thr = P.iou_thr[t] < 1.0 - 1e-10 ? P.iou_thr[t] : 1.0 - 1e-10;
@@ -76,10 +93,10 @@ __device__ __forceinline__ void greedy_match(int tid, int D, int G, const double
   }
 }
 
-// Workspace of one match launch over n_gt ground truths: [n_gt, kMaxDet] IoUs and [n_gt, kT, kA] gtm bytes.
-inline size_t match_workspace_bytes(int n_gt) {
-  if (n_gt < 0) return 0;
-  return smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256) + smb::align_up((size_t)n_gt * kT * kA, 256) + 256;
+// Workspace of one match launch over n_gt ground truths: [n_gt, kMaxDet] IoUs and [n_gt, ta] gtm bytes, ta = T * A.
+inline size_t match_workspace_bytes(int n_gt, int ta = kT * kA) {
+  if (n_gt < 0 || ta < 0) return 0;
+  return smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256) + smb::align_up((size_t)n_gt * ta, 256) + 256;
 }
 
 }  // namespace smb_match

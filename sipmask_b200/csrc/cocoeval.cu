@@ -4,6 +4,9 @@
 //   smb_coco_det_from_record_dev : engine record -> detection rows as the result json carries them (coco.coco_json)
 //   smb_coco_match_dev           : computeIoU + evaluateImg for every (image, category) of a batch of images
 //   smb_coco_accumulate_dev      : accumulate's precision / recall / scores arrays from the globally sorted rows
+//   smb_coco_*_params_dev        : the same two with user-given Params (thresholds, area ranges, maxDets, recall
+//                                  thresholds as data); the default Params give what the two above give
+//   smb_coco_analysis_match_dev  : coco_error_analysis.py's Sim / Oth evaluations (relabelled ground truth) of a batch
 //
 // Every float64 operation whose result is compared with pycocotools is an explicit _rn intrinsic, so nvcc cannot
 // contract it into an FMA (x86-64 pycocotools has none).
@@ -150,6 +153,54 @@ __device__ __forceinline__ double box_iou(const double* d, const double* g, int 
   return __ddiv_rn(i, u);
 }
 
+// computeIoU's [D, G] matrix of the sorted detections (rows s_sorted[d] of drow) against ground truths gt_of(g) = {row in
+// gts (-1: none, IoU 0), iscrowd}: bbIou for metric 0, rleIou of the bit planes for metric 1 (one warp per pair).
+template <typename GtOf>
+__device__ __forceinline__ void iou_matrix(int metric, int D, int G, const smb_coco_det_t* __restrict__ drow,
+                                           const int* s_sorted, const smb_coco_gt_t* __restrict__ gts, GtOf gt_of, int H,
+                                           int dpitch, int gpitch, const uint32_t* __restrict__ det_planes,
+                                           int64_t det_plane_words, const uint32_t* __restrict__ gt_planes,
+                                           int64_t gt_plane_words, double* __restrict__ ious) {
+  const int tid = threadIdx.x, warp = tid >> 5, lid = tid & 31;
+  if (metric == 0) {
+    for (int p = tid; p < D * G; p += kThreads) {
+      const int d = p / G, g = p - d * G;
+      const int2 gc = gt_of(g);
+      ious[p] = gc.x < 0 ? 0.0 : box_iou(drow[s_sorted[d]].box, gts[gc.x].box, gc.y);
+    }
+  } else {
+    for (int p = warp; p < D * G; p += kWarps) {
+      const int d = p / G, g = p - d * G;
+      const int2 gc = gt_of(g);
+      const smb_coco_det_t& dr = drow[s_sorted[d]];
+      const smb_coco_gt_t& gr = gts[max(gc.x, 0)];
+      const int y0 = max(max(dr.ext[0], gr.ext[0]), 0), y1 = min(min(dr.ext[1], gr.ext[1]), H);
+      const int x0 = max(max(dr.ext[2], gr.ext[2]), 0), x1 = min(min(min(dr.ext[3], gr.ext[3]), dpitch), gpitch);
+      const int nx = x1 - x0;
+      int inter = 0;
+      const bool dok = dr.plane >= 0 && dr.plane + (int64_t)H * dpitch <= det_plane_words;
+      const bool gok = gc.x >= 0 && gr.plane >= 0 && gr.plane + (int64_t)H * gpitch <= gt_plane_words;
+      if (dok && gok && nx > 0 && y1 > y0) {
+        const uint32_t* pd = det_planes + dr.plane;
+        const uint32_t* pg = gt_planes + gr.plane;
+        for (int e = lid; e < (y1 - y0) * nx; e += 32) {
+          const int y = y0 + e / nx, x = x0 + e % nx;
+          inter += __popc(pd[(size_t)y * dpitch + x] & pg[(size_t)y * gpitch + x]);
+        }
+      }
+      for (int o = 16; o > 0; o >>= 1) inter += __shfl_xor_sync(0xffffffffu, inter, o);
+      if (lid == 0) {
+        double v = 0.0;                            // rleIou: i == 0 -> 0
+        if (inter > 0) {
+          const long long u = gc.y ? (long long)dr.area_mask : (long long)dr.area_mask + gr.area_mask - inter;
+          v = __ddiv_rn((double)inter, (double)u);
+        }
+        ious[p] = v;
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kThreads) match_kernel(
     const smb_coco_img_t* __restrict__ imgs, const smb_coco_det_t* __restrict__ dets, int det_cap,
     const uint32_t* __restrict__ det_planes, int64_t det_plane_words, const smb_coco_gt_t* __restrict__ gts, int n_gt,
@@ -157,7 +208,7 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
     int metric, MatchParams P, smb_coco_out_t* __restrict__ out, int64_t n_out, int* __restrict__ npig,
     double* __restrict__ iou_ws, uint8_t* __restrict__ gtm_ws, int* __restrict__ status) {
   extern __shared__ __align__(16) unsigned char smem[];
-  uint64_t* s_m = (uint64_t*)smem;                 // [kMaxDet] matched bits (t * kA + a) of the sorted detections
+  uint64_t* s_m = (uint64_t*)smem;                 // [kMaxDet] matched bits (t * P.A + a) of the sorted detections
   uint64_t* s_ig = s_m + kMaxDet;                  // [kMaxDet] ignore bits
   int* s_sorted = (int*)(s_ig + kMaxDet);          // [kMaxDet] detection row of rank r
   int* s_start = s_sorted + kMaxDet;               // [K + 1] per category: first entry of s_list
@@ -197,7 +248,7 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
     const int l0 = s_start[k], n = s_start[k + 1] - l0;
     const int g0 = min(max(goff[k], 0), n_gt), g1 = min(max(goff[k + 1], g0), n_gt), G = g1 - g0;
     if (n == 0 && G == 0) continue;                // evaluateImg returns None
-    const int D = min(n, kMaxDet);
+    const int D = min(n, P.max_det);
     // ---- rank inside (image, category): score descending, stable over the json order
     for (int i = tid; i < n; i += kThreads) {
       const int j = s_list[l0 + i];
@@ -210,51 +261,18 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
         const int oq = drow[jq].order;
         r += (sq > s) || (sq == s && (oq < oj || (oq == oj && jq < j)));
       }
-      if (r < kMaxDet) s_sorted[r] = j;            // computeIoU keeps the first maxDets[-1]
+      if (r < P.max_det) s_sorted[r] = j;          // computeIoU keeps the first maxDets[-1]
     }
     for (int i = tid; i < D; i += kThreads) { s_m[i] = 0; s_ig[i] = 0; }
     __syncthreads();
     // ---- IoU [D, G] (ground truths in annotation order)
     double* ious = iou_ws + (size_t)kMaxDet * g0;
-    if (metric == 0) {
-      for (int p = tid; p < D * G; p += kThreads) {
-        const int d = p / G, g = p - d * G;
-        ious[p] = box_iou(drow[s_sorted[d]].box, gts[g0 + g].box, gts[g0 + g].crowd);
-      }
-    } else {
-      for (int p = warp; p < D * G; p += kWarps) {
-        const int d = p / G, g = p - d * G;
-        const smb_coco_det_t& dr = drow[s_sorted[d]];
-        const smb_coco_gt_t& gr = gts[g0 + g];
-        const int y0 = max(max(dr.ext[0], gr.ext[0]), 0), y1 = min(min(dr.ext[1], gr.ext[1]), H);
-        const int x0 = max(max(dr.ext[2], gr.ext[2]), 0), x1 = min(min(min(dr.ext[3], gr.ext[3]), dpitch), gpitch);
-        const int nx = x1 - x0;
-        int inter = 0;
-        const bool dok = dr.plane >= 0 && dr.plane + (int64_t)H * dpitch <= det_plane_words;
-        const bool gok = gr.plane >= 0 && gr.plane + (int64_t)H * gpitch <= gt_plane_words;
-        if (dok && gok && nx > 0 && y1 > y0) {
-          const uint32_t* pd = det_planes + dr.plane;
-          const uint32_t* pg = gt_planes + gr.plane;
-          for (int e = lid; e < (y1 - y0) * nx; e += 32) {
-            const int y = y0 + e / nx, x = x0 + e % nx;
-            inter += __popc(pd[(size_t)y * dpitch + x] & pg[(size_t)y * gpitch + x]);
-          }
-        }
-        for (int o = 16; o > 0; o >>= 1) inter += __shfl_xor_sync(0xffffffffu, inter, o);
-        if (lid == 0) {
-          double v = 0.0;                          // rleIou: i == 0 -> 0
-          if (inter > 0) {
-            const long long u = gr.crowd ? (long long)dr.area_mask : (long long)dr.area_mask + gr.area_mask - inter;
-            v = __ddiv_rn((double)inter, (double)u);
-          }
-          ious[p] = v;
-        }
-      }
-    }
+    iou_matrix(metric, D, G, drow, s_sorted, gts, [&](int g) { return make_int2(g0 + g, gts[g0 + g].crowd); }, H, dpitch,
+               gpitch, det_planes, det_plane_words, gt_planes, gt_plane_words, ious);
     __syncthreads();
     // ---- evaluateImg's greedy matching, one thread per (threshold, area range)
     smb_match::greedy_match(
-        tid, D, G, ious, gtm_ws + (size_t)kT * kA * g0, P,
+        tid, D, G, ious, gtm_ws + (size_t)P.T * P.A * g0, P,
         [&](int g) {
           const smb_coco_gt_t& gr = gts[g0 + g];
           return smb_match::MatchGt{gr.area, gr.id, gr.crowd};
@@ -263,7 +281,141 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
           const smb_coco_det_t& dr = drow[s_sorted[d]];
           return metric == 0 ? dr.area_box : (double)dr.area_mask;
         },
-        npig + k * kA, s_m, s_ig);
+        npig + k * P.A, s_m, s_ig);
+    __syncthreads();
+    for (int r = tid; r < D; r += kThreads) {
+      const int j = s_sorted[r];
+      smb_coco_out_t* o = out_row(j);
+      if (o) {
+        o->score = drow[j].score[metric];
+        o->matched = s_m[r];
+        o->ignored = s_ig[r];
+        o->cat = k;
+        o->rank = r;
+      } else {
+        atomicOr(status, SMB_COCO_CAPACITY);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ 2e: error analysis
+// coco_error_analysis.py evaluates category k's detections alone against a ground truth in which the annotations of
+// other categories become crowd (ignored) annotations of k: those of k's supercategory (Sim, variant 0) or all of them
+// (Oth, variant 1); iouThrs [.1], maxDets [100].  Its rows are one CTA per image, per category with detections there:
+// rank as match_kernel, one IoU matrix against every ground truth of the image (a relabelled one is crowd, IoU =
+// inter / area_d), and the greedy loop once per (variant v, area range a) over the image's annotations in file order,
+// filtered to the variant's set; bit v * A + a of the row.  npig is the plain evaluation's (only k's own ground truths
+// count), so none is written here.
+//   gt_pos [n_gt]: position of ground-truth row r in its image's annotation order; sup [K]: supercategory index
+//   pos_ws : [n_gt] rows by annotation position (base + p), then [n_gt] their category
+__global__ void __launch_bounds__(kThreads) analysis_match_kernel(
+    const smb_coco_img_t* __restrict__ imgs, const smb_coco_det_t* __restrict__ dets, int det_cap,
+    const uint32_t* __restrict__ det_planes, int64_t det_plane_words, const smb_coco_gt_t* __restrict__ gts, int n_gt,
+    const uint32_t* __restrict__ gt_planes, int64_t gt_plane_words, const int32_t* __restrict__ gt_cat_off,
+    const int32_t* __restrict__ gt_pos, const int32_t* __restrict__ sup, int n_sup, int K, int metric, MatchParams P,
+    smb_coco_out_t* __restrict__ out, int64_t n_out, double* __restrict__ iou_ws, uint8_t* __restrict__ gtm_ws,
+    int32_t* __restrict__ pos_ws, int* __restrict__ status) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  uint64_t* s_m = (uint64_t*)smem;                 // [kMaxDet] matched bits (v * P.A + a) of the sorted detections
+  uint64_t* s_ig = s_m + kMaxDet;                  // [kMaxDet] ignore bits
+  int* s_sorted = (int*)(s_ig + kMaxDet);          // [kMaxDet] detection row of rank r
+  int* s_start = s_sorted + kMaxDet;               // [K + 1] per category: first entry of s_list
+  int* s_list = s_start + K + 1;                   // [det_cap] detections grouped by category, record order inside
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const smb_coco_img_t im = imgs[b];
+  const int nd = min(max(im.n_det, 0), det_cap);
+  const smb_coco_det_t* drow = dets + (size_t)b * det_cap;
+  const int32_t* goff = gt_cat_off + (size_t)b * (K + 1);
+  const int H = max(im.h, 0), gpitch = max(im.gt_pitch, 0), dpitch = max(im.det_pitch, 0);
+  const int base = min(max(goff[0], 0), n_gt), Gi = min(max(goff[K], base), n_gt) - base;
+  int32_t* pos_row = pos_ws + base;
+  int32_t* pos_cat = pos_ws + n_gt + base;
+  auto out_row = [&](int j) -> smb_coco_out_t* {
+    const int64_t o = im.out_off + j;
+    return (o >= 0 && o < n_out) ? out + o : nullptr;
+  };
+  for (int j = tid; j < det_cap; j += kThreads) {
+    smb_coco_out_t* o = out_row(j);
+    if (o) { o->score = 0; o->image_id = im.image_id; o->matched = 0; o->ignored = 0; o->cat = K; o->rank = -1; }
+  }
+  for (int p = tid; p < Gi; p += kThreads) pos_row[p] = -1;
+  if (tid == 0) {
+    for (int k = 0; k <= K; ++k) s_start[k] = 0;
+    for (int j = 0; j < nd; ++j) {
+      const int c = drow[j].cat;
+      if (c >= 0 && c < K) s_start[c + 1]++;
+    }
+    for (int k = 0; k < K; ++k) s_start[k + 1] += s_start[k];
+    for (int j = 0; j < nd; ++j) {
+      const int c = drow[j].cat;
+      if (c >= 0 && c < K) s_list[s_start[c]++] = j;
+    }
+    for (int k = K; k > 0; --k) s_start[k] = s_start[k - 1];
+    s_start[0] = 0;
+  }
+  __syncthreads();
+  // ---- the image's ground truths in annotation order: row and category of position p
+  for (int k = 0; k < K; ++k) {
+    const int g0 = min(max(goff[k], base), base + Gi), g1 = min(max(goff[k + 1], g0), base + Gi);
+    for (int r = g0 + tid; r < g1; r += kThreads) {
+      const int p = gt_pos[r];
+      if (p < 0 || p >= Gi) { atomicOr(status, SMB_COCO_ANALYSIS_RANGE); continue; }
+      pos_row[p] = r;
+      pos_cat[p] = k;
+    }
+  }
+  for (int k = tid; k < K; k += kThreads)
+    if (sup[k] < 0 || sup[k] >= n_sup) atomicOr(status, SMB_COCO_ANALYSIS_RANGE);
+  __syncthreads();
+  for (int p = tid; p < Gi; p += kThreads)
+    if (pos_row[p] < 0) atomicOr(status, SMB_COCO_ANALYSIS_RANGE);  // a position no row holds (or two rows share)
+  for (int k = 0; k < K; ++k) {
+    const int l0 = s_start[k], n = s_start[k + 1] - l0;
+    if (n == 0) continue;                          // no rows; npig comes from the plain evaluation
+    const int D = min(n, P.max_det);
+    for (int i = tid; i < n; i += kThreads) {
+      const int j = s_list[l0 + i];
+      const double s = drow[j].score[metric];
+      const int oj = drow[j].order;
+      int r = 0;
+      for (int q = 0; q < n; ++q) {
+        const int jq = s_list[l0 + q];
+        const double sq = drow[jq].score[metric];
+        const int oq = drow[jq].order;
+        r += (sq > s) || (sq == s && (oq < oj || (oq == oj && jq < j)));
+      }
+      if (r < P.max_det) s_sorted[r] = j;
+    }
+    for (int i = tid; i < D; i += kThreads) { s_m[i] = 0; s_ig[i] = 0; }
+    __syncthreads();
+    double* ious = iou_ws + (size_t)kMaxDet * base;
+    iou_matrix(metric, D, Gi, drow, s_sorted, gts,
+               [&](int g) {
+                 const int r = pos_row[g];
+                 return make_int2(r, r < 0 ? 1 : (pos_cat[g] == k ? gts[r].crowd : 1));
+               },
+               H, dpitch, gpitch, det_planes, det_plane_words, gt_planes, gt_plane_words, ious);
+    __syncthreads();
+    const int sup_k = sup[k];
+    const int v = tid / P.A;
+    smb_match::greedy_match(
+        tid, D, Gi, ious, gtm_ws + (size_t)P.T * P.A * base, P,
+        [&](int g) {
+          const int r = pos_row[g];
+          if (r < 0) return smb_match::MatchGt{0.0, 0, 1, 1};
+          const int c = pos_cat[g];
+          const smb_coco_gt_t& gr = gts[r];
+          const bool own = c == k;
+          const bool in_set = own || v == 1 || sup[c] == sup_k;
+          return smb_match::MatchGt{gr.area, gr.id, own ? gr.crowd : 1, in_set ? 0 : 1};
+        },
+        [&](int d) {
+          const smb_coco_det_t& dr = drow[s_sorted[d]];
+          return metric == 0 ? dr.area_box : (double)dr.area_mask;
+        },
+        nullptr, s_m, s_ig);
     __syncthreads();
     for (int r = tid; r < D; r += kThreads) {
       const int j = s_sorted[r];
@@ -283,28 +435,38 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------ 2d: accumulate
+// What accumulate reads of the Params: A area ranges, M maxDets, R recall thresholds (rec_thr, unless the launch passes
+// them as a device array).
+struct AccParams {
+  int A, M, R;
+  int max_dets[SMB_COCO_MAX_M];
+  double rec_thr[kR];
+};
+
+// grid (K, A * M, T)
 __global__ void __launch_bounds__(kThreads) accumulate_kernel(
     const smb_coco_out_t* __restrict__ rows, const int32_t* __restrict__ cat_off, int64_t n_rows, int K,
-    const int* __restrict__ npig_in, const double* __restrict__ rec_thr, int3 max_dets, double* __restrict__ precision,
+    const int* __restrict__ npig_in, const double* __restrict__ rec_thr_dev, AccParams P, double* __restrict__ precision,
     double* __restrict__ recall, double* __restrict__ scores) {
   __shared__ int s_wi[kWarps];
   __shared__ double s_wd[kWarps];
   __shared__ double s_q[kR], s_ss[kR];
-  const int k = blockIdx.x, a = blockIdx.y / 3, mi = blockIdx.y % 3, t = blockIdx.z, tid = threadIdx.x;
-  const int M = 3;
-  const int max_det = mi == 0 ? max_dets.x : (mi == 1 ? max_dets.y : max_dets.z);
+  const int A = P.A, M = P.M, R = P.R;
+  const int k = blockIdx.x, a = blockIdx.y / M, mi = blockIdx.y % M, t = blockIdx.z, tid = threadIdx.x;
+  const int max_det = P.max_dets[mi];
+  auto rec_thr = [&](int r) { return rec_thr_dev ? rec_thr_dev[r] : P.rec_thr[r]; };
   const int64_t s0 = min(max((int64_t)cat_off[k], (int64_t)0), n_rows);
   const int64_t s1 = min(max((int64_t)cat_off[k + 1], s0), n_rows);
-  const uint64_t bit = 1ull << (t * kA + a);
-  const int npig = npig_in[k * kA + a];
-  auto p_idx = [&](int r) { return ((((size_t)t * kR + r) * K + k) * kA + a) * M + mi; };
-  const size_t r_idx = (((size_t)t * K + k) * kA + a) * M + mi;
+  const uint64_t bit = 1ull << (t * A + a);
+  const int npig = npig_in[k * A + a];
+  auto p_idx = [&](int r) { return ((((size_t)t * R + r) * K + k) * A + a) * M + mi; };
+  const size_t r_idx = (((size_t)t * K + k) * A + a) * M + mi;
   if (npig <= 0) {                                 // no ground truth to recall: every entry stays -1
-    for (int r = tid; r < kR; r += kThreads) { precision[p_idx(r)] = -1.0; scores[p_idx(r)] = -1.0; }
+    for (int r = tid; r < R; r += kThreads) { precision[p_idx(r)] = -1.0; scores[p_idx(r)] = -1.0; }
     if (tid == 0) recall[r_idx] = -1.0;
     return;
   }
-  for (int r = tid; r < kR; r += kThreads) { s_q[r] = 0.0; s_ss[r] = 0.0; }
+  for (int r = tid; r < R; r += kThreads) { s_q[r] = 0.0; s_ss[r] = 0.0; }
   // ---- totals: included detections (rank < maxDet), tp, fp
   int nd = 0, tp_tot = 0, fp_tot = 0;
   for (int64_t base = s0; base < s1; base += kThreads) {
@@ -355,8 +517,8 @@ __global__ void __launch_bounds__(kThreads) accumulate_kernel(
       const double rc = __ddiv_rn((double)tp, dn);
       const double rc_prev = first ? -INFINITY : __ddiv_rn((double)(tp - tpf), dn);
       if (rc > rc_prev) {
-        for (int r = 0; r < kR; ++r) {
-          const double x = rec_thr[r];
+        for (int r = 0; r < R; ++r) {
+          const double x = rec_thr(r);
           if (rc_prev < x && x <= rc) { s_q[r] = env; s_ss[r] = score; }
         }
       }
@@ -365,7 +527,16 @@ __global__ void __launch_bounds__(kThreads) accumulate_kernel(
     c_max = c_max > tm ? c_max : tm;
   }
   __syncthreads();
-  for (int r = tid; r < kR; r += kThreads) { precision[p_idx(r)] = s_q[r]; scores[p_idx(r)] = s_ss[r]; }
+  // searchsorted past the last detection raises IndexError in pycocotools, which leaves that recall threshold and every
+  // later one at 0 (with ascending thresholds they are exactly the ones no detection reaches)
+  if (tid == 0) {
+    const double rc_last = nd ? __ddiv_rn((double)tp_tot, dn) : -INFINITY;
+    int r0 = 0;
+    while (r0 < R && rec_thr(r0) <= rc_last) ++r0;
+    for (int r = r0; r < R; ++r) { s_q[r] = 0.0; s_ss[r] = 0.0; }
+  }
+  __syncthreads();
+  for (int r = tid; r < R; r += kThreads) { precision[p_idx(r)] = s_q[r]; scores[p_idx(r)] = s_ss[r]; }
 }
 
 // ------------------------------------------------------------------------------------------------ host rasterizer
@@ -524,6 +695,24 @@ extern "C" int smb_coco_plane_stats(const uint32_t* host_plane, int h, int w, in
 }
 
 // ------------------------------------------------------------------------------------------------ device entry points
+namespace {
+
+int launch_match(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap, const uint32_t* det_planes,
+                 int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt, const uint32_t* gt_planes,
+                 int64_t gt_plane_words, const int32_t* gt_cat_off, int K, int metric, const MatchParams& P,
+                 smb_coco_out_t* out, int64_t n_out, int* npig, int* status, void* workspace, smb_stream_t stream) {
+  double* iou_ws = (double*)workspace;
+  uint8_t* gtm_ws = (uint8_t*)workspace + smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256);
+  const size_t smem = 2 * kMaxDet * sizeof(uint64_t) + (size_t)(kMaxDet + K + 1 + det_cap) * sizeof(int);
+  match_kernel<<<n_img, kThreads, smem, (cudaStream_t)stream>>>(imgs, dets, det_cap, det_planes, det_plane_words, gts, n_gt,
+                                                               gt_planes, gt_plane_words, gt_cat_off, K, metric, P, out, n_out,
+                                                               npig, iou_ws, gtm_ws, status);
+  SMB_LAUNCH_OK("match_kernel");
+  return SMB_OK;
+}
+
+}  // namespace
+
 extern "C" int smb_coco_det_from_record_dev(const float* det, const int64_t* labels, const int* count, const float* mask_scores,
                                             const uint32_t* mask_bits, int N, int max_num, int cap_h, int words,
                                             const smb_img_geom_t* geom, const int32_t* label_cat, int num_labels,
@@ -560,17 +749,9 @@ extern "C" int smb_coco_match_dev(const smb_coco_img_t* imgs, int n_img, const s
   SMB_CHECK_ARG(metric == 0 || (det_planes && (gt_planes || n_gt == 0)), "smb_coco_match_dev: segm needs the planes");
   SMB_CHECK_ARG(workspace_bytes >= smb_coco_match_workspace_bytes(n_gt), "smb_coco_match_dev: workspace of %zu bytes, %zu needed",
                 workspace_bytes, smb_coco_match_workspace_bytes(n_gt));
-  MatchParams P;
-  for (int t = 0; t < kT; ++t) P.iou_thr[t] = host_iou_thr[t];
-  for (int a = 0; a < kA; ++a) { P.area_rng[a][0] = host_area_rng[2 * a]; P.area_rng[a][1] = host_area_rng[2 * a + 1]; }
-  double* iou_ws = (double*)workspace;
-  uint8_t* gtm_ws = (uint8_t*)workspace + smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256);
-  const size_t smem = 2 * kMaxDet * sizeof(uint64_t) + (size_t)(kMaxDet + K + 1 + det_cap) * sizeof(int);
-  match_kernel<<<n_img, kThreads, smem, (cudaStream_t)stream>>>(imgs, dets, det_cap, det_planes, det_plane_words, gts, n_gt,
-                                                               gt_planes, gt_plane_words, gt_cat_off, K, metric, P, out, n_out,
-                                                               npig, iou_ws, gtm_ws, status);
-  SMB_LAUNCH_OK("match_kernel");
-  return SMB_OK;
+  return launch_match(imgs, n_img, dets, det_cap, det_planes, det_plane_words, gts, n_gt, gt_planes, gt_plane_words,
+                      gt_cat_off, K, metric, smb_match::default_params(host_iou_thr, host_area_rng), out, n_out, npig, status,
+                      workspace, stream);
 }
 
 extern "C" int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
@@ -580,9 +761,131 @@ extern "C" int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_row
                 (long long)n_rows, K);
   SMB_CHECK_ARG(cat_off && npig && rec_thr && host_max_dets3 && precision && recall && scores && (rows || n_rows == 0),
                 "smb_coco_accumulate_dev: null pointer");
-  const int3 md = make_int3(host_max_dets3[0], host_max_dets3[1], host_max_dets3[2]);
-  accumulate_kernel<<<dim3(K, kA * 3, kT), kThreads, 0, (cudaStream_t)stream>>>(rows, cat_off, n_rows, K, npig, rec_thr, md,
+  AccParams P;
+  P.A = kA;
+  P.M = 3;
+  P.R = kR;
+  for (int m = 0; m < 3; ++m) P.max_dets[m] = host_max_dets3[m];
+  accumulate_kernel<<<dim3(K, kA * 3, kT), kThreads, 0, (cudaStream_t)stream>>>(rows, cat_off, n_rows, K, npig, rec_thr, P,
                                                                                precision, recall, scores);
+  SMB_LAUNCH_OK("accumulate_kernel");
+  return SMB_OK;
+}
+
+extern "C" size_t smb_coco_analysis_workspace_bytes(int n_gt) {
+  if (n_gt < 0) return 0;
+  return smb_match::match_workspace_bytes(n_gt, 2 * kA) + smb::align_up((size_t)n_gt * 2 * sizeof(int32_t), 256);
+}
+
+extern "C" int smb_coco_analysis_match_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                                           const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts,
+                                           int n_gt, const uint32_t* gt_planes, int64_t gt_plane_words,
+                                           const int32_t* gt_cat_off, const int32_t* gt_pos, const int32_t* sup,
+                                           int n_sup, int K, int metric, const double* host_area_rng,
+                                           smb_coco_out_t* out, int64_t n_out, int* status, void* workspace,
+                                           size_t workspace_bytes, smb_stream_t stream) {
+  SMB_CHECK_ARG(n_img >= 0 && det_cap >= 1 && det_cap <= SMB_COCO_DET_CAP && K >= 1 && K <= SMB_COCO_MAX_CATS && n_gt >= 0 &&
+                    n_sup >= 1 && (metric == 0 || metric == 1) && n_out >= 0 && det_plane_words >= 0 && gt_plane_words >= 0,
+                "smb_coco_analysis_match_dev: bad sizes (n_img %d, det_cap %d, K %d, n_gt %d, n_sup %d, metric %d)", n_img,
+                det_cap, K, n_gt, n_sup, metric);
+  SMB_CHECK_ARG(host_area_rng, "smb_coco_analysis_match_dev: null area ranges");
+  if (n_img == 0) return SMB_OK;
+  SMB_CHECK_ARG(imgs && dets && gt_cat_off && sup && out && status && ((gts && gt_pos) || n_gt == 0) && workspace,
+                "smb_coco_analysis_match_dev: null pointer");
+  SMB_CHECK_ARG(metric == 0 || (det_planes && (gt_planes || n_gt == 0)), "smb_coco_analysis_match_dev: segm needs the planes");
+  SMB_CHECK_ARG(workspace_bytes >= smb_coco_analysis_workspace_bytes(n_gt),
+                "smb_coco_analysis_match_dev: workspace of %zu bytes, %zu needed", workspace_bytes,
+                smb_coco_analysis_workspace_bytes(n_gt));
+  MatchParams P;                                   // variants Sim / Oth as two "thresholds" of .1; maxDets [100]
+  P.T = 2;
+  P.A = kA;
+  P.max_det = kMaxDet;
+  P.iou_thr[0] = P.iou_thr[1] = 0.1;
+  for (int a = 0; a < kA; ++a) { P.area_rng[a][0] = host_area_rng[2 * a]; P.area_rng[a][1] = host_area_rng[2 * a + 1]; }
+  const size_t match_ws = smb_match::match_workspace_bytes(n_gt, 2 * kA);
+  double* iou_ws = (double*)workspace;
+  uint8_t* gtm_ws = (uint8_t*)workspace + smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256);
+  int32_t* pos_ws = (int32_t*)((uint8_t*)workspace + match_ws);
+  const size_t smem = 2 * kMaxDet * sizeof(uint64_t) + (size_t)(kMaxDet + K + 1 + det_cap) * sizeof(int);
+  analysis_match_kernel<<<n_img, kThreads, smem, (cudaStream_t)stream>>>(
+      imgs, dets, det_cap, det_planes, det_plane_words, gts, n_gt, gt_planes, gt_plane_words, gt_cat_off, gt_pos, sup, n_sup,
+      K, metric, P, out, n_out, iou_ws, gtm_ws, pos_ws, status);
+  SMB_LAUNCH_OK("analysis_match_kernel");
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_params_check(const smb_coco_params_t* p) {
+  SMB_CHECK_ARG(p, "smb_coco_params_check: null Params");
+  SMB_CHECK_ARG(p->T >= 1 && p->A >= 1 && p->T * p->A <= SMB_COCO_MAX_TA,
+                "Params: %d IoU thresholds x %d area ranges; 1 <= T, 1 <= A and T * A <= %d (one uint64 of bits per row)",
+                p->T, p->A, SMB_COCO_MAX_TA);
+  SMB_CHECK_ARG(p->M >= 1 && p->M <= SMB_COCO_MAX_M, "Params: %d maxDets; 1 to %d", p->M, SMB_COCO_MAX_M);
+  for (int m = 0; m < p->M; ++m) {
+    SMB_CHECK_ARG(p->max_dets[m] >= 1 && p->max_dets[m] <= SMB_COCO_MAX_DET, "Params: maxDet %d outside [1, %d]",
+                  p->max_dets[m], SMB_COCO_MAX_DET);
+    // COCOeval.evaluate() sorts maxDets before anything reads them; the last one is the number of detections kept
+    SMB_CHECK_ARG(m == 0 || p->max_dets[m] >= p->max_dets[m - 1], "Params: maxDets must be ascending (%d after %d)",
+                  p->max_dets[m], p->max_dets[m - 1]);
+  }
+  SMB_CHECK_ARG(p->R >= 1 && p->R <= SMB_COCO_R, "Params: %d recall thresholds; 1 to %d", p->R, SMB_COCO_R);
+  for (int t = 0; t < p->T; ++t) SMB_CHECK_ARG(!isnan(p->iou_thr[t]), "Params: IoU threshold %d is NaN", t);
+  for (int a = 0; a < p->A; ++a)
+    SMB_CHECK_ARG(!isnan(p->area_rng[a][0]) && !isnan(p->area_rng[a][1]), "Params: area range %d has a NaN", a);
+  for (int r = 0; r < p->R; ++r) SMB_CHECK_ARG(!isnan(p->rec_thr[r]), "Params: recall threshold %d is NaN", r);
+  return SMB_OK;
+}
+
+extern "C" size_t smb_coco_match_params_workspace_bytes(int n_gt, const smb_coco_params_t* p) {
+  if (!p || smb_coco_params_check(p) != SMB_OK) return 0;
+  return smb_match::match_workspace_bytes(n_gt, p->T * p->A);
+}
+
+extern "C" int smb_coco_match_params_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                                         const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts,
+                                         int n_gt, const uint32_t* gt_planes, int64_t gt_plane_words,
+                                         const int32_t* gt_cat_off, int K, int metric, const smb_coco_params_t* p,
+                                         smb_coco_out_t* out, int64_t n_out, int* npig, int* status, void* workspace,
+                                         size_t workspace_bytes, smb_stream_t stream) {
+  const int rc = smb_coco_params_check(p);
+  if (rc != SMB_OK) return rc;
+  SMB_CHECK_ARG(n_img >= 0 && det_cap >= 1 && det_cap <= SMB_COCO_DET_CAP && K >= 1 && K <= SMB_COCO_MAX_CATS && n_gt >= 0 &&
+                    (metric == 0 || metric == 1) && n_out >= 0 && det_plane_words >= 0 && gt_plane_words >= 0,
+                "smb_coco_match_params_dev: bad sizes (n_img %d, det_cap %d, K %d, n_gt %d, metric %d)", n_img, det_cap, K,
+                n_gt, metric);
+  if (n_img == 0) return SMB_OK;
+  SMB_CHECK_ARG(imgs && dets && gt_cat_off && out && npig && status && (gts || n_gt == 0) && workspace,
+                "smb_coco_match_params_dev: null pointer");
+  SMB_CHECK_ARG(metric == 0 || (det_planes && (gt_planes || n_gt == 0)), "smb_coco_match_params_dev: segm needs the planes");
+  const size_t need = smb_match::match_workspace_bytes(n_gt, p->T * p->A);
+  SMB_CHECK_ARG(workspace_bytes >= need, "smb_coco_match_params_dev: workspace of %zu bytes, %zu needed", workspace_bytes,
+                need);
+  MatchParams P;
+  P.T = p->T;
+  P.A = p->A;
+  P.max_det = p->max_dets[p->M - 1];
+  for (int t = 0; t < p->T; ++t) P.iou_thr[t] = p->iou_thr[t];
+  for (int a = 0; a < p->A; ++a) { P.area_rng[a][0] = p->area_rng[a][0]; P.area_rng[a][1] = p->area_rng[a][1]; }
+  return launch_match(imgs, n_img, dets, det_cap, det_planes, det_plane_words, gts, n_gt, gt_planes, gt_plane_words,
+                      gt_cat_off, K, metric, P, out, n_out, npig, status, workspace, stream);
+}
+
+extern "C" int smb_coco_accumulate_params_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
+                                              const int* npig, const smb_coco_params_t* p, double* precision,
+                                              double* recall, double* scores, smb_stream_t stream) {
+  const int rc = smb_coco_params_check(p);
+  if (rc != SMB_OK) return rc;
+  SMB_CHECK_ARG(n_rows >= 0 && K >= 1 && K <= SMB_COCO_MAX_CATS,
+                "smb_coco_accumulate_params_dev: bad sizes (n_rows %lld, K %d)", (long long)n_rows, K);
+  SMB_CHECK_ARG(cat_off && npig && precision && recall && scores && (rows || n_rows == 0),
+                "smb_coco_accumulate_params_dev: null pointer");
+  AccParams P;
+  P.A = p->A;
+  P.M = p->M;
+  P.R = p->R;
+  for (int m = 0; m < p->M; ++m) P.max_dets[m] = p->max_dets[m];
+  for (int r = 0; r < p->R; ++r) P.rec_thr[r] = p->rec_thr[r];
+  accumulate_kernel<<<dim3(K, p->A * p->M, p->T), kThreads, 0, (cudaStream_t)stream>>>(rows, cat_off, n_rows, K, npig,
+                                                                                      nullptr, P, precision, recall, scores);
   SMB_LAUNCH_OK("accumulate_kernel");
   return SMB_OK;
 }

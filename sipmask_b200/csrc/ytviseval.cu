@@ -300,9 +300,7 @@ extern "C" int smb_ytvis_match_dev(const smb_ytvis_entry_t* ents, int n_ent, con
   SMB_CHECK_ARG(workspace_bytes >= smb_match::match_workspace_bytes(n_gt),
                 "smb_ytvis_match_dev: workspace of %zu bytes, %zu needed", workspace_bytes,
                 smb_match::match_workspace_bytes(n_gt));
-  MatchParams P;
-  for (int t = 0; t < kT; ++t) P.iou_thr[t] = host_iou_thr[t];
-  for (int a = 0; a < kA; ++a) { P.area_rng[a][0] = host_area_rng[2 * a]; P.area_rng[a][1] = host_area_rng[2 * a + 1]; }
+  const MatchParams P = smb_match::default_params(host_iou_thr, host_area_rng);
   double* iou_ws = (double*)workspace;
   uint8_t* gtm_ws = (uint8_t*)workspace + smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256);
   const size_t smem = 3 * kMaxDet * 8 + (size_t)(kMaxDet + K + 1 + n_ent) * sizeof(int);

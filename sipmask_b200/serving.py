@@ -982,14 +982,22 @@ class CocoEvalRunner(StreamRunner):
     stats and arrays.  result(ticket) still returns each record, so the result json can be written as well.
       gt      : cocoeval.CocoGroundTruth; cat_ids: COCO category id per 0-based label (as coco.coco_json takes it)
       metrics : 'bbox' and / or 'segm'
+      params  : cocoeval.CocoParams (None: COCOeval's default Params)
+      analyze : also run coco_error_analysis.py's matches after every batch; evaluate() then returns its arrays under
+                'analysis' (cocoeval.CocoEvaluator)
     Every other argument is StreamRunner's; SipMask-VIS (vis=True) is not supported."""
 
-    def __init__(self, state_dict, gt, cat_ids, metrics=('bbox', 'segm'), **kw):
-        from .cocoeval import CocoEvaluator
+    def __init__(self, state_dict, gt, cat_ids, metrics=('bbox', 'segm'), params=None, analyze=False, **kw):
+        from .cocoeval import CocoEvaluator, CocoParams
         if kw.get('vis'):
             raise ValueError('CocoEvalRunner: YouTube-VIS evaluation (vis=True) is not supported')
+        if params is not None and not isinstance(params, CocoParams):
+            raise ValueError('CocoEvalRunner: params must be a cocoeval.CocoParams')
+        if analyze:
+            gt.supercategory_index()                      # raises before the engines are built
         super(CocoEvalRunner, self).__init__(state_dict, **kw)
-        self.evaluator = CocoEvaluator(gt, cat_ids, metrics=metrics, benchmark=self.benchmark, device=self.dev)
+        self.evaluator = CocoEvaluator(gt, cat_ids, metrics=metrics, benchmark=self.benchmark, device=self.dev,
+                                       params=params, analyze=analyze)
         torch.cuda.current_stream(self.dev).synchronize()   # the evaluator's zeroed state, before the slots use it
         self._eval_rows = {}                # ticket -> (image id, its staged ground truth) until its batch is evaluated
         self._submitted = set()
