@@ -169,11 +169,13 @@ def nms(dets, iou_thr, cmp_ge=False, plus_one=True):
 
 
 def multiclass_nms_idx(multi_bboxes, multi_scores, score_thr, iou_thr, max_num=-1,
-                       score_factors=None, cmp_ge=False):
+                       score_factors=None, cmp_ge=False, nms_fn=None):
     """MM/mmdet/core/post_processing/bbox_nms.py:79-146.
 
-    multi_bboxes [n,4], multi_scores [n,C+1] (col 0 = background).
+    multi_bboxes [n,4], multi_scores [n,C+1] (col 0 = background).  nms_fn(dets, thr, cmp_ge) may replace the numpy
+    `nms` with a restatement of the same contract (oracle.cbind.nms, for speed).
     Returns dets [k,5] f32, labels [k] i64 (0-based), idxs [k] i64."""
+    nms_fn = nms_fn or (lambda d, thr, cmp_ge: nms(d, thr, cmp_ge=cmp_ge))
     num_classes = multi_scores.shape[1]
     bboxes, labels, idxs = [], [], []
     multi_idxs = torch.arange(0, multi_scores.shape[0], dtype=torch.long)
@@ -187,7 +189,7 @@ def multiclass_nms_idx(multi_bboxes, multi_scores, score_thr, iou_thr, max_num=-
         if score_factors is not None:
             _scores = _scores * score_factors[cls_inds]           # bbox_nms.py:122
         cls_dets = torch.cat([_bboxes, _scores[:, None]], dim=1)
-        ki = torch.from_numpy(nms(cls_dets.numpy(), iou_thr, cmp_ge=cmp_ge))
+        ki = torch.from_numpy(nms_fn(cls_dets.numpy(), iou_thr, cmp_ge))
         cls_dets = cls_dets[ki]
         bboxes.append(cls_dets)
         labels.append(torch.full((cls_dets.shape[0],), i - 1, dtype=torch.long))

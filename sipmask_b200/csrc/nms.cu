@@ -15,6 +15,8 @@ namespace smb {
 
 constexpr int NT = 1024;          // threads per CTA for all kernels in this file
 constexpr int MAXN = 5120;        // max candidates per class list held in shared memory (>= 5 levels x nms_pre = 1000)
+constexpr int MAXP = 8192;        // power of two >= MAXN: the bitonic sorts of up to MAXN keys pad to this many
+static_assert(MAXP >= MAXN && (MAXP & (MAXP - 1)) == 0, "MAXP must be the padded sort length of MAXN keys");
 constexpr int NMS1 = 8192;        // max boxes of the single-list operator smb_nms
 
 // ---------------------------------------------------------------------------------------------
@@ -256,7 +258,7 @@ __device__ void greedy_sweep_n(const float4* sb, int m, float thr, int cmp_ge, f
 //   w_keys[c][r]     sorted composite keys (low 32 bits = pos)    w_sbox[c][r]  boxes in sorted order
 //   w_m[c]           number of candidates
 struct McPrepSmem {
-  unsigned long long keys[MAXN];
+  unsigned long long keys[MAXP];
   int cidx[MAXN];
   float cscore[MAXN];
   int warp[33];
@@ -543,7 +545,7 @@ __global__ void __launch_bounds__(NT) finalize_kernel(const float* __restrict__ 
 // fast_nms stage 1: one CTA per class (sipmask_head.py:868-891).
 // ---------------------------------------------------------------------------------------------
 struct FastSmem {
-  unsigned long long keys[MAXN];
+  unsigned long long keys[MAXP];
   float4 sb[256];
   float sscore[256];
   unsigned char kept[256];

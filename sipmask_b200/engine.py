@@ -684,7 +684,7 @@ class SipMaskEngine(object):
         ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, nms_pre)
         ws = self._t(ws_bytes, dtype=torch.uint8)
 
-        def decode():
+        def decode(n=n):
             L.check(lib.smb_decode_topk_dev(nl, lv, ncls, nms_pre, L.ptr(self.geom[n]), L.ptr(boxes), L.ptr(scores), L.ptr(ctr),
                                             L.ptr(loc), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_decode_topk_dev')
         self._add(decode, 3, name='decode_topk')
@@ -692,7 +692,7 @@ class SipMaskEngine(object):
             nws_bytes = lib.smb_multiclass_nms_workspace_bytes(ncand, ncls)
             nws = self._t(nws_bytes, dtype=torch.uint8)
 
-            def nms():
+            def nms(n=n):
                 L.check(lib.smb_multiclass_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls, ctypes.c_float(cfg['score_thr']),
                                                ctypes.c_float(iou_thr), self.max_num, 0, L.ptr(det), L.ptr(labels), L.ptr(idx),
                                                L.ptr(count), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()),
@@ -702,7 +702,7 @@ class SipMaskEngine(object):
             nws_bytes = lib.smb_fast_nms_workspace_bytes(ncand, ncls, 200)
             nws = self._t(nws_bytes, dtype=torch.uint8)
 
-            def nms():
+            def nms(n=n):
                 L.check(lib.smb_fast_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls, ctypes.c_float(cfg['score_thr']),
                                          ctypes.c_float(iou_thr), 200, self.max_num, L.ptr(det), L.ptr(labels), L.ptr(idx),
                                          L.ptr(count), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()), 'smb_fast_nms')
@@ -720,7 +720,7 @@ class SipMaskEngine(object):
         ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, ncls, nms_pre)
         ws = self._t(ws_bytes, dtype=torch.uint8)
 
-        def decode():
+        def decode(n=n):
             L.check(lib.smb_pair_decode_topk_dev(nl, lv, ncls, ctypes.c_float(cfg['score_thr']), nms_pre, L.ptr(self.geom[n]),
                                                  L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(loc), L.ptr(n_cand), ncand,
                                                  L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
@@ -729,7 +729,7 @@ class SipMaskEngine(object):
         nws_bytes = lib.smb_ml_nms_workspace_bytes(ncand)
         nws = self._t(nws_bytes, dtype=torch.uint8)
 
-        def nms():
+        def nms(n=n):
             L.check(lib.smb_ml_nms_topk(L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(n_cand), ncand,
                                         ctypes.c_float(cfg['nms']['iou_thr']), self.max_num, self.max_num, L.ptr(self.det[n]),
                                         L.ptr(self.labels[n]), L.ptr(self.idx[n]), L.ptr(self.count[n:n + 1]),

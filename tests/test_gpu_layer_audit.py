@@ -4,7 +4,10 @@ reference of the operands it was actually given (teacher forcing), with the per-
 Around every op: its output region is NaN-filled first (a tile the op no longer writes cannot pass on a previous
 forward's values), and every other CUDA tensor the engine owns (activations, plan operands, packed weights) must be
 bitwise unchanged afterwards.  After the stepped forward the same engine replays as a CUDA graph (two streams) and must
-reproduce every activation buffer and the record bit for bit.  An op name without a rule fails the audit."""
+reproduce every activation buffer and the record bit for bit.  An op name without a rule fails the audit.
+
+The post-processing ops (candidates, NMS, gathers) are checked per image by oracle/postproc_check.py: bit-exact
+restatements, except the MM candidate selection, where the device sigmoid's proven bound decides what is certain."""
 import numpy as np
 import pytest
 import torch
@@ -14,7 +17,7 @@ from oracle import numerics as NU
 
 pytestmark = pytest.mark.gpu
 
-POSTPROC = {'gather_cofs', 'gather_track', 'decode_topk', 'nms'}      # bit-exact elsewhere
+POSTPROC = ('decode_topk', 'nms', 'gather_cofs', 'gather_track')
 MASKS = ('mask_fused', 'mask_dense')
 PATCHED = ('image_to_s2d16', 'maxpool3x3s2', 'upsample_bilinear', 'groupnorm_relu_apply_multi', 'offset_conv1x1_multi',
            'deform_im2col', 'deform_im2col_multi')
@@ -274,6 +277,72 @@ def _check_mask_dense(eng, n):
     return dict(ratio=NU.check_mask_values(eng.pos_masks[n], vals, what='mask_dense image %d' % n), count=k)
 
 
+def _closure(f):
+    return dict(zip(f.__code__.co_freevars, (c.cell_contents for c in f.__closure__ or ())))
+
+
+def _postproc_outputs(eng, f, name, n):
+    """Everything a post-processing op of image n writes, its workspace included."""
+    if name == 'gather_cofs':
+        return [eng.det_cofs[n], eng.det_boxes4[n], eng.loc_kept[n]]
+    if name == 'gather_track':
+        return [eng.det_track[n]]
+    if name == 'decode_topk':
+        ws = _closure(f)['ws']
+        if eng.benchmark:
+            return [eng.cand_boxes[n], eng.cand_scores[n], eng.cand_labels[n], eng.cand_loc[n], eng.n_cand[n:n + 1], ws]
+        return [eng.cand_boxes[n], eng.cand_scores[n], eng.cand_ctr[n], eng.cand_loc[n], ws]
+    outs = [eng.det[n], eng.labels[n], eng.idx[n], eng.count[n:n + 1], _closure(f)['nws']]
+    return outs + [eng.kept_total[n:n + 1]] if eng.benchmark else outs
+
+
+def _np(t):
+    return t.detach().cpu().numpy()
+
+
+def _check_postproc(eng, name, n):
+    """Image n's decode_topk / nms / gather_cofs / gather_track against oracle/postproc_check.py, on the buffers the op
+    read."""
+    from oracle import postproc_check as PC
+    from sipmask_b200 import _lib as L
+    gm = L.ImgGeom.from_buffer_copy(eng.geom[n].cpu().numpy().tobytes())
+    geom = PC.geometry_from_row(gm)
+    cfg, what = eng.cfg, '%s image %d' % (name, n)
+    if name == 'decode_topk':
+        levels = [PC.level_inputs(v['cls'][n], v['box'][n], v['ctr'][n], s, eng.scales[l], s)
+                  for l, (v, s) in enumerate(zip(eng.level_views, eng.strides))]
+        if eng.benchmark:
+            k = PC.check_pair_decode(levels, eng.ncls, cfg['score_thr'], int(cfg['nms_pre']), geom, _np(eng.cand_boxes[n]),
+                                     _np(eng.cand_scores[n]), _np(eng.cand_labels[n]), _np(eng.cand_loc[n]),
+                                     _np(eng.n_cand[n]), what=what)
+            return dict(what='%d pair candidates, bit-exact' % k)
+        st = PC.check_candidates(levels, int(cfg['nms_pre']), geom, _np(eng.cand_boxes[n]), _np(eng.cand_scores[n]),
+                                 _np(eng.cand_ctr[n]), _np(eng.cand_loc[n]), what=what)
+        return dict(what='%d locations, %d in cut levels' % (st['locations'], st['cut_locations']),
+                    ambiguous=st['ambiguous'], cut=st['cut_locations'])
+    rec = (_np(eng.det[n]), _np(eng.labels[n]), _np(eng.idx[n]), _np(eng.count[n]))
+    iou = float(cfg['nms']['iou_thr'])
+    if name == 'nms':
+        if eng.benchmark:
+            k = PC.check_ml_nms(_np(eng.cand_boxes[n]), _np(eng.cand_scores[n]), _np(eng.cand_labels[n]), _np(eng.n_cand[n]),
+                                iou, eng.max_num, eng.max_num, *rec, _np(eng.kept_total[n]), what=what)
+        elif eng.ssd or eng.vis:
+            k = PC.check_fast_nms(_np(eng.cand_boxes[n]), _np(eng.cand_scores[n]), _np(eng.cand_ctr[n]), eng.ncand,
+                                  cfg['score_thr'], iou, 200, eng.max_num, *rec, what=what)
+        else:
+            k = PC.check_multiclass_nms(_np(eng.cand_boxes[n]), _np(eng.cand_scores[n]), _np(eng.cand_ctr[n]), eng.ncand,
+                                        cfg['score_thr'], iou, eng.max_num, False, *rec, what=what, use_c=True)
+        return dict(what='%d detections, bit-exact' % k)
+    if name == 'gather_cofs':
+        hw = [h * w for h, w in eng.level_sizes] if eng.N > 1 else None
+        k = PC.check_gather_cofs(_np(eng.cof_src), _np(eng.cand_loc[n]), rec[2], rec[0], rec[3], hw, eng.N, n,
+                                 _np(eng.det_cofs[n]), _np(eng.det_boxes4[n]), _np(eng.loc_kept[n]), what=what)
+        return dict(what='%d rows, bit-exact' % k)
+    k = PC.check_gather_track(_np(eng.track_feats[n]), rec[0], rec[3], gm.track_sx, gm.track_sy, 8.0, _np(eng.det_track[n]),
+                              what=what)
+    return dict(what='%d rows, bit-exact' % k)
+
+
 # ------------------------------------------------------------------------------------------------------- the audit
 def audit(eng, log=print):
     """Steps through eng.ops; returns {kind: [ratio, misrounded, count]} and checks the graph replay afterwards."""
@@ -343,7 +412,22 @@ def audit(eng, log=print):
             if f is None:
                 continue
             if name in POSTPROC:
+                n = f.__defaults__[0]                     # the image the per-image closure was built for
+                outs = _postproc_outputs(eng, f, name, n)
+                for t in outs:
+                    if not t.is_floating_point():
+                        t.fill_(-1)                       # poison: the kernels must write every element
+                guard.prepare(outs)
                 f()
+                torch.cuda.synchronize()
+                guard.verify('op %d %s image %d' % (i, name, n))
+                st = _check_postproc(eng, name, n)
+                log('     %s image %d: %s, ambiguous %d' % (name, n, st['what'], st.get('ambiguous', 0)))
+                if 'cut' in st:
+                    amb = summary.setdefault('ambiguous candidates', [0, 0])
+                    amb[0] += st['ambiguous']
+                    amb[1] += st['cut']
+                note(name, i, '%s image %d' % (name, n), tuple(outs[0].shape), None, dict(ratio=0.0))
                 continue
             if name in MASKS:
                 n = f.__defaults__[0]                     # the image the per-image closure was built for
@@ -456,7 +540,7 @@ def _engine(cfg):
     from sipmask_b200.engine import SipMaskEngine
     if cfg == 'mm_r50_b2':
         sd = synth.detector_state_dict(50, 4, gn=True, seed=1, cls_bias=-2.5)
-        return SipMaskEngine(sd, (128, 192), batch=2, img_shape=(128, 187, 3), use_graph=False), (128, 192, 2)
+        return SipMaskEngine(sd, (128, 192), batch=2, img_shape=(128, 187, 3), max_ori_hw=(200, 260), use_graph=False), (128, 192, 2)
     if cfg == 'workload_a':
         sd = synth.detector_state_dict(50, 4, gn=True, seed=1, cls_bias=-2.5)
         return SipMaskEngine(sd, (800, 1344), batch=1, img_shape=(800, 1333, 3), use_graph=False), (800, 1344, 1)
@@ -466,11 +550,12 @@ def _engine(cfg):
         cfg_ = dict(nms_pre=200, score_thr=0.1, nms=dict(type='nms', iou_thr=0.5), max_per_img=100)
         return SipMaskEngine(sd, (256, 256), batch=2, depth=50, stacked_convs=2, gn=False, ssd_flag=True, backbone_dcn=True,
                              test_cfg=cfg_, rescoring_flag=True, scale_factor=np.ones(4, dtype=np.float32),
-                             use_graph=False), (256, 256, 2)
+                             max_ori_hw=(320, 320), use_graph=False), (256, 256, 2)
     if cfg == 'bm':
         from sipmask_b200 import benchmark as B
         sd = B.convert_state_dict(B.synthetic_state_dict())
-        return SipMaskEngine(sd, (128, 192), batch=2, img_shape=(120, 187, 3), use_graph=False, benchmark=True), (128, 192, 2)
+        return SipMaskEngine(sd, (128, 192), batch=2, img_shape=(120, 187, 3), max_ori_hw=(160, 240), use_graph=False,
+                             benchmark=True), (128, 192, 2)
     if cfg == 'vis':
         sd = {}
         sd.update(synth.backbone_state_dict(50, 1))
@@ -487,9 +572,21 @@ def _engine(cfg):
     if cfg == 'workload_b':
         sd = synth.detector_state_dict(50, 2, gn=False, seed=1, cls_bias=-2.5)
         return SipMaskEngine(sd, (544, 544), batch=3, stacked_convs=2, gn=False, ssd_flag=True,
-                             scale_factor=np.ones(4, dtype=np.float32), use_graph=False), (544, 544, 3)
+                             scale_factor=np.ones(4, dtype=np.float32), max_ori_hw=(640, 640), use_graph=False), (544, 544, 3)
     raise KeyError(cfg)
 
+
+# per-image shapes and scale factors of the batched configs, so the geometry rows and the N > 1 coefficient layout matter
+# (per-axis factors in mm_r50_b2)
+_SY = float(np.float32(112.0 / 150.0))
+METAS = {
+    'mm_r50_b2': [((128, 187, 3), (128, 187, 3), 1.0),
+                  ((112, 160, 3), (150, 200, 3), np.array([0.8, _SY, 0.8, _SY], np.float32))],
+    'pp': [((256, 256, 3), (256, 256, 3), 1.0), ((240, 224, 3), (300, 280, 3), np.full(4, 0.8, np.float32))],
+    'bm': [((120, 187, 3), (120, 187, 3), 1.0), ((104, 150, 3), (130, 190, 3), 1.0)],
+    'workload_b': [((544, 544, 3), (544, 544, 3), 1.0), ((512, 480, 3), (640, 600, 3), np.full(4, 0.8, np.float32)),
+                   ((400, 544, 3), (400, 544, 3), 1.0)],
+}
 
 CONFIGS = ['mm_r50_b2', 'workload_a', 'pp', 'bm', 'vis', 'fcos_head', 'workload_b']
 
@@ -498,6 +595,9 @@ CONFIGS = ['mm_r50_b2', 'workload_a', 'pp', 'bm', 'vis', 'fcos_head', 'workload_
 def test_every_engine_layer_within_its_bound(cfg):
     from sipmask_b200 import synth
     eng, shp = _engine(cfg)
+    if cfg in METAS:
+        eng.set_image_meta(METAS[cfg])
+        torch.cuda.synchronize()
     if shp is None:
         g = torch.Generator().manual_seed(5)
         for t in eng.fpn_outs:
@@ -509,7 +609,14 @@ def test_every_engine_layer_within_its_bound(cfg):
     summary = audit(eng, log=lines.append)
     print('\n'.join(lines))
     by_k = summary.pop('misrounded by K')
+    amb, cut = summary.pop('ambiguous candidates', [0, 0])
+    print('%s ambiguous candidate selections: %d of %d locations of cut levels (%.2e)' % (cfg, amb, cut, amb / max(cut, 1)))
     print('%s ops audited: ' % cfg + ', '.join('%s x%d (worst err/bound %.3f, misrounded %.4f)' % (k, v[2], v[0], v[1])
                                                for k, v in sorted(summary.items())))
     print('%s misrounded fp16 outputs by K: ' % cfg + ', '.join('K=%d %.4f' % kv for kv in sorted(by_k.items())))
     assert summary['conv'][2] > 0 and summary['conv fp32 out'][2] > 0
+    if cfg != 'fcos_head':
+        n_img = shp[2]
+        for op in POSTPROC[:3] + (('gather_track',) if cfg == 'vis' else ()):
+            got = summary.get(op, [0, 0, 0])[2]
+            assert got == n_img, '%s: %s audited %d times for %d images' % (cfg, op, got, n_img)
