@@ -12,6 +12,7 @@ copy of the packed weights but own their activations and CUDA graph; `EnginePool
 round-robin on n streams with the persistent conv grids capped (64 CTAs), so the images fill each other's bubbles.
 Every forward is still one image (imgs_per_gpu == 1, base.py:118-119); only the throughput changes.
 """
+import contextlib
 import gc
 
 import numpy as np
@@ -43,86 +44,223 @@ def _masks_mode(masks):
 DEFAULT_RLE_BYTES = 1 << 16
 
 
+@contextlib.contextmanager
+def _min_tiles(n):
+    """Engines built inside the block plan their convolutions with the planner's min_tiles set to n."""
+    prev = C.set_min_tiles(n)
+    try:
+        yield
+    finally:
+        C.set_min_tiles(prev)
+
+
 def make_engines(state_dict, img_hw, in_flight=1, **kw):
     """n engines for n images in flight (weights shared, activations private)."""
     tune = _tuning(in_flight)
-    prev = C.set_min_tiles(kw.pop('min_tiles', tune.pop('min_tiles')))
+    min_tiles = kw.pop('min_tiles', tune.pop('min_tiles'))
     for k, v in tune.items():
         kw.setdefault(k, v)
-    try:
-        engs = []
+    engs = []
+    with _min_tiles(min_tiles):
         for i in range(in_flight):
             engs.append(SipMaskEngine(state_dict, img_hw, share_weights=engs[0] if engs else None, **kw))
-    finally:
-        C.set_min_tiles(prev)
     return engs
 
 
+def _image_segms(region, eng, j, ori, planes):
+    """Image j's list of RLE dicts from the pinned region eng's encoder wrote a slot's strings into; an image whose
+    strings overflowed the encoder's capacities is encoded on the host from planes[j] (the forward's device bit planes)."""
+    from . import rle as R
+    ib = eng.rle_img_bytes
+    return R.image_segms(region.numpy()[j * ib:(j + 1) * ib], eng.max_num, ori, lambda n: planes[j, :n].cpu().numpy())
+
+
+def _record(o):
+    """The record of a slot's buffers (device or host), under the engine's record names."""
+    rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'])
+    for name, key in (('idx', 'idxs_keep'), ('bits', 'mask_bits'), ('trk', 'track_feats'), ('msc', 'mask_scores')):
+        if name in o:
+            rec[key] = o[name]
+    return rec
+
+
+def _queue_step(pending, n, ks, fn, consume):
+    """Queue the slots just launched (ks) in pending; with fn, hand the OLDEST to consume(slot, fn) while all n slots are
+    in flight, so the consumer (e.g. the all-gather) never stalls the slots behind it.  Without fn nothing is queued."""
+    pending += ks
+    if fn is None:
+        pending.clear()
+    while len(pending) >= n:
+        consume(pending.pop(0), fn)
+
+
+def _queue_flush(pending, fn, consume):
+    """Hand every queued slot to consume(slot, fn), oldest first (fn=None: drop them)."""
+    while pending:
+        k = pending.pop(0)
+        if fn is not None:
+            consume(k, fn)
+
+
+class _Slots(object):
+    """The streams and events of n staging slots, and the order of the work on them.  Slot k has an input (what
+    the H2D stream uploads and compute reads) and an output (the record compute writes, the D2H stream downloads and a
+    consumer reads on its own stream).  Five events per slot decide when each may be overwritten:
+      ev_in_ready   the uploads into slot k are done: its compute waits for them;
+      ev_in_free    compute consumed slot k's input: the next upload into slot k waits for it;
+      ev_out_ready  compute wrote slot k's record: its download and its consumer wait for it;
+      ev_out_free   slot k's download is done: the slot's next record and result() wait for it;
+      ev_hold       slot k's last consumer is done with the record (None before the first): the next record waits for it.
+    copies=False: no H2D / D2H streams (the inputs are in the engines, the records are read where compute wrote them).
+    streams=False: every slot computes on the current stream."""
+
+    def __init__(self, dev, n, streams=True, copies=True):
+        self.dev, self.n = dev, n
+        self.h2d = torch.cuda.Stream(device=dev) if copies else None
+        self.d2h = torch.cuda.Stream(device=dev) if copies else None
+        self.streams = [torch.cuda.Stream(device=dev) for _ in range(n)] if streams else None
+        self.ev_in_ready, self.ev_in_free, self.ev_out_ready, self.ev_out_free = ([torch.cuda.Event() for _ in range(n)]
+                                                                                  for _ in range(4))
+        self.ev_hold = [None] * n
+
+    def warm_up(self, engs, fwd):
+        """fwd(engine) twice per engine on its slot's stream (warm-up + graph capture), then wait for them."""
+        cur = torch.cuda.current_stream(self.dev)
+        for st, eng in zip(self.streams or [cur], engs):
+            if self.streams:
+                st.wait_stream(cur)
+            with torch.cuda.stream(st):
+                fwd(eng)
+                fwd(eng)
+        for st in self.streams or [cur]:
+            st.synchronize()
+
+    def mark_free(self):
+        """Every slot's input and output may be overwritten once the current stream's work so far is done."""
+        cur = torch.cuda.current_stream(self.dev)
+        for e in self.ev_in_free + self.ev_out_free:
+            e.record(cur)
+
+    def claim_input(self, k):
+        """The uploads that follow wait until compute consumed slot k's previous input."""
+        self.h2d.wait_event(self.ev_in_free[k])
+
+    def upload(self, dst, src):
+        with torch.cuda.stream(self.h2d):
+            dst.copy_(src, non_blocking=True)
+
+    def begin_compute(self, k):
+        """What the H2D stream uploaded so far is slot k's input: returns the slot's compute stream, made to wait for it."""
+        self.ev_in_ready[k].record(self.h2d)
+        cs = self.streams[k] if self.streams else torch.cuda.current_stream(self.dev)
+        cs.wait_event(self.ev_in_ready[k])
+        return cs
+
+    def input_free(self, k, cs):
+        """Slot k's input is consumed once cs's work so far is done."""
+        self.ev_in_free[k].record(cs)
+
+    def claim_output(self, k, cs):
+        """cs's next work, which writes slot k's record, waits until the slot's previous record is downloaded and
+        released by its consumer."""
+        if self.d2h is not None:
+            cs.wait_event(self.ev_out_free[k])
+        if self.ev_hold[k] is not None:
+            cs.wait_event(self.ev_hold[k])
+
+    def publish(self, k, cs):
+        """Slot k's record is complete once cs's work so far is done."""
+        self.ev_out_ready[k].record(cs)
+
+    def await_record(self, k, stream):
+        """stream waits until slot k's record is published."""
+        stream.wait_event(self.ev_out_ready[k])
+
+    def download(self, k, copies, after=None):
+        """The (host, device) copies on the D2H stream once slot k's record is published, or once the event `after` (of
+        work that waited for the record) is; the slot's output is free when they are done."""
+        with torch.cuda.stream(self.d2h):
+            self.d2h.wait_event(self.ev_out_ready[k] if after is None else after)
+            for dst, src in copies:
+                dst.copy_(src, non_blocking=True)
+            self.ev_out_free[k].record(self.d2h)
+
+    def hold(self, k, stream):
+        """Slot k's next record waits until stream's work so far is done."""
+        if self.ev_hold[k] is None:
+            self.ev_hold[k] = torch.cuda.Event()
+        self.ev_hold[k].record(stream)
+
+    def hand_over(self, k, work):
+        """work() on the CURRENT stream once slot k's record is published; the slot's next record waits for what work
+        enqueued.  Returns work's result."""
+        cur = torch.cuda.current_stream(self.dev)
+        self.await_record(k, cur)
+        r = work()
+        self.hold(k, cur)
+        return r
+
+    def join(self, *streams):
+        """Make the current stream wait for `streams`, by default for the downloads (and so for every record in flight),
+        or for the compute streams when there are none."""
+        cur = torch.cuda.current_stream(self.dev)
+        for s in streams or ([self.d2h] if self.d2h is not None else self.streams):
+            cur.wait_stream(s)
+
+    def wait(self, k):
+        """Block the host until slot k's download has finished."""
+        self.ev_out_free[k].synchronize()
+
+
 class EnginePool(object):
-    """Round-robin replay of n resident engines on n streams (inputs already in each engine's `img`)."""
+    """Round-robin replay of n resident engines on n streams (inputs already in each engine's `img`).  Each engine's
+    outputs are its slot's record."""
 
     def __init__(self, engines):
         self.engs = list(engines)
         self.n = len(self.engs)
         dev = self.engs[0].dev
         self.dev = dev
-        self.streams = [torch.cuda.Stream(device=dev) for _ in self.engs]
-        self.ev_done = [torch.cuda.Event() for _ in self.engs]
-        self.ev_consumed = [torch.cuda.Event() for _ in self.engs]
+        self.slots = _Slots(dev, self.n, copies=False)
         self.i = 0
         self.pending = []
-        cur = torch.cuda.current_stream(dev)
-        for st, eng in zip(self.streams, self.engs):
-            st.wait_stream(cur)
-            with torch.cuda.stream(st):
-                eng.forward(None)                  # warm-up + graph capture on the engine's own stream
-                eng.forward(None)
-        for st in self.streams:
-            st.synchronize()
-        for e in self.ev_consumed:
-            e.record(cur)
+        self.slots.warm_up(self.engs, lambda eng: eng.forward(None))
+        for k in range(self.n):
+            self.slots.hold(k, torch.cuda.current_stream(dev))
+
+    @property
+    def streams(self):
+        return self.slots.streams
 
     def launch(self):
         """Enqueue one image on the next engine; returns its index.  Does not block the host."""
         k = self.i % self.n
         st = self.streams[k]
-        st.wait_event(self.ev_consumed[k])
+        self.slots.claim_output(k, st)
         with torch.cuda.stream(st):
             self.engs[k].forward(None)
-        self.ev_done[k].record(st)
+        self.slots.publish(k, st)
         self.i += 1
         return k
 
     def consume(self, k, fn):
         """Run fn(engine_k_outputs) on the CURRENT stream once image k is done; engine k is not replayed again before fn's
         work has finished (used for the all-gather of the detection record)."""
-        cur = torch.cuda.current_stream(self.dev)
-        cur.wait_event(self.ev_done[k])
-        eng = self.engs[k]
-        r = fn(eng._result())
-        self.ev_consumed[k].record(cur)
-        return r
+        return self.slots.hand_over(k, lambda: fn(self.engs[k]._result()))
 
     def step(self, fn=None):
         """One image: launch it, and (if fn is given) hand the OLDEST image in flight to fn on the current stream, so the
         consumer (e.g. the all-gather) never stalls the images behind it."""
-        self.pending.append(self.launch())
-        if fn is not None and len(self.pending) >= self.n:
-            self.consume(self.pending.pop(0), fn)
+        _queue_step(self.pending, self.n, [self.launch()], fn, self.consume)
 
     def flush(self, fn=None):
         """Consume what is still in flight and make the current stream wait for all of it."""
-        while self.pending:
-            k = self.pending.pop(0)
-            if fn is not None:
-                self.consume(k, fn)
+        _queue_flush(self.pending, fn, self.consume)
         self.join()
 
     def join(self):
         """Make the current stream wait for everything in flight."""
-        cur = torch.cuda.current_stream(self.dev)
-        for st in self.streams:
-            cur.wait_stream(st)
+        self.slots.join()
 
 
 class PipelinedRunner(object):
@@ -147,9 +285,8 @@ class PipelinedRunner(object):
         ns = self.nslots
         dev = engine.dev
         self.dev = dev
-        self.s_h2d = torch.cuda.Stream(device=dev)
-        self.s_d2h = torch.cuda.Stream(device=dev)
-        self.s_comp = [torch.cuda.Stream(device=dev) for _ in self.engs] if self.n > 1 else [None]
+        # several engines: each slot computes on its engine's stream; one engine: every slot on the current stream
+        self.slots = _Slots(dev, ns, streams=self.n > 1)
         self.raw = raw_hw is not None
         if self.raw:
             assert engine.N == 1, 'raw uint8 input: one image per forward'
@@ -170,31 +307,13 @@ class PipelinedRunner(object):
         if self.rle:
             self.rle_regions = [torch.zeros(engine.N * engine.rle_img_bytes, dtype=torch.uint8).pin_memory() for _ in range(ns)]
             self.slot_oris = [None] * ns
-        self.ev_in_ready = [torch.cuda.Event() for _ in range(ns)]      # H2D of slot finished
-        self.ev_in_free = [torch.cuda.Event() for _ in range(ns)]       # compute consumed the slot's input
-        self.ev_out_ready = [torch.cuda.Event() for _ in range(ns)]     # compute wrote the slot's output
-        self.ev_out_free = [torch.cuda.Event() for _ in range(ns)]      # D2H of slot finished
-        self.ev_hold = [None] * ns                                      # optional: a consumer still reads out_dev[slot]
         self.i = 0
         self.pending = []
         self.h2d_bytes = self.in_dev[0].numel() * self.in_dev[0].element_size()
         # fixed-size downloads per forward (rle: plus the strings and headers the encoder writes, which vary per image)
         self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.out_host[0].values())
-        cur = torch.cuda.current_stream(dev)
-        if self.n > 1:
-            for st, eng in zip(self.s_comp, self.engs):
-                st.wait_stream(cur)
-                with torch.cuda.stream(st):
-                    self._fwd(eng, 0)              # warm-up + graph capture on the engine's own stream
-                    self._fwd(eng, 0)
-            for st in self.s_comp:
-                st.synchronize()
-        else:
-            self._fwd(engine, 0)
-            self._fwd(engine, 0)
-            cur.synchronize()
-        for e in self.ev_in_free + self.ev_out_free:
-            e.record(cur)
+        self.slots.warm_up(self.engs, lambda eng: self._fwd(eng, 0))
+        self.slots.mark_free()
 
     def _fwd(self, eng, k):
         if self.raw:
@@ -207,28 +326,23 @@ class PipelinedRunner(object):
         Nothing here blocks the host."""
         k = self.i % self.nslots
         eng = self.engs[k % self.n]
-        cur = torch.cuda.current_stream(self.dev)
-        cs = self.s_comp[k % self.n] or cur
-        with torch.cuda.stream(self.s_h2d):
-            self.s_h2d.wait_event(self.ev_in_free[k])
-            self.in_dev[k].copy_(host_img, non_blocking=True)
-            self.ev_in_ready[k].record(self.s_h2d)
+        sl = self.slots
+        sl.claim_input(k)
+        sl.upload(self.in_dev[k], host_img)
+        o = self.out_dev[k]
+        cs = sl.begin_compute(k)
         with torch.cuda.stream(cs):
-            cs.wait_event(self.ev_in_ready[k])
             if self.rle:
                 eng.set_rle_dest(self.rle_regions[k])      # this slot's strings go to this slot's region
                 self.slot_oris[k] = [m[1][:2] for m in eng.image_metas]
             if self.raw:
                 eng.forward_raw(self.in_dev[k])            # preprocess kernel reads the staged uint8 image, then the graph
-                self.ev_in_free[k].record(cs)
+                sl.input_free(k, cs)
             else:
                 eng.img.copy_(self.in_dev[k], non_blocking=True)
-                self.ev_in_free[k].record(cs)
+                sl.input_free(k, cs)
                 eng.forward(None)
-            cs.wait_event(self.ev_out_free[k])
-            if self.ev_hold[k] is not None:
-                cs.wait_event(self.ev_hold[k])
-            o = self.out_dev[k]
+            sl.claim_output(k, cs)
             o['det'].copy_(eng.det, non_blocking=True)
             o['lab'].copy_(eng.labels, non_blocking=True)
             o['cnt'].copy_(eng.count, non_blocking=True)
@@ -237,71 +351,46 @@ class PipelinedRunner(object):
                 o['trk'].copy_(eng.det_track, non_blocking=True)
             if 'msc' in o:
                 o['msc'].copy_(eng.mask_scores, non_blocking=True)
-            self.ev_out_ready[k].record(cs)
-        with torch.cuda.stream(self.s_d2h):
-            self.s_d2h.wait_event(self.ev_out_ready[k])
-            for name in self.out_host[k]:
-                self.out_host[k][name].copy_(o[name], non_blocking=True)
-            self.ev_out_free[k].record(self.s_d2h)
+            sl.publish(k, cs)
+        sl.download(k, [(h, o[name]) for name, h in self.out_host[k].items()])
         self.i += 1
         return k
 
     def consume(self, slot, fn):
         """Run fn(slot's device record) on the CURRENT stream once it is ready; the slot is not overwritten before fn's
         work has finished (used for the all-gather of the detection record)."""
-        cur = torch.cuda.current_stream(self.dev)
-        cur.wait_event(self.ev_out_ready[slot])
-        o = self.out_dev[slot]
-        rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'], mask_bits=o['bits'])
-        if 'trk' in o:
-            rec['track_feats'] = o['trk']
-        if 'msc' in o:
-            rec['mask_scores'] = o['msc']
-        r = fn(rec)
-        if self.ev_hold[slot] is None:
-            self.ev_hold[slot] = torch.cuda.Event()
-        self.ev_hold[slot].record(cur)
-        return r
+        rec = _record(self.out_dev[slot])
+        return self.slots.hand_over(slot, lambda: fn(rec))
 
     def step(self, host_img, fn=None):
         """submit() + hand the OLDEST slot in flight to fn (see EnginePool.step).  Returns the submitted slot."""
         k = self.submit(host_img)
-        self.pending.append(k)
-        if fn is not None and len(self.pending) >= self.nslots:
-            self.consume(self.pending.pop(0), fn)
-        elif fn is None:
-            self.pending.clear()
+        _queue_step(self.pending, self.nslots, [k], fn, self.consume)
         return k
 
     def flush(self, fn=None):
-        while self.pending:
-            k = self.pending.pop(0)
-            if fn is not None:
-                self.consume(k, fn)
+        _queue_flush(self.pending, fn, self.consume)
         self.join()
 
     def result(self, slot):
         """Blocks until the slot's download finished; returns pinned host tensors (valid until the slot is reused).
         masks='rle': a dict of them with 'segms' (one list of RLE dicts per image of the forward) in place of 'bits'."""
-        self.ev_out_free[slot].synchronize()
+        self.slots.wait(slot)
         if not self.rle:
             return self.out_host[slot]
-        from . import rle as R
         eng = self.engs[slot % self.n]
-        ib, bits = eng.rle_img_bytes, self.out_dev[slot]['bits']
-        region = self.rle_regions[slot].numpy()
         rec = dict(self.out_host[slot])
-        rec['segms'] = [R.image_segms(region[i * ib:(i + 1) * ib], eng.max_num, ori, lambda k, i=i: bits[i, :k].cpu().numpy())
+        rec['segms'] = [_image_segms(self.rle_regions[slot], eng, i, ori, self.out_dev[slot]['bits'])
                         for i, ori in enumerate(self.slot_oris[slot])]
         return rec
 
     def join(self):
         """Make the current stream wait for the downloads (and so for every image in flight)."""
-        torch.cuda.current_stream(self.dev).wait_stream(self.s_d2h)
+        self.slots.join()
 
     def drain(self):
-        self.s_d2h.synchronize()
-        self.s_h2d.synchronize()
+        self.slots.d2h.synchronize()
+        self.slots.h2d.synchronize()
 
 
 def rescale_size(h, w, scale=(1333, 800)):
@@ -321,19 +410,20 @@ def image_meta(h, w, resize=(1333, 800), keep_ratio=True, size_divisor=32):
     else:
         nw, nh = int(resize[0]), int(resize[1])
         sf = np.array([nw / w, nh / h, nw / w, nh / h], dtype=np.float32)
-    ph = (nh + size_divisor - 1) // size_divisor * size_divisor
-    pw = (nw + size_divisor - 1) // size_divisor * size_divisor
-    return (nh, nw, 3), (ph, pw, 3), sf
+    return (nh, nw, 3), (_pad(nh, size_divisor), _pad(nw, size_divisor), 3), sf
+
+
+def _pad(v, size_divisor):
+    """v rounded up to a multiple of size_divisor (the Pad transform)."""
+    return (int(v) + size_divisor - 1) // size_divisor * size_divisor
 
 
 def largest_pad_shapes(resize=(1333, 800), keep_ratio=True, size_divisor=32):
     """The padded shapes no other image exceeds under the rule: (short, long) and (long, short) for keep_ratio,
     the one fixed shape otherwise."""
-    def up(v):
-        return (int(v) + size_divisor - 1) // size_divisor * size_divisor
     if not keep_ratio:
-        return [(up(resize[1]), up(resize[0]))]
-    s, l = up(min(resize)), up(max(resize))
+        return [(_pad(resize[1], size_divisor), _pad(resize[0], size_divisor))]
+    s, l = _pad(min(resize), size_divisor), _pad(max(resize), size_divisor)
     return [(s, l), (l, s)] if s != l else [(s, l)]
 
 
@@ -360,9 +450,7 @@ def bm_image_meta(h, w, min_size=800, max_size=1333, size_divisor=32):
     then to_image_list(size_divisible=32)).  The benchmark post-processing reads only img_shape and ori_shape
     (postproc.image_geometry(benchmark=True)); scale_factor = min(oh / h, ow / w) is the ratio its mask resize uses."""
     nh, nw = bm_resize_size(h, w, min_size, max_size)
-    ph = (nh + size_divisor - 1) // size_divisor * size_divisor
-    pw = (nw + size_divisor - 1) // size_divisor * size_divisor
-    return (nh, nw, 3), (ph, pw, 3), min(nh / h, nw / w)
+    return (nh, nw, 3), (_pad(nh, size_divisor), _pad(nw, size_divisor), 3), min(nh / h, nw / w)
 
 
 class StreamRunner(object):
@@ -445,9 +533,7 @@ class StreamRunner(object):
         torch.cuda.synchronize(self.dev)
         self.arena_bytes = need
         self.arenas = [torch.empty(need, dtype=torch.uint8, device=self.dev) for _ in range(self.n)]
-        self.streams = [torch.cuda.Stream(device=self.dev) for _ in range(self.n)]
-        self.s_h2d = torch.cuda.Stream(device=self.dev)
-        self.s_d2h = torch.cuda.Stream(device=self.dev)
+        self.slots = _Slots(self.dev, self.n)
         if self.benchmark and not self.bm_raw:
             ph, pw = max(largest_pad_shapes(self.resize, self.keep_ratio), key=lambda s: s[0] * s[1])
             self.src_elems = 3 * max(ph, pw) ** 2
@@ -458,13 +544,8 @@ class StreamRunner(object):
             self.in_dev = [torch.empty(self.B * self.src_elems, dtype=torch.uint8, device=self.dev) for _ in range(self.n)]
         self.out_dev, self.out_host = [], []
         self.rle_regions = [None] * self.n                # masks='rle': per slot, the pinned region of its batch's strings
-        self.ev_in_ready, self.ev_in_free, self.ev_out_ready, self.ev_out_free = ([torch.cuda.Event() for _ in range(self.n)]
-                                                                                  for _ in range(4))
-        self.ev_hold = [None] * self.n
         self._init_queue()
-        cur = torch.cuda.current_stream(self.dev)
-        for e in self.ev_in_free + self.ev_out_free:
-            e.record(cur)
+        self.slots.mark_free()
 
     def _init_queue(self):
         """Host bookkeeping of the batches: tickets, the open batch, what each slot holds."""
@@ -476,17 +557,13 @@ class StreamRunner(object):
         self.pending = []
 
     def _new_engine(self, hw, arena):
-        from .engine import SipMaskEngine
         H, W = hw
         cap = self.max_ori_hw
         ori = (min(H, cap[0]), min(W, cap[1]), 3)
-        prev = C.set_min_tiles(self.kw.get('min_tiles', self.tune['min_tiles']))
-        try:
-            kw = {k: v for k, v in self.kw.items() if k != 'min_tiles'}
+        kw = {k: v for k, v in self.kw.items() if k != 'min_tiles'}
+        with _min_tiles(self.kw.get('min_tiles', self.tune['min_tiles'])):
             return SipMaskEngine(self.sd, (H, W), batch=self.B, img_shape=(H, W, 3), ori_shape=ori, scale_factor=1.0,
                                  share_weights=self._wcache, arena=arena, device=self.dev, **kw)
-        finally:
-            C.set_min_tiles(prev)
 
     def _engine(self, k, hw):
         """The slot's engine for padded shape hw, built in the slot's arena and captured on first use."""
@@ -496,7 +573,7 @@ class StreamRunner(object):
             torch.cuda.synchronize(self.dev)
             t0 = time.perf_counter()
             eng = self._new_engine(hw, self.arenas[k])
-            with torch.cuda.stream(self.streams[k]):
+            with torch.cuda.stream(self.slots.streams[k]):
                 if self.benchmark and not self.bm_raw:
                     eng.forward(None)                  # warm-up + capture
                 else:
@@ -630,13 +707,12 @@ class StreamRunner(object):
         """A batch opens in slot k: its engine exists, and the uploads wait until the slot's previous batch consumed its
         input."""
         self._engine(k, hw)
-        self.s_h2d.wait_event(self.ev_in_free[k])
+        self.slots.claim_input(k)
 
     def _stage(self, k, j, img):
         """Upload image j of slot k's open batch into its staging on the H2D stream; returns the device view."""
         src = self.in_dev[k][j * self.src_elems:j * self.src_elems + img.numel()].view(img.shape)
-        with torch.cuda.stream(self.s_h2d):
-            src.copy_(img, non_blocking=True)
+        self.slots.upload(src, img)
         return src
 
     def _dispatch(self):
@@ -653,12 +729,11 @@ class StreamRunner(object):
 
     def _launch(self, k, pad, images):
         eng = self._engine(k, pad)
-        cs = self.streams[k]
-        self.ev_in_ready[k].record(self.s_h2d)
+        sl = self.slots
         nr = len(images)
         metas = [(m['img_shape'], m['ori_shape'], m['scale_factor']) for m in images]
+        cs = sl.begin_compute(k)
         with torch.cuda.stream(cs):
-            cs.wait_event(self.ev_in_ready[k])
             eng.set_image_meta(metas + [metas[-1]] * (self.B - nr))      # fillers: the last real image's geometry
             if self.rle:
                 if self.rle_regions[k] is None:
@@ -669,10 +744,8 @@ class StreamRunner(object):
                 eng.forward(None)
             else:
                 eng.forward_raw([m['src'] for m in images] + [None] * (self.B - nr), self.mean, self._pipeline)
-            self.ev_in_free[k].record(cs)
-            cs.wait_event(self.ev_out_free[k])
-            if self.ev_hold[k] is not None:
-                cs.wait_event(self.ev_hold[k])
+            sl.input_free(k, cs)
+            sl.claim_output(k, cs)
             dev, host, used = self._out(k, eng, [m['ori_shape'][:2] for m in images])
             flat = self.out_dev[k]
             mx = eng.max_num
@@ -688,7 +761,7 @@ class StreamRunner(object):
                 if 'bits' in o:
                     oh, wq = o['bits'].shape[1:]
                     o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
-            self.ev_out_ready[k].record(cs)
+            sl.publish(k, cs)
             self._after_forward(k, eng, images)
         self._download(k, used, images)
         for m, o, h in zip(images, dev, host):
@@ -701,47 +774,21 @@ class StreamRunner(object):
 
     def _download(self, k, used, images):
         """Enqueue the download of slot k's record (the first used[name] elements of every field) once its batch is done."""
-        flat = self.out_dev[k]
-        with torch.cuda.stream(self.s_d2h):
-            self.s_d2h.wait_event(self.ev_out_ready[k])
-            for name, n in used.items():
-                self.out_host[k][name][:n].copy_(flat[name][:n], non_blocking=True)
-            self.ev_out_free[k].record(self.s_d2h)
+        self.slots.download(k, [(self.out_host[k][name][:n], self.out_dev[k][name][:n]) for name, n in used.items()])
 
     def consume(self, slot, fn):
         """Run fn(record on the device) on the CURRENT stream for every image of the slot's batch, in submission order,
         once the batch is done; the slot is not overwritten before fn's work has finished.  Returns fn's result (batch=1)
         or the list of them."""
-        cur = torch.cuda.current_stream(self.dev)
-        cur.wait_event(self.ev_out_ready[slot])
-        rs = [fn(self._record(m['dev'])) for m in self.slot_images[slot]]
-        if self.ev_hold[slot] is None:
-            self.ev_hold[slot] = torch.cuda.Event()
-        self.ev_hold[slot].record(cur)
+        rs = self.slots.hand_over(slot, lambda: [fn(_record(m['dev'])) for m in self.slot_images[slot]])
         return rs[0] if self.B == 1 else rs
-
-    @staticmethod
-    def _record(o):
-        rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'], idxs_keep=o['idx'])
-        if 'bits' in o:
-            rec['mask_bits'] = o['bits']
-        if 'trk' in o:
-            rec['track_feats'] = o['trk']
-        if 'msc' in o:
-            rec['mask_scores'] = o['msc']
-        return rec
 
     def step(self, img, fn=None, meta=None):
         """submit() + hand the images of the OLDEST batch in flight to fn once in_flight batches are dispatched (see
         EnginePool.step).  Returns what submit() returned."""
         before = self.dispatched
         r = self.submit(img, meta)
-        self.pending += [b % self.n for b in range(before, self.dispatched)]
-        if fn is not None:
-            while len(self.pending) >= self.n:
-                self.consume(self.pending.pop(0), fn)
-        else:
-            self.pending.clear()
+        _queue_step(self.pending, self.n, [b % self.n for b in range(before, self.dispatched)], fn, self.consume)
         return r
 
     def flush(self, fn=None):
@@ -749,14 +796,11 @@ class StreamRunner(object):
         downloads."""
         if self._open is not None:
             self.pending.append(self._dispatch())
-        while self.pending:
-            k = self.pending.pop(0)
-            if fn is not None:
-                self.consume(k, fn)
+        _queue_flush(self.pending, fn, self.consume)
         self._join()
 
     def _join(self):
-        torch.cuda.current_stream(self.dev).wait_stream(self.s_d2h)
+        self.slots.join()
 
     def _locate(self, ticket):
         if self._open is not None and any(m['ticket'] == ticket for m in self._open['images']):
@@ -773,15 +817,12 @@ class StreamRunner(object):
         ceil(ori_w / 32)], track_feats / mask_scores when enabled) and the image's meta.  Valid until the slot is reused.
         masks='rle': segms (the image's RLE dicts, in detection order) in place of mask_bits."""
         k, j = (key, 0) if self.B == 1 else self._locate(key)
-        self.ev_out_free[k].synchronize()
+        self.slots.wait(k)
         m = self.slot_images[k][j]
-        rec = self._record(m['host'])
+        rec = _record(m['host'])
         if self.rle:
-            from . import rle as R
             eng = self.engines[k][m['pad_shape'][:2]]
-            ib = eng.rle_img_bytes
-            rec['segms'] = R.image_segms(self.rle_regions[k].numpy()[j * ib:(j + 1) * ib], eng.max_num, m['ori_shape'][:2],
-                                         lambda n: eng.mask_bits[j, :n].cpu().numpy())
+            rec['segms'] = _image_segms(self.rle_regions[k], eng, j, m['ori_shape'][:2], eng.mask_bits)
         rec['meta'] = dict(img_shape=m['img_shape'], pad_shape=m['pad_shape'], ori_shape=m['ori_shape'],
                            scale_factor=m['scale_factor'])
         return rec
@@ -894,7 +935,7 @@ class VideoRunner(StreamRunner):
             self.ids_host[k] = torch.empty((self.B, mx), dtype=torch.int32).pin_memory()
         flat, st, trk = self.out_dev[k], self.s_trk, self.tracker
         with torch.cuda.stream(st):
-            st.wait_event(self.ev_out_ready[k])
+            self.slots.await_record(k, st)
             trk.associate([self.rows[m['ticket']][:2] for m in images], flat['det'][:nr * mx * 5].view(nr, mx, 5),
                           flat['lab'][:nr * mx].view(nr, mx), flat['cnt'][:nr], flat['trk'][:nr * mx * 512].view(nr, mx, 512),
                           ids=self.ids_dev[k][:nr])
@@ -902,14 +943,10 @@ class VideoRunner(StreamRunner):
             trk.status.zero_()
             self._after_associate(k, images)
             self.ev_assoc[k].record(st)
-        with torch.cuda.stream(self.s_d2h):
-            self.s_d2h.wait_event(self.ev_assoc[k])
-            for name, n in used.items():
-                if name != 'trk':                           # the tracking features stay on the device
-                    self.out_host[k][name][:n].copy_(flat[name][:n], non_blocking=True)
-            self.ids_host[k][:nr].copy_(self.ids_dev[k][:nr], non_blocking=True)
-            self.status_host[k].copy_(self.status_dev[k], non_blocking=True)
-            self.ev_out_free[k].record(self.s_d2h)
+        # the tracking features stay on the device
+        copies = [(self.out_host[k][name][:n], flat[name][:n]) for name, n in used.items() if name != 'trk']
+        self.slots.download(k, copies + [(self.ids_host[k][:nr], self.ids_dev[k][:nr]),
+                                         (self.status_host[k], self.status_dev[k])], after=self.ev_assoc[k])
 
     def _after_associate(self, k, images):
         """Work on the tracker stream right after slot k's batch is associated (its object ids are in ids_dev[k]); the
@@ -1010,7 +1047,7 @@ class CocoEvalRunner(StreamRunner):
             raise ValueError('image id %d is evaluated twice' % image_id)
         self.evaluator.check_image(image_id, ori)
         t = self.i
-        self._eval_rows[t] = (image_id, self.evaluator.stage_gt(image_id, self.s_h2d))
+        self._eval_rows[t] = (image_id, self.evaluator.stage_gt(image_id, self.slots.h2d))
         try:
             r = super(CocoEvalRunner, self).submit(img, meta)
         except Exception:
@@ -1032,9 +1069,7 @@ class CocoEvalRunner(StreamRunner):
     def evaluate(self):
         """Dispatch the open batch, wait for every slot's evaluation and return CocoEvaluator.evaluate()'s dict."""
         self.flush()
-        cur = torch.cuda.current_stream(self.dev)
-        for s in self.streams:
-            cur.wait_stream(s)
+        self.slots.join(*self.slots.streams)
         return self.evaluator.evaluate()
 
 
@@ -1093,7 +1128,7 @@ class VideoEvalRunner(VideoRunner):
                 self.evaluator.begin_video(video_id, slot)
         t = self.i
         try:
-            staged = self._staged[t] = self.evaluator.stage_frame(video_id, frame_id, self.s_h2d)
+            staged = self._staged[t] = self.evaluator.stage_frame(video_id, frame_id, self.slots.h2d)
             super(VideoEvalRunner, self).submit(img, video_id, frame_id)
         except Exception:
             self._staged.pop(t, None)
@@ -1178,7 +1213,5 @@ class VideoEvalRunner(VideoRunner):
             raise ValueError('video %r has not ended: end_video() first' % (open_videos[0],))
         for v in list(self._vslot):
             self._finish(v)
-        cur = torch.cuda.current_stream(self.dev)
-        for s in self.streams + [self.s_trk]:
-            cur.wait_stream(s)
+        self.slots.join(*self.slots.streams, self.s_trk)
         return self.evaluator.evaluate()
