@@ -603,6 +603,39 @@ int smb_segm_raster_dev(const smb_segm_item_t* items, int n_items, const double*
                         int32_t* ext, int64_t ext_stride, int* status, void* workspace, size_t workspace_bytes,
                         smb_stream_t stream);
 
+/* ------------------------------------------------------------------ detections drawn onto images on the device
+ * The picture of the reference's show_result, for a batch of uint8 HWC 3-channel images in one launch:
+ *   rule SMB_RENDER_IMAGES : SipMask-mmdetection/mmdet/apis/inference.py:119-184 (show_result).  Drawn: the detections
+ *                            with score > score_thr (fp32), class-major (ascending label, detection order within a label),
+ *                            colour palette[label % palette_rows], blend p <- (p + c) >> 1 (= uint8(p * 0.5 + c * 0.5)).
+ *   rule SMB_RENDER_VIDEO  : SipMask-VIS/mmdet/models/detectors/base.py:90-192 (gen_colormask, show_result(is_video)).
+ *                            Drawn: one entry per object id >= 0, at the position of the id's first detection and with
+ *                            its last detection's score, box and mask (bbox2result_with_id's dict), when that score >
+ *                            score_thr; colour palette[obj_id % palette_rows], blend p <- uint8(c * 0.6 + p * 0.4) in
+ *                            float64 (each product and the sum rounded on its own).
+ * Masks are blended in draw order, every channel c of a set pixel with the colour's byte c.  boxes != 0: then every
+ * drawn box's outline in (0, 255, 0): corners truncated toward zero, the border of the inclusive rectangle [min x, max x]
+ * x [min y, max y] clipped to the image (what cv2.rectangle(thickness=1) sets).  The label text is not drawn.
+ *   imgs      : device rows [N]; image n is read from src and written to dst (src == dst: in place), h x w pixels
+ *               (its ori_shape) of 3 bytes, rows 3 * w bytes apart.  A row with h or w <= 0, a null pointer, h > max_h
+ *               or w > max_w is left untouched.  An image with nothing to draw is copied (src != dst) or left as it is.
+ *   mask_bits : the engine's record [N, max_num, cap_h, words] (pixel x = bit x&31 of word x>>5); only the planes of
+ *               image n's first count[n] (clamped to [0, max_num]) detections, rows < min(h, cap_h) and bits < w are read
+ *   det       : [N, max_num, 5] fp32 boxes + score; labels [N, max_num] int64 (images), obj_ids [N, max_num] int32 (videos;
+ *               the other may be NULL); palette [palette_rows, 3] uint8 device table.
+ * max_num <= SMB_RENDER_MAX_NUM; max_w is bounded by the shared memory a CTA may use (about 70,000 pixels on sm_90). */
+typedef struct {
+  const uint8_t* src;
+  uint8_t* dst;
+  int32_t h, w;
+} smb_render_img_t;
+#define SMB_RENDER_IMAGES 0
+#define SMB_RENDER_VIDEO 1
+#define SMB_RENDER_MAX_NUM 1024
+int smb_render_dev(const smb_render_img_t* imgs, int N, int max_h, int max_w, const uint32_t* mask_bits, int max_num,
+                   int cap_h, int words, const float* det, const int64_t* labels, const int* count, const int32_t* obj_ids,
+                   const uint8_t* palette, int palette_rows, int rule, float score_thr, int boxes, smb_stream_t stream);
+
 /* gather rows: dst[i,:] = src[idx[i],:] for i < *count (device count), zero otherwise. */
 int smb_gather_rows_f32(const float* src, int src_pitch, const int64_t* idx, const int* count_dev,
                         int max_rows, int row_elems, float* dst, smb_stream_t stream);

@@ -53,6 +53,13 @@ class TrackFrame(ctypes.Structure):
     _fields_ = [('lane', ctypes.c_int32), ('is_first', ctypes.c_int32)]
 
 
+class RenderImg(ctypes.Structure):
+    """smb_render_img_t: one image of a render launch (include/sipmask_b200.h)."""
+    _fields_ = [('src', ctypes.c_void_p), ('dst', ctypes.c_void_p), ('h', ctypes.c_int32), ('w', ctypes.c_int32)]
+
+
+RENDER_IMAGES, RENDER_VIDEO, RENDER_MAX_NUM = 0, 1, 1024    # SMB_RENDER_IMAGES / SMB_RENDER_VIDEO / SMB_RENDER_MAX_NUM
+
 TRACK_CAPACITY = 1                   # SMB_TRACK_CAPACITY: a lane had more tracked objects than its capacity
 
 
@@ -83,7 +90,7 @@ SYMBOLS = [
     'smb_coco_match_params_dev', 'smb_coco_accumulate_params_dev', 'smb_coco_analysis_workspace_bytes',
     'smb_coco_analysis_match_dev',
     'smb_ytvis_overlap_dev', 'smb_ytvis_scatter_dev', 'smb_ytvis_match_workspace_bytes', 'smb_ytvis_match_dev',
-    'smb_segm_raster_workspace_bytes', 'smb_segm_raster_dev',
+    'smb_segm_raster_workspace_bytes', 'smb_segm_raster_dev', 'smb_render_dev',
 ]
 
 

@@ -616,6 +616,30 @@ def segm_raster_workspace_bytes(n_items, max_hw, max_w):
 
 
 @L.device_guard
+def render(rows, n, max_hw, mask_bits, det, count, palette, rule, score_thr, boxes=True, labels=None, obj_ids=None):
+    """smb_render_dev on the current stream: n images (rows: device smb_render_img_t rows, uint8) drawn from a record
+    mask_bits [n, max, cap_h, words] int32, det [n, max, 5] fp32, count [n] int32 and labels [n, max] int64
+    (rule RENDER_IMAGES) or obj_ids [n, max] int32 (RENDER_VIDEO); palette [rows, 3] uint8 on the device.  score_thr is
+    compared in fp32.  The caller validates the rows against max_hw and the record (render.render_images does)."""
+    _need_cuda(rows, mask_bits, det, count, palette, labels, obj_ids)
+    mx = det.shape[1]
+    assert mask_bits.dtype == torch.int32 and mask_bits.dim() == 4 and mask_bits.is_contiguous()
+    assert tuple(mask_bits.shape[:2]) == (n, mx) and tuple(det.shape) == (n, mx, 5) and det.dtype == torch.float32
+    assert det.is_contiguous() and count.dtype == torch.int32 and count.numel() >= n and count.is_contiguous()
+    assert palette.dtype == torch.uint8 and palette.dim() == 2 and palette.shape[1] == 3 and palette.is_contiguous()
+    assert rows.dtype == torch.uint8 and rows.numel() >= n * ctypes.sizeof(L.RenderImg)
+    for t, dt in ((labels, torch.int64), (obj_ids, torch.int32)):
+        if t is not None:
+            assert t.dtype == dt and tuple(t.shape) == (n, mx) and t.is_contiguous()
+    cap_h, words = mask_bits.shape[2:]
+    L.check(L.lib().smb_render_dev(L.ptr(rows), int(n), int(max_hw[0]), int(max_hw[1]), L.ptr(mask_bits), int(mx),
+                                   int(cap_h), int(words), L.ptr(det), L.ptr(labels), L.ptr(count), L.ptr(obj_ids),
+                                   L.ptr(palette), int(palette.shape[0]), int(rule),
+                                   ctypes.c_float(float(np.float32(score_thr))), int(bool(boxes)), L.stream_ptr()),
+            'smb_render_dev')
+
+
+@L.device_guard
 def segm_raster(items, n_items, xy, n_xy, counts, n_counts, max_hw, max_w, planes, n_planes, plane_stride, pitch, status,
                 area=None, area_stride=1, ext=None, ext_stride=4, workspace=None):
     """smb_segm_raster_dev: zero planes [n_planes, plane_stride words] (int32, rows of `pitch` words) and rasterize

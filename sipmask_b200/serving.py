@@ -18,7 +18,9 @@ import gc
 import numpy as np
 import torch
 
+from . import _lib as L
 from . import conv as C
+from . import render as R
 from ._lib import TRACK_CAPACITY, SmbError
 from .engine import SipMaskEngine
 
@@ -78,7 +80,8 @@ def _image_segms(region, eng, j, ori, planes):
 def _record(o):
     """The record of a slot's buffers (device or host), under the engine's record names."""
     rec = dict(det_bboxes=o['det'], det_labels=o['lab'], count=o['cnt'])
-    for name, key in (('idx', 'idxs_keep'), ('bits', 'mask_bits'), ('trk', 'track_feats'), ('msc', 'mask_scores')):
+    for name, key in (('idx', 'idxs_keep'), ('bits', 'mask_bits'), ('trk', 'track_feats'), ('msc', 'mask_scores'),
+                      ('render', 'render')):
         if name in o:
             rec[key] = o[name]
     return rec
@@ -486,14 +489,28 @@ class StreamRunner(object):
     neither copied nor downloaded.  result() returns 'segms' (the image's list of RLE dicts {'size': [ori_h, ori_w],
     'counts': bytes}) in place of mask_bits; an image whose strings overflowed the encoder's capacities is encoded on the
     host from the bucket engine's planes, which stay valid until the slot is reused.  consume() hands fn the device record
-    without mask_bits."""
+    without mask_bits.
 
-    bm_raw = False                                    # benchmark=True, raw=True: raw RGB images, PIL resize on the GPU
+    render=True: every image is also drawn with its detections on the device (render.render_images: the masks blended in
+    their labels' colours and the boxes of the detections with score > render_score_thr, as SipMask-mmdetection's
+    show_result draws them) and result() / consume() carry 'render', the uint8 [ori_h, ori_w, 3] picture in the image's
+    channel order.  The drawing reads the source image from the slot's input staging and writes the slot's render
+    buffer, right after the record copies: so the slot's input is released after it (once the slot's output is claimed)
+    instead of right after the forward.  Each slot holds a device and a pinned host render buffer of
+    batch * max_src_hw[0] * max_src_hw[1] * 3 bytes.  benchmark=True runners do not render."""
+
+    bm_raw = False
+    _render_rule = L.RENDER_IMAGES                   # render=True: the rule render.draw applies                                    # benchmark=True, raw=True: raw RGB images, PIL resize on the GPU
 
     def __init__(self, state_dict, in_flight=1, resize=(1333, 800), keep_ratio=True, max_src_hw=(2048, 2048),
                  max_ori_hw=None, min_mask_up=0.5, mean=(102.9801, 115.9465, 122.7717), device='cuda', batch=1,
-                 raw=False, masks='bits', **engine_kw):
+                 raw=False, masks='bits', render=False, render_score_thr=R.DEFAULT_SCORE_THR, **engine_kw):
         self.rle = _masks_mode(masks)
+        self.render = bool(render)
+        if self.render:
+            if engine_kw.get('benchmark', False):
+                raise ValueError('render=True: benchmark=True runners do not render')
+            self.render_thr = R.score_threshold(render_score_thr, 'render_score_thr')
         if self.rle:
             engine_kw.setdefault('rle_bytes', DEFAULT_RLE_BYTES)
             if int(engine_kw['rle_bytes']) <= 0:
@@ -544,6 +561,10 @@ class StreamRunner(object):
             self.in_dev = [torch.empty(self.B * self.src_elems, dtype=torch.uint8, device=self.dev) for _ in range(self.n)]
         self.out_dev, self.out_host = [], []
         self.rle_regions = [None] * self.n                # masks='rle': per slot, the pinned region of its batch's strings
+        if self.render:
+            table = (R.image_palette(self.kw.get('num_classes', 81)) if self._render_rule == L.RENDER_IMAGES
+                     else R.video_palette())
+            self.render_palette = R.device_palette(table, self.dev)
         self._init_queue()
         self.slots.mark_free()
 
@@ -650,11 +671,13 @@ class StreamRunner(object):
             spec['trk'] = ((mx, 512), torch.float32)
         if eng.rescoring:
             spec['msc'] = ((mx,), torch.float32)
+        if self.render:
+            spec['render'] = (None, torch.uint8)
         if k >= len(self.out_dev):
             self.out_dev += [None] * (k + 1 - len(self.out_dev))
             self.out_host += [None] * (k + 1 - len(self.out_host))
         if self.out_dev[k] is None:
-            cap = dict(bits=mx * self.max_ori_hw[0] * ((self.max_ori_hw[1] + 31) // 32))
+            cap = dict(bits=mx * self.max_ori_hw[0] * ((self.max_ori_hw[1] + 31) // 32), render=self.src_elems)
             self.out_dev[k] = {n: torch.empty(self.B * cap.get(n, int(np.prod(s or ()))), dtype=d, device=self.dev)
                                for n, (s, d) in spec.items()}
             self.out_host[k] = {n: torch.empty(v.numel(), dtype=v.dtype).pin_memory() for n, v in self.out_dev[k].items()}
@@ -664,6 +687,8 @@ class StreamRunner(object):
             shape = dict((n, s) for n, (s, d) in spec.items())
             if 'bits' in shape:
                 shape['bits'] = (mx, oh, (ow + 31) // 32)
+            if 'render' in shape:
+                shape['render'] = (oh, ow, 3)
             dev.append({})
             host.append({})
             for n, sh in shape.items():
@@ -744,7 +769,8 @@ class StreamRunner(object):
                 eng.forward(None)
             else:
                 eng.forward_raw([m['src'] for m in images] + [None] * (self.B - nr), self.mean, self._pipeline)
-            sl.input_free(k, cs)
+            if not self.render:
+                sl.input_free(k, cs)
             sl.claim_output(k, cs)
             dev, host, used = self._out(k, eng, [m['ori_shape'][:2] for m in images])
             flat = self.out_dev[k]
@@ -761,11 +787,24 @@ class StreamRunner(object):
                 if 'bits' in o:
                     oh, wq = o['bits'].shape[1:]
                     o['bits'].copy_(eng.mask_bits[j, :, :oh, :wq])
+            if self.render:
+                # the source images are still in the slot's input staging and the render buffer is claimed output: the
+                # input is released only once this has read it
+                self._render_batch(k, eng, images, dev)
+                sl.input_free(k, cs)
             sl.publish(k, cs)
             self._after_forward(k, eng, images)
-        self._download(k, used, images)
         for m, o, h in zip(images, dev, host):
             m['dev'], m['host'] = o, h
+        self._download(k, used, images)
+
+    def _render_batch(self, k, eng, images, dev):
+        """render=True, on slot k's stream after the record copies: draw each real image of the batch from its staged
+        source into its render buffer, from the bucket engine's record."""
+        nr = len(images)
+        R.draw([(m['src'], o['render'], m['ori_shape'][0], m['ori_shape'][1]) for m, o in zip(images, dev)],
+               eng.det[:nr], eng.count[:nr], eng.mask_bits[:nr], L.RENDER_IMAGES, self.render_palette, self.render_thr,
+               labels=eng.labels[:nr])
 
     def _after_forward(self, k, eng, images):
         """Work on slot k's stream right after the batch's forward and record copies, while the bucket engine still holds
@@ -859,7 +898,15 @@ class VideoRunner(StreamRunner):
     video_json(video_id) -> the video's results2json_videoseg entries (ytvis.video_json), once the video has ended and
     its frames are dispatched.  The runner keeps every frame's pair until then (before a slot takes a new batch, the
     frames it holds are read into their videos) and forgets the video afterwards, so its video_id may be served again.
-    For a video whose lane overflowed max_objects, video_json forgets the video and raises SmbError."""
+    For a video whose lane overflowed max_objects, video_json forgets the video and raises SmbError.
+
+    render=True (render_score_thr as StreamRunner's): result() also carries 'render', the frame drawn as SipMask-VIS's
+    show_result(is_video=True) draws it (render.render_frames), coloured by the object ids of the association.  The
+    source frames are copied into the slot's render buffer before the slot's input is released, and the bucket engine's
+    planes into a device buffer of the slot (also with masks='rle'; it is not downloaded); the drawing runs on the tracker
+    stream after the association, from the slot's buffers only, before the download that waits for the association."""
+
+    _render_rule = L.RENDER_VIDEO
 
     def __init__(self, state_dict, lanes=8, batch=1, in_flight=6, resize=(640, 360), keep_ratio=True,
                  max_src_hw=(1920, 1920), max_ori_hw=None, masks='rle', max_objects=4096, match_coeff=(1.0, 2.0, 10.0),
@@ -879,6 +926,7 @@ class VideoRunner(StreamRunner):
         self.s_trk.wait_stream(torch.cuda.current_stream(self.dev))        # the lanes' initial state
         self.ev_assoc = [torch.cuda.Event() for _ in range(self.n)]
         self.ids_dev, self.ids_host = [None] * self.n, [None] * self.n
+        self.planes_dev = [None] * self.n           # render=True: per slot, its batch's bit planes for the drawing
         self.status_dev = [torch.zeros(self.tracker.lanes, dtype=torch.int32, device=self.dev) for _ in range(self.n)]
         self.status_host = [torch.zeros(self.tracker.lanes, dtype=torch.int32).pin_memory() for _ in range(self.n)]
         self.rows = {}                      # ticket -> (lane, is_first, video_id, frame_id)
@@ -927,6 +975,16 @@ class VideoRunner(StreamRunner):
         super(VideoRunner, self)._launch(k, pad, images)
         self._unread.update(m['ticket'] for m in images)
 
+    def _render_batch(self, k, eng, images, dev):
+        # the slot's next forward rewrites the bucket engine's planes without waiting for the tracker stream: the drawing
+        # after the association reads the slot's own copies of the sources and planes
+        if self.planes_dev[k] is None:
+            self.planes_dev[k] = torch.empty_like(eng.mask_bits)
+        nr = len(images)
+        self.planes_dev[k][:nr].copy_(eng.mask_bits[:nr])
+        for m, o in zip(images, dev):
+            o['render'].copy_(m['src'])
+
     def _download(self, k, used, images):
         nr = len(images)
         mx = used['lab'] // nr
@@ -942,6 +1000,10 @@ class VideoRunner(StreamRunner):
             self.status_dev[k].copy_(trk.status)            # this launch's status bits, then clear them for the next
             trk.status.zero_()
             self._after_associate(k, images)
+            if self.render:
+                R.draw([(m['dev']['render'], m['dev']['render']) + tuple(m['ori_shape'][:2]) for m in images],
+                       flat['det'][:nr * mx * 5].view(nr, mx, 5), flat['cnt'][:nr], self.planes_dev[k][:nr],
+                       L.RENDER_VIDEO, self.render_palette, self.render_thr, obj_ids=self.ids_dev[k][:nr])
             self.ev_assoc[k].record(st)
         # the tracking features stay on the device
         copies = [(self.out_host[k][name][:n], flat[name][:n]) for name, n in used.items() if name != 'trk']
