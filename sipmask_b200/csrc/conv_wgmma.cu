@@ -57,6 +57,24 @@ static_assert(ring_stages(256) == 4 && ring_stages(128) == 6 && ring_stages(64) 
               "the epilogue slots must not cost any N tile an operand stage");
 static_assert(4 * kEpiSlots * 8 <= 256, "epilogue barriers exceed their reserve");
 
+#ifdef SMB_CONV_PHASES
+// Timing build only (tools/conv_tile_phases.py compiles it; the library never does).  clock64 stamps per CTA:
+//   [0, 4): globaltimer / clock64 at the first and last stamp (cycles -> ns);
+//   [4, 8): warp 9: cycles blocked in bulk_wait_read, cycles blocked on epi_ready, stores committed, fills;  [8]: tiles;
+//   [16 + (sample * 2 + wg) * 4, + 4): the sample-th recorded tile of consumer warpgroup wg (every phase_every-th tile of the
+//   CTA): mainloop start, last wgmma_wait<0> returned, epilogue end, cycles blocked in epi_full waits.
+constexpr int kPhaseSamples = 64;
+constexpr int kPhaseWords = 16 + kPhaseSamples * 2 * 4;
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define PHASE(...) __VA_ARGS__
+#else
+#define PHASE(...)
+#endif
+
 // One pyramid level (or the only tensor) of a launch.  Convolutions whose weights are shared by several feature-pyramid
 // levels (the FCOS towers and heads, sipmask_head.py:250-257) run as ONE launch over the union of the levels' tiles.
 struct LevelDesc {
@@ -89,6 +107,7 @@ struct ConvParams {
   int gn_group;                   // channels per GroupNorm group (8 or 16), 0 = no statistics
   int relu;
   int epi_tma;                    // epilogue through shared memory and TMA (fp16 output, res_mode 0 / 1)
+  PHASE(unsigned long long* phases; int phase_every;)
 };
 static_assert(sizeof(ConvParams) <= 4096, "ConvParams must fit the 4 KB kernel-parameter space");
 
@@ -415,7 +434,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
 template <int N>
 __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp,
                                              int lane, GnPart& gn_part, uint32_t slots, uint64_t* epi_full,
-                                             uint64_t* epi_ready, int& es, uint32_t& eph) {
+                                             uint64_t* epi_ready, int& es, uint32_t& eph PHASE(, long long& blocked)) {
   const LevelDesc& L = p.lv[tc.lvl];
   const int bw_shift = 31 - __clz(L.BW);
   bool valid[2];
@@ -432,11 +451,29 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
   const uint32_t q1 = (uint32_t)((2 + (lane >> 4)) ^ ((mrow >> 1) & 3)) << 4;
   const int cq = 2 * (lane & 3);
   const int nchunks = (min(N, p.Cout - tc.n0) + 31) >> 5;
+  // bias of 8-channel block jj of chunk cc (zero past Cout).  The slot wait's memory clobber keeps every load after it, so
+  // a chunk's bias is loaded one chunk ahead, before that wait: one global round trip per tile instead of one per chunk.
+  auto chunk_bias = [&](int cc, float2* b) {
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int ch0 = tc.n0 + 8 * (4 * cc + jj);
+      b[jj] = make_float2(0.f, 0.f);
+      if (p.bias && ch0 < p.Cout) b[jj] = make_float2(__ldg(p.bias + ch0 + cq), __ldg(p.bias + ch0 + cq + 1));
+    }
+  };
+  float2 bnext[4];
+  chunk_bias(0, bnext);
   float gsum = 0.f, gsq = 0.f;
 #pragma unroll
   for (int c = 0; c < N / 32; ++c) {
     if (c >= nchunks) break;
+    float2 bias[4];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) bias[jj] = bnext[jj];
+    if (c + 1 < nchunks) chunk_bias(c + 1, bnext);
+    PHASE(const long long w0 = clock64();)
     mbar_wait(&epi_full[wg * kEpiSlots + es], eph);
+    PHASE(blocked += clock64() - w0;)
     const uint32_t sa = row_addr + (uint32_t)es * kEpiSlotBytes;
     uint32_t rh[8], oh[8];                           // residual / output: block jj, row half i in register 2 jj + i
     if (p.res_mode) { ldmatrix_x4(sa + q0, rh); ldmatrix_x4(sa + q1, rh + 4); }
@@ -444,9 +481,7 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
     for (int jj = 0; jj < 4; ++jj) {
       const int j = 4 * c + jj;
       const int ch0 = tc.n0 + 8 * j;                 // warp-uniform; blocks past Cout are clipped by the TMA store
-      const int ch = ch0 + cq;
-      float2 bb = make_float2(0.f, 0.f);
-      if (p.bias && ch0 < p.Cout) bb = make_float2(__ldg(p.bias + ch), __ldg(p.bias + ch + 1));
+      const float2 bb = bias[jj];
       float s = 0.f, q = 0.f;
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -560,6 +595,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       if (p.res_mode) tma_prefetch_desc(&p.rmap);
       int s = 0, c = 0, nchunks = 0, filled = 0;
       uint32_t ph = 0;
+      PHASE(long long read_wait = 0, ready_wait = 0, stores = 0;)
       int unit = blockIdx.x;
       TileCoord tc = {};
       for (int step = 0;; ++step) {
@@ -572,17 +608,22 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           for (int wg = 0; wg < 2; ++wg) {
             int x, y;
             epi_box_origin(L, q.y, q.z, wg, x, y);
+            PHASE(const long long w0 = clock64();)
             mbar_wait(&epi_ready[wg * kEpiSlots + s], ph ^ 1);
+            PHASE(ready_wait += clock64() - w0;)
             tma_store_4d(&p.omap[q.w & 7], epi_slots + (wg * kEpiSlots + s) * kEpiSlotBytes, q.x, x, y, q.w >> 3);
           }
           bulk_commit();
+          PHASE(++stores;)
         }
         if (fill) {
           if (c == 0) {
             tc = decode_tile(p, unit);
             nchunks = (min(N, p.Cout - tc.n0) + 31) >> 5;
           }
+          PHASE(const long long w0 = clock64();)
           bulk_wait_read_all();                        // the store above has read the slot
+          PHASE(read_wait += clock64() - w0;)
 #pragma unroll
           for (int wg = 0; wg < 2; ++wg) {
             uint64_t* bar = &epi_full[wg * kEpiSlots + s];
@@ -602,6 +643,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (++s == kEpiSlots) { s = 0; ph ^= 1; }
       }
       bulk_wait_read_all();                          // the slots stay allocated until the last store has read them
+      PHASE(if (p.phases) {
+              unsigned long long* r = p.phases + (size_t)blockIdx.x * kPhaseWords;
+              r[4] = read_wait; r[5] = ready_wait; r[6] = stores; r[7] = filled;
+            })
     }
   } else {
     // ===================== consumers: warpgroup wg computes pixels 64*wg .. 64*wg+63 of the tile =====================
@@ -613,8 +658,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
     int s = 0, es = 0;
     uint32_t ph = 0, eph = 0;
+    PHASE(unsigned long long* const rec = p.phases + (size_t)blockIdx.x * kPhaseWords;
+          const bool stamp = p.phases && (threadIdx.x & 127) == 0;
+          if (threadIdx.x == 0 && p.phases) { rec[0] = globaltimer(); rec[1] = clock64(); }
+          int tile_i = 0;)
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
       const TileCoord tc = decode_tile(p, unit);
+      PHASE(const int sample = tile_i % p.phase_every == 0 ? tile_i / p.phase_every : kPhaseSamples;
+            const long long t_main = clock64(); long long blocked = 0; ++tile_i;)
       int prev = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(&full_bar[s], ph);
@@ -632,14 +683,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (++s == nstages) { s = 0; ph ^= 1; }
       }
       wgmma_wait<0>();
+      PHASE(const long long t_mma = clock64();)
       fence_regs<N / 2>(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
       if (p.epi_tma)
-        epilogue_tma<N>(p, tc, acc, wg, warp, lane, gn_part, smem_u32(epi_slots), epi_full, epi_ready, es, eph);
+        epilogue_tma<N>(p, tc, acc, wg, warp, lane, gn_part, smem_u32(epi_slots), epi_full, epi_ready, es,
+                        eph PHASE(, blocked));
       else
         epilogue<N>(p, tc, acc, wg, warp, lane, gn_part);
       if (p.gn_group) gn_flush(p, tc, gn_part, N);
+      PHASE(if (stamp && sample < kPhaseSamples) {
+              unsigned long long* r = rec + 16 + (sample * 2 + wg) * 4;
+              r[0] = t_main; r[1] = t_mma; r[2] = clock64(); r[3] = blocked;
+            })
     }
+    PHASE(if (threadIdx.x == 0 && p.phases) { rec[2] = globaltimer(); rec[3] = clock64(); rec[8] = tile_i; })
   }
 }
 
@@ -919,11 +977,24 @@ extern "C" int smb_conv_plan_set_max_ctas(smb_conv_plan_t* plan, int max_ctas) {
   return SMB_OK;
 }
 
+#ifdef SMB_CONV_PHASES
+// Timing build only: launches after this call stamp into buf (kPhaseWords 64-bit words per CTA, zeroed by the caller),
+// every every-th tile of each CTA; buf = null stops stamping.
+static unsigned long long* g_phases = nullptr;
+static int g_phase_every = 1;
+extern "C" int smb_conv_phase_buffer(void* buf, int every) {
+  g_phases = (unsigned long long*)buf;
+  g_phase_every = every > 0 ? every : 1;
+  return kPhaseWords;
+}
+#endif
+
 extern "C" int smb_conv_run(const smb_conv_plan_t* plan, const float* bias, const void* residual, void* gn_stats,
                             float alpha, smb_stream_t stream) {
   SMB_CHECK_ARG(plan, "smb_conv_run: null plan");
   SMB_CHECK_ARG(!plan->has_bias || bias, "smb_conv_run: plan expects a bias");
   ConvParams p = plan->p;
+  PHASE(p.phases = g_phases; p.phase_every = g_phase_every;)
   p.bias = plan->has_bias ? bias : nullptr;
   // single-level plans take residual / statistics pointers at run time; multi-level plans bake them per level
   if (p.num_levels == 1) {
