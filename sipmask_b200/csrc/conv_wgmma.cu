@@ -33,12 +33,14 @@ constexpr int kMaxMaps = 8;
 constexpr int kMaxLevels = 5;
 constexpr int kConsumerWarps = 8;
 // + a producer warpgroup: warp 8 issues the operand TMA loads, warp 9 the epilogue's residual loads and output stores
-// (epi_tma plans), warps 10-11 exist only so that the CTA is whole warpgroups, which setmaxnreg needs to move registers
-// from the producer (40 per thread) to the consumers (232 instead of 168)
+// (epi_tma plans), warp 10 the GroupNorm statistics' global atomics (GN plans), warp 11 exists only so that the CTA is
+// whole warpgroups, which setmaxnreg needs to move registers from the producer (40 per thread) to the consumers (232
+// instead of 168)
 constexpr int kThreads = 32 * (kConsumerWarps + 4);
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int kProducerWarp = kConsumerWarps;
 constexpr int kEpiWarp = kConsumerWarps + 1;
+constexpr int kGnWarp = kConsumerWarps + 2;
 constexpr int kABytes = 128 * 64 * 2;                // one A stage: 128 pixels x 64 channels fp16
 constexpr size_t kSmemBudget = 220 * 1024;           // epilogue slots + operand stages + barriers (227 KB per block on sm_90)
 // Epilogue slots (epi_tma plans): per consumer warpgroup a ring of kEpiSlots chunks of 64 pixels x 32 channels fp16, one
@@ -61,10 +63,13 @@ static_assert(4 * kEpiSlots * 8 <= 256, "epilogue barriers exceed their reserve"
 // Timing build only (tools/conv_tile_phases.py compiles it; the library never does).  clock64 stamps per CTA:
 //   [0, 4): globaltimer / clock64 at the first and last stamp (cycles -> ns);
 //   [4, 8): warp 9: cycles blocked in bulk_wait_read, cycles blocked on epi_ready, stores committed, fills;  [8]: tiles;
-//   [16 + (sample * 2 + wg) * 4, + 4): the sample-th recorded tile of consumer warpgroup wg (every phase_every-th tile of the
-//   CTA): mainloop start, last wgmma_wait<0> returned, epilogue end, cycles blocked in epi_full waits.
+//   [16 + (sample * 2 + wg) * kPhaseTile, + kPhaseTile): the sample-th recorded tile of consumer warpgroup wg (every
+//   phase_every-th tile of the CTA): mainloop start, last wgmma_wait<0> returned, epilogue end, cycles blocked in epi_full
+//   waits, cycles in the GroupNorm statistics' shuffle reductions, cycles handing the tile's statistics to warp 10 (the
+//   wait for the previous tile's flush and the arrival).
 constexpr int kPhaseSamples = 64;
-constexpr int kPhaseWords = 16 + kPhaseSamples * 2 * 4;
+constexpr int kPhaseTile = 6;
+constexpr int kPhaseWords = 16 + kPhaseSamples * 2 * kPhaseTile;
 __device__ __forceinline__ unsigned long long globaltimer() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -312,31 +317,70 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int unit) 
   return t;
 }
 
-// Epilogue of one consumer warp: rows (warp%4)*16 + lane/4 + {0, 8} of its warpgroup's 64-pixel half of the tile.
-// Per element: acc + bias, * alpha, + residual -> GroupNorm statistics (pre-activation) -> ReLU -> fp16 / fp32 store.
-// GroupNorm partials of one tile: [consumer warp][group within the N tile (<= 256 / 8)][sum, sum of squares], fixed point
+// GroupNorm partials of one tile: [consumer warp][group within the N tile (<= 256 / 8)][sum, sum of squares], fixed point.
+// Warp 10 sums the eight warps' partials of a tile and issues one global atomic per (group, statistic): per-warp atomics
+// on the same few addresses serialised in L2 when every SM ran a tower convolution.  Integer sums are exact, so the
+// statistics are the same bits in any order.
 typedef unsigned long long GnPart[kConsumerWarps][32][2];
 
-// After every consumer warp has written its partials of the tile: one global atomic per (group, statistic) of the tile
-// instead of one per warp.  When all SMs run tower convolutions, per-warp atomics on the same few addresses serialised
-// in L2 and stretched every tile.  Integer sums are exact, so the statistics are the same bits.
-__device__ __forceinline__ void gn_flush(const ConvParams& p, const TileCoord& tc, GnPart& gn_part, int N) {
-  asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory");       // partials of all consumer warps written
-  const int t = threadIdx.x, ngl = min(N, p.Cout - tc.n0) / p.gn_group;
-  if (t < 2 * ngl) {
-    unsigned long long v = 0;
+// GroupNorm statistics of one 32-channel chunk of a consumer warp (pre-activation values of its 16 rows): v[2 g + s] is
+// the lane's fp32 partial of group g of the chunk, statistic s (sum, sum of squares); NV = 8 for 8-channel groups (four
+// per chunk), 4 for 16-channel groups (two; each already the sum of its two 8-channel blocks, in block order).  Writes
+// the warp's sums to part[g][s] in 64-bit fixed point.
+// A reduce-scatter: xor 16 exchanges NV / 2 values (a lane keeps the upper half when its bit 4 is set and sends the other
+// half), xor 8 exchanges NV / 4, ..., and once one value is left the remaining offsets are butterfly steps; lane l ends
+// with the warp's sum of value (l >> 2) & 7 (NV = 8) or (l >> 3) & 3 (NV = 4), and lanes with those bits alone convert
+// it.  9 (NV = 8) or 5 (NV = 4) shuffles per chunk instead of 5 per value.  The sums are the same bits as a full
+// butterfly per value: every value still goes through the pairing tree with offsets 16, 8, 4, 2, 1, step o adding the
+// lane's running sum and that of lane ^ o, and fp32 addition is commutative, so each running sum is the same bits in
+// every lane that holds it; so is every fixed-point partial.
+template <int NV>
+__device__ __forceinline__ void gn_reduce_chunk(float* v, int lane, unsigned long long (*part)[2]) {
+  int n = NV;
 #pragma unroll
-    for (int w = 0; w < kConsumerWarps; ++w) v += gn_part[w][t >> 1][t & 1];
-    const int ngroups = p.Cout / p.gn_group;
-    atomicAdd(reinterpret_cast<unsigned long long*>(p.lv[tc.lvl].gn_stats) +
-                  ((size_t)tc.img * ngroups + tc.n0 / p.gn_group + (t >> 1)) * 2 + (t & 1), v);
+  for (int o = 16; o > 0; o >>= 1) {
+    if (n > 1) {
+      n >>= 1;
+      const bool hi = lane & o;
+#pragma unroll
+      for (int i = 0; i < n; ++i) {
+        const float send = hi ? v[i] : v[i + n];
+        v[i] = (hi ? v[i + n] : v[i]) + __shfl_xor_sync(0xffffffffu, send, o);
+      }
+    } else {
+      v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
+    }
   }
-  asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory");       // read before the next tile overwrites
+  constexpr int kShift = NV == 8 ? 2 : 3;
+  const int idx = (lane >> kShift) & (NV - 1);
+  if ((lane & ((1 << kShift) - 1)) == 0)
+    part[idx >> 1][idx & 1] = (unsigned long long)__float2ll_rn(v[0] * ((idx & 1) ? kGnSqScale : kGnSumScale));
 }
 
+// Collects one 8-channel block's statistics (s, q: the lane's sum and sum of squares over its valid rows) into the
+// chunk's v[] of gn_reduce_chunk; after the chunk's last block (jj = 3) reduces them into the warp's partials of chunk c.
+__device__ __forceinline__ void gn_block(const ConvParams& p, float* v, int jj, float s, float q, int lane,
+                                         unsigned long long (*part)[2], int c PHASE(, unsigned& shfl)) {
+  if (p.gn_group == 8) {
+    v[2 * jj] = s; v[2 * jj + 1] = q;
+  } else {                                           // 16-channel groups: blocks 2g and 2g + 1 summed in that order
+    const int g = jj >> 1;
+    v[2 * g] = (jj & 1) ? v[2 * g] + s : s;
+    v[2 * g + 1] = (jj & 1) ? v[2 * g + 1] + q : q;
+  }
+  if (jj == 3) {
+    PHASE(const unsigned w0 = clock();)
+    if (p.gn_group == 8) gn_reduce_chunk<8>(v, lane, part + 4 * c);
+    else gn_reduce_chunk<4>(v, lane, part + 2 * c);
+    PHASE(shfl += clock() - w0;)
+  }
+}
+
+// Epilogue of one consumer warp: rows (warp%4)*16 + lane/4 + {0, 8} of its warpgroup's 64-pixel half of the tile.
+// Per element: acc + bias, * alpha, + residual -> GroupNorm statistics (pre-activation) -> ReLU -> fp16 / fp32 store.
 template <int N>
 __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp, int lane,
-                                         GnPart& gn_part) {
+                                         GnPart& gn_part PHASE(, unsigned& shfl)) {
   const LevelDesc& L = p.lv[tc.lvl];
   const int bw_shift = 31 - __clz(L.BW);            // BW is a power of two (choose_patch)
   bool valid[2];
@@ -361,7 +405,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
     }
   }
   const int cq = 2 * (lane & 3);
-  float gsum = 0.f, gsq = 0.f;                       // GroupNorm partials of the current 16-channel group (gn_group 16)
+  float gv[8];                                       // GroupNorm partials of the current 32-channel chunk (gn_block)
   // The output may alias the residual as far as the compiler knows, so a residual load written after a store cannot be
   // issued before it: one 8-channel block at a time, every residual load would wait a full memory round trip.  The
   // bias and residual operands of kEpiChunk blocks are therefore loaded together, then combined and stored (at N = 256
@@ -404,24 +448,10 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
           }
         }
       }
-      if (p.gn_group) {
-        // per-(image, group) sum / sum of squares of the conv output (pre-activation): fp32 over the warp's 16 rows, then
-        // 64-bit fixed point, summed over the tile by gn_flush (integer sums: bit-reproducible whatever the tile order).
-        gsum += s; gsq += q;
-        if (p.gn_group == 8 || (j & 1)) {
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
-            gsq += __shfl_xor_sync(0xffffffffu, gsq, o);
-          }
-          if (lane == 0) {
-            unsigned long long* part = gn_part[warp][(ch0 - tc.n0) / p.gn_group];
-            part[0] = (unsigned long long)__float2ll_rn(gsum * kGnSumScale);
-            part[1] = (unsigned long long)__float2ll_rn(gsq * kGnSqScale);
-          }
-          gsum = 0.f; gsq = 0.f;
-        }
-      }
+      // per-(image, group) sum / sum of squares of the conv output (pre-activation): fp32 over the warp's 16 rows, then
+      // 64-bit fixed point, summed over the tile by warp 10 (integer sums: bit-reproducible whatever the tile order).
+      // GroupNorm plans have Cout 256 or 512, so every 32-channel chunk is whole.
+      if (p.gn_group) gn_block(p, gv, j & 3, s, q, lane, gn_part[warp], j >> 2 PHASE(, shfl));
     }
   }
 }
@@ -434,7 +464,8 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
 template <int N>
 __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp,
                                              int lane, GnPart& gn_part, uint32_t slots, uint64_t* epi_full,
-                                             uint64_t* epi_ready, int& es, uint32_t& eph PHASE(, long long& blocked)) {
+                                             uint64_t* epi_ready, int& es, uint32_t& eph
+                                             PHASE(, long long& blocked, unsigned& shfl)) {
   const LevelDesc& L = p.lv[tc.lvl];
   const int bw_shift = 31 - __clz(L.BW);
   bool valid[2];
@@ -463,7 +494,7 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
   };
   float2 bnext[4];
   chunk_bias(0, bnext);
-  float gsum = 0.f, gsq = 0.f;
+  float gv[8];                                       // GroupNorm partials of the chunk (gn_block)
 #pragma unroll
   for (int c = 0; c < N / 32; ++c) {
     if (c >= nchunks) break;
@@ -480,8 +511,7 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       const int j = 4 * c + jj;
-      const int ch0 = tc.n0 + 8 * j;                 // warp-uniform; blocks past Cout are clipped by the TMA store
-      const float2 bb = bias[jj];
+      const float2 bb = bias[jj];                      // blocks past Cout are clipped by the TMA store
       float s = 0.f, q = 0.f;
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -496,22 +526,7 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
         const __half2 h = __floats2half2_rn(f0, f1);
         oh[2 * jj + i] = *reinterpret_cast<const uint32_t*>(&h);
       }
-      if (p.gn_group && ch0 < p.Cout) {
-        gsum += s; gsq += q;
-        if (p.gn_group == 8 || (j & 1)) {
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
-            gsq += __shfl_xor_sync(0xffffffffu, gsq, o);
-          }
-          if (lane == 0) {
-            unsigned long long* part = gn_part[warp][(ch0 - tc.n0) / p.gn_group];
-            part[0] = (unsigned long long)__float2ll_rn(gsum * kGnSumScale);
-            part[1] = (unsigned long long)__float2ll_rn(gsq * kGnSqScale);
-          }
-          gsum = 0.f; gsq = 0.f;
-        }
-      }
+      if (p.gn_group) gn_block(p, gv, jj, s, q, lane, gn_part[warp], c PHASE(, shfl));   // whole chunks (Cout 256 / 512)
     }
     stmatrix_x4(sa + q0, oh);
     stmatrix_x4(sa + q1, oh + 4);
@@ -531,6 +546,9 @@ template <int N>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __shared__ GnPart gn_part;                         // 4 KB beside the <= 220 KB of operand stages
+  // GroupNorm plans: gn_bar[0] = a tile's partials written (every consumer thread), gn_bar[1] = summed by warp 10 (its 32
+  // lanes), so the consumers may overwrite them with the next tile's
+  __shared__ uint64_t gn_bar[2];
   // the 128-byte swizzle atoms (8 rows x 128 B) must start on 1024-byte boundaries
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -548,6 +566,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   if (threadIdx.x == 0) {
     for (int i = 0; i < nstages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerWarps); }
     for (int i = 0; i < 2 * kEpiSlots; ++i) { mbar_init(&epi_full[i], 1); mbar_init(&epi_ready[i], 128); }
+    mbar_init(&gn_bar[0], 32 * kConsumerWarps);
+    mbar_init(&gn_bar[1], 32);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -647,6 +667,28 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
               unsigned long long* r = p.phases + (size_t)blockIdx.x * kPhaseWords;
               r[4] = read_wait; r[5] = ready_wait; r[6] = stores; r[7] = filled;
             })
+    } else if (warp == kGnWarp && p.gn_group) {
+      // ===================== GroupNorm statistics (whole warp): the consumers' tile sequence =====================
+      // Once every consumer thread has written its partials of a tile: sum the eight warps' partials, one global atomic per
+      // (group, statistic), then release the partials.  The consumers hand a tile over with an mbarrier arrival and go on
+      // to their next mainloop: no CTA barrier on their path, and the next tile's partials are written an entire
+      // mainloop later, long after this warp has read these.
+      uint32_t ph = 0;
+      for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
+        const TileCoord tc = decode_tile(p, unit);
+        const int ngl = min(N, p.Cout - tc.n0) / p.gn_group, ngroups = p.Cout / p.gn_group;
+        unsigned long long* st = reinterpret_cast<unsigned long long*>(p.lv[tc.lvl].gn_stats) +
+                                 ((size_t)tc.img * ngroups + tc.n0 / p.gn_group) * 2;
+        mbar_wait(&gn_bar[0], ph);
+        for (int e = lane; e < 2 * ngl; e += 32) {
+          unsigned long long v = 0;
+#pragma unroll
+          for (int w = 0; w < kConsumerWarps; ++w) v += gn_part[w][e >> 1][e & 1];
+          atomicAdd(st + e, v);
+        }
+        mbar_arrive(&gn_bar[1]);
+        ph ^= 1;
+      }
     }
   } else {
     // ===================== consumers: warpgroup wg computes pixels 64*wg .. 64*wg+63 of the tile =====================
@@ -657,7 +699,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
     int s = 0, es = 0;
-    uint32_t ph = 0, eph = 0;
+    uint32_t ph = 0, eph = 0, gph = 0;
     PHASE(unsigned long long* const rec = p.phases + (size_t)blockIdx.x * kPhaseWords;
           const bool stamp = p.phases && (threadIdx.x & 127) == 0;
           if (threadIdx.x == 0 && p.phases) { rec[0] = globaltimer(); rec[1] = clock64(); }
@@ -665,7 +707,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
       const TileCoord tc = decode_tile(p, unit);
       PHASE(const int sample = tile_i % p.phase_every == 0 ? tile_i / p.phase_every : kPhaseSamples;
-            const long long t_main = clock64(); long long blocked = 0; ++tile_i;)
+            const long long t_main = clock64(); long long blocked = 0; unsigned shfl = 0, hand = 0; ++tile_i;)
       int prev = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(&full_bar[s], ph);
@@ -686,15 +728,20 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       PHASE(const long long t_mma = clock64();)
       fence_regs<N / 2>(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      PHASE(unsigned t_hand = clock();)
+      if (p.gn_group) mbar_wait(&gn_bar[1], gph ^ 1);    // warp 10 has summed the previous tile's partials
+      PHASE(hand = clock() - t_hand;)
       if (p.epi_tma)
         epilogue_tma<N>(p, tc, acc, wg, warp, lane, gn_part, smem_u32(epi_slots), epi_full, epi_ready, es,
-                        eph PHASE(, blocked));
+                        eph PHASE(, blocked, shfl));
       else
-        epilogue<N>(p, tc, acc, wg, warp, lane, gn_part);
-      if (p.gn_group) gn_flush(p, tc, gn_part, N);
-      PHASE(if (stamp && sample < kPhaseSamples) {
-              unsigned long long* r = rec + 16 + (sample * 2 + wg) * 4;
-              r[0] = t_main; r[1] = t_mma; r[2] = clock64(); r[3] = blocked;
+        epilogue<N>(p, tc, acc, wg, warp, lane, gn_part PHASE(, shfl));
+      PHASE(t_hand = clock();)
+      if (p.gn_group) { mbar_arrive(&gn_bar[0]); gph ^= 1; }
+      PHASE(hand += clock() - t_hand;
+            if (stamp && sample < kPhaseSamples) {
+              unsigned long long* r = rec + 16 + (sample * 2 + wg) * kPhaseTile;
+              r[0] = t_main; r[1] = t_mma; r[2] = clock64(); r[3] = blocked; r[4] = shfl; r[5] = hand;
             })
     }
     PHASE(if (threadIdx.x == 0 && p.phases) { rec[2] = globaltimer(); rec[3] = clock64(); rec[8] = tile_i; })
