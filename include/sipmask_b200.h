@@ -479,7 +479,8 @@ int smb_coco_accumulate_dev(const smb_coco_out_t* rows, int64_t n_rows, const in
  * COCOeval.evaluate() sorts them).
  * Limits: 1 <= T, 1 <= A, T * A <= SMB_COCO_MAX_TA (the matched / ignored bits of a row are one uint64 each);
  * 1 <= M <= SMB_COCO_MAX_M with every maxDet in [1, SMB_COCO_MAX_DET], in ascending order; 1 <= R <= SMB_COCO_R; no NaN.  A launch with
- * Params outside them returns SMB_EINVAL.  The default Params make these entry points compute what the two above do. */
+ * Params outside them returns SMB_EINVAL.  The default Params make these entry points compute what the two above do.
+ * useCats = 0 and maxDets above SMB_COCO_MAX_DET go through smb_coco_params2_t below. */
 #define SMB_COCO_MAX_TA 64
 #define SMB_COCO_MAX_M 3
 typedef struct {
@@ -505,6 +506,39 @@ int smb_coco_match_params_dev(const smb_coco_img_t* imgs, int n_img, const smb_c
 int smb_coco_accumulate_params_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
                                    const int* npig, const smb_coco_params_t* host_params, double* precision,
                                    double* recall, double* scores, smb_stream_t stream);
+
+/* COCOeval Params with p.useCats and maxDets up to SMB_COCO_MAX_DET2 (the *_params2_* entry points).  The fields are
+ * smb_coco_params_t's, with use_cats in place of its padding:
+ *   use_cats 1: one group per (image, category), as the entry points above;
+ *   use_cats 0: one pooled group per image (computeIoU / evaluateImg over the concatenation of the image's rows of every
+ *               category), rows written with category index 0 and npig [1, A], so accumulate runs with K = 1.
+ * The K categories of a launch are p.catIds: the host packs an image's ground truth category-major (category index,
+ * then annotation order) and gives a detection the index of its category (-1: not evaluated).  In a pooled group,
+ * detections rank by score descending, then category index, then json order, which is np.argsort(-score,
+ * kind='mergesort') over pycocotools' concatenation; ground truths keep the packed order.
+ * Limits: those of smb_coco_params_t, except every maxDet in [1, SMB_COCO_MAX_DET2]; use_cats 0 or 1.  The shared memory
+ * of a match launch grows with det_cap and maxDets[M-1] (about 122 KB at 4096 rows and 1000). */
+#define SMB_COCO_MAX_DET2 1000
+typedef struct {
+  int32_t T, A, M, R;
+  int32_t max_dets[SMB_COCO_MAX_M];
+  int32_t use_cats;
+  double iou_thr[SMB_COCO_MAX_TA];
+  double area_rng[SMB_COCO_MAX_TA][2];
+  double rec_thr[SMB_COCO_R];
+} smb_coco_params2_t;
+int smb_coco_params2_check(const smb_coco_params2_t* host_params);
+/* workspace >= smb_coco_match_params2_workspace_bytes(n_gt, host_params): [n_gt, maxDets[M-1]] IoUs, [n_gt, T*A] bytes. */
+size_t smb_coco_match_params2_workspace_bytes(int n_gt, const smb_coco_params2_t* host_params);
+int smb_coco_match_params2_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                               const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts, int n_gt,
+                               const uint32_t* gt_planes, int64_t gt_plane_words, const int32_t* gt_cat_off, int K,
+                               int metric, const smb_coco_params2_t* host_params, smb_coco_out_t* out, int64_t n_out,
+                               int* npig, int* status, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+/* smb_coco_accumulate_params_dev with these Params (K = 1 for use_cats 0). */
+int smb_coco_accumulate_params2_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
+                                    const int* npig, const smb_coco_params2_t* host_params, double* precision,
+                                    double* recall, double* scores, smb_stream_t stream);
 
 /* coco_error_analysis.py's per-category evaluations with relabelled ground truth (iouThrs [.1], maxDets [100], the four
  * area ranges host_area_rng[4][2]), for every (image, category) with detections: category k's detections against the

@@ -89,7 +89,8 @@ SYMBOLS = [
     'smb_coco_plane_stats', 'smb_coco_det_from_record_dev', 'smb_coco_match_workspace_bytes', 'smb_coco_match_dev',
     'smb_coco_accumulate_dev', 'smb_coco_params_check', 'smb_coco_match_params_workspace_bytes',
     'smb_coco_match_params_dev', 'smb_coco_accumulate_params_dev', 'smb_coco_analysis_workspace_bytes',
-    'smb_coco_analysis_match_dev',
+    'smb_coco_analysis_match_dev', 'smb_coco_params2_check', 'smb_coco_match_params2_workspace_bytes',
+    'smb_coco_match_params2_dev', 'smb_coco_accumulate_params2_dev',
     'smb_ytvis_overlap_dev', 'smb_ytvis_scatter_dev', 'smb_ytvis_match_workspace_bytes', 'smb_ytvis_match_dev',
     'smb_segm_raster_workspace_bytes', 'smb_segm_raster_dev', 'smb_render_dev',
 ]
@@ -108,7 +109,8 @@ def lib():
                   'smb_mask_rescore_f16_workspace_bytes', 'smb_pair_decode_workspace_bytes', 'smb_ml_nms_workspace_bytes',
                   'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes', 'smb_coco_match_workspace_bytes',
                   'smb_ytvis_match_workspace_bytes', 'smb_segm_raster_workspace_bytes',
-                  'smb_coco_match_params_workspace_bytes', 'smb_coco_analysis_workspace_bytes'):
+                  'smb_coco_match_params_workspace_bytes', 'smb_coco_analysis_workspace_bytes',
+                  'smb_coco_match_params2_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

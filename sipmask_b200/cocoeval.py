@@ -1,6 +1,7 @@
 """COCO box and mask AP on the device: pycocotools 2.0 COCOeval (iouType 'bbox' / 'segm') as MM's CocoDataset.evaluate
 (SipMask-mmdetection/mmdet/datasets/coco.py:290-392) and SipMask-benchmark's coco_eval.py run it, with the default Params
-or user-given ones (CocoParams: IoU thresholds, recall thresholds, maxDets and area ranges as data).
+or user-given ones (CocoParams: IoU thresholds, recall thresholds, maxDets and area ranges as data; CocoParams2: also
+useCats, catIds and maxDets up to 1000), and MM's class-agnostic 'proposal' metric.
 
 Host: the ground truth (CocoGroundTruth: pycocotools COCO's indexing; annToRLE through the library's C restatement of
 rleFrPoly / rleFrString as the public host rasterizer, segm_plane) and summarize (numpy, the code of COCOeval.summarize).
@@ -11,6 +12,7 @@ accumulate's precision / recall / scores arrays at evaluate() (csrc/cocoeval.cu)
 Restated only: pycocotools is neither vendored in the reference nor installed where this was written, so the semantics
 are pycocotools 2.0's as read from its source, not pinned by running it.
 """
+import copy
 import ctypes
 
 import numpy as np
@@ -39,6 +41,9 @@ DET_CAP = 4096                       # SMB_COCO_DET_CAP: detections of one image
 MAX_CATS = 2048                      # SMB_COCO_MAX_CATS
 LABEL_RANGE, CAPACITY, ANALYSIS_RANGE = 1, 2, 4   # status bits
 MAX_TA, MAX_M, MAX_DET = 64, 3, 100  # SMB_COCO_MAX_TA, SMB_COCO_MAX_M, SMB_COCO_MAX_DET
+MAX_DET2 = 1000                      # SMB_COCO_MAX_DET2: maxDets through the Params2 entry points
+PROPOSAL_NUMS = (100, 300, 1000)     # CocoDataset.evaluate's default proposal_nums
+PROPOSAL_ITEMS = ['AR@100', 'AR@300', 'AR@1000', 'AR_s@1000', 'AR_m@1000', 'AR_l@1000']
 
 
 class _ParamsC(ctypes.Structure):
@@ -46,6 +51,14 @@ class _ParamsC(ctypes.Structure):
     _fields_ = [('T', ctypes.c_int32), ('A', ctypes.c_int32), ('M', ctypes.c_int32), ('R', ctypes.c_int32),
                 ('max_dets', ctypes.c_int32 * MAX_M), ('pad', ctypes.c_int32), ('iou_thr', ctypes.c_double * MAX_TA),
                 ('area_rng', ctypes.c_double * (2 * MAX_TA)), ('rec_thr', ctypes.c_double * 101)]
+
+
+class _Params2C(ctypes.Structure):
+    """smb_coco_params2_t (include/sipmask_b200.h): smb_coco_params_t with use_cats in place of its padding."""
+    _fields_ = [('T', ctypes.c_int32), ('A', ctypes.c_int32), ('M', ctypes.c_int32), ('R', ctypes.c_int32),
+                ('max_dets', ctypes.c_int32 * MAX_M), ('use_cats', ctypes.c_int32),
+                ('iou_thr', ctypes.c_double * MAX_TA), ('area_rng', ctypes.c_double * (2 * MAX_TA)),
+                ('rec_thr', ctypes.c_double * 101)]
 
 
 class CocoParams:
@@ -56,34 +69,43 @@ class CocoParams:
       1 <= T (IoU thresholds), 1 <= A (area ranges), T * A <= 64: a detection's matched / ignored bits are one uint64;
       1 <= M <= 3 maxDets, each an integer in [1, 100]; 1 <= R <= 101 recall thresholds; no NaN;
       one label per area range.
-    Not supported: useCats = 0 and catIds subsets (every category of the ground truth is evaluated)."""
+    Not supported here: useCats = 0, catIds subsets and maxDets above 100 (every category of the ground truth is
+    evaluated); CocoParams2 takes them."""
+    _MAX_DET = MAX_DET
 
     def __init__(self, iou_thrs=None, rec_thrs=None, max_dets=None, area_rng=None, area_rng_lbl=None, use_cats=1,
                  cat_ids=None):
         if use_cats != 1:
-            raise ValueError('CocoParams: useCats = 0 is not supported (categories are always used)')
+            raise ValueError('CocoParams: useCats = 0 is not supported (categories are always used; CocoParams2 '
+                             'takes it)')
         if cat_ids is not None:
-            raise ValueError('CocoParams: catIds subsets are not supported (every ground-truth category is evaluated)')
+            raise ValueError('CocoParams: catIds subsets are not supported (every ground-truth category is evaluated; '
+                             'CocoParams2 takes them)')
+        self.use_cats, self.cat_ids = 1, None
+        self._set(iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
+
+    def _set(self, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl):
+        name = type(self).__name__
         self.iou_thrs = self._floats(IOU_THRS if iou_thrs is None else iou_thrs, 'iou_thrs')
         self.rec_thrs = self._floats(REC_THRS if rec_thrs is None else rec_thrs, 'rec_thrs')
         self.area_rng = self._floats(AREA_RNG if area_rng is None else area_rng, 'area_rng', (-1, 2))
         self.area_rng_lbl = list(AREA_RNG_LBL if area_rng_lbl is None else area_rng_lbl)
         md = list(MAX_DETS if max_dets is None else max_dets)
         if not all(isinstance(m, (int, np.integer)) and not isinstance(m, bool) for m in md):
-            raise ValueError('CocoParams: maxDets must be integers, got %r' % (md,))
+            raise ValueError('%s: maxDets must be integers, got %r' % (name, md))
         self.max_dets = sorted(int(m) for m in md)
         T, A, M, R = len(self.iou_thrs), len(self.area_rng), len(self.max_dets), len(self.rec_thrs)
         if T < 1 or A < 1 or T * A > MAX_TA:
-            raise ValueError('CocoParams: %d IoU thresholds x %d area ranges; need 1 <= T, 1 <= A and T * A <= %d '
-                             '(the matched / ignored bits of a detection are one uint64)' % (T, A, MAX_TA))
+            raise ValueError('%s: %d IoU thresholds x %d area ranges; need 1 <= T, 1 <= A and T * A <= %d '
+                             '(the matched / ignored bits of a detection are one uint64)' % (name, T, A, MAX_TA))
         if not 1 <= M <= MAX_M:
-            raise ValueError('CocoParams: %d maxDets; 1 to %d are supported' % (M, MAX_M))
-        if any(not 1 <= m <= MAX_DET for m in self.max_dets):
-            raise ValueError('CocoParams: maxDets %r; each must be in [1, %d]' % (self.max_dets, MAX_DET))
+            raise ValueError('%s: %d maxDets; 1 to %d are supported' % (name, M, MAX_M))
+        if any(not 1 <= m <= self._MAX_DET for m in self.max_dets):
+            raise ValueError('%s: maxDets %r; each must be in [1, %d]' % (name, self.max_dets, self._MAX_DET))
         if not 1 <= R <= 101:
-            raise ValueError('CocoParams: %d recall thresholds; 1 to 101 are supported' % R)
+            raise ValueError('%s: %d recall thresholds; 1 to 101 are supported' % (name, R))
         if len(self.area_rng_lbl) != A:
-            raise ValueError('CocoParams: %d area range labels for %d area ranges' % (len(self.area_rng_lbl), A))
+            raise ValueError('%s: %d area range labels for %d area ranges' % (name, len(self.area_rng_lbl), A))
 
     @staticmethod
     def _floats(v, name, shape=(-1,)):
@@ -100,18 +122,71 @@ class CocoParams:
         """(T, R, A, M): precision / scores are [T, R, K, A, M], recall [T, K, A, M]."""
         return len(self.iou_thrs), len(self.rec_thrs), len(self.area_rng), len(self.max_dets)
 
+    @property
+    def extended(self):
+        """Whether these Params need the Params2 entry points (useCats = 0 or a maxDet above 100)."""
+        return self.use_cats == 0 or self.max_dets[-1] > MAX_DET
+
+    def eval_cats(self, gt_cat_ids):
+        """The category ids evaluated against a ground truth whose categories are gt_cat_ids (sorted), in the order of
+        their category index on the device: cat_ids as normalized here, or the ground truth's."""
+        return list(gt_cat_ids) if self.cat_ids is None else list(self.cat_ids)
+
+    def cat_axis(self, gt_cat_ids):
+        """The category ids along K of precision / recall / scores: eval_cats with useCats 1, [-1] with useCats 0 (as
+        accumulate sets p.catIds)."""
+        return self.eval_cats(gt_cat_ids) if self.use_cats else [-1]
+
     def summarizable(self):
         """Whether COCOeval.summarize runs on these Params: three maxDets and the labels all / small / medium / large."""
         return len(self.max_dets) == 3 and all(l in self.area_rng_lbl for l in AREA_RNG_LBL)
 
     def c_struct(self):
         T, R, A, M = self.shape
-        p = _ParamsC(T=T, A=A, M=M, R=R)
+        p = _Params2C(T=T, A=A, M=M, R=R, use_cats=self.use_cats) if self.extended else _ParamsC(T=T, A=A, M=M, R=R)
         p.max_dets[:M] = self.max_dets
         p.iou_thr[:T] = self.iou_thrs.tolist()
         p.area_rng[:2 * A] = self.area_rng.reshape(-1).tolist()
         p.rec_thr[:R] = self.rec_thrs.tolist()
         return p
+
+
+class CocoParams2(CocoParams):
+    """CocoParams plus p.useCats, p.catIds and maxDets up to 1000 (smb_coco_params2_t where needed).
+      use_cats 1: one evaluation per category of cat_ids (None: every ground-truth category), sorted and de-duplicated
+                  as evaluate() does (p.catIds = list(np.unique(p.catIds))); the K axis of the arrays is that list.
+                  An id no ground-truth annotation has gets a column of -1.
+      use_cats 0: one pooled evaluation per image over the ground truth and results of cat_ids (None: every
+                  ground-truth category, sorted), concatenated in the order given (computeIoU / evaluateImg); K = 1.
+                  pycocotools would repeat a repeated id's annotations, so duplicates are refused.
+    Results and annotations of other categories are not evaluated.  Limits: CocoParams', except each maxDet in
+    [1, 1000]; use_cats 0 or 1; cat_ids non-empty, at most 2048 ids.  With use_cats 1, no cat_ids and maxDets up to 100
+    these Params compute what the same CocoParams compute, through the same entry points."""
+    _MAX_DET = MAX_DET2
+
+    def __init__(self, iou_thrs=None, rec_thrs=None, max_dets=None, area_rng=None, area_rng_lbl=None, use_cats=1,
+                 cat_ids=None):
+        if isinstance(use_cats, (bool, np.bool_)) or (isinstance(use_cats, (int, np.integer)) and use_cats in (0, 1)):
+            self.use_cats = int(use_cats)
+        else:
+            raise ValueError('CocoParams2: useCats must be 0 or 1, got %r' % (use_cats,))
+        self.cat_ids = None
+        if cat_ids is not None:
+            ids = list(cat_ids)
+            if not all(isinstance(c, (int, np.integer)) and not isinstance(c, bool) for c in ids):
+                raise ValueError('CocoParams2: catIds must be integers, got %r' % (ids[:8],))
+            ids = [int(c) for c in ids]
+            if not ids:
+                raise ValueError('CocoParams2: catIds is empty')
+            if self.use_cats:
+                ids = sorted(set(ids))                                # evaluate(): list(np.unique(p.catIds))
+            elif len(set(ids)) != len(ids):
+                raise ValueError('CocoParams2: catIds %r repeats an id; with useCats = 0 pycocotools would evaluate '
+                                 'its annotations twice' % (ids[:8],))
+            if len(ids) > MAX_CATS:
+                raise ValueError('CocoParams2: %d catIds; at most %d' % (len(ids), MAX_CATS))
+            self.cat_ids = ids
+        self._set(iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
 
 
 def _ptr(a):
@@ -225,6 +300,7 @@ class CocoGroundTruth:
         self.names = [str(info[c].get('name', c)) for c in self.cat_ids]
         self.supercategories = [info[c].get('supercategory') for c in self.cat_ids]
         self.anns = {i: [] for i in self.img_ids}
+        self._all_anns = {i: [] for i in self.img_ids}       # imgToAnns, whatever the category (subset() filters it)
         for a in anns:
             try:
                 img, cat = int(a['image_id']), int(a['category_id'])
@@ -237,6 +313,22 @@ class CocoGroundTruth:
                 raise ValueError('CocoGroundTruth: annotation %d: bbox needs 4 numbers' % row['id'])
             if img in self.anns and cat in self.cat_index:        # getAnnIds(imgIds=p.imgIds, catIds=p.catIds)
                 self.anns[img].append(row)
+            if img in self._all_anns:
+                self._all_anns[img].append(row)
+
+    def subset(self, cat_ids):
+        """The ground truth as COCOeval indexes it with p.catIds = cat_ids: the same images, category index = position in
+        cat_ids (in the order given), and per image its annotations of those ids in file order (getAnnIds(imgIds,
+        catIds), which also keeps an id the file's categories do not list).  Rows of image() are then category-major in
+        that order, which is the order useCats = 0 concatenates them in."""
+        v = copy.copy(self)
+        v.cat_ids = [int(c) for c in cat_ids]
+        v.cat_index = {c: i for i, c in enumerate(v.cat_ids)}
+        info = dict(zip(self.cat_ids, zip(self.names, self.supercategories)))
+        v.names = [info[c][0] if c in info else str(c) for c in v.cat_ids]
+        v.supercategories = [info[c][1] if c in info else None for c in v.cat_ids]
+        v.anns = {i: [a for a in self._all_anns[i] if a['cat'] in v.cat_index] for i in self.img_ids}
+        return v
 
     def image(self, img_id, masks=True):
         """One image's ground truth for a match launch: (rows GT_DTYPE, per-category offsets [K+1], planes [G, h, pitch]
@@ -373,7 +465,12 @@ def accumulate(row_parts, npig, K, dev, params=None):
     precision = torch.empty((T, R, K, A, M), dtype=torch.float64, device=dev)
     scores = torch.empty_like(precision)
     recall = torch.empty((T, K, A, M), dtype=torch.float64, device=dev)
-    if params is None:
+    if params is not None and params.extended:
+        pc = params.c_struct()
+        L.check(L.lib().smb_coco_accumulate_params2_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K,
+                                                        L.ptr(npig), ctypes.byref(pc), L.ptr(precision), L.ptr(recall),
+                                                        L.ptr(scores), L.stream_ptr()), 'smb_coco_accumulate_params2_dev')
+    elif params is None:
         rec_thr = torch.from_numpy(np.ascontiguousarray(REC_THRS)).to(dev)
         md = (ctypes.c_int * 3)(*MAX_DETS)
         L.check(L.lib().smb_coco_accumulate_dev(L.ptr(srt), ctypes.c_int64(srt.shape[0]), L.ptr(cat_off), K, L.ptr(npig),
@@ -432,6 +529,44 @@ def _dev_bytes(arr, dev):
     return torch.from_numpy(np.ascontiguousarray(arr).view(np.uint8).reshape(-1)).to(dev)
 
 
+def check_metrics(metrics, benchmark=False):
+    """CocoDataset.evaluate's metric names this evaluator runs: 'bbox', 'segm' and 'proposal' (box recall of the bbox
+    results, class-agnostic).  Raises KeyError for a name CocoDataset.evaluate does not know either, ValueError for
+    'proposal_fast' and, on SipMask-benchmark records, for 'proposal'."""
+    metrics = [metrics] if isinstance(metrics, str) else list(metrics)
+    for m in metrics:
+        if m == 'proposal_fast':
+            raise ValueError("metric 'proposal_fast' is not supported: it evaluates proposal arrays (eval_recalls reads "
+                             "proposals[i].ndim), which SipMask's (bboxes, masks) results are not; 'proposal' gives "
+                             "AR@100 / 300 / 1000 of the bbox results")
+        if m not in ('bbox', 'segm', 'proposal'):
+            raise KeyError('metric {} is not supported'.format(m))
+    if benchmark and 'proposal' in metrics:
+        raise ValueError("metric 'proposal' is not supported on SipMask-benchmark records: its evaluation never "
+                         "evaluates box proposals of SipMask (box_only=False)")
+    return metrics
+
+
+def proposal_results(stats):
+    """CocoDataset.evaluate's entries of metric 'proposal': stats[6:12] rounded, under its names whatever proposal_nums
+    are."""
+    return {item: float('{:.3f}'.format(stats[i + 6])) for i, item in enumerate(PROPOSAL_ITEMS)}
+
+
+class _View:
+    """What one metric is matched and accumulated with: its Params (None: the default entry points), the ground truth as
+    they index it (gv: index into the evaluator's distinct views), the category index of each record label, K of the
+    match launches (categories the rows index) and of accumulate (1 with useCats 0)."""
+
+    def __init__(self, params, gv, label_cat_host, dev, K):
+        self.params, self.gv, self.K = params, gv, K
+        self.K_acc = K if params is None or params.use_cats else 1
+        self.A = len(AREA_RNG) if params is None else params.shape[2]
+        self.pc = params.c_struct() if params is not None else None
+        self.label_cat_host = label_cat_host
+        self.label_cat = torch.from_numpy(label_cat_host).to(dev)
+
+
 class CocoEvaluator:
     """Device state of one COCO evaluation: per evaluated image, its detections' matched / ignored flags (per metric),
     and npig per (category, area range).  Images are added as engine records (add_records) or result lists
@@ -439,24 +574,38 @@ class CocoEvaluator:
       gt      : CocoGroundTruth
       cat_ids : COCO category id per 0-based record label (as coco.coco_json takes it)
       benchmark: SipMask-benchmark records (BoxList.resize boxes, box scores for segm)
-      params  : CocoParams (None: COCOeval's default Params)
+      params  : CocoParams or CocoParams2 (None: COCOeval's default Params)
       analyze : also run, for every image added, the matches of coco_error_analysis.py (see analysis_arrays), so that
-                evaluate() returns its precision arrays as well."""
+                evaluate() returns its precision arrays as well (every ground-truth category: not with a cat_ids
+                subset)
+      metrics : 'bbox', 'segm' and / or 'proposal': MM's proposal metric, COCOeval of the bbox results (boxes and box
+                scores) with the default Params but useCats = 0 and maxDets = proposal_nums, whatever `params` are."""
 
-    def __init__(self, gt, cat_ids, metrics=('bbox', 'segm'), benchmark=False, device=None, params=None, analyze=False):
-        metrics = [metrics] if isinstance(metrics, str) else list(metrics)
-        for m in metrics:
-            if m not in ('bbox', 'segm'):
-                raise KeyError('metric {} is not supported'.format(m))
+    def __init__(self, gt, cat_ids, metrics=('bbox', 'segm'), benchmark=False, device=None, params=None, analyze=False,
+                 proposal_nums=PROPOSAL_NUMS):
+        metrics = check_metrics(metrics, benchmark)
         if params is not None and not isinstance(params, CocoParams):
             raise ValueError('params must be a CocoParams')
         self.gt, self.metrics, self.benchmark, self.params = gt, metrics, bool(benchmark), params
-        A = len(AREA_RNG) if params is None else params.shape[2]
         self.dev = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
         self.K = len(gt.cat_ids)
         self.label_cat_host = np.array([gt.cat_index.get(int(c), -1) for c in cat_ids], np.int32)
-        self.label_cat = torch.from_numpy(self.label_cat_host).to(self.dev)
-        self.npig = {m: torch.zeros(self.K * A, dtype=torch.int32, device=self.dev) for m in metrics}
+        self.proposal_params = (CocoParams2(max_dets=[int(n) for n in proposal_nums], use_cats=0)
+                                if 'proposal' in metrics else None)
+        self._gviews, self._gcats, self.views = [], [], {}
+        for m in metrics:
+            p = self.proposal_params if m == 'proposal' else params
+            cats = list(gt.cat_ids) if p is None else p.eval_cats(gt.cat_ids)
+            if cats not in self._gcats:
+                self._gcats.append(cats)
+                self._gviews.append(gt if cats == list(gt.cat_ids) else gt.subset(cats))
+            gv = self._gcats.index(cats)
+            lc = np.array([self._gviews[gv].cat_index.get(int(c), -1) for c in cat_ids], np.int32)
+            self.views[m] = _View(p, gv, lc, self.dev, len(cats))
+        self._segm_gv = self.views['segm'].gv if 'segm' in metrics else 0
+        if analyze and any(self._gviews[self.views[m].gv] is not gt for m in metrics if m != 'proposal'):
+            raise ValueError('analyze: the error analysis evaluates every ground-truth category (no cat_ids subset)')
+        self.npig = {m: torch.zeros(v.K_acc * v.A, dtype=torch.int32, device=self.dev) for m, v in self.views.items()}
         self.rows = {m: [] for m in metrics}
         self.status = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.raster_status = torch.zeros(1, dtype=torch.int32, device=self.dev)
@@ -465,15 +614,15 @@ class CocoEvaluator:
         self._seen = set()
         self._iou_thr = np.ascontiguousarray(IOU_THRS, dtype=np.float64)
         self._area_rng = np.ascontiguousarray(np.array(AREA_RNG, dtype=np.float64).reshape(-1))
-        self._params_c = params.c_struct() if params is not None else None
         self.analyze = bool(analyze)
         if self.analyze:
             sup, self.n_sup = gt.supercategory_index()
             self.sup = torch.from_numpy(sup).to(self.dev)
             self._ana_c = ANALYSIS_PARAMS.c_struct()
-            self.npig_ana = {m: torch.zeros(self.K * len(AREA_RNG), dtype=torch.int32, device=self.dev) for m in metrics}
-            self.rows_c = {m: [] for m in metrics}         # ps[0:3]: iouThrs [.75, .5, .1], maxDets [100]
-            self.rows_so = {m: [] for m in metrics}        # ps[3:5]: Sim / Oth rows
+            ana = [m for m in metrics if m != 'proposal']
+            self.npig_ana = {m: torch.zeros(self.K * len(AREA_RNG), dtype=torch.int32, device=self.dev) for m in ana}
+            self.rows_c = {m: [] for m in ana}             # ps[0:3]: iouThrs [.75, .5, .1], maxDets [100]
+            self.rows_so = {m: [] for m in ana}            # ps[3:5]: Sim / Oth rows
 
     # ---- bookkeeping
     def _claim(self, image_ids, ori_hws=None):
@@ -493,18 +642,24 @@ class CocoEvaluator:
         vertices and run lengths) and upload it from pinned memory on `stream` (default: the current stream); its planes
         are reserved on the device and rasterized there right before the image's first segm match.  Returns its device
         tensors, for add_records(..., gts=[...]) on a stream that is ordered after `stream`.  masks: whether the masks
-        are needed (default: when 'segm' is evaluated)."""
+        are needed (default: when 'segm' is evaluated).  When the metrics index the ground truth differently (a cat_ids
+        subset beside 'proposal'), each such view is staged too, under 'views'."""
+        want = 'segm' in self.metrics if masks is None else bool(masks)
+        staged = [self._stage_view(g, int(image_id), stream, want and v == self._segm_gv)
+                  for v, g in enumerate(self._gviews)]
+        staged[0]['views'] = staged
+        return staged[0]
+
+    def _stage_view(self, gv, image_id, stream, segm):
         from . import segm_raster as SR
-        image_id = int(image_id)
-        segm = 'segm' in self.metrics if masks is None else bool(masks)
-        rows, off, pack = self.gt.packed(image_id) if segm else self.gt.image(image_id, False)[:2] + (None,)
+        rows, off, pack = gv.packed(image_id) if segm else gv.image(image_id, False)[:2] + (None,)
         h, w = self.gt.hw[image_id]
         pitch = (w + 31) // 32
         n_gt = len(rows)
         if segm:
             rows['plane'] = np.arange(n_gt, dtype=np.int64) * (h * pitch)
         stream = stream or torch.cuda.current_stream(self.dev)
-        extra = (rows, off) + ((self.gt.positions(image_id),) if self.analyze else ())
+        extra = (rows, off) + ((gv.positions(image_id),) if self.analyze else ())
         with torch.cuda.device(self.dev), torch.cuda.stream(stream):
             st, views = SR.staged(pack if segm else SR.SegmPack(), self.dev, extra)
             planes = torch.empty(max(n_gt * h * pitch, 1) if segm else 1, dtype=torch.int32, device=self.dev)
@@ -523,20 +678,22 @@ class CocoEvaluator:
         SR.raster(r, gt['planes'], gt['n_gt'], r['stride'], r['pitch'], self.raster_status, area=rows[15:],
                   area_stride=GT_DTYPE.itemsize // 4, ext=rows[16:], ext_stride=GT_DTYPE.itemsize // 4)
 
-    def _outs(self, n_rows):
+    def _outs(self, metric, n_rows):
         """Output rows of a batch: the plain match's and, when analyzing, those of the two analysis matches."""
         return [torch.empty(n_rows * OUT_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
-                for _ in range(3 if self.analyze else 1)]
+                for _ in range(3 if self.analyze and metric != 'proposal' else 1)]
 
     def _keep(self, metric, outs):
         self.rows[metric].append(outs[0])
-        if self.analyze:
+        if self.analyze and metric != 'proposal':
             self.rows_c[metric].append(outs[1])
             self.rows_so[metric].append(outs[2])
 
     def _match(self, metric, imgs, n, dets, det_cap, det_planes, det_plane_words, gt, outs):
         """The match launches of image n of a batch (imgs / dets: the batch's device rows) on the current stream."""
         lib = L.lib()
+        view = self.views[metric]
+        gt = gt['views'][view.gv] if 'views' in gt else gt
         cur = torch.cuda.current_stream(self.dev)
         if gt['stream'] != cur:                          # uploaded on another stream: keep it until this stream is done
             for key in ('rows', 'off', 'planes', 'pos'):
@@ -549,20 +706,26 @@ class CocoEvaluator:
         args = (ctypes.c_void_p(imgs.data_ptr() + n * IMG_DTYPE.itemsize), 1,
                 ctypes.c_void_p(dets.data_ptr() + n * det_cap * DET_DTYPE.itemsize), det_cap, L.ptr(det_planes),
                 ctypes.c_int64(det_plane_words), L.ptr(gt['rows']), gt['n_gt'], L.ptr(gt['planes']),
-                ctypes.c_int64(gt['plane_words']), L.ptr(gt['off']), self.K, 0 if metric == 'bbox' else 1)
+                ctypes.c_int64(gt['plane_words']), L.ptr(gt['off']), view.K, 1 if metric == 'segm' else 0)
         tail = (L.ptr(out_rows), ctypes.c_int64(n_out), L.ptr(self.npig[metric]), L.ptr(self.status))
-        if self._params_c is None:
+        if view.pc is None:
             ws_bytes = lib.smb_coco_match_workspace_bytes(gt['n_gt'])
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
             L.check(lib.smb_coco_match_dev(*args, _ptr(self._iou_thr), _ptr(self._area_rng), *tail, L.ptr(ws),
                                            ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_coco_match_dev')
+        elif view.params.extended:
+            pc = ctypes.byref(view.pc)
+            ws_bytes = lib.smb_coco_match_params2_workspace_bytes(gt['n_gt'], pc)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
+            L.check(lib.smb_coco_match_params2_dev(*args, pc, *tail, L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
+                    'smb_coco_match_params2_dev')
         else:
-            pc = ctypes.byref(self._params_c)
+            pc = ctypes.byref(view.pc)
             ws_bytes = lib.smb_coco_match_params_workspace_bytes(gt['n_gt'], pc)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.dev)
             L.check(lib.smb_coco_match_params_dev(*args, pc, *tail, L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
                     'smb_coco_match_params_dev')
-        if not self.analyze:
+        if not self.analyze or metric == 'proposal':
             return
         pc = ctypes.byref(self._ana_c)
         ws_bytes = lib.smb_coco_match_params_workspace_bytes(gt['n_gt'], pc)
@@ -621,16 +784,22 @@ class CocoEvaluator:
                 gts = [self.stage_gt(i) for i in ids]
             lib = L.lib()
             imgs = _dev_bytes(self._img_rows(ids, words, max_num), self.dev)
-            dets = torch.empty(B * max_num * DET_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
-            L.check(lib.smb_coco_det_from_record_dev(L.ptr(det), L.ptr(labels), L.ptr(count), L.ptr(ms), L.ptr(bits), B,
-                                                     max_num, cap_h, words, L.ptr(geom), L.ptr(self.label_cat),
-                                                     len(self.label_cat_host), int(self.benchmark), L.ptr(dets), L.ptr(imgs),
-                                                     L.ptr(self.status), L.stream_ptr()), 'smb_coco_det_from_record_dev')
+            dets = {}                                     # per ground-truth view: its category index of every label
+            for m in self.metrics:
+                v = self.views[m]
+                if v.gv in dets:
+                    continue
+                dets[v.gv] = torch.empty(B * max_num * DET_DTYPE.itemsize, dtype=torch.uint8, device=self.dev)
+                L.check(lib.smb_coco_det_from_record_dev(L.ptr(det), L.ptr(labels), L.ptr(count), L.ptr(ms), L.ptr(bits),
+                                                         B, max_num, cap_h, words, L.ptr(geom), L.ptr(v.label_cat),
+                                                         len(v.label_cat_host), int(self.benchmark), L.ptr(dets[v.gv]),
+                                                         L.ptr(imgs), L.ptr(self.status), L.stream_ptr()),
+                        'smb_coco_det_from_record_dev')
             n_json = count[:B].clamp(0, max_num).sum()
             for m in self.metrics:
-                outs = self._outs(B * max_num)
+                outs = self._outs(m, B * max_num)
                 for n in range(B):
-                    self._match(m, imgs, n, dets, max_num, bits, bits.numel(), gts[n], outs)
+                    self._match(m, imgs, n, dets[self.views[m].gv], max_num, bits, bits.numel(), gts[n], outs)
                 self._keep(m, outs)
                 self.n_results[m] += n_json
             self.image_ids += ids
@@ -640,7 +809,9 @@ class CocoEvaluator:
     def add_results(self, per_image, metric):
         """Evaluate `metric` of images from result-json entries (dicts with image_id, category_id, score, and bbox or
         segmentation).  per_image: [(image_id, its entries in list order)].  Used by evaluate_json, one metric at a time,
-        for images it has claimed."""
+        for images it has claimed.  'proposal' reads the bbox results."""
+        gv = self._gviews[self.views[metric].gv]
+        box = metric != 'segm'
         with torch.cuda.device(self.dev):
             ids = [int(i) for i, _ in per_image]
             det_cap = max([1] + [len(v) for _, v in per_image])
@@ -664,7 +835,7 @@ class CocoEvaluator:
                     try:
                         score = float(r['score'])
                         cat = int(r['category_id'])
-                        if metric == 'bbox':
+                        if box:
                             bb = [float(v) for v in r['bbox']]
                             if len(bb) != 4:
                                 raise ValueError('bbox needs 4 numbers')
@@ -679,8 +850,8 @@ class CocoEvaluator:
                             rows_of_plane.append(n * det_cap + j)
                     except (KeyError, TypeError) as e:
                         raise ValueError('add_results: malformed result %r: %r' % (r, e))
-                    d['score'][0 if metric == 'bbox' else 1] = score
-                    d['cat'] = self.gt.cat_index.get(cat, -1)
+                    d['score'][0 if box else 1] = score
+                    d['cat'] = gv.cat_index.get(cat, -1)
             imgs = _dev_bytes(self._img_rows(ids, pitch, det_cap, n_det), self.dev)
             P = len(rows_of_plane)
             st, (dd, at) = SR.staged(pack, self.dev, (dets, np.array(rows_of_plane, np.int64)))
@@ -695,20 +866,22 @@ class CocoEvaluator:
                 rows32 = dd.view(torch.int32)[:B * det_cap * 24].view(B * det_cap, 24)
                 rows32[at, 16] = stats[:, 0]
                 rows32[at[:, None], torch.arange(18, 22, device=self.dev)[None]] = stats[:, 1:]
-            outs = self._outs(B * det_cap)
+            outs = self._outs(metric, B * det_cap)
             for n, i in enumerate(ids):
                 self._match(metric, imgs, n, dd, det_cap, pd, pd.numel(), self.stage_gt(i, masks=metric == 'segm'), outs)
             self._keep(metric, outs)
 
     # ---- accumulate + summarize
     def _accumulate(self, metric):
-        return accumulate(self.rows[metric], self.npig[metric], self.K, self.dev, self.params)
+        v = self.views[metric]
+        return accumulate(self.rows[metric], self.npig[metric], v.K_acc, self.dev, v.params)
 
     def evaluate(self):
         """Accumulate and summarize every metric.  Returns 'arrays' ({metric: {'precision', 'recall', 'scores'}}) with
-        COCOeval's eval arrays in the Params' shapes and, where COCOeval.summarize runs on the Params (three maxDets and
-        the labels all / small / medium / large), MM's dict (bbox_mAP, ..., segm_mAP_copypaste) and 'stats'.  With
-        analyze=True, also 'analysis' ({metric: ps}, see analysis_arrays)."""
+        COCOeval's eval arrays in the Params' shapes (K along CocoParams.cat_axis) and, where COCOeval.summarize runs on
+        the Params (three maxDets and the labels all / small / medium / large), MM's dict (bbox_mAP, ...,
+        segm_mAP_copypaste; AR@100, ..., AR_l@1000 for 'proposal') and 'stats'.  With analyze=True, also 'analysis'
+        ({metric: ps}, see analysis_arrays)."""
         with torch.cuda.device(self.dev):
             status = int(self.status.item())
             if status & LABEL_RANGE:
@@ -725,18 +898,19 @@ class CocoEvaluator:
                     raise ValueError('%s: the results of the evaluated images are empty' % m)
                 p, r, s = self._accumulate(m)
                 arrays[m] = dict(precision=p, recall=r, scores=s)
-                if self.params is None:
+                prm = self.views[m].params
+                if prm is None:
                     stats[m] = summarize(p, r)
-                elif self.params.summarizable():
-                    stats[m] = summarize(p, r, self.params.area_rng_lbl, self.params.max_dets, self.params.iou_thrs)
+                elif prm.summarizable():
+                    stats[m] = summarize(p, r, prm.area_rng_lbl, prm.max_dets, prm.iou_thrs)
                 else:
                     continue
-                out.update(mm_results(m, stats[m]))
+                out.update(proposal_results(stats[m]) if m == 'proposal' else mm_results(m, stats[m]))
             if stats:
                 out['stats'] = stats
             out['arrays'] = arrays
             if self.analyze:
-                out['analysis'] = {m: self._analysis(m) for m in self.metrics}
+                out['analysis'] = {m: self._analysis(m) for m in self.metrics if m != 'proposal'}
             return out
 
     def _analysis(self, m):
@@ -745,22 +919,30 @@ class CocoEvaluator:
         return analysis_arrays(p3, p2)
 
 
-def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None, params=None):
+def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None, params=None,
+                  proposal=False, proposal_nums=PROPOSAL_NUMS):
     """COCOeval of result lists (coco.coco_json output or a loaded results file) against `gt` on the device: the same
     kernels as CocoEvaluator, with the detections' RLE strings parsed to run lengths on the host and rasterized on the
     device.  img_ids: the evaluated images
     (p.imgIds; default every ground-truth image).  As in pycocotools, a result whose image is not in the ground truth
     raises (loadRes), and results of ground-truth images outside img_ids are not evaluated (_prepare).  params:
-    CocoParams (None: the default Params).  Returns CocoEvaluator.evaluate()'s dict for the metrics given."""
+    CocoParams (None: the default Params).  proposal: also MM's 'proposal' metric of bbox_json (useCats = 0, maxDets =
+    proposal_nums).  Returns CocoEvaluator.evaluate()'s dict for the metrics given."""
     metrics = [m for m, j in (('bbox', bbox_json), ('segm', segm_json)) if j is not None]
-    return _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, False, metrics)
+    if proposal:
+        if bbox_json is None:
+            raise ValueError("evaluate_json: 'proposal' evaluates the bbox results; bbox_json is None")
+        metrics.append('proposal')
+    return _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, False, metrics, proposal_nums)
 
 
-def _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, analyze, metrics):
-    ev = CocoEvaluator(gt, cat_ids, metrics=metrics, device=device, params=params, analyze=analyze)
+def _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, analyze, metrics,
+              proposal_nums=PROPOSAL_NUMS):
+    ev = CocoEvaluator(gt, cat_ids, metrics=metrics, device=device, params=params, analyze=analyze,
+                       proposal_nums=proposal_nums)
     ids = ev._claim(gt.img_ids if img_ids is None else sorted(set(int(i) for i in img_ids)))
-    for m, res in (('bbox', bbox_json), ('segm', segm_json)):
-        if res is None:
+    for m, res in (('bbox', bbox_json), ('segm', segm_json), ('proposal', bbox_json)):
+        if res is None or m not in metrics:
             continue
         per = {i: [] for i in ids}
         for r in res:

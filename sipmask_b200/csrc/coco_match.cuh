@@ -93,10 +93,10 @@ __device__ __forceinline__ void greedy_match(int tid, int D, int G, const double
   }
 }
 
-// Workspace of one match launch over n_gt ground truths: [n_gt, kMaxDet] IoUs and [n_gt, ta] gtm bytes, ta = T * A.
-inline size_t match_workspace_bytes(int n_gt, int ta = kT * kA) {
-  if (n_gt < 0 || ta < 0) return 0;
-  return smb::align_up((size_t)n_gt * kMaxDet * sizeof(double), 256) + smb::align_up((size_t)n_gt * ta, 256) + 256;
+// Workspace of one match launch over n_gt ground truths: [n_gt, max_det] IoUs and [n_gt, ta] gtm bytes, ta = T * A.
+inline size_t match_workspace_bytes(int n_gt, int ta = kT * kA, int max_det = kMaxDet) {
+  if (n_gt < 0 || ta < 0 || max_det < 0) return 0;
+  return smb::align_up((size_t)n_gt * max_det * sizeof(double), 256) + smb::align_up((size_t)n_gt * ta, 256) + 256;
 }
 
 }  // namespace smb_match

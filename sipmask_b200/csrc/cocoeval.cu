@@ -6,6 +6,7 @@
 //   smb_coco_accumulate_dev      : accumulate's precision / recall / scores arrays from the globally sorted rows
 //   smb_coco_*_params_dev        : the same two with user-given Params (thresholds, area ranges, maxDets, recall
 //                                  thresholds as data); the default Params give what the two above give
+//   smb_coco_*_params2_dev       : the same with useCats 0 (one pooled group per image) and maxDets up to 1000
 //   smb_coco_analysis_match_dev  : coco_error_analysis.py's Sim / Oth evaluations (relabelled ground truth) of a batch
 //
 // Every float64 operation whose result is compared with pycocotools is an explicit _rn intrinsic, so nvcc cannot
@@ -285,6 +286,140 @@ __global__ void __launch_bounds__(kThreads) match_kernel(
     __syncthreads();
     for (int r = tid; r < D; r += kThreads) {
       const int j = s_sorted[r];
+      smb_coco_out_t* o = out_row(j);
+      if (o) {
+        o->score = drow[j].score[metric];
+        o->matched = s_m[r];
+        o->ignored = s_ig[r];
+        o->cat = k;
+        o->rank = r;
+      } else {
+        atomicOr(status, SMB_COCO_CAPACITY);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ 2b' + 2c': Params2
+// match_kernel for smb_coco_params2_t: useCats 0 (one pooled group per image) or 1, and up to SMB_COCO_MAX_DET2 ranked
+// detections per group.  The image's detections are ranked at once by a bitonic sort of their indices in shared memory,
+// with the keys staged there too: (group, score descending, category index, json order, row), a total order, so the sort
+// needs no stability.  group = category index with useCats 1, 0 with useCats 0; rows of no evaluated category sort last.
+// A group is then a run of the sorted indices, found by binary search, and its first min(n, maxDet) entries are its
+// ranked detections, as computeIoU keeps them.  IoU, the greedy loop and the output rows are match_kernel's.
+// Dynamic shared memory: s_m / s_ig [max_det] uint64, then per padded row (n_pad = det_cap rounded up to a power of two)
+// score double, tie uint64 = (category index << 32 | order), group int, sorted index int, then s_start [groups + 1].
+constexpr int kMaxDet2 = SMB_COCO_MAX_DET2;
+
+__host__ __device__ inline int pad_pow2(int n) {
+  int p = 1;
+  while (p < n) p <<= 1;
+  return p;
+}
+
+inline size_t match2_smem_bytes(int det_cap, int K, int max_det, int use_cats) {
+  const size_t n_pad = (size_t)pad_pow2(det_cap);
+  return 2 * (size_t)max_det * sizeof(uint64_t) + n_pad * (sizeof(double) + sizeof(uint64_t) + 2 * sizeof(int)) +
+         (size_t)((use_cats ? K : 1) + 1) * sizeof(int);
+}
+
+__global__ void __launch_bounds__(kThreads) match2_kernel(
+    const smb_coco_img_t* __restrict__ imgs, const smb_coco_det_t* __restrict__ dets, int det_cap,
+    const uint32_t* __restrict__ det_planes, int64_t det_plane_words, const smb_coco_gt_t* __restrict__ gts, int n_gt,
+    const uint32_t* __restrict__ gt_planes, int64_t gt_plane_words, const int32_t* __restrict__ gt_cat_off, int K,
+    int metric, int use_cats, MatchParams P, smb_coco_out_t* __restrict__ out, int64_t n_out, int* __restrict__ npig,
+    double* __restrict__ iou_ws, uint8_t* __restrict__ gtm_ws, int* __restrict__ status) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int n_pad = pad_pow2(det_cap), n_grp = use_cats ? K : 1;
+  uint64_t* s_m = (uint64_t*)smem;                 // [max_det] matched bits of the ranked detections of a group
+  uint64_t* s_ig = s_m + P.max_det;                // [max_det] ignore bits
+  double* s_score = (double*)(s_ig + P.max_det);   // [n_pad] per row
+  uint64_t* s_tie = (uint64_t*)(s_score + n_pad);  // [n_pad] per row
+  int* s_grp = (int*)(s_tie + n_pad);              // [n_pad] per row (INT_MAX: not evaluated)
+  int* s_idx = s_grp + n_pad;                      // [n_pad] rows in rank order (-1: padding)
+  int* s_start = s_idx + n_pad;                    // [n_grp + 1] first sorted position of each group
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const smb_coco_img_t im = imgs[b];
+  const int nd = min(max(im.n_det, 0), det_cap);
+  const smb_coco_det_t* drow = dets + (size_t)b * det_cap;
+  const int32_t* goff = gt_cat_off + (size_t)b * (K + 1);
+  const int H = max(im.h, 0), gpitch = max(im.gt_pitch, 0), dpitch = max(im.det_pitch, 0);
+  auto out_row = [&](int j) -> smb_coco_out_t* {
+    const int64_t o = im.out_off + j;
+    return (o >= 0 && o < n_out) ? out + o : nullptr;
+  };
+  for (int j = tid; j < det_cap; j += kThreads) {
+    smb_coco_out_t* o = out_row(j);
+    if (o) { o->score = 0; o->image_id = im.image_id; o->matched = 0; o->ignored = 0; o->cat = n_grp; o->rank = -1; }
+  }
+  for (int j = tid; j < n_pad; j += kThreads) {
+    s_idx[j] = j < nd ? j : -1;
+    if (j < nd) {
+      const int c = drow[j].cat;
+      const bool ok = c >= 0 && c < K;
+      s_grp[j] = ok ? (use_cats ? c : 0) : INT_MAX;
+      s_score[j] = drow[j].score[metric];
+      s_tie[j] = ((uint64_t)(uint32_t)c << 32) | (uint32_t)drow[j].order;
+    }
+  }
+  __syncthreads();
+  auto before = [&](int x, int y) -> bool {        // x ranks before y; padding (-1) after everything
+    if (y < 0) return x >= 0;
+    if (x < 0) return false;
+    if (s_grp[x] != s_grp[y]) return s_grp[x] < s_grp[y];
+    if (s_score[x] != s_score[y]) return s_score[x] > s_score[y];
+    if (s_tie[x] != s_tie[y]) return s_tie[x] < s_tie[y];
+    return x < y;
+  };
+  for (int k = 2; k <= n_pad; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < n_pad; i += kThreads) {
+        const int l = i ^ j;
+        if (l > i) {
+          const int x = s_idx[i], y = s_idx[l];
+          if ((i & k) == 0 ? before(y, x) : before(x, y)) { s_idx[i] = y; s_idx[l] = x; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  // group g's sorted positions are [s_start[g], s_start[g + 1]): the first position whose group is >= g
+  for (int g = tid; g <= n_grp; g += kThreads) {
+    int lo = 0, hi = nd;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (s_grp[s_idx[mid]] < g) lo = mid + 1; else hi = mid;
+    }
+    s_start[g] = lo;
+  }
+  __syncthreads();
+  for (int k = 0; k < n_grp; ++k) {
+    const int l0 = s_start[k], n = s_start[k + 1] - l0;
+    const int c0 = use_cats ? k : 0, c1 = use_cats ? k + 1 : K;
+    const int g0 = min(max(goff[c0], 0), n_gt), g1 = min(max(goff[c1], g0), n_gt), G = g1 - g0;
+    if (n == 0 && G == 0) continue;                // evaluateImg returns None
+    const int D = min(n, P.max_det);
+    const int* ranked = s_idx + l0;
+    for (int i = tid; i < D; i += kThreads) { s_m[i] = 0; s_ig[i] = 0; }
+    double* ious = iou_ws + (size_t)P.max_det * g0;
+    iou_matrix(metric, D, G, drow, ranked, gts, [&](int g) { return make_int2(g0 + g, gts[g0 + g].crowd); }, H, dpitch,
+               gpitch, det_planes, det_plane_words, gt_planes, gt_plane_words, ious);
+    __syncthreads();
+    smb_match::greedy_match(
+        tid, D, G, ious, gtm_ws + (size_t)P.T * P.A * g0, P,
+        [&](int g) {
+          const smb_coco_gt_t& gr = gts[g0 + g];
+          return smb_match::MatchGt{gr.area, gr.id, gr.crowd};
+        },
+        [&](int d) {
+          const smb_coco_det_t& dr = drow[ranked[d]];
+          return metric == 0 ? dr.area_box : (double)dr.area_mask;
+        },
+        npig + k * P.A, s_m, s_ig);
+    __syncthreads();
+    for (int r = tid; r < D; r += kThreads) {
+      const int j = ranked[r];
       smb_coco_out_t* o = out_row(j);
       if (o) {
         o->score = drow[j].score[metric];
@@ -878,6 +1013,91 @@ extern "C" int smb_coco_accumulate_params_dev(const smb_coco_out_t* rows, int64_
                 "smb_coco_accumulate_params_dev: bad sizes (n_rows %lld, K %d)", (long long)n_rows, K);
   SMB_CHECK_ARG(cat_off && npig && precision && recall && scores && (rows || n_rows == 0),
                 "smb_coco_accumulate_params_dev: null pointer");
+  AccParams P;
+  P.A = p->A;
+  P.M = p->M;
+  P.R = p->R;
+  for (int m = 0; m < p->M; ++m) P.max_dets[m] = p->max_dets[m];
+  for (int r = 0; r < p->R; ++r) P.rec_thr[r] = p->rec_thr[r];
+  accumulate_kernel<<<dim3(K, p->A * p->M, p->T), kThreads, 0, (cudaStream_t)stream>>>(rows, cat_off, n_rows, K, npig,
+                                                                                      nullptr, P, precision, recall, scores);
+  SMB_LAUNCH_OK("accumulate_kernel");
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_params2_check(const smb_coco_params2_t* p) {
+  SMB_CHECK_ARG(p, "smb_coco_params2_check: null Params");
+  SMB_CHECK_ARG(p->use_cats == 0 || p->use_cats == 1, "Params: useCats %d; 0 or 1", p->use_cats);
+  SMB_CHECK_ARG(p->T >= 1 && p->A >= 1 && p->T * p->A <= SMB_COCO_MAX_TA,
+                "Params: %d IoU thresholds x %d area ranges; 1 <= T, 1 <= A and T * A <= %d (one uint64 of bits per row)",
+                p->T, p->A, SMB_COCO_MAX_TA);
+  SMB_CHECK_ARG(p->M >= 1 && p->M <= SMB_COCO_MAX_M, "Params: %d maxDets; 1 to %d", p->M, SMB_COCO_MAX_M);
+  for (int m = 0; m < p->M; ++m) {
+    SMB_CHECK_ARG(p->max_dets[m] >= 1 && p->max_dets[m] <= SMB_COCO_MAX_DET2, "Params: maxDet %d outside [1, %d]",
+                  p->max_dets[m], SMB_COCO_MAX_DET2);
+    SMB_CHECK_ARG(m == 0 || p->max_dets[m] >= p->max_dets[m - 1], "Params: maxDets must be ascending (%d after %d)",
+                  p->max_dets[m], p->max_dets[m - 1]);
+  }
+  SMB_CHECK_ARG(p->R >= 1 && p->R <= SMB_COCO_R, "Params: %d recall thresholds; 1 to %d", p->R, SMB_COCO_R);
+  for (int t = 0; t < p->T; ++t) SMB_CHECK_ARG(!isnan(p->iou_thr[t]), "Params: IoU threshold %d is NaN", t);
+  for (int a = 0; a < p->A; ++a)
+    SMB_CHECK_ARG(!isnan(p->area_rng[a][0]) && !isnan(p->area_rng[a][1]), "Params: area range %d has a NaN", a);
+  for (int r = 0; r < p->R; ++r) SMB_CHECK_ARG(!isnan(p->rec_thr[r]), "Params: recall threshold %d is NaN", r);
+  return SMB_OK;
+}
+
+extern "C" size_t smb_coco_match_params2_workspace_bytes(int n_gt, const smb_coco_params2_t* p) {
+  if (!p || smb_coco_params2_check(p) != SMB_OK) return 0;
+  return smb_match::match_workspace_bytes(n_gt, p->T * p->A, p->max_dets[p->M - 1]);
+}
+
+extern "C" int smb_coco_match_params2_dev(const smb_coco_img_t* imgs, int n_img, const smb_coco_det_t* dets, int det_cap,
+                                          const uint32_t* det_planes, int64_t det_plane_words, const smb_coco_gt_t* gts,
+                                          int n_gt, const uint32_t* gt_planes, int64_t gt_plane_words,
+                                          const int32_t* gt_cat_off, int K, int metric, const smb_coco_params2_t* p,
+                                          smb_coco_out_t* out, int64_t n_out, int* npig, int* status, void* workspace,
+                                          size_t workspace_bytes, smb_stream_t stream) {
+  const int rc = smb_coco_params2_check(p);
+  if (rc != SMB_OK) return rc;
+  SMB_CHECK_ARG(n_img >= 0 && det_cap >= 1 && det_cap <= SMB_COCO_DET_CAP && K >= 1 && K <= SMB_COCO_MAX_CATS && n_gt >= 0 &&
+                    (metric == 0 || metric == 1) && n_out >= 0 && det_plane_words >= 0 && gt_plane_words >= 0,
+                "smb_coco_match_params2_dev: bad sizes (n_img %d, det_cap %d, K %d, n_gt %d, metric %d)", n_img, det_cap, K,
+                n_gt, metric);
+  if (n_img == 0) return SMB_OK;
+  SMB_CHECK_ARG(imgs && dets && gt_cat_off && out && npig && status && (gts || n_gt == 0) && workspace,
+                "smb_coco_match_params2_dev: null pointer");
+  SMB_CHECK_ARG(metric == 0 || (det_planes && (gt_planes || n_gt == 0)), "smb_coco_match_params2_dev: segm needs the planes");
+  const int max_det = p->max_dets[p->M - 1];
+  const size_t need = smb_match::match_workspace_bytes(n_gt, p->T * p->A, max_det);
+  SMB_CHECK_ARG(workspace_bytes >= need, "smb_coco_match_params2_dev: workspace of %zu bytes, %zu needed", workspace_bytes,
+                need);
+  MatchParams P;
+  P.T = p->T;
+  P.A = p->A;
+  P.max_det = max_det;
+  for (int t = 0; t < p->T; ++t) P.iou_thr[t] = p->iou_thr[t];
+  for (int a = 0; a < p->A; ++a) { P.area_rng[a][0] = p->area_rng[a][0]; P.area_rng[a][1] = p->area_rng[a][1]; }
+  double* iou_ws = (double*)workspace;
+  uint8_t* gtm_ws = (uint8_t*)workspace + smb::align_up((size_t)n_gt * max_det * sizeof(double), 256);
+  const size_t smem = match2_smem_bytes(det_cap, K, max_det, p->use_cats);
+  if (smem > 48 * 1024)
+    SMB_CUDA_OK(cudaFuncSetAttribute(match2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  match2_kernel<<<n_img, kThreads, smem, (cudaStream_t)stream>>>(imgs, dets, det_cap, det_planes, det_plane_words, gts, n_gt,
+                                                                gt_planes, gt_plane_words, gt_cat_off, K, metric, p->use_cats,
+                                                                P, out, n_out, npig, iou_ws, gtm_ws, status);
+  SMB_LAUNCH_OK("match2_kernel");
+  return SMB_OK;
+}
+
+extern "C" int smb_coco_accumulate_params2_dev(const smb_coco_out_t* rows, int64_t n_rows, const int32_t* cat_off, int K,
+                                               const int* npig, const smb_coco_params2_t* p, double* precision,
+                                               double* recall, double* scores, smb_stream_t stream) {
+  const int rc = smb_coco_params2_check(p);
+  if (rc != SMB_OK) return rc;
+  SMB_CHECK_ARG(n_rows >= 0 && K >= 1 && K <= SMB_COCO_MAX_CATS,
+                "smb_coco_accumulate_params2_dev: bad sizes (n_rows %lld, K %d)", (long long)n_rows, K);
+  SMB_CHECK_ARG(cat_off && npig && precision && recall && scores && (rows || n_rows == 0),
+                "smb_coco_accumulate_params2_dev: null pointer");
   AccParams P;
   P.A = p->A;
   P.M = p->M;

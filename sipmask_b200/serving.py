@@ -1080,14 +1080,19 @@ class CocoEvalRunner(StreamRunner):
     evaluate() accumulates and summarizes every image submitted so far and returns MM's evaluate() dict plus the raw
     stats and arrays.  result(ticket) still returns each record, so the result json can be written as well.
       gt      : cocoeval.CocoGroundTruth; cat_ids: COCO category id per 0-based label (as coco.coco_json takes it)
-      metrics : 'bbox' and / or 'segm'
-      params  : cocoeval.CocoParams (None: COCOeval's default Params)
+      metrics : 'bbox', 'segm' and / or 'proposal' (MM's class-agnostic AR@100 / 300 / 1000 of the boxes and box scores,
+                matched on the slot's stream like the others; not on SipMask-benchmark checkpoints)
+      params  : cocoeval.CocoParams or CocoParams2 for 'bbox' / 'segm' (None: COCOeval's default Params), e.g. a
+                cat_ids subset
+      proposal_nums: the maxDets of 'proposal' (a record holds at most max_per_img detections, as the bbox json does)
       analyze : also run coco_error_analysis.py's matches after every batch; evaluate() then returns its arrays under
                 'analysis' (cocoeval.CocoEvaluator)
     Every other argument is StreamRunner's; SipMask-VIS (vis=True) is not supported."""
 
-    def __init__(self, state_dict, gt, cat_ids, metrics=('bbox', 'segm'), params=None, analyze=False, **kw):
-        from .cocoeval import CocoEvaluator, CocoParams
+    def __init__(self, state_dict, gt, cat_ids, metrics=('bbox', 'segm'), params=None, analyze=False,
+                 proposal_nums=(100, 300, 1000), **kw):
+        from .cocoeval import CocoEvaluator, CocoParams, check_metrics
+        check_metrics(metrics)                            # names raise before the engines are built
         if kw.get('vis'):
             raise ValueError('CocoEvalRunner: YouTube-VIS evaluation (vis=True) is not supported')
         if params is not None and not isinstance(params, CocoParams):
@@ -1096,7 +1101,7 @@ class CocoEvalRunner(StreamRunner):
             gt.supercategory_index()                      # raises before the engines are built
         super(CocoEvalRunner, self).__init__(state_dict, **kw)
         self.evaluator = CocoEvaluator(gt, cat_ids, metrics=metrics, benchmark=self.benchmark, device=self.dev,
-                                       params=params, analyze=analyze)
+                                       params=params, analyze=analyze, proposal_nums=proposal_nums)
         torch.cuda.current_stream(self.dev).synchronize()   # the evaluator's zeroed state, before the slots use it
         self._eval_rows = {}                # ticket -> (image id, its staged ground truth) until its batch is evaluated
         self._submitted = set()
