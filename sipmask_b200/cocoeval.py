@@ -434,6 +434,21 @@ def summarize(precision, recall, area_rng_lbl=AREA_RNG_LBL, max_dets=MAX_DETS, i
     return stats
 
 
+def classwise_table(precision, names):
+    """Per-category AP of an accumulated precision array [T, R, K, A, M] (as CocoDataset.evaluate(classwise=True) of
+    later mmdetection computes it): for category k, the mean of precision[:, :, k, 0, -1] (area range 'all', the last
+    maxDet) over its values > -1, nan when there are none.  Returns [(name, ap)] in the order of K."""
+    precision = np.asarray(precision)
+    if precision.shape[2] != len(names):
+        raise ValueError('classwise: %d names for %d categories' % (len(names), precision.shape[2]))
+    out = []
+    for k, name in enumerate(names):
+        p = precision[:, :, k, 0, -1]
+        p = p[p > -1]
+        out.append((name, float(np.mean(p)) if p.size else float('nan')))
+    return out
+
+
 def mm_results(metric, stats):
     """CocoDataset.evaluate's entries of one metric: rounded stats[:6] and the copypaste string."""
     out = {}
@@ -876,12 +891,83 @@ class CocoEvaluator:
         v = self.views[metric]
         return accumulate(self.rows[metric], self.npig[metric], v.K_acc, self.dev, v.params)
 
-    def evaluate(self):
+    # ---- state across processes
+    def state(self):
+        """This evaluator's device state as a flat dict of 1-D tensors on its device, for merge() in another evaluator
+        of the same settings (dist.gather_eval_state carries it between ranks): 'image_ids' (int64), 'status' and
+        'raster_status', and per metric m 'rows/m' (the OUT_DTYPE rows, uint8), 'npig/m', 'n_results/m' and, when
+        analyzing, 'rows_c/m', 'rows_so/m' and 'npig_ana/m'."""
+        def cat(parts):
+            return torch.cat(parts) if parts else torch.zeros(0, dtype=torch.uint8, device=self.dev)
+        st = {'image_ids': torch.tensor(self.image_ids, dtype=torch.int64).to(self.dev),
+              'status': self.status.clone(), 'raster_status': self.raster_status.clone()}
+        for m in self.metrics:
+            st['rows/' + m] = cat(self.rows[m])
+            st['npig/' + m] = self.npig[m].clone()
+            st['n_results/' + m] = self.n_results[m].reshape(1).clone()
+            if self.analyze and m != 'proposal':
+                st['rows_c/' + m] = cat(self.rows_c[m])
+                st['rows_so/' + m] = cat(self.rows_so[m])
+                st['npig_ana/' + m] = self.npig_ana[m].clone()
+        return st
+
+    def merge(self, states):
+        """Add other evaluators' state() (same ground truth, cat_ids, metrics, Params and analyze) to this one: their
+        rows are appended, npig and n_results summed, status bits OR-ed.  evaluate() then gives what one evaluator of
+        all their images gives (accumulate orders the rows itself).  Raises ValueError for a state of other settings
+        and for an image id evaluated here or in two states, before anything is merged."""
+        states = list(states)
+        want = set(self.state_keys())
+        seen = set(self._seen)
+        ids = []
+        for st in states:
+            if set(st) != want:
+                raise ValueError('merge: a state of an evaluator with other metrics / analyze settings')
+            for m in self.metrics:
+                if st['npig/' + m].numel() != self.npig[m].numel():
+                    raise ValueError('merge: a state of an evaluator with another ground truth or Params (%s)' % m)
+            for i in st['image_ids'].cpu().tolist():
+                if i in seen:
+                    raise ValueError('merge: image id %d is evaluated twice (in two states, or here and in a state)' % i)
+                if i not in self.gt.hw:
+                    raise ValueError('merge: image id %d is not in the ground truth' % i)
+                seen.add(i)
+                ids.append(i)
+        for st in states:
+            self.status |= st['status'].to(self.dev)
+            self.raster_status |= st['raster_status'].to(self.dev)
+            for m in self.metrics:
+                self.rows[m].append(st['rows/' + m].to(self.dev))
+                self.npig[m] += st['npig/' + m].to(self.dev)
+                self.n_results[m] += st['n_results/' + m].to(self.dev).reshape(())
+                if self.analyze and m != 'proposal':
+                    self.rows_c[m].append(st['rows_c/' + m].to(self.dev))
+                    self.rows_so[m].append(st['rows_so/' + m].to(self.dev))
+                    self.npig_ana[m] += st['npig_ana/' + m].to(self.dev)
+        self.image_ids += ids
+        self._seen.update(ids)
+
+    def state_keys(self):
+        """The keys of state(), in a fixed order."""
+        keys = ['image_ids', 'status', 'raster_status']
+        for m in self.metrics:
+            keys += [s + m for s in ('rows/', 'npig/', 'n_results/')]
+            if self.analyze and m != 'proposal':
+                keys += [s + m for s in ('rows_c/', 'rows_so/', 'npig_ana/')]
+        return keys
+
+    def evaluate(self, classwise=False):
         """Accumulate and summarize every metric.  Returns 'arrays' ({metric: {'precision', 'recall', 'scores'}}) with
         COCOeval's eval arrays in the Params' shapes (K along CocoParams.cat_axis) and, where COCOeval.summarize runs on
         the Params (three maxDets and the labels all / small / medium / large), MM's dict (bbox_mAP, ...,
         segm_mAP_copypaste; AR@100, ..., AR_l@1000 for 'proposal') and 'stats'.  With analyze=True, also 'analysis'
-        ({metric: ps}, see analysis_arrays)."""
+        ({metric: ps}, see analysis_arrays).  classwise=True adds 'classwise' ({metric: classwise_table} for 'bbox' /
+        'segm': per-category AP with the ground truth's category names); it needs per-category arrays (useCats = 1)."""
+        if classwise:
+            for m in self.metrics:
+                p = self.views[m].params
+                if m != 'proposal' and p is not None and not p.use_cats:
+                    raise ValueError('classwise: %s is evaluated class-agnostically (useCats = 0)' % m)
         with torch.cuda.device(self.dev):
             status = int(self.status.item())
             if status & LABEL_RANGE:
@@ -911,6 +997,9 @@ class CocoEvaluator:
             out['arrays'] = arrays
             if self.analyze:
                 out['analysis'] = {m: self._analysis(m) for m in self.metrics if m != 'proposal'}
+            if classwise:
+                out['classwise'] = {m: classwise_table(arrays[m]['precision'], self._gviews[self.views[m].gv].names)
+                                    for m in self.metrics if m != 'proposal'}
             return out
 
     def _analysis(self, m):
@@ -920,24 +1009,26 @@ class CocoEvaluator:
 
 
 def evaluate_json(gt, cat_ids, bbox_json=None, segm_json=None, img_ids=None, chunk=64, device=None, params=None,
-                  proposal=False, proposal_nums=PROPOSAL_NUMS):
+                  proposal=False, proposal_nums=PROPOSAL_NUMS, classwise=False):
     """COCOeval of result lists (coco.coco_json output or a loaded results file) against `gt` on the device: the same
     kernels as CocoEvaluator, with the detections' RLE strings parsed to run lengths on the host and rasterized on the
     device.  img_ids: the evaluated images
     (p.imgIds; default every ground-truth image).  As in pycocotools, a result whose image is not in the ground truth
     raises (loadRes), and results of ground-truth images outside img_ids are not evaluated (_prepare).  params:
     CocoParams (None: the default Params).  proposal: also MM's 'proposal' metric of bbox_json (useCats = 0, maxDets =
-    proposal_nums).  Returns CocoEvaluator.evaluate()'s dict for the metrics given."""
+    proposal_nums).  classwise: also the per-category AP tables (CocoEvaluator.evaluate).  Returns
+    CocoEvaluator.evaluate()'s dict for the metrics given."""
     metrics = [m for m, j in (('bbox', bbox_json), ('segm', segm_json)) if j is not None]
     if proposal:
         if bbox_json is None:
             raise ValueError("evaluate_json: 'proposal' evaluates the bbox results; bbox_json is None")
         metrics.append('proposal')
-    return _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, False, metrics, proposal_nums)
+    return _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, False, metrics, proposal_nums,
+                     classwise)
 
 
 def _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params, analyze, metrics,
-              proposal_nums=PROPOSAL_NUMS):
+              proposal_nums=PROPOSAL_NUMS, classwise=False):
     ev = CocoEvaluator(gt, cat_ids, metrics=metrics, device=device, params=params, analyze=analyze,
                        proposal_nums=proposal_nums)
     ids = ev._claim(gt.img_ids if img_ids is None else sorted(set(int(i) for i in img_ids)))
@@ -958,4 +1049,4 @@ def _run_json(gt, cat_ids, bbox_json, segm_json, img_ids, chunk, device, params,
         ev.n_results[m] += len(res)                   # loadRes fails on an empty list
     ev.image_ids = list(ids)
     ev._seen.update(ids)
-    return ev.evaluate()
+    return ev.evaluate(classwise)

@@ -118,3 +118,46 @@ def track_gathered(gathered, n_frames, tracker, first_frames=(0,)):
         k = int(rec[:, 6].sum())
         ids.append(tracker.step(rec[:k, :5], rec[:k, 5].astype('int64'), rec[:k, 7:], f in first_frames))
     return ids
+
+
+def gather_parts(parts):
+    """Variable-size byte buffers of every rank, in two collectives: an all-gather of the sizes (one int64 per part),
+    then one of the parts concatenated and padded to the largest rank's total (apis/test.py's collect_results_gpu does
+    the same with one pickled buffer).  parts: a list of 1-D uint8 tensors on this rank's device (the same number on
+    every rank).  Returns, per rank in rank order, its list of parts (views of the gathered buffer)."""
+    dev = parts[0].device if parts else torch.device('cpu')
+    sizes = torch.tensor([p.numel() for p in parts], dtype=torch.int64, device=dev)
+    world = dist.get_world_size() if dist.is_initialized() else 1
+    if world == 1:
+        return [list(parts)]
+    all_sizes = [torch.empty_like(sizes) for _ in range(world)]
+    dist.all_gather(all_sizes, sizes)
+    totals = [int(s.sum()) for s in all_sizes]
+    buf = torch.zeros(max(totals + [1]), dtype=torch.uint8, device=dev)
+    if parts:
+        flat = torch.cat(parts)
+        buf[:flat.numel()].copy_(flat)
+    bufs = [torch.empty_like(buf) for _ in range(world)]
+    dist.all_gather(bufs, buf)
+    out = []
+    for b, s in zip(bufs, all_sizes):
+        offs = [0] + torch.cumsum(s, 0).tolist()
+        out.append([b[offs[i]:offs[i + 1]] for i in range(len(parts))])
+    return out
+
+
+def gather_bytes(data, device):
+    """Every rank's `data` (bytes) through gather_parts (staged on `device`: NCCL moves device memory).  Returns the list
+    of bytes in rank order."""
+    t = torch.frombuffer(bytearray(data), dtype=torch.uint8) if len(data) else torch.zeros(0, dtype=torch.uint8)
+    return [p[0].cpu().numpy().tobytes() for p in gather_parts([t.to(device)])]
+
+
+def gather_eval_state(evaluator):
+    """Every rank's cocoeval.CocoEvaluator.state(), in rank order, on every rank: the state's tensors as bytes through
+    gather_parts (one all-gather of the sizes, one of the padded bytes), read back with the local state's dtypes.  Call
+    it once, after the last image; rank 0 then merges the others' states (CocoEvaluator.merge) and evaluates."""
+    local = evaluator.state()
+    keys = evaluator.state_keys()
+    parts = [local[k].contiguous().view(-1).view(torch.uint8) for k in keys]
+    return [{k: p.clone().view(local[k].dtype) for k, p in zip(keys, ps)} for ps in gather_parts(parts)]

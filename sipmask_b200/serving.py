@@ -1133,11 +1133,16 @@ class CocoEvalRunner(StreamRunner):
         ids, gts = zip(*[self._eval_rows.pop(m['ticket']) for m in images])
         self.evaluator.add_records(rec, eng.geom, list(ids), [m['ori_shape'] for m in images], gts=list(gts))
 
-    def evaluate(self):
-        """Dispatch the open batch, wait for every slot's evaluation and return CocoEvaluator.evaluate()'s dict."""
+    def finish(self):
+        """Dispatch the open batch and make the current stream wait for every slot's evaluation: the evaluator then holds
+        every image submitted (its state() can be gathered across ranks)."""
         self.flush()
         self.slots.join(*self.slots.streams)
-        return self.evaluator.evaluate()
+
+    def evaluate(self, classwise=False):
+        """finish() and return CocoEvaluator.evaluate(classwise)'s dict."""
+        self.finish()
+        return self.evaluator.evaluate(classwise)
 
 
 class VideoEvalRunner(VideoRunner):

@@ -130,6 +130,41 @@ def detector_state_dict(depth=50, stacked_convs=4, gn=True, num_classes=81, resc
     return sd
 
 
+def detector_keys(depth=50, stacked_convs=4, gn=True, rescoring_flag=False, backbone_dcn=False, track=False,
+                  num_levels=5):
+    """The parameter / buffer names of an MM (track=True: SipMask-VIS) detector's state dict: the keys
+    backbone_state_dict + neck_state_dict + head_state_dict write, without making the tensors."""
+    bn = ('weight', 'bias', 'running_mean', 'running_var', 'num_batches_tracked')
+    keys = ['backbone.conv1.weight'] + ['backbone.bn1.' + s for s in bn]
+    for i, nb in enumerate(ARCH[depth]):
+        for j in range(nb):
+            p = 'backbone.layer%d.%d.' % (i + 1, j)
+            keys += [p + 'conv1.weight', p + 'conv2.weight', p + 'conv3.weight']
+            if backbone_dcn and i > 0 and j % 3 == 0:
+                keys += [p + 'conv2.conv_offset.weight', p + 'conv2.conv_offset.bias']
+            keys += [p + 'bn%d.%s' % (c, s) for c in (1, 2, 3) for s in bn]
+            if j == 0:
+                keys += [p + 'downsample.0.weight'] + [p + 'downsample.1.' + s for s in bn]
+    keys += ['neck.lateral_convs.%d.conv.%s' % (i, s) for i in range(3) for s in ('weight', 'bias')]
+    keys += ['neck.fpn_convs.%d.conv.%s' % (i, s) for i in range(5) for s in ('weight', 'bias')]
+    h = 'bbox_head.'
+    conv = ('conv.weight', 'gn.weight', 'gn.bias') if gn else ('conv.weight', 'conv.bias')
+    towers = [('cls_convs', stacked_convs - 1), ('reg_convs', stacked_convs)]
+    towers += [('track_convs', stacked_convs - 1)] if track else []
+    for name, n in towers:
+        keys += ['%s%s.%d.%s' % (h, name, i, c) for i in range(n) for c in conv]
+    for m in ('fcos_cls', 'fcos_reg', 'fcos_centerness', 'sip_cof', 'sip_mask_lat', 'sip_mask_lat0', 'feat_align.norm'):
+        keys += [h + m + '.weight', h + m + '.bias']
+    keys += [h + 'feat_align.conv_offset.weight', h + 'feat_align.conv_adaption.weight']
+    keys += [h + 'scales.%d.scale' % i for i in range(num_levels)]
+    if rescoring_flag:
+        keys += ['%sconvs_scoring.%d.conv.%s' % (h, i, s) for i in range(6) for s in ('weight', 'bias')]
+        keys += [h + 'mask_scoring.weight', h + 'mask_scoring.bias']
+    if track:
+        keys += [h + 'sipmask_track.weight', h + 'sipmask_track.bias']
+    return keys
+
+
 def synthetic_image(h=800, w=1344, batch=1, seed=0):
     """uniform [0,255) BGR minus mean (SURVEY.md §8d); NCHW fp32."""
     g = torch.Generator().manual_seed(seed)
