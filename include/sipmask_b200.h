@@ -744,9 +744,22 @@ int smb_conv_plan_set_max_ctas(smb_conv_plan_t* plan, int max_ctas);
  * L2 -> SM per FLOP), large values favour occupancy of a single stream.  Returns the previous value. */
 int smb_conv_set_min_tiles(int min_tiles);
 /* out = relu?( (acc + bias) * alpha + residual ); alpha carries the per-level `Scale` of fcos_reg
- * (sipmask_head.py:261, ops/scale.py:12-15). */
+ * (sipmask_head.py:261, ops/scale.py:12-15).  The residual must be 4-byte aligned (SMB_EINVAL without a launch). */
 int smb_conv_run(const smb_conv_plan_t* plan, const float* bias, const void* residual, void* gn_stats,
                  float alpha, smb_stream_t stream);
+/* What the planner chose for a plan, so that tests can state which kernel path a shape reaches.  Per level: the
+ * BH x BW = 128-pixel output patch and the tile counts; per plan: the N tile (256 / 128 / 64) and the number of N tiles,
+ * the operand ring's stages, whether fp16 outputs go through the shared-memory / TMA epilogue (as decided at creation:
+ * a same-shape residual that is not 16-byte aligned still takes the register epilogue at run time), the persistent grid
+ * and the dynamic shared memory of a launch. */
+#define SMB_CONV_MAX_LEVELS 5
+typedef struct {
+  int num_levels, tiles_m;
+  int n_tile, n_tiles_n, stages, epi_tma, grid, smem_bytes;
+  int H_out[SMB_CONV_MAX_LEVELS], W_out[SMB_CONV_MAX_LEVELS];
+  int BH[SMB_CONV_MAX_LEVELS], BW[SMB_CONV_MAX_LEVELS], tiles_x[SMB_CONV_MAX_LEVELS], tiles_y[SMB_CONV_MAX_LEVELS];
+} smb_conv_plan_info_t;
+int smb_conv_plan_info(const smb_conv_plan_t* plan, smb_conv_plan_info_t* info);
 
 /* ------------------------------------------------------------------ elementwise / gather kernels (NHWC fp16) */
 /* GroupNorm(32 groups, eps) + ReLU applied in place from precomputed per-(image,group) sum/sumsq

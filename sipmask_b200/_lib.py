@@ -34,6 +34,16 @@ class ConvLevel(ctypes.Structure):
                 ('res_w', ctypes.c_int)]
 
 
+CONV_MAX_LEVELS = 5                  # SMB_CONV_MAX_LEVELS
+
+
+class ConvPlanInfo(ctypes.Structure):
+    """smb_conv_plan_info_t: what the planner chose for a convolution plan (include/sipmask_b200.h)."""
+    _fields_ = [(n, ctypes.c_int) for n in ('num_levels', 'tiles_m', 'n_tile', 'n_tiles_n', 'stages', 'epi_tma', 'grid',
+                                            'smem_bytes')] + \
+        [(n, ctypes.c_int * CONV_MAX_LEVELS) for n in ('H_out', 'W_out', 'BH', 'BW', 'tiles_x', 'tiles_y')]
+
+
 class ImgGeom(ctypes.Structure):
     """smb_img_geom_t: one image's post-processing geometry (include/sipmask_b200.h)."""
     _fields_ = [('img_h', ctypes.c_int), ('img_w', ctypes.c_int), ('scale', ctypes.c_float * 4),
@@ -78,7 +88,7 @@ SYMBOLS = [
     'smb_multiclass_soft_nms', 'smb_pair_decode_slots', 'smb_pair_decode_workspace_bytes',
     'smb_pair_decode_topk', 'smb_ml_nms_workspace_bytes', 'smb_ml_nms_topk', 'smb_fast_nms_workspace_bytes', 'smb_fast_nms',
     'smb_gather_rows_f32', 'smb_gather_det_inputs', 'smb_gather_track_feats', 'smb_track_step', 'smb_conv_plan_create', 'smb_conv_plan_create_multi', 'smb_conv_plan_destroy', 'smb_conv_plan_set_max_ctas', 'smb_conv_set_min_tiles',
-    'smb_conv_run',
+    'smb_conv_run', 'smb_conv_plan_info',
     'smb_groupnorm_relu_apply', 'smb_groupnorm_stats', 'smb_deform_im2col', 'smb_offset_conv1x1', 'smb_groupnorm_relu_apply_multi', 'smb_offset_conv1x1_multi', 'smb_offset_conv1x1_relu_multi', 'smb_deform_im2col_multi', 'smb_maxpool3x3s2',
     'smb_upsample_bilinear', 'smb_stem_plan_create_s2d', 'smb_image_to_s2d16', 'smb_preprocess_u8_s2d',
     'smb_mask_assemble_dev', 'smb_mask_assemble_pack_dev', 'smb_decode_topk_dev', 'smb_pair_decode_topk_dev',

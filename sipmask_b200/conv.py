@@ -103,6 +103,17 @@ class ConvPlan(object):
         L.check(L.lib().smb_conv_plan_set_max_ctas(self.handle, int(n)), 'smb_conv_plan_set_max_ctas')
         return self
 
+    def info(self):
+        """What the planner chose (smb_conv_plan_info): dict with num_levels, tiles_m, n_tile, n_tiles_n, stages, epi_tma
+        (as decided at creation), grid, smem_bytes, and per level a list of dicts H_out, W_out, BH, BW, tiles_x, tiles_y."""
+        i = L.ConvPlanInfo()
+        L.check(L.lib().smb_conv_plan_info(self.handle, ctypes.byref(i)), 'smb_conv_plan_info')
+        keys = ('H_out', 'W_out', 'BH', 'BW', 'tiles_x', 'tiles_y')
+        res = {n: int(getattr(i, n)) for n in ('num_levels', 'tiles_m', 'n_tile', 'n_tiles_n', 'stages', 'epi_tma', 'grid',
+                                               'smem_bytes')}
+        res['levels'] = [{k: int(getattr(i, k)[l]) for k in keys} for l in range(i.num_levels)]
+        return res
+
     def run(self, stream=None):
         if self.dev.index != torch.cuda.current_device():        # launch on the plan's device and ITS current stream
             with torch.cuda.device(self.dev):

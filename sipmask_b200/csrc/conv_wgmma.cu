@@ -909,7 +909,7 @@ extern "C" int smb_conv_plan_create_multi(const smb_conv_desc_t* d, int num_leve
     LevelDesc& L = p.lv[l];
     const int H = lv.H, W = lv.W;
     if (!lv.in || !lv.out || H <= 0 || W <= 0 || ((uintptr_t)lv.in % 16) || ((uintptr_t)lv.out % 16) ||
-        (d->has_residual && !lv.residual) || (d->gn_stats && !lv.gn_stats)) {
+        (d->has_residual && (!lv.residual || (uintptr_t)lv.residual % 4)) || (d->gn_stats && !lv.gn_stats)) {
       set_error("smb_conv_plan_create: level %d has a null / misaligned pointer or empty shape", l);
       rc = SMB_EINVAL;
       break;
@@ -955,6 +955,11 @@ extern "C" int smb_conv_plan_create_multi(const smb_conv_desc_t* d, int num_leve
           p.tap_map[t] = py * 2 + pxp;
           p.tap_dy[t] = (oy - py) / 2;                           // exact: oy - py is even
           p.tap_dx[t] = (ox - pxp) / 2;
+          // A parity with no rows (H == 1, py == 1) or no columns (W == 1, pxp == 1) is encoded with one so that its map
+          // is valid, but that row / column is the next image's or lies past the tensor.  Its taps read at offset 1
+          // instead: every box row / column is then at a coordinate >= 1, past the map's single one, so TMA fills zeros.
+          if ((levels[0].H - py + 1) / 2 == 0) p.tap_dy[t] = 1;
+          if ((levels[0].W - pxp + 1) / 2 == 0) p.tap_dx[t] = 1;
         }
       }
     rc = finish_plan(pl, d->Cout, k * k * d->Cin, weight);
@@ -1016,6 +1021,23 @@ extern "C" int smb_stem_plan_create_s2d(int N, int H, int W, const void* img_s2d
 
 extern "C" void smb_conv_plan_destroy(smb_conv_plan_t* plan) { delete plan; }
 
+static_assert(SMB_CONV_MAX_LEVELS == kMaxLevels, "smb_conv_plan_info_t holds every level of a plan");
+
+extern "C" int smb_conv_plan_info(const smb_conv_plan_t* plan, smb_conv_plan_info_t* info) {
+  SMB_CHECK_ARG(plan && info, "smb_conv_plan_info: null pointer");
+  const ConvParams& p = plan->p;
+  memset(info, 0, sizeof(*info));
+  info->num_levels = p.num_levels; info->tiles_m = p.tiles_m;
+  info->n_tile = p.n_tile; info->n_tiles_n = p.n_tiles_n; info->stages = p.stages; info->epi_tma = p.epi_tma;
+  info->grid = plan->grid; info->smem_bytes = (int)plan->smem_bytes;
+  for (int l = 0; l < p.num_levels; ++l) {
+    const LevelDesc& L = p.lv[l];
+    info->H_out[l] = L.H_out; info->W_out[l] = L.W_out;
+    info->BH[l] = L.BH; info->BW[l] = L.BW; info->tiles_x[l] = L.tiles_x; info->tiles_y[l] = L.tiles_y;
+  }
+  return SMB_OK;
+}
+
 // Cap the persistent grid (e.g. to half the SMs) so that two independent convolutions captured on different streams
 // can run side by side and fill each other's partial waves.
 extern "C" int smb_conv_plan_set_max_ctas(smb_conv_plan_t* plan, int max_ctas) {
@@ -1047,6 +1069,8 @@ extern "C" int smb_conv_run(const smb_conv_plan_t* plan, const float* bias, cons
   if (p.num_levels == 1) {
     if (plan->has_residual) {
       SMB_CHECK_ARG(residual, "smb_conv_run: plan expects a residual");
+      // the register epilogue reads the residual as __half2 pairs of even channels
+      SMB_CHECK_ARG((uintptr_t)residual % 4 == 0, "smb_conv_run: residual must be 4-byte aligned");
       p.lv[0].residual = (const __half*)residual;
       // the residual's TMA map goes into this launch's parameters (a captured graph keeps them by value); a residual
       // TMA cannot address (not 16-byte aligned) takes the register epilogue

@@ -22,6 +22,30 @@ def test_library_exports_every_declared_symbol():
     assert lib.smb_version() >= 100
 
 
+def test_conv_plan_info_layout_and_null_arguments():
+    """ConvPlanInfo lays out smb_conv_plan_info_t's fields in the header's order, and smb_conv_plan_info refuses null
+    pointers (no device needed)."""
+    from sipmask_b200 import _lib, build
+    header = open(os.path.join(ROOT, 'include', 'sipmask_b200.h')).read()
+    body = re.search(r'typedef struct \{([^}]*)\} smb_conv_plan_info_t;', header).group(1)
+    fields = []
+    for decl in body.split(';'):
+        decl = decl.strip()
+        if decl:
+            assert decl.startswith('int '), decl
+            fields += [re.match(r'(\w+)', f.strip()).group(1) for f in decl[4:].split(',')]
+    assert [f[0] for f in _lib.ConvPlanInfo._fields_] == fields
+    n = int(re.search(r'#define SMB_CONV_MAX_LEVELS (\d+)', header).group(1))
+    assert _lib.CONV_MAX_LEVELS == n
+    arrays = [f for f in fields if '%s[SMB_CONV_MAX_LEVELS]' % f in body]
+    assert ctypes.sizeof(_lib.ConvPlanInfo) == 4 * (len(fields) - len(arrays) + n * len(arrays))
+    lib = ctypes.CDLL(build.build())
+    lib.smb_last_error.restype = ctypes.c_char_p
+    info = _lib.ConvPlanInfo()
+    assert lib.smb_conv_plan_info(None, ctypes.byref(info)) == -1
+    assert b'smb_conv_plan_info' in lib.smb_last_error()
+
+
 def test_ops_fail_loudly_without_cuda():
     import torch
     from sipmask_b200 import ops, _lib
