@@ -855,6 +855,48 @@ int smb_preprocess_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out_s2d16,
  * N*(H/2+3)*(W/2+4)*32 bytes. */
 int smb_preprocess_pil_u8_s2d_dev(const smb_raw_src_t* rows, int N, void* out_s2d16, int H, int W, smb_stream_t stream);
 
+/* ------------------------------------------------------------------ training-side operators (train_ops.cu)
+ * DeformConv backward, 3x3 / stride 1 / pad 1 / dilation 1 / groups 1, channel-last like smb_deform_im2col.  Replaces
+ * deform_conv_backward_input_cuda and deform_conv_backward_parameters_cuda (ops/dcn/src/deform_conv_cuda.cpp:262-470).
+ *
+ * smb_deform_grad_scale: grad_out [N, C, H, W] fp32 (NCHW, as autograd passes it) -> out_f16 [N, H, W, C] = s * grad_out,
+ * with s = 2^k chosen on the device so that amax |grad_out| lands in [2^14, 2^15) (s = 1 when amax is 0 or not finite),
+ * no host synchronisation.  scale (device, 2 floats) receives {s, 1 / s}.  C % 8 == 0.  One cooperative launch;
+ * workspace: smb_deform_grad_scale_workspace_bytes(). */
+size_t smb_deform_grad_scale_workspace_bytes(void);
+int smb_deform_grad_scale(const float* grad_out, int n_img, int C, int H, int W, void* out_f16, float* scale,
+                          void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
+/* smb_deform_col2im: deformable_col2im_coord and deformable_col2im (ops/dcn/src/deform_conv_cuda_kernel.cu:337-465) in one
+ * pass over grad_col [N, H, W, 9 * C] fp32 (column k = tap * C + c, holding s * the column gradient):
+ *   grad_offset [N, H, W, dg * 18] fp32 (channel g * 18 + 2 * tap + {0: h, 1: w}), every element written, each a
+ *     fixed-order sum over the group's C / dg channels of get_coordinate_weight (kernel.cu:145-188) x grad_col / s;
+ *   grad_input [N, H, W, C] fp32, ACCUMULATED (zero it first) with float atomics: get_gradient_weight (kernel.cu:117-143)
+ *     x grad_col / s.
+ * Either output may be null (not both).  x [N, H, W, C] fp16, offset [N, H, W, >= dg * 18] fp32 with pitch off_pitch,
+ * scale = smb_deform_grad_scale's {s, 1 / s}.  C % 8 == 0, C <= 1024, (C / dg) % 8 == 0. */
+int smb_deform_col2im(const float* grad_col, const void* x, const float* offset, int off_pitch, const float* scale,
+                      float* grad_input, float* grad_offset, int n_img, int H, int W, int C, int deformable_groups,
+                      smb_stream_t stream);
+
+/* smb_deform_weight_grad: grad_weight [Cout, K] fp32 = sum_p grad_f16[p, co] * col[p, k] / s over P pixels, the
+ * columns' GEMM of deform_conv_backward_parameters_cuda (deform_conv_cuda.cpp:376-470; col recomputed by
+ * smb_deform_im2col, K = 9 * C).  grad_f16 [P, Cout] fp16 (smb_deform_grad_scale's output), col [P, K] fp16.  wgmma with
+ * MN-major operands, split over pixels; the splits are summed in a fixed order, so the result is the same bits on every
+ * run.  Cout % 8 == 0, K % 8 == 0, 16-byte aligned pointers; workspace: smb_deform_weight_grad_workspace_bytes. */
+size_t smb_deform_weight_grad_workspace_bytes(int Cout, int K, long long P);
+int smb_deform_weight_grad(const void* grad_f16, const void* col, long long P, int Cout, int K, const float* scale,
+                           float* grad_weight, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
+/* Sigmoid focal loss (ops/sigmoid_focal_loss/src/sigmoid_focal_loss_cuda.cu:23-100, SigmoidFocalLoss_forward_cuda /
+ * _backward_cuda): logits [N, C] fp32, targets [N] int64 (1-based class, 0 = background, < 0 ignored), d_losses [N, C]
+ * fp32 -> losses / d_logits [N, C] fp32, every element written.  The reference's expressions operation by operation,
+ * so the results are the reference kernel's bits.  N = 0 launches nothing. */
+int smb_sigmoid_focal_loss_forward(const float* logits, const int64_t* targets, int N, int num_classes, float gamma,
+                                   float alpha, float* losses, smb_stream_t stream);
+int smb_sigmoid_focal_loss_backward(const float* logits, const int64_t* targets, const float* d_losses, int N,
+                                    int num_classes, float gamma, float alpha, float* d_logits, smb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

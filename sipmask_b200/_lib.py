@@ -103,6 +103,9 @@ SYMBOLS = [
     'smb_coco_match_params2_dev', 'smb_coco_accumulate_params2_dev',
     'smb_ytvis_overlap_dev', 'smb_ytvis_scatter_dev', 'smb_ytvis_match_workspace_bytes', 'smb_ytvis_match_dev',
     'smb_segm_raster_workspace_bytes', 'smb_segm_raster_dev', 'smb_render_dev',
+    'smb_deform_grad_scale_workspace_bytes', 'smb_deform_grad_scale', 'smb_deform_col2im',
+    'smb_deform_weight_grad_workspace_bytes', 'smb_deform_weight_grad', 'smb_sigmoid_focal_loss_forward',
+    'smb_sigmoid_focal_loss_backward',
 ]
 
 
@@ -120,7 +123,8 @@ def lib():
                   'smb_rle_encode_workspace_bytes', 'smb_track_assoc_workspace_bytes', 'smb_coco_match_workspace_bytes',
                   'smb_ytvis_match_workspace_bytes', 'smb_segm_raster_workspace_bytes',
                   'smb_coco_match_params_workspace_bytes', 'smb_coco_analysis_workspace_bytes',
-                  'smb_coco_match_params2_workspace_bytes'):
+                  'smb_coco_match_params2_workspace_bytes', 'smb_deform_grad_scale_workspace_bytes',
+                  'smb_deform_weight_grad_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

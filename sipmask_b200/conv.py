@@ -327,6 +327,47 @@ def deform_im2col(x, offset, dg, out=None):
 
 
 @L.device_guard
+def deform_grad_scale(grad_out):
+    """grad_out [N,C,H,W] fp32 contiguous -> (s * grad_out as [N,H,W,C] fp16, device {s, 1/s} fp32) with s a power of two
+    chosen on the device from amax |grad_out| (smb_deform_grad_scale)."""
+    N, C, H, W = grad_out.shape
+    out = torch.empty((N, H, W, C), dtype=torch.float16, device=grad_out.device)
+    scale = torch.empty(2, dtype=torch.float32, device=grad_out.device)
+    ws = torch.empty(int(L.lib().smb_deform_grad_scale_workspace_bytes()), dtype=torch.uint8, device=grad_out.device)
+    L.check(L.lib().smb_deform_grad_scale(L.ptr(grad_out), N, C, H, W, L.ptr(out), L.ptr(scale), L.ptr(ws),
+                                          ctypes.c_size_t(ws.numel()), L.stream_ptr()), 'smb_deform_grad_scale')
+    return out, scale
+
+
+@L.device_guard
+def deform_col2im(grad_col, x, offset, dg, scale, grad_input=True, grad_offset=True):
+    """grad_col [N,H,W,9C] fp32 (s * the column gradient), x [N,H,W,C] fp16, offset [N,H,W,dg*18] fp32, scale {s, 1/s}
+    -> (grad_input [N,H,W,C] fp32 | None, grad_offset [N,H,W,dg*18] fp32 | None) (smb_deform_col2im)."""
+    N, H, W, C = x.shape
+    assert x.is_contiguous() and grad_col.is_contiguous() and offset.stride(3) == 1
+    gin = torch.zeros((N, H, W, C), dtype=torch.float32, device=x.device) if grad_input else None
+    goff = torch.empty((N, H, W, dg * 18), dtype=torch.float32, device=x.device) if grad_offset else None
+    L.check(L.lib().smb_deform_col2im(L.ptr(grad_col), L.ptr(x), L.ptr(offset), offset.stride(2), L.ptr(scale), L.ptr(gin),
+                                      L.ptr(goff), N, H, W, C, int(dg), L.stream_ptr()), 'smb_deform_col2im')
+    return gin, goff
+
+
+@L.device_guard
+def deform_weight_grad(grad_f16, col, scale):
+    """grad_f16 [N,H,W,Cout] fp16, col [N,H,W,K] fp16 -> dW [Cout, K] fp32 = sum over pixels / s (smb_deform_weight_grad)."""
+    cout, k = grad_f16.shape[-1], col.shape[-1]
+    P = grad_f16.numel() // cout
+    assert grad_f16.is_contiguous() and col.is_contiguous() and col.numel() == P * k
+    dw = torch.empty((cout, k), dtype=torch.float32, device=col.device)
+    ws = torch.empty(max(int(L.lib().smb_deform_weight_grad_workspace_bytes(cout, k, ctypes.c_longlong(P))), 16),
+                     dtype=torch.uint8, device=col.device)
+    L.check(L.lib().smb_deform_weight_grad(L.ptr(grad_f16), L.ptr(col), ctypes.c_longlong(P), cout, k, L.ptr(scale),
+                                           L.ptr(dw), L.ptr(ws), ctypes.c_size_t(ws.numel()), L.stream_ptr()),
+            'smb_deform_weight_grad')
+    return dw
+
+
+@L.device_guard
 def upsample_bilinear(x, factor, out=None, out_choff=0, relu=False):
     N, H, W, C = x.shape
     if out is None:

@@ -6,6 +6,8 @@ and `mmdet.core` entry points, backed by the C ABI (PyTorch tensors in, PyTorch 
   multiclass_nms_idx       <- MM/mmdet/core/post_processing/bbox_nms.py:79-146
   fast_nms                 <- MM/mmdet/models/anchor_heads/sipmask_head.py:868-910
   mask_assemble            <- MM/mmdet/models/anchor_heads/sipmask_head.py:609-627 (fused)
+  DeformConv(Pack) / deform_conv        <- MM/mmdet/ops/dcn/deform_conv.py:14-94,192-300 (with the backward)
+  SigmoidFocalLoss / sigmoid_focal_loss <- MM/mmdet/ops/sigmoid_focal_loss/sigmoid_focal_loss.py:8-52
 All tensors must be CUDA tensors on an sm_90 device; there is no CPU path.
 """
 import ctypes
@@ -13,6 +15,7 @@ import ctypes
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib as L
 
@@ -950,14 +953,228 @@ class DeformConv(nn.Module):
         key = (self.weight._version, self.weight.data_ptr(), x.device)
         if self._packed is None or self._packed[0] != key:
             self._packed = (key, C.pack_weight(self.weight, device=x.device)[0])
-        wk = self._packed[1]
-        with torch.cuda.device(x.device):
-            xh = x.permute(0, 2, 3, 1).contiguous().to(torch.float16)
-            off = offset.permute(0, 2, 3, 1).contiguous().float()
-            col = C.deform_im2col(xh, off, self.deformable_groups)
-            out = torch.empty((N, H, W, self.out_channels), dtype=torch.float16, device=x.device)
-            C.ConvPlan(col, wk, out, 1, 1).run()
-            y = out.permute(0, 3, 1, 2).to(x.dtype)
+        y = _deform_conv_forward(x, offset, self._packed[1], self.deformable_groups)
         if input_pad:
             y = y[:, :, :y.size(2) - pad_h, :y.size(3) - pad_w]
         return y.contiguous()
+
+
+def _channels_last(x, offset):
+    """x [N,C,H,W] -> fp16 [N,H,W,C]; offset [N,dg*18,H,W] -> fp32 [N,H,W,dg*18] (the layouts smb_deform_im2col reads)."""
+    return (x.permute(0, 2, 3, 1).contiguous().to(torch.float16), offset.permute(0, 2, 3, 1).contiguous().float())
+
+
+def _deform_conv_forward(x, offset, wk, dg):
+    """The DeformConv forward on an input at least as large as the kernel: `smb_deform_im2col` + the wgmma GEMM with the
+    packed weight wk [Cout, 9*C] fp16 -> y [N, Cout, H, W] in x.dtype (a permuted view)."""
+    from . import conv as C
+    N, _, H, W = x.shape
+    with torch.cuda.device(x.device):
+        xh, off = _channels_last(x, offset)
+        col = C.deform_im2col(xh, off, dg)
+        out = torch.empty((N, H, W, wk.shape[0]), dtype=torch.float16, device=x.device)
+        C.ConvPlan(col, wk, out, 1, 1).run()
+        return out.permute(0, 3, 1, 2).to(x.dtype)
+
+
+# ------------------------------------------------------------------------------ DeformConv with autograd (fine-tuning)
+def _check_deform_args(x, offset, weight, stride, padding, dilation, groups, dg):
+    """What the sm_90a forward and backward support; raises before anything is launched."""
+    if x.dtype not in (torch.float32, torch.float16) or offset.dtype not in (torch.float32, torch.float16) \
+            or weight.dtype != torch.float32:
+        raise L.SmbError('deform_conv: input / offset must be fp32 or fp16 and weight fp32 (got %s, %s, %s)'
+                         % (x.dtype, offset.dtype, weight.dtype))
+    pair = lambda v: tuple(v) if isinstance(v, (tuple, list)) else (v, v)       # noqa: E731
+    cout, cin = weight.shape[0], weight.shape[1]
+    if not (tuple(weight.shape[2:]) == (3, 3) and pair(stride) == (1, 1) and pair(padding) == (1, 1)
+            and pair(dilation) == (1, 1) and groups == 1):
+        raise NotImplementedError('sipmask_b200.ops.deform_conv: only 3x3 / stride 1 / padding 1 / dilation 1 / groups 1')
+    if x.size(1) != cin or cin % 64 or cout % 64 or cin % dg or (cin // dg) % 8 or cin > 1024:
+        raise NotImplementedError('sipmask_b200.ops.deform_conv: in_channels %% 64 (<= 1024), out_channels %% 64 and '
+                                  '(in_channels / deformable_groups) %% 8 must be 0 (got %d, %d, dg=%d)' % (cin, cout, dg))
+    N, _, H, W = x.shape
+    if tuple(offset.shape) != (N, dg * 18, H, W):
+        raise L.SmbError('deform_conv: offset shape %s does not match input %s (deform_conv_cuda.cpp:62-150)'
+                         % (tuple(offset.shape), tuple(x.shape)))
+    _need_cuda(x, offset, weight)
+
+
+class DeformConvFunction(torch.autograd.Function):
+    """mmdet.ops.dcn.DeformConvFunction (MM/mmdet/ops/dcn/deform_conv.py:14-94) on sm_90a, same arguments.
+
+    forward: the path of ops.DeformConv (smb_deform_im2col + the wgmma GEMM), bit for bit.
+    backward (deform_conv_cuda.cpp:262-470), for the inputs that need a gradient:
+      s * grad_out -> fp16 NHWC (smb_deform_grad_scale, s a power of two chosen on the device);
+      x or offset: grad_col = (s * grad_out) . W on the convolution GEMM (fp32 out), then smb_deform_col2im -> grad_offset
+        (deterministic) and grad_input (atomics), divided by s;
+      weight: the columns recomputed by smb_deform_im2col (as the reference does), dW by smb_deform_weight_grad (wgmma,
+        fixed-order split reduction: the same bits on every run), divided by s.
+    Only the SipMask geometry: 3x3 / stride 1 / padding 1 / dilation 1 / groups 1, in_channels and out_channels
+    multiples of 64."""
+
+    @staticmethod
+    def forward(ctx, input, offset, weight, stride=1, padding=0, dilation=1, groups=1, deformable_groups=1,
+                im2col_step=64):
+        from . import conv as C
+        if input is not None and input.dim() != 4:
+            raise ValueError('Expected 4D tensor as input, got {}D tensor instead.'.format(input.dim()))
+        cur_im2col_step = min(im2col_step, input.shape[0])
+        assert (input.shape[0] % cur_im2col_step) == 0, 'im2col step must divide batchsize'
+        _check_deform_args(input, offset, weight, stride, padding, dilation, groups, deformable_groups)
+        ctx.deformable_groups = deformable_groups
+        ctx.save_for_backward(input, offset, weight)
+        wk = C.pack_weight(weight, device=input.device)[0]
+        return _deform_conv_forward(input, offset, wk, deformable_groups).contiguous()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        from . import conv as C
+        x, offset, weight = ctx.saved_tensors
+        need_x, need_off, need_w = ctx.needs_input_grad[:3]
+        grad_input = grad_offset = grad_weight = None
+        _need_cuda(grad_output)
+        if need_x or need_off or need_w:
+            dg = ctx.deformable_groups
+            N, cin, H, W = x.shape
+            cout = weight.shape[0]
+            with torch.cuda.device(x.device):
+                g16, scale = C.deform_grad_scale(grad_output.float().contiguous())
+                xh, off = _channels_last(x, offset)
+                if need_x or need_off:
+                    wt = C.pack_weight(weight)[0].t().contiguous().to(x.device)     # W^T [9*C, Cout], K-major
+                    gcol = torch.empty((N, H, W, 9 * cin), dtype=torch.float32, device=x.device)
+                    C.ConvPlan(g16, wt, gcol, 1, 1).run()
+                    gin, goff = C.deform_col2im(gcol, xh, off, dg, scale, grad_input=need_x, grad_offset=need_off)
+                    if need_x:
+                        grad_input = gin.permute(0, 3, 1, 2).to(x.dtype).contiguous()
+                    if need_off:
+                        grad_offset = goff.permute(0, 3, 1, 2).to(offset.dtype).contiguous()
+                if need_w:
+                    col = C.deform_im2col(xh, off, dg)
+                    dw = C.deform_weight_grad(g16, col, scale)
+                    grad_weight = dw.view(cout, 3, 3, cin).permute(0, 3, 1, 2).contiguous()
+        return grad_input, grad_offset, grad_weight, None, None, None, None, None, None
+
+
+deform_conv = DeformConvFunction.apply
+
+
+class TrainableDeformConv(DeformConv):
+    """ops.DeformConv whose forward runs through `deform_conv`, so x, the offsets and `weight` get gradients (ops.DeformConv
+    itself runs under no_grad).  Inputs smaller than the kernel are zero-padded outside the Function and the output
+    cropped back, as MM/mmdet/ops/dcn/deform_conv.py:242-254 does."""
+
+    def forward(self, x, offset):
+        kh, kw = self.kernel_size
+        input_pad = x.size(2) < kh or x.size(3) < kw
+        if input_pad:
+            pad_h, pad_w = max(kh - x.size(2), 0), max(kw - x.size(3), 0)
+            x = torch.nn.functional.pad(x, (0, pad_w, 0, pad_h), 'constant', 0).contiguous()
+            offset = torch.nn.functional.pad(offset, (0, pad_w, 0, pad_h), 'constant', 0).contiguous()
+        out = deform_conv(x, offset, self.weight, self.stride, self.padding, self.dilation, self.groups,
+                          self.deformable_groups)
+        if input_pad:
+            out = out[:, :, :out.size(2) - pad_h, :out.size(3) - pad_w].contiguous()
+        return out
+
+
+class DeformConvPack(TrainableDeformConv):
+    """mmdet.ops.DeformConvPack (MM/mmdet/ops/dcn/deform_conv.py:258-300): the offsets come from `conv_offset`, an
+    nn.Conv2d with bias initialised to zero, so the state-dict keys (weight, conv_offset.weight, conv_offset.bias) are the
+    reference's and SipMask++ checkpoints load strictly.  Version-1 checkpoints' `<name>_offset.*` keys are renamed on load
+    as the reference does."""
+
+    _version = 2
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.conv_offset = nn.Conv2d(self.in_channels, self.deformable_groups * 2 * self.kernel_size[0] * self.kernel_size[1],
+                                     kernel_size=self.kernel_size, stride=self.stride, padding=self.padding, bias=True)
+        self.init_offset()
+
+    def init_offset(self):
+        self.conv_offset.weight.data.zero_()
+        self.conv_offset.bias.data.zero_()
+
+    def forward(self, x):
+        offset = self.conv_offset(x)
+        return deform_conv(x, offset, self.weight, self.stride, self.padding, self.dilation, self.groups,
+                           self.deformable_groups)
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
+        version = local_metadata.get('version', None)
+        if version is None or version < 2:
+            for k in ('weight', 'bias'):
+                if prefix + 'conv_offset.' + k not in state_dict and prefix[:-1] + '_offset.' + k in state_dict:
+                    state_dict[prefix + 'conv_offset.' + k] = state_dict.pop(prefix[:-1] + '_offset.' + k)
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                      error_msgs)
+
+
+# ----------------------------------------------------------------------------------------------- sigmoid focal loss
+def _check_focal(pred, target):
+    if pred.dtype != torch.float32 or pred.dim() != 2:
+        raise L.SmbError('sigmoid_focal_loss: logits must be a 2-D fp32 tensor [N, C] (got %s %s)'
+                         % (pred.dtype, tuple(pred.shape)))
+    if target.dtype != torch.int64 or target.dim() != 1 or target.shape[0] != pred.shape[0]:
+        raise L.SmbError('sigmoid_focal_loss: targets must be int64 [N] (got %s %s)' % (target.dtype, tuple(target.shape)))
+    if pred.shape[1] < 1:
+        raise L.SmbError('sigmoid_focal_loss: no classes')
+    _need_cuda(pred, target)
+
+
+class SigmoidFocalLossFunction(torch.autograd.Function):
+    """mmdet.ops.sigmoid_focal_loss (MM/mmdet/ops/sigmoid_focal_loss/sigmoid_focal_loss.py:8-33): per-element loss
+    [N, C] and its gradient by smb_sigmoid_focal_loss_forward / _backward, the reference kernel's bits."""
+
+    @staticmethod
+    def forward(ctx, input, target, gamma=2.0, alpha=0.25):
+        _check_focal(input, target)
+        input, target = input.contiguous(), target.contiguous()
+        ctx.save_for_backward(input, target)
+        ctx.gamma, ctx.alpha = float(gamma), float(alpha)
+        loss = torch.empty_like(input)
+        if input.numel():
+            with torch.cuda.device(input.device):
+                L.check(L.lib().smb_sigmoid_focal_loss_forward(L.ptr(input), L.ptr(target), input.shape[0], input.shape[1],
+                                                               ctypes.c_float(ctx.gamma), ctypes.c_float(ctx.alpha),
+                                                               L.ptr(loss), L.stream_ptr()),
+                        'smb_sigmoid_focal_loss_forward')
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_loss):
+        input, target = ctx.saved_tensors
+        _need_cuda(d_loss)
+        d_loss = d_loss.float().contiguous()
+        d_input = torch.empty_like(input)
+        if input.numel():
+            with torch.cuda.device(input.device):
+                L.check(L.lib().smb_sigmoid_focal_loss_backward(L.ptr(input), L.ptr(target), L.ptr(d_loss), input.shape[0],
+                                                                input.shape[1], ctypes.c_float(ctx.gamma),
+                                                                ctypes.c_float(ctx.alpha), L.ptr(d_input), L.stream_ptr()),
+                        'smb_sigmoid_focal_loss_backward')
+        return d_input, None, None, None
+
+
+def sigmoid_focal_loss(pred, target, gamma=2.0, alpha=0.25):
+    """Per-element sigmoid focal loss [N, C] of fp32 CUDA logits and int64 targets (1-based, 0 background, < 0 ignored),
+    differentiable w.r.t. `pred`."""
+    return SigmoidFocalLossFunction.apply(pred, target, gamma, alpha)
+
+
+class SigmoidFocalLoss(nn.Module):
+    """mmdet.ops.SigmoidFocalLoss (sigmoid_focal_loss.py:36-52): the summed loss."""
+
+    def __init__(self, gamma, alpha):
+        super().__init__()
+        self.gamma = gamma
+        self.alpha = alpha
+
+    def forward(self, logits, targets):
+        return sigmoid_focal_loss(logits, targets, self.gamma, self.alpha).sum()
+
+    def __repr__(self):
+        return self.__class__.__name__ + '(gamma={}, alpha={})'.format(self.gamma, self.alpha)
