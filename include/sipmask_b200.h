@@ -897,6 +897,31 @@ int smb_sigmoid_focal_loss_forward(const float* logits, const int64_t* targets, 
 int smb_sigmoid_focal_loss_backward(const float* logits, const int64_t* targets, const float* d_losses, int N,
                                     int num_classes, float gamma, float alpha, float* d_logits, smb_stream_t stream);
 
+/* ------------------------------------------------------------------ SipMask mask loss (mask_loss.cu)
+ * The mask-loss block of SipMaskHead.loss (models/anchor_heads/sipmask_head.py:437-463), fused: no [H, W, M] tensor is
+ * stored.
+ *
+ * smb_mask_targets: gt mask planes -> bits [G, H, ceil(W / 32)] uint32 (bit x % 32 of word x / 32 is pixel x), equal to
+ * F.interpolate(scale_factor=0.5, bilinear, align_corners=False) -> zero pad / crop to H x W -> gt(0.5) on {0, 1} masks
+ * (any non-zero byte counts as 1).  src: uint8 planes; planes [G, 3] int64 (device) = {byte offset of the plane in src,
+ * Hf, Wf}.  One launch; G = 0 launches nothing. */
+int smb_mask_targets(const void* src, const long long* planes, int G, int H, int W, uint32_t* bits, smb_stream_t stream);
+
+/* smb_mask_loss: feat [B, 32, H, W] fp32 NCHW, cofs [M, 128] fp32, boxes [M, 4] fp32 (mask coordinates), img_offsets
+ * [B + 1] int32 (instances of image b are img_offsets[b] .. img_offsets[b + 1] - 1), targets from smb_mask_targets with G
+ * planes, gt_rows [M] int32 (a row outside [0, G) reads as an empty mask), weights [M] fp32; all on the device.
+ *   g == NULL (forward): loss [B] fp32, loss[b] = sum over b's instances n and the pixels inside n's box of
+ *     BCE(sigmoid(z), t) * w_n / (bw_n * bh_n * M_b) (torch's CUDA sigmoid and binary_cross_entropy, logs clamped at
+ *     -100; CropSplit's cell geometry).
+ *   g [B] (backward): d_feat [B, 32, H, W] (every element written) and / or d_cofs [M, 128] (every element written) for
+ *     the upstream gradient g of loss; either may be NULL, not both.
+ * Every sum has a fixed order (the same bits on every run); no host synchronisation.  M = 0, images without instances
+ * and boxes outside the map give 0.  workspace: smb_mask_loss_workspace_bytes(B, M, H, W). */
+size_t smb_mask_loss_workspace_bytes(int B, int M, int H, int W);
+int smb_mask_loss(const float* feat, const float* cofs, const float* boxes, const int* img_offsets, const uint32_t* targets,
+                  int G, const int* gt_rows, const float* weights, const float* g, int B, int M, int H, int W, float* loss,
+                  float* d_feat, float* d_cofs, void* workspace, size_t workspace_bytes, smb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -105,7 +105,7 @@ SYMBOLS = [
     'smb_segm_raster_workspace_bytes', 'smb_segm_raster_dev', 'smb_render_dev',
     'smb_deform_grad_scale_workspace_bytes', 'smb_deform_grad_scale', 'smb_deform_col2im',
     'smb_deform_weight_grad_workspace_bytes', 'smb_deform_weight_grad', 'smb_sigmoid_focal_loss_forward',
-    'smb_sigmoid_focal_loss_backward',
+    'smb_sigmoid_focal_loss_backward', 'smb_mask_targets', 'smb_mask_loss_workspace_bytes', 'smb_mask_loss',
 ]
 
 
@@ -124,7 +124,7 @@ def lib():
                   'smb_ytvis_match_workspace_bytes', 'smb_segm_raster_workspace_bytes',
                   'smb_coco_match_params_workspace_bytes', 'smb_coco_analysis_workspace_bytes',
                   'smb_coco_match_params2_workspace_bytes', 'smb_deform_grad_scale_workspace_bytes',
-                  'smb_deform_weight_grad_workspace_bytes'):
+                  'smb_deform_weight_grad_workspace_bytes', 'smb_mask_loss_workspace_bytes'):
             getattr(L, n).restype = ctypes.c_size_t
         L.smb_conv_plan_destroy.restype = None
         _lib = L

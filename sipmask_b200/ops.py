@@ -8,6 +8,8 @@ and `mmdet.core` entry points, backed by the C ABI (PyTorch tensors in, PyTorch 
   mask_assemble            <- MM/mmdet/models/anchor_heads/sipmask_head.py:609-627 (fused)
   DeformConv(Pack) / deform_conv        <- MM/mmdet/ops/dcn/deform_conv.py:14-94,192-300 (with the backward)
   SigmoidFocalLoss / sigmoid_focal_loss <- MM/mmdet/ops/sigmoid_focal_loss/sigmoid_focal_loss.py:8-52
+  sipmask_mask_targets / sipmask_mask_loss / sipmask_head_mask_loss
+                           <- MM/mmdet/models/anchor_heads/sipmask_head.py:403-484 (the mask loss, fused)
 All tensors must be CUDA tensors on an sm_90 device; there is no CPU path.
 """
 import ctypes
@@ -1178,3 +1180,191 @@ class SigmoidFocalLoss(nn.Module):
 
     def __repr__(self):
         return self.__class__.__name__ + '(gamma={}, alpha={})'.format(self.gamma, self.alpha)
+
+
+# ----------------------------------------------------------------------------------------------- SipMask mask loss
+def _mask_planes_u8(m, device):
+    """one image's gt masks -> uint8 {0, 1} [G, Hf, Wf] on `device` (bool / uint8 / float, tensor or numpy)"""
+    if isinstance(m, np.ndarray):
+        m = torch.from_numpy(m)
+    if m.dim() != 3:
+        raise L.SmbError('sipmask_mask_targets: masks must be [G, Hf, Wf] (got %s)' % (tuple(m.shape),))
+    if m.dtype not in (torch.uint8, torch.bool, torch.float32, torch.float64, torch.float16):
+        raise L.SmbError('sipmask_mask_targets: masks must be uint8, bool or float (got %s)' % m.dtype)
+    m = m.to(device)
+    return (m != 0).to(torch.uint8) if m.dtype != torch.uint8 else m
+
+
+@L.device_guard
+def sipmask_mask_targets(gt_masks, mask_hw, device=None):
+    """SipMaskHead.loss's targets (sipmask_head.py:437-442) for a batch, in one launch: per-image gt masks [G_i, Hf, Wf]
+    (uint8, bool or float; {0, 1}) -> (bits [sum G_i, H, ceil(W / 32)] int32 holding uint32 words, bit x % 32 of word
+    x / 32 is pixel x; gt_offsets [B + 1] int64, image i's planes are rows gt_offsets[i] .. gt_offsets[i + 1] - 1).
+    Bit for bit F.interpolate(scale_factor=0.5, bilinear, align_corners=False) -> zero pad / crop to (H, W) -> gt(0.5)."""
+    H, W = int(mask_hw[0]), int(mask_hw[1])
+    if H <= 0 or W <= 0:
+        raise L.SmbError('sipmask_mask_targets: bad mask size %s' % (tuple(mask_hw),))
+    if device is None:
+        device = next((m.device for m in gt_masks if isinstance(m, torch.Tensor) and m.is_cuda), None)
+    if device is None or torch.device(device).type != 'cuda':
+        raise L.SmbError('sipmask_mask_targets: needs a CUDA device (no CPU fallback)')
+    planes = [_mask_planes_u8(m, device) for m in gt_masks]
+    counts = [int(m.shape[0]) for m in planes]
+    gt_offsets = torch.tensor(np.concatenate([[0], np.cumsum(counts)]).astype(np.int64), device=device)
+    G = sum(counts)
+    bits = torch.empty((G, H, (W + 31) // 32), dtype=torch.int32, device=device)
+    if G == 0:
+        return bits, gt_offsets
+    table, off = [], 0
+    for m in planes:
+        for _ in range(m.shape[0]):
+            table.append((off, m.shape[1], m.shape[2]))
+            off += m.shape[1] * m.shape[2]
+    src = torch.cat([m.reshape(-1) for m in planes])
+    table = torch.tensor(table, dtype=torch.int64).to(device)
+    with torch.cuda.device(device):
+        L.check(L.lib().smb_mask_targets(L.ptr(src), L.ptr(table), G, H, W, L.ptr(bits), L.stream_ptr()),
+                'smb_mask_targets')
+    return bits, gt_offsets
+
+
+def _check_mask_loss(feat, cofs, boxes, img_offsets, targets, gt_rows, weights):
+    """What smb_mask_loss accepts; raises before anything is launched."""
+    def need(cond, msg):
+        if not cond:
+            raise L.SmbError('sipmask_mask_loss: ' + msg)
+    ts = dict(feat_masks=feat, cofs=cofs, boxes=boxes, img_offsets=img_offsets, targets=targets, gt_rows=gt_rows,
+              weights=weights)
+    for k, t in ts.items():
+        need(isinstance(t, torch.Tensor), '%s must be a tensor' % k)
+    need(feat.dtype == torch.float32 and feat.dim() == 4 and feat.shape[1] == 32,
+         'feat_masks must be fp32 [B, 32, H, W] (got %s %s)' % (feat.dtype, tuple(feat.shape)))
+    B, _, H, W = feat.shape
+    need(B > 0 and H > 0 and W > 0, 'empty feat_masks %s' % (tuple(feat.shape),))
+    need(cofs.dtype == torch.float32 and cofs.dim() == 2 and cofs.shape[1] == 128,
+         'cofs must be fp32 [M, 128] (got %s %s)' % (cofs.dtype, tuple(cofs.shape)))
+    M = cofs.shape[0]
+    need(boxes.dtype == torch.float32 and tuple(boxes.shape) == (M, 4),
+         'boxes must be fp32 [M, 4] (got %s %s)' % (boxes.dtype, tuple(boxes.shape)))
+    need(weights.dtype == torch.float32 and tuple(weights.shape) == (M,),
+         'weights must be fp32 [M] (got %s %s)' % (weights.dtype, tuple(weights.shape)))
+    need(gt_rows.dtype in (torch.int32, torch.int64) and tuple(gt_rows.shape) == (M,),
+         'gt_rows must be int32 / int64 [M] (got %s %s)' % (gt_rows.dtype, tuple(gt_rows.shape)))
+    need(img_offsets.dtype in (torch.int32, torch.int64) and tuple(img_offsets.shape) == (B + 1,),
+         'img_offsets must be int32 / int64 [B + 1] (got %s %s)' % (img_offsets.dtype, tuple(img_offsets.shape)))
+    need(targets.dtype == torch.int32 and targets.dim() == 3 and tuple(targets.shape[1:]) == (H, (W + 31) // 32),
+         'targets must be sipmask_mask_targets bits [G, %d, %d] (got %s %s)'
+         % (H, (W + 31) // 32, targets.dtype, tuple(targets.shape)))
+    _need_cuda(*ts.values())
+    for k, t in ts.items():
+        need(t.is_contiguous(), '%s must be contiguous' % k)
+        need(t.device == feat.device, '%s is on %s, feat_masks on %s' % (k, t.device, feat.device))
+
+
+def _mask_loss_launch(feat, cofs, boxes, offs, targets, rows, weights, g, loss, d_feat, d_cofs):
+    B, _, H, W = feat.shape
+    M = cofs.shape[0]
+    ws = torch.empty(max(int(L.lib().smb_mask_loss_workspace_bytes(B, M, H, W)), 1), dtype=torch.uint8, device=feat.device)
+    with torch.cuda.device(feat.device):
+        L.check(L.lib().smb_mask_loss(L.ptr(feat), L.ptr(cofs), L.ptr(boxes), L.ptr(offs), L.ptr(targets),
+                                      int(targets.shape[0]), L.ptr(rows), L.ptr(weights), L.ptr(g), B, M, H, W,
+                                      L.ptr(loss), L.ptr(d_feat), L.ptr(d_cofs), L.ptr(ws), ctypes.c_size_t(ws.numel()),
+                                      L.stream_ptr()), 'smb_mask_loss')
+
+
+class SipMaskMaskLossFunction(torch.autograd.Function):
+    """The mask loss of SipMaskHead.loss (sipmask_head.py:446-463) per image, fused: loss[b] and, in backward, d feat_masks
+    and d cofs, recomputing the logits (K = 32) instead of keeping any [H, W, M] tensor.  boxes, weights and the targets
+    get no gradient, as in the reference (bbox_dt and weighting are detached)."""
+
+    @staticmethod
+    def forward(ctx, feat_masks, cofs, boxes, img_offsets, targets, gt_rows, weights):
+        _check_mask_loss(feat_masks, cofs, boxes, img_offsets, targets, gt_rows, weights)
+        offs, rows = img_offsets.to(torch.int32), gt_rows.to(torch.int32)
+        ctx.save_for_backward(feat_masks, cofs, boxes, offs, targets, rows, weights)
+        loss = torch.empty(feat_masks.shape[0], dtype=torch.float32, device=feat_masks.device)
+        _mask_loss_launch(feat_masks, cofs, boxes, offs, targets, rows, weights, None, loss, None, None)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        feat, cofs, boxes, offs, targets, rows, weights = ctx.saved_tensors
+        need_x, need_c = ctx.needs_input_grad[:2]
+        d_feat = d_cofs = None
+        if need_x or need_c:
+            _need_cuda(g)
+            g = g.float().contiguous()
+            d_feat = torch.empty_like(feat) if need_x else None
+            d_cofs = torch.empty_like(cofs) if need_c else None
+            if need_x or cofs.shape[0]:
+                _mask_loss_launch(feat, cofs, boxes, offs, targets, rows, weights, g, None, d_feat, d_cofs)
+        return d_feat, d_cofs, None, None, None, None, None
+
+
+def sipmask_mask_loss(feat_masks, cofs, boxes, img_offsets, targets, gt_rows, weights):
+    """Per-image SipMask mask loss [B] (sipmask_head.py:446-463 before the sum over images):
+      feat_masks [B, 32, H, W] fp32, cofs [M, 128] fp32 (instances of image b are rows img_offsets[b] ..
+      img_offsets[b + 1] - 1), boxes [M, 4] fp32 in mask coordinates (bbox_dt), targets / gt_rows: the planes of
+      sipmask_mask_targets and each instance's row in them, weights [M] fp32 (the detached weighting).
+    loss[b] = sum_n w_n / (M_b bw_n bh_n) sum over n's box of BCE(CropSplit(sigmoid(feat . cof)), gt); differentiable
+    w.r.t. feat_masks and cofs."""
+    return SipMaskMaskLossFunction.apply(feat_masks, cofs, boxes, img_offsets, targets, gt_rows, weights)
+
+
+def _bbox_overlaps_aligned(b1, b2):
+    """mmdet v1 bbox_overlaps(b1, b2, is_aligned=True) (core/bbox/geometry.py:57-69), the +1 box convention"""
+    lt = torch.max(b1[:, :2], b2[:, :2])
+    rb = torch.min(b1[:, 2:], b2[:, 2:])
+    wh = (rb - lt + 1).clamp(min=0)
+    overlap = wh[:, 0] * wh[:, 1]
+    area1 = (b1[:, 2] - b1[:, 0] + 1) * (b1[:, 3] - b1[:, 1] + 1)
+    area2 = (b2[:, 2] - b2[:, 0] + 1) * (b2[:, 3] - b2[:, 1] + 1)
+    return overlap / (area1 + area2 - overlap)
+
+
+def sipmask_head_mask_loss(feat_masks, flatten_cof_preds, flatten_cls_scores1, det_bboxes, label_list, gt_inds, gt_bboxes,
+                           gt_masks):
+    """`loss_mask` of SipMaskHead.loss (SipMask-mmdetection sipmask_head.py:403-484, SipMask-VIS :467-548) without
+    rescoring, with the per-image block batched into one sipmask_mask_targets and one sipmask_mask_loss call.  The
+    arguments are the reference's local variables of the same names (gt_masks: the per-image mask arrays).  Per image:
+    the positives (labels > 0) of det_bboxes / 2 with area > 1; weighting = sigmoid(cls score of the label) x aligned IoU
+    with the gt box / 2 (+1 convention), normalised to mean ~1 (/ (sum + 1e-4) * count).  Returns the batch mean; the
+    gradient flows to feat_masks and flatten_cof_preds only."""
+    num_imgs = feat_masks.shape[0]
+    H, W = int(feat_masks.shape[2]), int(feat_masks.shape[3])
+    device = feat_masks.device
+    bits, _ = sipmask_mask_targets(gt_masks, (H, W), device=device)
+    gt_off = np.concatenate([[0], np.cumsum([int(m.shape[0]) for m in gt_masks])]).tolist()   # on the host: no sync
+    cofs, boxes, rows, weights, offsets = [], [], [], [], [0]
+    for i in range(num_imgs):
+        labels = torch.cat([lv.flatten() for lv in label_list[i]])
+        bbox_dt = (det_bboxes[i] / 2).detach()
+        pos_inds = (labels > 0).nonzero().view(-1)
+        keep_box = bbox_dt[pos_inds, :4]
+        area = (keep_box[:, 2] - keep_box[:, 0]) * (keep_box[:, 3] - keep_box[:, 1])
+        keep = area > 1.0
+        bbox = keep_box[keep]
+        idx_gt = gt_inds[i][keep]
+        if bbox.shape[0] > 0:
+            cls_score = flatten_cls_scores1[i, pos_inds, labels[pos_inds] - 1].sigmoid().detach()[keep]
+            ious = _bbox_overlaps_aligned(gt_bboxes[i][idx_gt] / 2, bbox)
+            with torch.no_grad():
+                weighting = cls_score * ious
+                weighting = weighting / (torch.sum(weighting) + 0.0001) * len(weighting)
+            cofs.append(flatten_cof_preds[i][pos_inds][keep])
+            boxes.append(bbox)
+            rows.append(idx_gt.to(torch.int64) + gt_off[i])
+            weights.append(weighting.detach())
+        offsets.append(offsets[-1] + int(bbox.shape[0]))
+    if offsets[-1] == 0:
+        cofs = flatten_cof_preds.new_zeros((0, 128)) + flatten_cof_preds.sum() * 0
+        boxes = torch.zeros((0, 4), dtype=torch.float32, device=device)
+        rows = torch.zeros((0,), dtype=torch.int64, device=device)
+        weights = torch.zeros((0,), dtype=torch.float32, device=device)
+    else:
+        cofs, boxes = torch.cat(cofs).float().contiguous(), torch.cat(boxes).float().contiguous()
+        rows, weights = torch.cat(rows), torch.cat(weights).float().contiguous()
+    offs = torch.tensor(offsets, dtype=torch.int32).to(device)
+    loss = sipmask_mask_loss(feat_masks.float().contiguous(), cofs, boxes, offs, bits, rows, weights)
+    return loss.sum() / num_imgs
