@@ -770,7 +770,7 @@ int smb_groupnorm_relu_apply(void* x, int n_img, int hw, int C, int pitch, const
 int smb_groupnorm_stats(const void* x, int n_img, int hw, int C, int pitch, void* stats /* int64 */, smb_stream_t stream);
 
 /* Deformable im2col (ops/dcn/src/deform_conv_cuda_kernel.cu:85-115,191-243), channel-last:
- *   x [H,W,C] fp16, offset [H,W,dg*18] fp32 (per dg: 2*(i*3+j)=dh, +1=dw) with pitch off_pitch
+ *   x [H,W,C] fp16, offset [H,W,dg*18] fp32 (per dg: 2*(i*3+j)=dh, +1=dw) with pitch off_pitch >= dg*18
  *   -> col [H*W, 9*C] fp16, K index = tap*C + c (3x3, stride 1, pad 1, dil 1). */
 int smb_deform_im2col(const void* x, const float* offset, int off_pitch, void* col,
                       int n_img, int H, int W, int C, int deformable_groups, smb_stream_t stream);

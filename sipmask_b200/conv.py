@@ -314,6 +314,16 @@ def offset_conv1x1(bbox, scale, weight, out=None):
     return out
 
 
+def _pixel_pitch(t):
+    """Elements between neighbouring pixels of an [N, H, W, C] view whose pixels are evenly spaced (a channel slice of a
+    wider tensor included).  The stride of a size-1 dimension is arbitrary (a permuted 1 x 1 map counts as contiguous
+    with stride(2) == 1), so the pitch comes from the innermost dimension longer than 1."""
+    N, H, W, C = t.shape
+    p = t.stride(2) if W > 1 else t.stride(1) if H > 1 else t.stride(0) if N > 1 else C
+    assert (C == 1 or t.stride(3) == 1) and (H == 1 or t.stride(1) == W * p) and (N == 1 or t.stride(0) == H * W * p)
+    return p
+
+
 @L.device_guard
 def deform_im2col(x, offset, dg, out=None):
     """x [N,H,W,C] fp16, offset [N,H,W,dg*18] fp32 -> col [N,H,W,9*C] fp16."""
@@ -321,7 +331,7 @@ def deform_im2col(x, offset, dg, out=None):
     assert x.is_contiguous()
     if out is None:
         out = torch.empty((N, H, W, 9 * C), dtype=torch.float16, device=x.device)
-    L.check(L.lib().smb_deform_im2col(L.ptr(x), L.ptr(offset), offset.stride(2), L.ptr(out), N, H, W, C, int(dg),
+    L.check(L.lib().smb_deform_im2col(L.ptr(x), L.ptr(offset), _pixel_pitch(offset), L.ptr(out), N, H, W, C, int(dg),
                                       L.stream_ptr()), 'smb_deform_im2col')
     return out
 
@@ -344,10 +354,10 @@ def deform_col2im(grad_col, x, offset, dg, scale, grad_input=True, grad_offset=T
     """grad_col [N,H,W,9C] fp32 (s * the column gradient), x [N,H,W,C] fp16, offset [N,H,W,dg*18] fp32, scale {s, 1/s}
     -> (grad_input [N,H,W,C] fp32 | None, grad_offset [N,H,W,dg*18] fp32 | None) (smb_deform_col2im)."""
     N, H, W, C = x.shape
-    assert x.is_contiguous() and grad_col.is_contiguous() and offset.stride(3) == 1
+    assert x.is_contiguous() and grad_col.is_contiguous()
     gin = torch.zeros((N, H, W, C), dtype=torch.float32, device=x.device) if grad_input else None
     goff = torch.empty((N, H, W, dg * 18), dtype=torch.float32, device=x.device) if grad_offset else None
-    L.check(L.lib().smb_deform_col2im(L.ptr(grad_col), L.ptr(x), L.ptr(offset), offset.stride(2), L.ptr(scale), L.ptr(gin),
+    L.check(L.lib().smb_deform_col2im(L.ptr(grad_col), L.ptr(x), L.ptr(offset), _pixel_pitch(offset), L.ptr(scale), L.ptr(gin),
                                       L.ptr(goff), N, H, W, C, int(dg), L.stream_ptr()), 'smb_deform_col2im')
     return gin, goff
 

@@ -492,6 +492,8 @@ extern "C" int smb_deform_im2col(const void* x, const float* offset, int off_pit
   SMB_CHECK_ARG(x && offset && col, "smb_deform_im2col: null pointer");
   SMB_CHECK_ARG(C % 8 == 0 && deformable_groups > 0 && C % deformable_groups == 0 && (C / deformable_groups) % 8 == 0,
                 "smb_deform_im2col: C=%d dg=%d unsupported", C, deformable_groups);
+  SMB_CHECK_ARG(off_pitch >= deformable_groups * 18, "smb_deform_im2col: offset pitch %d < %d", off_pitch,
+                deformable_groups * 18);
   const long long warps = (long long)n_img * H * W * 9;
   deform_im2col_kernel<<<grid_for(warps * 32, 256), 256, 0, (cudaStream_t)stream>>>((const __half*)x, offset, off_pitch,
                                                                                     (__half*)col, n_img, H, W, C,

@@ -4,6 +4,8 @@ tests/train_ops_inputs.py.
 Needs a GPU and oracle/_ref/libsipmask_ref_train_cuda.so (built by oracle/build_train.py from the reference sources).
     python tests/golden/gen_golden_ref_train_ops.py OUT_DIR
 
+Arrays of an existing OUT_DIR/ref_train_ops.npz are kept (see main), so adding cases leaves the other keys' bits alone.
+
   * `deformable_col2im` / `deformable_col2im_coord` (MM/mmdet/ops/dcn/src/deform_conv_cuda_kernel.cu:279-465) on each
     COL2IM_CASES input: grad_input [B,C,H,W] and grad_offset [B,dg*18,H,W] as the fp32 values at a fixed, seeded sample of
     flat indices (`train_ops_inputs.sample_index`), as in ref_cuda_kernels.npz;
@@ -69,6 +71,16 @@ def main(out_dir):
         g[T.focal_key(C, gamma, alpha) + '_loss'] = loss.cpu().numpy()
         g[T.focal_key(C, gamma, alpha) + '_grad'] = grad.cpu().numpy()
     path = os.path.join(out_dir, 'ref_train_ops.npz')
+    if os.path.exists(path):
+        # deformable_col2im sums grad_input with float atomics, so a second run reproduces it only to rounding: arrays
+        # already in the file keep their bits (after checking they agree), and added cases only add keys
+        old = np.load(path)
+        for k in old.files:
+            if k in g:
+                tol = 1e-6 * float(np.abs(g[k]).max()) if k.startswith('col2im_input_') else 0.0
+                assert old[k].shape == g[k].shape and np.abs(old[k].astype(np.float64) - g[k]).max() <= tol, k
+                g[k] = old[k]
+        print('kept %d existing arrays' % len([k for k in old.files if k in g]))
     np.savez_compressed(path, **g)
     print('wrote %s (%d arrays)' % (path, len(g)))
 

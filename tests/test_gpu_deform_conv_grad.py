@@ -6,6 +6,7 @@
   * module level against the float64 autograd of oracle.ops.deform_conv at the FeatureAlign and SipMask++ DCN sizes;
   * the gradient scaling, determinism, needs_input_grad, a FeatureAlign step, DeformConvPack.
 """
+import math
 import os
 
 import numpy as np
@@ -27,6 +28,10 @@ REL = 3e-3
 
 FEATURE_ALIGN = [(2, 256, 256, h, w, 4) for h, w in [(100, 168), (50, 84), (25, 42), (13, 21), (7, 11), (2, 2)]]
 PP_DCN = [(2, 128, 128, 68, 68, 1), (2, 256, 256, 34, 34, 1), (2, 512, 512, 17, 17, 1)]
+# shapes the API accepts beyond the models': ragged M and N tiles in both GEMMs, Cin != Cout, dg up to Cin / 8, and maps
+# smaller than the kernel (TrainableDeformConv pads them to 3 x 3 and crops the output)
+EDGES = [(1, 64, 64, 13, 21, 1), (3, 64, 128, 9, 11, 8), (2, 256, 64, 25, 42, 4), (1, 1024, 64, 7, 9, 128)] + \
+    [(1, 256, 256, h, w, 4) for h, w in [(1, 1), (1, 5), (5, 1), (2, 1)]]
 
 
 def _rel(a, b):
@@ -95,9 +100,49 @@ def test_col2im_reference_kernel_vs_float64_autograd_vs_smb(B, C, H, W, dg):
 
 
 # ---------------------------------------------------------------------------------------------------- module level
-@pytest.mark.parametrize('B,C,Cout,H,W,dg', FEATURE_ALIGN + PP_DCN)
+def _wgrad_split(cout, kc, P):
+    """smb_deform_weight_grad's split of the P pixels (wgrad_split in csrc/train_ops.cu): 128 x 128 tiles, 64-pixel
+    blocks, about 264 CTAs -> (blocks, blocks per split, splits)."""
+    tiles = -(-cout // 128) * -(-kc // 128)
+    kb_total = -(-P // 64)
+    want = max(1, min(-(-264 // tiles), kb_total))
+    kps = -(-kb_total // want)
+    return kb_total, kps, -(-kb_total // kps)
+
+
+def _dw_bound(x, off, gy, dg, splits_cfg):
+    """Per-element bound on |dW - dW64| [Cout, Cin, 3, 3]: the weight GEMM's accumulation (gamma of the pixels in one
+    split, one fp32 rounding per split added) over m = sum_p |g| |col|, plus the fp16 rounding of s * g and of the columns
+    (2^-11 each, their product 2^-22, fp16's subnormal spacing 2^-25 in absolute terms) and the fp32 interpolation of the
+    columns (2^-20).  |col| is bounded by the columns of |x| (the bilinear weights are non-negative)."""
+    from oracle import ops as O
+    from oracle import numerics as NU
+    kb_total, kps, splits = splits_cfg
+    B, Cout, H, W = gy.shape
+    C = x.shape[1]
+    with torch.device('cuda'):
+        ph, pw = max(3 - H, 0), max(3 - W, 0)                    # TrainableDeformConv's padding of small maps
+        xa = torch.nn.functional.pad(x.double().abs(), (0, pw, 0, ph))
+        oa = torch.nn.functional.pad(off.double(), (0, pw, 0, ph))
+        cols, _, _ = O.deform_im2col(xa, oa, 3, 3, 1, 1, 1, dg)             # [B, C*9, Hp*Wp], row c*9 + tap
+    ga = torch.nn.functional.pad(gy.double().abs(), (0, pw, 0, ph)).reshape(B, Cout, -1)
+    m = torch.einsum('bop,bkp->ok', ga, cols).view(Cout, C, 3, 3)
+    amax = float(gy.abs().max())
+    e = math.frexp(amax)[1] - 1 if amax > 0 else 0
+    s = 2.0 ** min(max(14 - e, -126), 126) if amax > 0 else 1.0
+    g_sum = ga.sum((0, 2)).view(Cout, 1, 1, 1)
+    c_sum = cols.sum((0, 2)).view(1, C, 3, 3)
+    u = 2.0 ** -11
+    rel = NU.gamma_k(64 * kps) + (splits - 1) * 2.0 ** -24 + 2 * u + u * u + 2.0 ** -20
+    return rel * m + 2.0 ** -25 * (c_sum / s + g_sum)
+
+
+@pytest.mark.parametrize('B,C,Cout,H,W,dg', FEATURE_ALIGN + PP_DCN + EDGES)
 def test_module_gradients_vs_float64(B, C, Cout, H, W, dg):
     x, off, w, gy = _module_inputs(B, C, Cout, H, W, dg)
+    cfg = _wgrad_split(Cout, 9 * C, B * max(H, 3) * max(W, 3))
+    print('module B %d Cin %4d Cout %4d map %3dx%-3d dg %3d: weight GEMM %d x %d tiles, %d blocks, %d per split, %d splits'
+          % (B, C, Cout, H, W, dg, -(-Cout // 128), -(-9 * C // 128), cfg[0], cfg[1], cfg[2]))
     got = _smb_grads(x, off, w, gy, dg)
     want = _ref64_grads(x, off, w, gy, dg)
     errs = {}
@@ -105,20 +150,29 @@ def test_module_gradients_vs_float64(B, C, Cout, H, W, dg):
         assert a.shape == b.shape and a.dtype == torch.float32, name
         errs[name] = _rel(a, b)
     assert max(errs.values()) <= REL, errs
+    err = (got[2].double() - want[2]).abs()
+    bound = _dw_bound(x, off, gy, dg, cfg)
+    worst = float((err / bound).max())
+    assert worst <= 1.0, ('grad_weight per-element bound', worst)
 
 
 def test_gradient_scaling_is_exact():
-    """grad_out * 2^-24 (far below fp16's normal range: cast to fp16 it would mostly flush to zero) gives dW and
-    grad_offset of exactly 2^-24 times the unscaled ones; grad_input (float atomics, any order) agrees to rounding."""
+    """grad_out * 2^-24 (far below fp16's normal range: cast to fp16 it would mostly flush to zero) and grad_out * 2^25
+    (amax above fp16's 65504, so the scale s < 1) give dW and grad_offset of exactly 2^e times the unscaled ones;
+    grad_input (float atomics, any order) agrees to rounding."""
     x, off, w, gy = _module_inputs(1, 256, 256, 25, 42, 4)
-    tiny = gy * 2.0 ** -24
-    assert (tiny.half() == 0).float().mean().item() > 0.9
     a = _smb_grads(x, off, w, gy, 4)
-    b = _smb_grads(x, off, w, tiny, 4)
-    assert torch.equal(b[2], a[2] * 2.0 ** -24)
-    assert torch.equal(b[1], a[1] * 2.0 ** -24)
-    assert _rel(b[0] * 2.0 ** 24, a[0]) <= 1e-6
     assert a[2].abs().max() > 0 and a[1].abs().max() > 0
+    for e in (-24, 25):
+        scaled = gy * 2.0 ** e
+        if e < 0:
+            assert (scaled.half() == 0).float().mean().item() > 0.9
+        else:
+            assert scaled.abs().max().item() > 65504
+        b = _smb_grads(x, off, w, scaled, 4)
+        assert torch.equal(b[2], a[2] * 2.0 ** e), e
+        assert torch.equal(b[1], a[1] * 2.0 ** e), e
+        assert _rel(b[0] * 2.0 ** -e, a[0]) <= 1e-6, e
 
 
 def test_backward_is_deterministic():

@@ -38,6 +38,30 @@ def test_forward_backward_bit_equal_to_reference_kernel(gold, C, gamma, alpha):
     assert set(targets.tolist()) >= set(range(-1, C + 1))
 
 
+FOCAL_GRID = 4096 * 512                    # threads of the largest focal-loss grid; beyond that the kernels stride
+
+
+@pytest.mark.parametrize('C,gamma,alpha', [(80, 2.0, 0.25), (80, 1.5, 0.5), (1, 2.0, 0.25), (1, 0.0, 0.5)])
+def test_past_one_grid(gold, C, gamma, alpha):
+    """The fixture's rows tiled to more than two grids' worth of elements (two 1333 x 800 images at 80 classes give about
+    3.6 M), with a partial last stride.  Every element depends only on its logit, target and class, so the loss and the
+    gradient must be the fixture's bits tiled the same way."""
+    from sipmask_b200 import ops
+    logits, targets, d_loss = T.focal_inputs(C)
+    N = logits.shape[0]
+    reps = 2 * FOCAL_GRID // (N * C) + 1
+    n = reps * N * C
+    assert n > 2 * FOCAL_GRID and n % FOCAL_GRID != 0
+    print('focal loss C %d: %d rows x %d = %d elements, %d grid strides, last one %d elements' % (
+        C, N, reps, n, -(-n // FOCAL_GRID), n % FOCAL_GRID))
+    x = logits.repeat(reps, 1).cuda().requires_grad_(True)
+    loss = ops.sigmoid_focal_loss(x, targets.repeat(reps).cuda(), gamma, alpha)
+    loss.backward(d_loss.repeat(reps, 1).cuda())
+    key = T.focal_key(C, gamma, alpha)
+    np.testing.assert_array_equal(_bits(loss.detach().cpu().numpy()), np.tile(_bits(gold[key + '_loss']), (reps, 1)))
+    np.testing.assert_array_equal(_bits(x.grad.cpu().numpy()), np.tile(_bits(gold[key + '_grad']), (reps, 1)))
+
+
 def test_module_returns_the_sum():
     from sipmask_b200 import ops
     logits, targets, _ = [t.cuda() for t in T.focal_inputs(40)]

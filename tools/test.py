@@ -76,11 +76,13 @@ def _decode(path, rgb):
         arr = cv2.imread(path, cv2.IMREAD_COLOR)
         if arr is None:
             raise FileNotFoundError('cannot read image %s' % path)
-    return torch.from_numpy(np.ascontiguousarray(arr)).pin_memory()
+    return torch.from_numpy(np.ascontiguousarray(arr))
 
 
 def _decoded(paths, rgb, workers):
-    """The decoded images of `paths` in order, decoded ahead by a pool of `workers` threads (a bounded window)."""
+    """The decoded images of `paths` in order, in pinned memory, decoded ahead by a pool of `workers` threads (a bounded
+    window).  The pinning happens here, on the caller's thread: pinning allocates through CUDA, and a CUDA allocation
+    from another thread while the runner captures an engine's CUDA graph (on its first forward) invalidates the capture."""
     with ThreadPoolExecutor(max_workers=max(1, workers)) as pool:
         window = collections.deque()
         it = iter(paths)
@@ -89,10 +91,10 @@ def _decoded(paths, rgb, workers):
             if len(window) >= 4 * max(1, workers):
                 break
         for p in it:
-            yield window.popleft().result()
+            yield window.popleft().result().pin_memory()
             window.append(pool.submit(_decode, p, rgb))
         while window:
-            yield window.popleft().result()
+            yield window.popleft().result().pin_memory()
 
 
 class _Reader:
