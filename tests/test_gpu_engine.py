@@ -98,7 +98,8 @@ def test_images_in_flight_match_serial(small_case):
     from sipmask_b200.serving import make_engines, EnginePool, PipelinedRunner
     sd, cfg, H, W = small_case['sd'], small_case['cfg'], small_case['H'], small_case['W']
     serial = make_engines(sd, (H, W), in_flight=1, test_cfg=cfg, img_shape=(H, W - 5, 3), use_graph=True)[0]
-    imgs = [synth.synthetic_image(H, W, seed=s) for s in range(3)]
+    # 7 images over 3 slots: consecutive uses of a slot get different images, so a stale input or record shows
+    imgs = [synth.synthetic_image(H, W, seed=s) for s in range(7)]
     want = []
     for im in imgs:
         o = serial.forward(im.cuda())
@@ -121,21 +122,26 @@ def test_images_in_flight_match_serial(small_case):
         assert torch.equal(e.mask_bits, w['mask_bits'])
     # the same through the host <-> device pipeline (pinned host in, pinned host out), lagged consumer included
     runner = PipelinedRunner(engs)
+    pinned = [im.pin_memory() for im in imgs]
     seen = []
     slots = []
-    for i in range(8):
-        slots.append(runner.step(imgs[i % 3].pin_memory(), lambda rec: seen.append(int(rec['count'][0]))))
-        if i >= 5:
-            continue
+
+    def check(i):                                      # image i % 7, read before its slot takes image i + 3
+        host = runner.result(slots[i])
+        w = want[i % 7]
+        assert torch.equal(host['det'], w['det_bboxes'].cpu()), i
+        assert torch.equal(host['lab'], w['det_labels'].cpu()), i
+        assert torch.equal(host['cnt'], w['count'].cpu()), i
+        assert torch.equal(host['bits'], w['mask_bits'].cpu()), i
+    for i in range(10):
+        if i >= 3:
+            check(i - 3)
+        slots.append(runner.step(pinned[i % 7], lambda rec: seen.append(int(rec['count'][0]))))
     runner.flush(lambda rec: seen.append(int(rec['count'][0])))
     torch.cuda.synchronize()
-    assert len(seen) == 8
-    for i in (5, 6, 7):                                # the last use of each slot: image i % 3 on slot i % 3
-        host = runner.result(slots[i])
-        w = want[i % 3]
-        assert torch.equal(host['det'], w['det_bboxes'].cpu())
-        assert torch.equal(host['bits'], w['mask_bits'].cpu())
-        assert seen[i] == int(w['count'][0])
+    for i in (7, 8, 9):
+        check(i)
+    assert seen == [int(want[i % 7]['count'][0]) for i in range(10)]
 
 
 def _engine_vs_oracle(depth, stacked, gn, ssd, H, W, cfg, cls_bias, scale_factor=1.0, tol=2e-2):
