@@ -469,7 +469,7 @@ class SipMaskEngine(object):
         MM: rescale=True semantics, boxes / scale_factor and masks resized by 2 / scale_factor (sipmask_head.py:587-588,
         629-633,648-654).  BM (SipMask-benchmark/fcos_core/modeling/rpn/sipmask/inference.py:66-222): boxes stay in
         resized-image coordinates, rois = boxes / 2, masks are resized by 2 / sf with sf = min(h / ori_h, w / ori_w)."""
-        N, cfg, lib = self.N, self.cfg, L.lib()
+        N, cfg = self.N, self.cfg
         nl, ncls = len(self.level_sizes), self.ncls
         nms_pre = int(cfg['nms_pre'])
         Hm, Wm = self.protos.shape[1], self.protos.shape[2]
@@ -489,15 +489,12 @@ class SipMaskEngine(object):
         fused_mask_tile(*self.mask_tile_r, sizes=(Hm, Wm, g0.full_h, g0.full_w))
         self.set_image_meta([(self.img_shape, self.ori_shape, self.scale_factor)] * N)
         torch.cuda.current_stream(self.dev).synchronize()
-        levels = []                                     # per image: the smb_level_t array over its head outputs
-        for n in range(N):
-            lv, views = ops.level_descs([v['cls'][n] for v in self.level_views], [v['box'][n] for v in self.level_views],
-                                        [v['ctr'][n] for v in self.level_views], self.strides, self.scales)
-            self._keep += [lv, views]
-            levels.append(lv)
+        # per image: its (cls, box, ctr) head outputs, level by level; every image has image 0's level sizes
+        heads = [[[v[k][n] for v in self.level_views] for k in ('cls', 'box', 'ctr')] for n in range(N)]
+        lv, _ = ops.level_descs(*heads[0], self.strides, self.scales)
         if self.benchmark:
             self.max_num = int(cfg['max_per_img'])
-            self.ncand = lib.smb_pair_decode_slots(nl, levels[0], ncls, nms_pre)
+            self.ncand = L.lib().smb_pair_decode_slots(nl, lv, ncls, nms_pre)
             if self.ncand < 0 or self.ncand > 5120:
                 raise ValueError('benchmark: %d candidate slots (nms_pre=%d) exceed the NMS capacity 5120' % (self.ncand, nms_pre))
             self.cand_scores = self._t(N, self.ncand, dtype=torch.float32)
@@ -536,8 +533,7 @@ class SipMaskEngine(object):
                 self._w(hp + 'mask_scoring.weight'), self._w(hp + 'mask_scoring.bias'), self.dev))
             self._rescore_ws = self._t(ops.mask_rescore_f16_workspace_bytes(N * self.max_num, Hm, Wm), dtype=torch.uint8)
             self.rescore_flops = float(N * self.max_num * ops.rescore_flops_per_row(Hm, Wm))    # at full detection counts
-        level_hw = (ctypes.c_int * nl)(*[h * w for h, w in self.level_sizes])
-        self._keep.append(level_hw)
+        level_hw = [h * w for h, w in self.level_sizes] if N > 1 else None
         # the per-image chains are independent (get_bboxes loops over images, sipmask_head.py:517-540): with a batch they
         # are spread over a few streams of the captured graph
         pp_streams = min(N, 4) if N > 1 else 0
@@ -545,40 +541,30 @@ class SipMaskEngine(object):
             self._marker('fork')
         for n in range(N):
             self._tag = (n % pp_streams) + 1 if pp_streams else 0
-            cand_loc = candidates(n, levels[n])
+            cand_loc = candidates(n, heads[n], lv)
 
             def gather(n=n, cand_loc=cand_loc):
                 # candidate row -> level-concatenated location -> coefficient row (mlvl_cofs[idxs_keep], sipmask_head.py:612)
                 # and det[:, :4] -> contiguous rois input, one launch
-                L.check(lib.smb_gather_det_inputs(L.ptr(self.cof_src), self.cof_src.stride(0), L.ptr(cand_loc), L.ptr(self.idx[n]),
-                                                  L.ptr(self.det[n]), L.ptr(self.count[n:n + 1]), self.max_num, 128,
-                                                  L.ptr(self.det_cofs[n]), L.ptr(self.det_boxes4[n]), L.ptr(self.loc_kept[n]),
-                                                  nl if N > 1 else 0, level_hw, N, n, L.stream_ptr()), 'smb_gather_det_inputs')
+                ops.gather_det_inputs(self.cof_src, cand_loc, self.idx[n], self.det[n], self.count[n:n + 1], self.det_cofs[n],
+                                      self.det_boxes4[n], self.loc_kept[n], level_hw, N, n)
             self._add(gather, 1, name='gather_cofs')
 
             def masks(n=n):
                 # fused: prototypes -> sub-region dot/sigmoid/crop -> resize -> threshold -> bit-pack (no pos_masks tensor)
-                L.check(lib.smb_mask_assemble_pack_dev(L.ptr(self.protos[n]), L.F16, 1, L.ptr(self.det_cofs[n]),
-                                                       L.ptr(self.det_boxes4[n]), L.ptr(self.geom[n]),
-                                                       ctypes.c_float(self.mask_tile_r[0]), ctypes.c_float(self.mask_tile_r[1]),
-                                                       L.ptr(self.mask_bits[n]), Hm, Wm, self.max_num, cap_h, cap_w,
-                                                       ctypes.c_float(self.mask_thr), L.stream_ptr()), 'smb_mask_assemble_pack_dev')
+                ops.mask_assemble_pack_dev(self.protos[n], self.det_cofs[n], self.det_boxes4[n], self.geom[n], self.mask_tile_r,
+                                           (cap_h, cap_w), self.mask_thr, out=self.mask_bits[n])
             self._add(masks, 2, name='mask_fused')
             if self.rescoring:
                 def dense(n=n):
                     # the same rois as mask_fused; rows past the count have zero boxes and are skipped by the rescoring
-                    L.check(lib.smb_mask_assemble_dev(L.ptr(self.protos[n]), L.F16, 1, L.ptr(self.det_cofs[n]),
-                                                      L.ptr(self.det_boxes4[n]), L.ptr(self.geom[n]), L.ptr(self.pos_masks[n]),
-                                                      L.F16, Hm, Wm, self.max_num, L.stream_ptr()), 'smb_mask_assemble_dev')
+                    ops.mask_assemble(self.protos[n], self.det_cofs[n], self.det_boxes4[n], None, layout='hwc',
+                                      out=self.pos_masks[n], geom=self.geom[n])
                 self._add(dense, 1, name='mask_dense')
             if self.vis:
-                th, tw = self.track_feats.shape[1], self.track_feats.shape[2]
-
-                def track(n=n, th=th, tw=tw):
-                    L.check(lib.smb_gather_track_feats_dev(L.ptr(self.track_feats[n]), th, tw, 512, L.ptr(self.det[n]),
-                                                           L.ptr(self.count[n:n + 1]), self.max_num, L.ptr(self.geom[n]),
-                                                           ctypes.c_float(8.0), L.ptr(self.det_track[n]), L.stream_ptr()),
-                            'smb_gather_track_feats_dev')
+                def track(n=n):
+                    ops.gather_track_feats(self.track_feats[n], self.det[n], self.count[n:n + 1], geom=self.geom[n],
+                                           out=self.det_track[n])
                 self._add(track, 1, name='gather_track')
         if pp_streams:
             self._marker('join')
@@ -683,85 +669,59 @@ class SipMaskEngine(object):
         self._geom_copied.record(torch.cuda.current_stream(self.dev))
         self.image_metas = [tuple(m) for m in metas]
 
-    def _mm_candidates(self, n, lv):
-        """MM candidates of image n: decode + per-level top-k (smb_decode_topk), then multi-class NMS (soft-NMS when the
-        nms type is soft_nms), or fast NMS for SSD and VIS (fast_nms with cfg.max_per_img, VIS/...:986).  Returns the
-        candidate -> location table."""
-        cfg, lib, ncls, ncand = self.cfg, L.lib(), self.ncls, self.ncand
-        nl, nms_pre = len(lv), int(cfg['nms_pre'])
+    def _mm_candidates(self, n, head, lv):
+        """MM candidates of image n (head: its (cls, box, ctr) level lists, lv: their level_descs): decode + per-level
+        top-k (decode_topk), then multi-class NMS (soft-NMS when the nms type is soft_nms), or fast NMS for SSD and VIS
+        (fast_nms with cfg.max_per_img, VIS/...:986).  Returns the candidate -> location table."""
+        cfg, ncls, ncand, nms_pre = self.cfg, self.ncls, self.ncand, int(self.cfg['nms_pre'])
         boxes, scores, ctr, loc = self.cand_boxes[n], self.cand_scores[n], self.cand_ctr[n], self.cand_loc[n]
-        det, labels, idx, count = self.det[n], self.labels[n], self.idx[n], self.count[n:n + 1]
-        ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, nms_pre)
-        ws = self._t(ws_bytes, dtype=torch.uint8)
+        rec = (self.det[n], self.labels[n], self.idx[n], self.count[n:n + 1])
+        ws = self._t(ops.decode_workspace_bytes(lv, nms_pre), dtype=torch.uint8)
 
         def decode(n=n):
-            L.check(lib.smb_decode_topk_dev(nl, lv, ncls, nms_pre, L.ptr(self.geom[n]), L.ptr(boxes), L.ptr(scores), L.ptr(ctr),
-                                            L.ptr(loc), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_decode_topk_dev')
+            ops.decode_topk(*head, self.strides, None, nms_pre, box_scales=self.scales, geom=self.geom[n],
+                            out=(boxes, scores, ctr, loc), workspace=ws)
         self._add(decode, 3, name='decode_topk')
-        if self.soft_nms is not None:
-            if ncand > ops.SOFT_NMS_MAX:
-                raise ValueError('soft_nms: %d candidates (nms_pre=%d) exceed the soft-NMS capacity %d'
-                                 % (ncand, nms_pre, ops.SOFT_NMS_MAX))
-            iou, method, sigma, min_score = self.soft_nms
-            nws_bytes = lib.smb_multiclass_soft_nms_workspace_bytes(ncand, ncls)
-            nws = self._t(nws_bytes, dtype=torch.uint8)
+        if self.ssd or self.vis:
+            iou_thr = float(cfg['nms']['iou_thr'])
+            nws = self._t(ops.fast_nms_workspace_bytes(ncand, ncls, 200), dtype=torch.uint8)
 
             def nms(n=n):
-                L.check(lib.smb_multiclass_soft_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls,
-                                                    ctypes.c_float(cfg['score_thr']), ctypes.c_float(iou), self.max_num,
-                                                    method, ctypes.c_float(sigma), ctypes.c_float(min_score), L.ptr(det),
-                                                    L.ptr(labels), L.ptr(idx), L.ptr(count), L.ptr(nws),
-                                                    ctypes.c_size_t(nws_bytes), L.stream_ptr()), 'smb_multiclass_soft_nms')
+                ops.fast_nms(boxes, scores, ctr, iou_thr, 200, cfg['score_thr'], self.max_num, out=rec, workspace=nws)
             self._add(nms, 2, name='nms')
             return loc
-        iou_thr = float(cfg['nms']['iou_thr'])
-        if not (self.ssd or self.vis):
-            nws_bytes = lib.smb_multiclass_nms_workspace_bytes(ncand, ncls)
-            nws = self._t(nws_bytes, dtype=torch.uint8)
-
-            def nms(n=n):
-                L.check(lib.smb_multiclass_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls, ctypes.c_float(cfg['score_thr']),
-                                               ctypes.c_float(iou_thr), self.max_num, 0, L.ptr(det), L.ptr(labels), L.ptr(idx),
-                                               L.ptr(count), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()),
-                        'smb_multiclass_nms')
-            self._add(nms, 4, name='nms')
-        else:
-            nws_bytes = lib.smb_fast_nms_workspace_bytes(ncand, ncls, 200)
-            nws = self._t(nws_bytes, dtype=torch.uint8)
-
-            def nms(n=n):
-                L.check(lib.smb_fast_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), ncand, ncls, ctypes.c_float(cfg['score_thr']),
-                                         ctypes.c_float(iou_thr), 200, self.max_num, L.ptr(det), L.ptr(labels), L.ptr(idx),
-                                         L.ptr(count), L.ptr(nws), ctypes.c_size_t(nws_bytes), L.stream_ptr()), 'smb_fast_nms')
-            self._add(nms, 2, name='nms')
-        return loc
-
-    def _bm_candidates(self, n, lv):
-        """BM candidates of image n: (location, class) pairs above score_thr, the top nms_pre per level
-        (smb_pair_decode_topk), then label-aware NMS and the k-th-value cut (smb_ml_nms_topk), which also writes
-        kept_total[n].  Returns the candidate -> location table."""
-        cfg, lib, ncls, ncand = self.cfg, L.lib(), self.ncls, self.ncand
-        nl, nms_pre = len(lv), int(cfg['nms_pre'])
-        boxes, scores, labels, loc = self.cand_boxes[n], self.cand_scores[n], self.cand_labels[n], self.cand_loc[n]
-        n_cand = self.n_cand[n:n + 1]
-        ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, ncls, nms_pre)
-        ws = self._t(ws_bytes, dtype=torch.uint8)
-
-        def decode(n=n):
-            L.check(lib.smb_pair_decode_topk_dev(nl, lv, ncls, ctypes.c_float(cfg['score_thr']), nms_pre, L.ptr(self.geom[n]),
-                                                 L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(loc), L.ptr(n_cand), ncand,
-                                                 L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
-                    'smb_pair_decode_topk_dev')
-        self._add(decode, 3, name='decode_topk')
-        nws_bytes = lib.smb_ml_nms_workspace_bytes(ncand)
-        nws = self._t(nws_bytes, dtype=torch.uint8)
+        soft = self.soft_nms is not None
+        if soft and ncand > ops.SOFT_NMS_MAX:
+            raise ValueError('soft_nms: %d candidates (nms_pre=%d) exceed the soft-NMS capacity %d'
+                             % (ncand, nms_pre, ops.SOFT_NMS_MAX))
+        nms_cfg = cfg['nms'] if soft else float(cfg['nms']['iou_thr'])
+        nws = self._t(ops.multiclass_nms_workspace_bytes(ncand, ncls, soft), dtype=torch.uint8)
 
         def nms(n=n):
-            L.check(lib.smb_ml_nms_topk(L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(n_cand), ncand,
-                                        ctypes.c_float(cfg['nms']['iou_thr']), self.max_num, self.max_num, L.ptr(self.det[n]),
-                                        L.ptr(self.labels[n]), L.ptr(self.idx[n]), L.ptr(self.count[n:n + 1]),
-                                        L.ptr(self.kept_total[n:n + 1]), L.ptr(nws), ctypes.c_size_t(nws_bytes),
-                                        L.stream_ptr()), 'smb_ml_nms_topk')
+            ops.multiclass_nms_idx(boxes, scores, cfg['score_thr'], nms_cfg, self.max_num, score_factors=ctr,
+                                   has_bg_column=False, out=rec, workspace=nws)
+        self._add(nms, 2 if soft else 4, name='nms')
+        return loc
+
+    def _bm_candidates(self, n, head, lv):
+        """BM candidates of image n (head, lv as _mm_candidates): (location, class) pairs above score_thr, the top nms_pre
+        per level (pair_decode_topk), then label-aware NMS and the k-th-value cut (ml_nms_topk), which also writes
+        kept_total[n].  Returns the candidate -> location table."""
+        cfg, ncls, ncand, nms_pre = self.cfg, self.ncls, self.ncand, int(self.cfg['nms_pre'])
+        boxes, scores, labels, loc = self.cand_boxes[n], self.cand_scores[n], self.cand_labels[n], self.cand_loc[n]
+        n_cand = self.n_cand[n:n + 1]
+        ws = self._t(ops.pair_decode_workspace_bytes(lv, ncls, nms_pre), dtype=torch.uint8)
+
+        def decode(n=n):
+            ops.pair_decode_topk(*head, self.strides, None, nms_pre, cfg['score_thr'], box_scales=self.scales,
+                                 geom=self.geom[n], out=(boxes, scores, labels, loc, n_cand), workspace=ws)
+        self._add(decode, 3, name='decode_topk')
+        nws = self._t(ops.ml_nms_workspace_bytes(ncand), dtype=torch.uint8)
+
+        def nms(n=n):
+            ops.ml_nms_topk(boxes, scores, labels, n_cand, cfg['nms']['iou_thr'], self.max_num, self.max_num,
+                            out=(self.det[n], self.labels[n], self.idx[n], self.count[n:n + 1], self.kept_total[n:n + 1]),
+                            workspace=nws)
         self._add(nms, 4, name='nms')
         return loc
 

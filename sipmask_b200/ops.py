@@ -242,9 +242,17 @@ def level_descs(cls_list, box_list, ctr_list, strides, box_scales):
     return lv, keep_alive
 
 
+def decode_workspace_bytes(levels, nms_pre):
+    return int(L.lib().smb_decode_workspace_bytes(len(levels), levels, int(nms_pre)))
+
+
 @L.device_guard
-def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale_factor=None, box_scales=None):
+def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale_factor=None, box_scales=None, geom=None,
+                out=None, workspace=None):
     """Per-level tensors channel-last fp32: cls [h,w,C], box [h,w,4] (distances x stride), ctr [h,w,1|].
+    geom: a device geometry row (geom_row), read when the kernels run in place of img_shape and scale_factor.
+    out / workspace: the (boxes, scores, ctr, loc) buffers and a uint8 tensor of decode_workspace_bytes to use; with both
+    the call only launches (graph-capturable).
 
     Returns cand_boxes [n,4], cand_scores [n,C], cand_ctr [n], cand_loc [n] int32."""
     nl = len(cls_list)
@@ -252,174 +260,174 @@ def decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre, scale
     lv, keep_alive = level_descs(cls_list, box_list, ctr_list, strides, box_scales)
     lib = L.lib()
     dev = cls_list[0].device
-    ws_bytes = lib.smb_decode_workspace_bytes(nl, lv, int(nms_pre))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    n = sum(min(c.shape[0] * c.shape[1], nms_pre) if nms_pre > 0 else c.shape[0] * c.shape[1] for c in cls_list)
-    boxes = torch.empty((n, 4), dtype=torch.float32, device=dev)
-    scores = torch.empty((n, C), dtype=torch.float32, device=dev)
-    ctr = torch.empty((n,), dtype=torch.float32, device=dev)
-    loc = torch.empty((n,), dtype=torch.int32, device=dev)
+    if workspace is None:
+        workspace = torch.empty(decode_workspace_bytes(lv, nms_pre), dtype=torch.uint8, device=dev)
+    if out is None:
+        n = sum(min(c.shape[0] * c.shape[1], nms_pre) if nms_pre > 0 else c.shape[0] * c.shape[1] for c in cls_list)
+        out = (torch.empty((n, 4), dtype=torch.float32, device=dev), torch.empty((n, C), dtype=torch.float32, device=dev),
+               torch.empty((n,), dtype=torch.float32, device=dev), torch.empty((n,), dtype=torch.int32, device=dev))
+    args = [L.ptr(t) for t in out] + [L.ptr(workspace), ctypes.c_size_t(workspace.numel()), L.stream_ptr()]
+    if geom is not None:
+        L.check(lib.smb_decode_topk_dev(nl, lv, C, int(nms_pre), L.ptr(geom), *args), 'smb_decode_topk_dev')
+        return out
     sf = None
     if scale_factor is not None:
         a = np.atleast_1d(np.asarray(scale_factor, dtype=np.float32))
         sf = L.f4(a if a.size == 4 else [a[0]] * 4)
-    L.check(lib.smb_decode_topk(nl, lv, C, int(nms_pre), int(img_shape[0]), int(img_shape[1]), sf, L.ptr(boxes),
-                                L.ptr(scores), L.ptr(ctr), L.ptr(loc), L.ptr(ws), ctypes.c_size_t(ws_bytes),
-                                L.stream_ptr()), 'smb_decode_topk')
-    return boxes, scores, ctr, loc
+    L.check(lib.smb_decode_topk(nl, lv, C, int(nms_pre), int(img_shape[0]), int(img_shape[1]), sf, *args), 'smb_decode_topk')
+    return out
+
+
+def pair_decode_workspace_bytes(levels, num_classes, nms_pre):
+    return int(L.lib().smb_pair_decode_workspace_bytes(len(levels), levels, int(num_classes), int(nms_pre)))
 
 
 @L.device_guard
-def pair_decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre=1000, score_thr=0.05, box_scales=None):
+def pair_decode_topk(cls_list, box_list, ctr_list, strides, img_shape, nms_pre=1000, score_thr=0.05, box_scales=None,
+                     geom=None, out=None, workspace=None):
     """SipMask-benchmark candidate selection (smb_pair_decode_topk).  Per-level channel-last fp32 tensors as decode_topk:
     cls [h,w,C] logits, ctr [h,w,1|], box [h,w,4]; distances are relu(box * box_scales[l]) * strides[l] when box_scales is
     given (raw bbox_pred), else relu(box).  Returns (boxes [n,4], scores [n] = sqrt(cls * ctr), labels [n] int32 0-based,
-    loc [n] int32, n_cand device int32 [1]); n is the slot capacity, rows past n_cand are zero / -1."""
+    loc [n] int32, n_cand device int32 [1]); n is the slot capacity, rows past n_cand are zero / -1.
+    geom / out / workspace as decode_topk (geom in place of img_shape; the workspace of pair_decode_workspace_bytes)."""
     nl = len(cls_list)
     C = cls_list[0].shape[-1]
     lv, keep_alive = level_descs(cls_list, box_list, ctr_list, strides, box_scales)
     lib = L.lib()
     dev = cls_list[0].device
-    n = lib.smb_pair_decode_slots(nl, lv, C, int(nms_pre))
-    if n < 0:
-        raise L.SmbError('pair_decode_topk: unsupported levels / nms_pre=%d' % nms_pre)
-    ws_bytes = lib.smb_pair_decode_workspace_bytes(nl, lv, C, int(nms_pre))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    boxes = torch.empty((n, 4), dtype=torch.float32, device=dev)
-    scores = torch.empty((n,), dtype=torch.float32, device=dev)
-    labels = torch.empty((n,), dtype=torch.int32, device=dev)
-    loc = torch.empty((n,), dtype=torch.int32, device=dev)
-    n_cand = torch.empty((1,), dtype=torch.int32, device=dev)
-    L.check(lib.smb_pair_decode_topk(nl, lv, C, ctypes.c_float(score_thr), int(nms_pre), int(img_shape[0]), int(img_shape[1]),
-                                     L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(loc), L.ptr(n_cand), n, L.ptr(ws),
-                                     ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_pair_decode_topk')
-    return boxes, scores, labels, loc, n_cand
+    if out is None:
+        n = lib.smb_pair_decode_slots(nl, lv, C, int(nms_pre))
+        if n < 0:
+            raise L.SmbError('pair_decode_topk: unsupported levels / nms_pre=%d' % nms_pre)
+        out = (torch.empty((n, 4), dtype=torch.float32, device=dev), torch.empty((n,), dtype=torch.float32, device=dev),
+               torch.empty((n,), dtype=torch.int32, device=dev), torch.empty((n,), dtype=torch.int32, device=dev),
+               torch.empty((1,), dtype=torch.int32, device=dev))
+    if workspace is None:
+        workspace = torch.empty(pair_decode_workspace_bytes(lv, C, nms_pre), dtype=torch.uint8, device=dev)
+    args = [L.ptr(t) for t in out] + [out[0].shape[0], L.ptr(workspace), ctypes.c_size_t(workspace.numel()), L.stream_ptr()]
+    if geom is not None:
+        L.check(lib.smb_pair_decode_topk_dev(nl, lv, C, ctypes.c_float(score_thr), int(nms_pre), L.ptr(geom), *args),
+                'smb_pair_decode_topk_dev')
+    else:
+        L.check(lib.smb_pair_decode_topk(nl, lv, C, ctypes.c_float(score_thr), int(nms_pre), int(img_shape[0]),
+                                         int(img_shape[1]), *args), 'smb_pair_decode_topk')
+    return out
+
+
+def ml_nms_workspace_bytes(cap):
+    return int(L.lib().smb_ml_nms_workspace_bytes(int(cap)))
 
 
 @L.device_guard
-def ml_nms_topk(boxes, scores, labels, n_cand, iou_thr=0.6, max_per_img=100, out_cap=None):
+def ml_nms_topk(boxes, scores, labels, n_cand, iou_thr=0.6, max_per_img=100, out_cap=None, out=None, workspace=None):
     """SipMask-benchmark label-aware NMS + k-th-value cut (smb_ml_nms_topk) over the first *n_cand rows of boxes [cap,4],
     scores [cap], labels [cap] int32.  Returns (det [out_cap,5], labels int64, idx int64, count int32 [1], kept_total
-    int32 [1]); out_cap defaults to cap."""
+    int32 [1]); out_cap defaults to cap.  out / workspace: those five buffers and a uint8 tensor of ml_nms_workspace_bytes
+    to use; with both the call only launches."""
     _need_cuda(boxes, scores, labels, n_cand)
     boxes, scores = boxes.float().contiguous(), scores.float().contiguous()
     labels, n_cand = labels.to(torch.int32).contiguous(), n_cand.to(torch.int32).contiguous()
     cap = boxes.shape[0]
     out_cap = cap if out_cap is None else int(out_cap)
     dev = boxes.device
-    lib = L.lib()
-    ws_bytes = lib.smb_ml_nms_workspace_bytes(cap)
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-    det = torch.empty((out_cap, 5), dtype=torch.float32, device=dev)
-    lab = torch.empty((out_cap,), dtype=torch.long, device=dev)
-    idx = torch.empty((out_cap,), dtype=torch.long, device=dev)
-    cnt = torch.empty((1,), dtype=torch.int32, device=dev)
-    total = torch.empty((1,), dtype=torch.int32, device=dev)
-    L.check(lib.smb_ml_nms_topk(L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(n_cand), cap, ctypes.c_float(iou_thr),
-                                int(max_per_img), out_cap, L.ptr(det), L.ptr(lab), L.ptr(idx), L.ptr(cnt), L.ptr(total),
-                                L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_ml_nms_topk')
-    return det, lab, idx, cnt, total
+    if workspace is None:
+        workspace = torch.empty(max(ml_nms_workspace_bytes(cap), 1), dtype=torch.uint8, device=dev)
+    if out is None:
+        out = (torch.empty((out_cap, 5), dtype=torch.float32, device=dev), torch.empty((out_cap,), dtype=torch.long, device=dev),
+               torch.empty((out_cap,), dtype=torch.long, device=dev), torch.empty((1,), dtype=torch.int32, device=dev),
+               torch.empty((1,), dtype=torch.int32, device=dev))
+    L.check(L.lib().smb_ml_nms_topk(L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(n_cand), cap, ctypes.c_float(iou_thr),
+                                    int(max_per_img), out_cap, *[L.ptr(t) for t in out], L.ptr(workspace),
+                                    ctypes.c_size_t(workspace.numel()), L.stream_ptr()), 'smb_ml_nms_topk')
+    return out
 
 
 # ------------------------------------------------------------------------------------ multi-class NMS
+def _nms_record(out, max_num, dev):
+    """The (det [max_num,5], labels int64, idx int64, count int32 [1]) buffers an NMS writes: `out`, or new ones."""
+    if out is not None:
+        return out
+    return (torch.empty((max_num, 5), dtype=torch.float32, device=dev), torch.empty((max_num,), dtype=torch.long, device=dev),
+            torch.empty((max_num,), dtype=torch.long, device=dev), torch.zeros(1, dtype=torch.int32, device=dev))
+
+
+def _nms_result(rec, whole):
+    """The record itself (whole), or its first count rows of (det, labels, idx) after reading the count on the host."""
+    if whole:
+        return rec
+    k = int(rec[3].item())
+    return rec[0][:k], rec[1][:k], rec[2][:k]
+
+
+def multiclass_nms_workspace_bytes(n, num_classes, soft=False):
+    lib = L.lib()
+    f = lib.smb_multiclass_soft_nms_workspace_bytes if soft else lib.smb_multiclass_nms_workspace_bytes
+    return int(f(int(n), int(num_classes)))
+
+
 @L.device_guard
 def multiclass_nms_idx(multi_bboxes, multi_scores, score_thr, nms_cfg, max_num=-1, score_factors=None,
-                       has_bg_column=True, cmp_ge=False, return_count_tensor=False):
+                       has_bg_column=True, cmp_ge=False, return_count_tensor=False, out=None, workspace=None):
     """Same contract as mmdet.core.multiclass_nms_idx (bbox_nms.py:79-146): returns
     (dets [k,5], labels [k] int64 0-based, idxs [k] int64).  `multi_scores` carries the background
     column 0 like the reference unless has_bg_column=False.  nms_cfg['type'] selects 'nms' (the default) or 'soft_nms'
-    (smb_multiclass_soft_nms: decayed scores in dets, each class in selection order); any other type raises."""
+    (smb_multiclass_soft_nms: decayed scores in dets, each class in selection order); any other type raises.
+    out / workspace: the (det, labels, idx, count) buffers and a uint8 tensor of multiclass_nms_workspace_bytes to use; with
+    both and score_factors the call only launches and returns the whole record, as return_count_tensor does."""
     _need_cuda(multi_bboxes, multi_scores)
     kind = nms_type(nms_cfg) if isinstance(nms_cfg, dict) else 'nms'
-    if kind == 'soft_nms':
-        return _multiclass_soft_nms(multi_bboxes, multi_scores, score_thr, nms_cfg, max_num, score_factors, has_bg_column,
-                                    return_count_tensor)
-    if kind != 'nms':
+    if kind not in ('nms', 'soft_nms'):
         raise ValueError("multiclass_nms_idx: nms type %r (supported: 'nms', 'soft_nms')" % (kind,))
-    iou_thr = nms_cfg.get('iou_thr', 0.5) if isinstance(nms_cfg, dict) else float(nms_cfg)
-    scores = multi_scores[:, 1:] if has_bg_column else multi_scores
-    scores = scores.float().contiguous()
-    boxes = multi_bboxes.float().contiguous()
-    n, C = scores.shape
-    dev = boxes.device
-    if score_factors is None:
-        score_factors = torch.ones(n, dtype=torch.float32, device=dev)
-    ctr = score_factors.float().contiguous()
-    if max_num is None or max_num <= 0:
-        max_num = 1024
-    lib = L.lib()
-    ws_bytes = lib.smb_multiclass_nms_workspace_bytes(n, C)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    det = torch.empty((max_num, 5), dtype=torch.float32, device=dev)
-    lab = torch.empty((max_num,), dtype=torch.long, device=dev)
-    idx = torch.empty((max_num,), dtype=torch.long, device=dev)
-    cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-    L.check(lib.smb_multiclass_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), n, C, ctypes.c_float(score_thr),
-                                   ctypes.c_float(iou_thr), int(max_num), int(cmp_ge), L.ptr(det), L.ptr(lab),
-                                   L.ptr(idx), L.ptr(cnt), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
-            'smb_multiclass_nms')
-    if return_count_tensor:
-        return det, lab, idx, cnt
-    k = int(cnt.item())
-    return det[:k], lab[:k], idx[:k]
-
-
-def _multiclass_soft_nms(multi_bboxes, multi_scores, score_thr, nms_cfg, max_num, score_factors, has_bg_column,
-                         return_count_tensor):
-    iou_thr, method, sigma, min_score = soft_nms_args(nms_cfg)
+    soft = kind == 'soft_nms'
+    if soft:
+        iou_thr, method, sigma, min_score = soft_nms_args(nms_cfg)
+    else:
+        iou_thr = nms_cfg.get('iou_thr', 0.5) if isinstance(nms_cfg, dict) else float(nms_cfg)
     scores = (multi_scores[:, 1:] if has_bg_column else multi_scores).float().contiguous()
     boxes = multi_bboxes.float().contiguous()
     n, C = scores.shape
-    if n > SOFT_NMS_MAX:
+    if soft and n > SOFT_NMS_MAX:
         raise L.SmbError('multiclass soft_nms: %d candidates, at most %d' % (n, SOFT_NMS_MAX))
     dev = boxes.device
-    ctr = (torch.ones(n, dtype=torch.float32, device=dev) if score_factors is None else score_factors.float().contiguous())
+    ctr = torch.ones(n, dtype=torch.float32, device=dev) if score_factors is None else score_factors.float().contiguous()
     if max_num is None or max_num <= 0:
         max_num = 1024
-    lib = L.lib()
-    ws_bytes = lib.smb_multiclass_soft_nms_workspace_bytes(n, C)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    det = torch.empty((max_num, 5), dtype=torch.float32, device=dev)
-    lab = torch.empty((max_num,), dtype=torch.long, device=dev)
-    idx = torch.empty((max_num,), dtype=torch.long, device=dev)
-    cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-    L.check(lib.smb_multiclass_soft_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), n, C, ctypes.c_float(score_thr),
-                                        ctypes.c_float(iou_thr), int(max_num), method, ctypes.c_float(sigma),
-                                        ctypes.c_float(min_score), L.ptr(det), L.ptr(lab), L.ptr(idx), L.ptr(cnt),
-                                        L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()), 'smb_multiclass_soft_nms')
-    if return_count_tensor:
-        return det, lab, idx, cnt
-    k = int(cnt.item())
-    return det[:k], lab[:k], idx[:k]
+    if workspace is None:
+        workspace = torch.empty(multiclass_nms_workspace_bytes(n, C, soft), dtype=torch.uint8, device=dev)
+    rec = _nms_record(out, max_num, dev)
+    head = (L.ptr(boxes), L.ptr(scores), L.ptr(ctr), n, C, ctypes.c_float(score_thr), ctypes.c_float(iou_thr), int(max_num))
+    tail = [L.ptr(t) for t in rec] + [L.ptr(workspace), ctypes.c_size_t(workspace.numel()), L.stream_ptr()]
+    if soft:
+        L.check(L.lib().smb_multiclass_soft_nms(*head, method, ctypes.c_float(sigma), ctypes.c_float(min_score), *tail),
+                'smb_multiclass_soft_nms')
+    else:
+        L.check(L.lib().smb_multiclass_nms(*head, int(cmp_ge), *tail), 'smb_multiclass_nms')
+    return _nms_result(rec, return_count_tensor or out is not None)
+
+
+def fast_nms_workspace_bytes(n, num_classes, top_k):
+    return int(L.lib().smb_fast_nms_workspace_bytes(int(n), int(num_classes), int(top_k)))
 
 
 @L.device_guard
 def fast_nms(boxes, scores, ctr, iou_threshold=0.5, top_k=200, score_thr=0.1, max_num=100,
-             return_count_tensor=False):
+             return_count_tensor=False, out=None, workspace=None):
     """boxes [n,4], scores [n,C] sigmoid (NOT yet multiplied by ctr), ctr [n].
     Returns (dets [k,5], classes [k], idx [k]) like SipMaskHead.fast_nms (sipmask_head.py:868-910)
-    with the coefficient gather left to the caller (`cofs[idx]`)."""
+    with the coefficient gather left to the caller (`cofs[idx]`).  out / workspace as multiclass_nms_idx (the workspace of
+    fast_nms_workspace_bytes)."""
     _need_cuda(boxes, scores, ctr)
     boxes = boxes.float().contiguous()
     scores = scores.float().contiguous()
     ctr = ctr.float().contiguous()
     n, C = scores.shape
-    dev = boxes.device
-    lib = L.lib()
-    ws_bytes = lib.smb_fast_nms_workspace_bytes(n, C, int(top_k))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    det = torch.empty((max_num, 5), dtype=torch.float32, device=dev)
-    lab = torch.empty((max_num,), dtype=torch.long, device=dev)
-    idx = torch.empty((max_num,), dtype=torch.long, device=dev)
-    cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-    L.check(lib.smb_fast_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), n, C, ctypes.c_float(score_thr),
-                             ctypes.c_float(iou_threshold), int(top_k), int(max_num), L.ptr(det), L.ptr(lab),
-                             L.ptr(idx), L.ptr(cnt), L.ptr(ws), ctypes.c_size_t(ws_bytes), L.stream_ptr()),
-            'smb_fast_nms')
-    if return_count_tensor:
-        return det, lab, idx, cnt
-    k = int(cnt.item())
-    return det[:k], lab[:k], idx[:k]
+    if workspace is None:
+        workspace = torch.empty(fast_nms_workspace_bytes(n, C, top_k), dtype=torch.uint8, device=boxes.device)
+    rec = _nms_record(out, max_num, boxes.device)
+    L.check(L.lib().smb_fast_nms(L.ptr(boxes), L.ptr(scores), L.ptr(ctr), n, C, ctypes.c_float(score_thr),
+                                 ctypes.c_float(iou_threshold), int(top_k), int(max_num), *[L.ptr(t) for t in rec],
+                                 L.ptr(workspace), ctypes.c_size_t(workspace.numel()), L.stream_ptr()), 'smb_fast_nms')
+    return _nms_result(rec, return_count_tensor or out is not None)
 
 
 @L.device_guard
@@ -435,22 +443,47 @@ def gather_rows(src, idx, count, max_rows):
 
 
 @L.device_guard
-def gather_track_feats(track_feats, det, count, scale_factor=1.0, feat_stride=8.0):
+def gather_det_inputs(cof_src, cand_loc, idx, det, count, det_cofs, det_boxes, loc_out=None, level_hw=None, n_img=1, img=0):
+    """smb_gather_det_inputs, the gather between NMS and mask assembly (mlvl_cofs[idxs_keep], det_bboxes[:, :4];
+    sipmask_head.py:612,623) in one launch: det_cofs[i] = cof_src[cand_loc[idx[i]]] and det_boxes[i] = det[i, :4] for
+    i < count (device int32 [1]), zeros after; loc_out (int64, optional) receives the kept locations, -1 after count.
+    cof_src [rows, E] fp32 with row pitch stride(0) is one image's level-concatenated table (level_hw None), or a batched
+    level-major buffer [level][n_img][h_l * w_l] of which image `img` is gathered (level_hw: h_l * w_l per level)."""
+    _need_cuda(cof_src, cand_loc, idx, det, count, det_cofs, det_boxes, loc_out)
+    max_rows, E = det_cofs.shape
+    hw = None if level_hw is None else (ctypes.c_int * len(level_hw))(*level_hw)
+    L.check(L.lib().smb_gather_det_inputs(L.ptr(cof_src), cof_src.stride(0), L.ptr(cand_loc), L.ptr(idx), L.ptr(det),
+                                          L.ptr(count), max_rows, E, L.ptr(det_cofs), L.ptr(det_boxes), L.ptr(loc_out),
+                                          0 if hw is None else len(hw), hw, int(n_img), int(img), L.stream_ptr()),
+            'smb_gather_det_inputs')
+
+
+@L.device_guard
+def gather_track_feats(track_feats, det, count, scale_factor=1.0, feat_stride=8.0, geom=None, out=None):
     """SipMask-VIS `extract_box_feature_center_single`: track_feats [512,h,w] (reference layout) or [h,w,512] channel-last
-    fp32, det [max,5], count device int -> [max,512] features at floor((x1+x2) * sf / 2 / 8) (zeros after count)."""
+    fp32, det [max,5], count device int -> [max,512] features at floor((x1+x2) * sf / 2 / 8) (zeros after count).
+    geom: a device geometry row whose track scale is read when the kernel runs, in place of scale_factor.  out: the
+    [max,512] buffer to write."""
     _need_cuda(track_feats, det, count)
     t = track_feats.float()
     if t.shape[0] == 512 and t.shape[-1] != 512:
         t = t.permute(1, 2, 0)
     t = t.contiguous()
     h, w, C = t.shape
+    det = det.float().contiguous()
+    count = count.to(torch.int32)
+    if out is None:
+        out = torch.empty((det.shape[0], C), dtype=torch.float32, device=det.device)
+    if geom is not None:
+        L.check(L.lib().smb_gather_track_feats_dev(L.ptr(t), h, w, C, L.ptr(det), L.ptr(count), det.shape[0], L.ptr(geom),
+                                                   ctypes.c_float(feat_stride), L.ptr(out), L.stream_ptr()),
+                'smb_gather_track_feats_dev')
+        return out
     a = np.atleast_1d(np.asarray(scale_factor, dtype=np.float32))
     sx, sy = float(a[0]), float(a[1] if a.size >= 2 else a[0])
-    det = det.float().contiguous()
-    out = torch.empty((det.shape[0], C), dtype=torch.float32, device=det.device)
-    L.check(L.lib().smb_gather_track_feats(L.ptr(t), h, w, C, L.ptr(det), L.ptr(count.to(torch.int32)), det.shape[0],
-                                           ctypes.c_float(sx), ctypes.c_float(sy), ctypes.c_float(feat_stride), L.ptr(out),
-                                           L.stream_ptr()), 'smb_gather_track_feats')
+    L.check(L.lib().smb_gather_track_feats(L.ptr(t), h, w, C, L.ptr(det), L.ptr(count), det.shape[0], ctypes.c_float(sx),
+                                           ctypes.c_float(sy), ctypes.c_float(feat_stride), L.ptr(out), L.stream_ptr()),
+            'smb_gather_track_feats')
     return out
 
 
@@ -462,9 +495,10 @@ def set_mask_tensor_dot(on):
     return bool(L.lib().smb_mask_set_tensor_dot(-1 if on is None else int(bool(on))))
 
 
-def mask_assemble(protos, cofs, boxes, box_scale, layout='chw', out_dtype=torch.float32, out=None):
+def mask_assemble(protos, cofs, boxes, box_scale, layout='chw', out_dtype=torch.float32, out=None, geom=None):
     """protos [32,H,W] ('chw') or [H,W,32] ('hwc'), fp32/fp16; cofs [N,128] fp32; boxes [N,4] fp32
-    (image space); rois = boxes * box_scale (scalar or 4-vector).  Returns pos_masks [N,H,W]."""
+    (image space); rois = boxes * box_scale (scalar or 4-vector), or * the roi scale of the device geometry row `geom`
+    read when the kernel runs (box_scale is then unused).  Returns pos_masks [N,H,W]."""
     _need_cuda(protos, cofs, boxes)
     protos = protos.contiguous()
     if layout == 'chw':
@@ -474,13 +508,17 @@ def mask_assemble(protos, cofs, boxes, box_scale, layout='chw', out_dtype=torch.
     N = cofs.shape[0]
     cofs = cofs.float().contiguous()
     boxes = boxes.float().contiguous()
-    a = np.atleast_1d(np.asarray(box_scale, dtype=np.float32))
-    bs = L.f4(a if a.size == 4 else [a[0]] * 4)
     if out is None:
         out = torch.empty((N, H, W), dtype=out_dtype, device=protos.device)
-    L.check(L.lib().smb_mask_assemble(L.ptr(protos), _dt(protos), 1 if layout == 'hwc' else 0, L.ptr(cofs),
-                                      L.ptr(boxes), bs, L.ptr(out), _dt(out), H, W, N, L.stream_ptr()),
-            'smb_mask_assemble')
+    hwc = 1 if layout == 'hwc' else 0
+    if geom is not None:
+        L.check(L.lib().smb_mask_assemble_dev(L.ptr(protos), _dt(protos), hwc, L.ptr(cofs), L.ptr(boxes), L.ptr(geom),
+                                              L.ptr(out), _dt(out), H, W, N, L.stream_ptr()), 'smb_mask_assemble_dev')
+        return out
+    a = np.atleast_1d(np.asarray(box_scale, dtype=np.float32))
+    bs = L.f4(a if a.size == 4 else [a[0]] * 4)
+    L.check(L.lib().smb_mask_assemble(L.ptr(protos), _dt(protos), hwc, L.ptr(cofs), L.ptr(boxes), bs, L.ptr(out), _dt(out),
+                                      H, W, N, L.stream_ptr()), 'smb_mask_assemble')
     return out
 
 
