@@ -130,14 +130,21 @@ __global__ void preprocess_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows,
 // in -> out axis, scale = in / out, fs = max(scale, 1) (= the bilinear support), center = (xx + 0.5) * scale, taps
 // [xmin, xmin + n) with xmin = max((int)(center - fs + 0.5), 0), xmin + n = min((int)(center + fs + 0.5), in), weights
 // tri(((x + xmin) - center + 0.5) * (1 / fs)) summed in order in double, divided by the sum and stored as
-// (int)(0.5 + k * 2^22).  The horizontal pass runs first and clips to uint8; each pass is clamp((2^21 + sum v * k) >> 22,
-// 0, 255).  An axis whose size does not change gets the taps {2^22, 0}, which copy it exactly (Pillow skips that pass).
+// (int)(0.5 + k * 2^22).  The first pass clips to uint8; each pass is clamp((2^21 + sum v * k) >> 22, 0, 255).  The
+// horizontal pass runs first, except where Image.resize runs the vertical one first: for an image more than 100 times
+// taller than wide whose height shrinks.  The order changes the bits, because the intermediate image is clipped.  An axis
+// whose size does not change gets the taps {2^22, 0}, which copy it exactly (Pillow skips that pass).
 // Every double operation is an explicit _rn intrinsic: the reference (x86-64 Pillow) does not contract to FMA, nvcc would.
 constexpr int PIL_TY = 8, PIL_TX = 32;                        // cells per CTA: 8 x 32 -> 16 output rows x 64 columns
 constexpr int PIL_OY = 2 * PIL_TY, PIL_OX = 2 * PIL_TX;
 constexpr int PIL_MAX_SCALE = 8;                              // steepest downscale per axis (validated by the host)
 constexpr int PIL_KMAX = 2 * PIL_MAX_SCALE + 1;               // taps per output index at that scale (< 2 * fs + 1)
 constexpr int PIL_RMAX = (PIL_OY - 1) * PIL_MAX_SCALE + PIL_KMAX;   // source rows the 16 output rows of a tile read
+constexpr int PIL_CMAX = (PIL_OX - 1) * PIL_MAX_SCALE + PIL_KMAX;   // source columns the 64 output columns of a tile read
+// The tile's intermediate image: horizontal pass first, PIL_RMAX source rows x PIL_OX output columns; vertical pass first,
+// PIL_OY output rows x PIL_CMAX source columns.  One buffer holds either.
+constexpr int PIL_HPASS_BYTES = PIL_RMAX * PIL_OX * 3, PIL_VPASS_BYTES = PIL_OY * PIL_CMAX * 3;
+constexpr int PIL_PASS_BYTES = PIL_HPASS_BYTES > PIL_VPASS_BYTES ? PIL_HPASS_BYTES : PIL_VPASS_BYTES;
 
 // Taps of output index xx of an in -> out axis: first source index, count, fixed-point weights.
 __device__ void pil_taps(int xx, int in, int out, int* lo, int* cnt, int* w) {
@@ -167,25 +174,33 @@ __device__ void pil_taps(int xx, int in, int out, int* lo, int* cnt, int* w) {
 __device__ __forceinline__ int pil_clip8(int v) { return min(max(v >> 22, 0), 255); }
 
 // One CTA = a tile of PIL_TY x PIL_TX cells of canvas blockIdx.z.  It computes the taps of the tile's output columns and
-// rows once, runs the horizontal pass over the source rows those output rows need into shared memory (uint8, as Pillow's
-// intermediate image), then each thread runs the vertical pass for its cell's four pixels and writes the cell.  Write
-// indices come from the canvas alone; source indices are clamped inside the row's image and shared-memory rows inside
+// rows once, runs the first pass into shared memory (uint8, as Pillow's intermediate image), then each thread runs the
+// second pass for its cell's four pixels and writes the cell.  Horizontal first: the first pass covers the source rows
+// the tile's output rows need, at its output columns.  Vertical first: it covers the tile's output rows, at the source
+// columns its output columns need.  The order is a property of the canvas's row, so it is uniform over the CTA.  Write
+// indices come from the canvas alone; source indices are clamped inside the row's image and shared-memory indices inside
 // the tile's buffer, so an unvalidated row cannot make the kernel touch memory outside them.
-__global__ void __launch_bounds__(PIL_TY * PIL_TX) preprocess_pil_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows,
-                                                                               __half* __restrict__ out, int H, int W) {
-  __shared__ int cx_lo[PIL_OX], cx_n[PIL_OX], cx_w[PIL_OX][PIL_KMAX];
-  __shared__ int cy_lo[PIL_OY], cy_n[PIL_OY], cy_w[PIL_OY][PIL_KMAX];
-  __shared__ uint8_t hpass[PIL_RMAX][PIL_OX * 3];
+struct PilSmem {
+  int cx_lo[PIL_OX], cx_n[PIL_OX], cx_w[PIL_OX][PIL_KMAX];
+  int cy_lo[PIL_OY], cy_n[PIL_OY], cy_w[PIL_OY][PIL_KMAX];
+  uint8_t pass[PIL_PASS_BYTES];
+};
+
+// The tile with the passes in one order, compiled once per order so that neither pays for the other's branches.
+template <bool VFIRST>
+__device__ __forceinline__ void pil_tile(PilSmem& s, const smb_raw_src_t& r, int dh, int dw, __half* __restrict__ out,
+                                         int H, int W) {
+  auto& cx_lo = s.cx_lo; auto& cx_n = s.cx_n; auto& cx_w = s.cx_w;
+  auto& cy_lo = s.cy_lo; auto& cy_n = s.cy_n; auto& cy_w = s.cy_w;
+  uint8_t(*hpass)[PIL_OX * 3] = reinterpret_cast<uint8_t(*)[PIL_OX * 3]>(s.pass);       // [PIL_RMAX][PIL_OX * 3]
+  uint8_t(*vpass)[PIL_CMAX * 3] = reinterpret_cast<uint8_t(*)[PIL_CMAX * 3]>(s.pass);   // [PIL_OY][PIL_CMAX * 3]
   const int Hq = H / 2 + 3, Wq = W / 2 + 4;
   const int n = blockIdx.z, Y0 = blockIdx.y * PIL_TY, X0 = blockIdx.x * PIL_TX, t = threadIdx.x;
-  const smb_raw_src_t r = rows[n];
-  const bool fill = r.dst_h <= 0 || r.dst_w <= 0;
-  const int dh = fill ? 0 : r.dst_h, dw = fill ? 0 : r.dst_w;
   const int py0 = 2 * Y0 - 3, px0 = 2 * X0 - 3;               // output pixel of the tile's local (0, 0)
   // the tile's output pixels inside the resized image (everything else is halo / padding: zero)
   const int ya = max(py0, 0), yb = min(py0 + PIL_OY, dh), xa = max(px0, 0), xb = min(px0 + PIL_OX, dw);
   const bool any = ya < yb && xa < xb;                        // uniform over the CTA
-  int ybase = 0;
+  int ybase = 0, xbase = 0;
   if (any) {
     if (t < PIL_OX) {
       const int x = px0 + t;
@@ -195,24 +210,46 @@ __global__ void __launch_bounds__(PIL_TY * PIL_TX) preprocess_pil_u8_s2d_kernel(
       if (y >= ya && y < yb) pil_taps(y, r.src_h, dh, &cy_lo[ly], &cy_n[ly], cy_w[ly]);
     }
     __syncthreads();
-    ybase = cy_lo[ya - py0];
-    const int nrows = min(cy_lo[yb - 1 - py0] + cy_n[yb - 1 - py0] - ybase, PIL_RMAX);
-    const int nx = xb - xa, lx0 = xa - px0;
-    for (int i = t; i < nrows * nx; i += PIL_TY * PIL_TX) {
-      const int rr = i / nx, lx = lx0 + i % nx;
-      const uint8_t* p = r.src + (size_t)min(ybase + rr, r.src_h - 1) * r.src_pitch_bytes;
-      const int lo = cx_lo[lx], cnt = cx_n[lx];
-      int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
-      for (int k = 0; k < cnt; ++k) {
-        const uint8_t* q = p + 3 * min(lo + k, r.src_w - 1);
-        const int w = cx_w[lx][k];
-        a0 += (int)q[0] * w;
-        a1 += (int)q[1] * w;
-        a2 += (int)q[2] * w;
+    if constexpr (!VFIRST) {                                  // horizontal pass over source rows [ybase, ybase + nrows)
+      ybase = cy_lo[ya - py0];
+      const int nrows = min(cy_lo[yb - 1 - py0] + cy_n[yb - 1 - py0] - ybase, PIL_RMAX);
+      const int nx = xb - xa, lx0 = xa - px0;
+      for (int i = t; i < nrows * nx; i += PIL_TY * PIL_TX) {
+        const int rr = i / nx, lx = lx0 + i % nx;
+        const uint8_t* p = r.src + (size_t)min(ybase + rr, r.src_h - 1) * r.src_pitch_bytes;
+        const int lo = cx_lo[lx], cnt = cx_n[lx];
+        int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+        for (int k = 0; k < cnt; ++k) {
+          const uint8_t* q = p + 3 * min(lo + k, r.src_w - 1);
+          const int w = cx_w[lx][k];
+          a0 += (int)q[0] * w;
+          a1 += (int)q[1] * w;
+          a2 += (int)q[2] * w;
+        }
+        hpass[rr][lx * 3 + 0] = (uint8_t)pil_clip8(a0);
+        hpass[rr][lx * 3 + 1] = (uint8_t)pil_clip8(a1);
+        hpass[rr][lx * 3 + 2] = (uint8_t)pil_clip8(a2);
       }
-      hpass[rr][lx * 3 + 0] = (uint8_t)pil_clip8(a0);
-      hpass[rr][lx * 3 + 1] = (uint8_t)pil_clip8(a1);
-      hpass[rr][lx * 3 + 2] = (uint8_t)pil_clip8(a2);
+    } else {                                                  // vertical pass over source columns [xbase, xbase + ncols)
+      xbase = cx_lo[xa - px0];
+      const int ncols = min(cx_lo[xb - 1 - px0] + cx_n[xb - 1 - px0] - xbase, PIL_CMAX);
+      const int ny = yb - ya, ly0 = ya - py0;
+      for (int i = t; i < ny * ncols; i += PIL_TY * PIL_TX) {
+        const int ly = ly0 + i / ncols, cc = i % ncols;
+        const uint8_t* p = r.src + 3 * min(xbase + cc, r.src_w - 1);
+        const int lo = cy_lo[ly], cnt = cy_n[ly];
+        int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+        for (int k = 0; k < cnt; ++k) {
+          const uint8_t* q = p + (size_t)min(lo + k, r.src_h - 1) * r.src_pitch_bytes;
+          const int w = cy_w[ly][k];
+          a0 += (int)q[0] * w;
+          a1 += (int)q[1] * w;
+          a2 += (int)q[2] * w;
+        }
+        vpass[ly][cc * 3 + 0] = (uint8_t)pil_clip8(a0);
+        vpass[ly][cc * 3 + 1] = (uint8_t)pil_clip8(a1);
+        vpass[ly][cc * 3 + 2] = (uint8_t)pil_clip8(a2);
+      }
     }
     __syncthreads();
   }
@@ -224,14 +261,25 @@ __global__ void __launch_bounds__(PIL_TY * PIL_TX) preprocess_pil_u8_s2d_kernel(
     const int ly = 2 * ty + (d >> 1), lx = 2 * tx + (d & 1), y = py0 + ly, x = px0 + lx;
     f[4 * d + 0] = f[4 * d + 1] = f[4 * d + 2] = f[4 * d + 3] = 0.f;
     if (any && y >= ya && y < yb && x >= xa && x < xb) {
-      const int lo = cy_lo[ly] - ybase, cnt = cy_n[ly];
       int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
-      for (int k = 0; k < cnt; ++k) {
-        const uint8_t* q = &hpass[min(lo + k, PIL_RMAX - 1)][lx * 3];
-        const int w = cy_w[ly][k];
-        a0 += (int)q[0] * w;
-        a1 += (int)q[1] * w;
-        a2 += (int)q[2] * w;
+      if constexpr (!VFIRST) {                                // vertical pass over the tile's rows of hpass
+        const int lo = cy_lo[ly] - ybase, cnt = cy_n[ly];
+        for (int k = 0; k < cnt; ++k) {
+          const uint8_t* q = &hpass[min(lo + k, PIL_RMAX - 1)][lx * 3];
+          const int w = cy_w[ly][k];
+          a0 += (int)q[0] * w;
+          a1 += (int)q[1] * w;
+          a2 += (int)q[2] * w;
+        }
+      } else {                                                // horizontal pass along the output row ly of vpass
+        const int lo = cx_lo[lx] - xbase, cnt = cx_n[lx];
+        for (int k = 0; k < cnt; ++k) {
+          const uint8_t* q = &vpass[ly][3 * min(lo + k, PIL_CMAX - 1)];
+          const int w = cx_w[lx][k];
+          a0 += (int)q[0] * w;
+          a1 += (int)q[1] * w;
+          a2 += (int)q[2] * w;
+        }
       }
       // RGB source -> BGR network input
       f[4 * d + 0] = __fsub_rn((float)pil_clip8(a2), r.mean[0]);
@@ -240,6 +288,20 @@ __global__ void __launch_bounds__(PIL_TY * PIL_TX) preprocess_pil_u8_s2d_kernel(
     }
   }
   store_cell(out, ((long long)n * Hq + Y) * Wq + X, f);
+}
+
+__global__ void __launch_bounds__(PIL_TY * PIL_TX) preprocess_pil_u8_s2d_kernel(const smb_raw_src_t* __restrict__ rows,
+                                                                               __half* __restrict__ out, int H, int W) {
+  __shared__ PilSmem s;
+  const smb_raw_src_t r = rows[blockIdx.z];
+  const bool fill = r.dst_h <= 0 || r.dst_w <= 0;
+  const int dh = fill ? 0 : r.dst_h, dw = fill ? 0 : r.dst_w;
+  // Image.resize's order (PIL/Image.py): vertical first when the image is more than 100 times taller than wide and its
+  // height shrinks.  64-bit: 100 * src_w overflows an int for widths a row admits.
+  if ((long long)r.src_h > 100LL * r.src_w && dh < r.src_h)
+    pil_tile<true>(s, r, dh, dw, out, H, W);
+  else
+    pil_tile<false>(s, r, dh, dw, out, H, W);
 }
 
 static int launch_preprocess(const smb_raw_src_t* rows, const smb_raw_src_t& row0, void* out, int N, int H, int W,

@@ -5,7 +5,8 @@ Reference: SipMask-benchmark/fcos_core/data/transforms/build.py:17-36 (test: Res
 ToTensor -> Normalize(PIXEL_MEAN, PIXEL_STD = 1, to_bgr255=True)), transforms.py:27-95, and to_image_list(size_divisible
 = 32) in the model.  The image is a PIL RGB image; Resize is torchvision F.resize = PIL Image.resize(BILINEAR).
 resize_pil_bilinear_u8 restates Pillow's libImaging/Resample.c for 8-bit images: separable, antialiased, 22-bit fixed
-point, horizontal pass first and clipped to uint8.  PIN: tests/test_bm_raw_host.py compares it bit for bit with the
+point, the first pass clipped to uint8.  The horizontal pass runs first, except where Pillow's Image.resize runs the
+vertical one first: for an image more than 100 times taller than wide whose height shrinks.  PIN: tests/test_bm_raw_host.py compares it bit for bit with the
 installed Pillow's Image.resize, and bm_preprocess with tensors the reference's own transforms produced
 (tests/golden/ref_bm_transforms.npz).
 """
@@ -28,15 +29,24 @@ def bm_resize_size(h, w, min_size=800, max_size=1333):
     return size, int(size * w / h)
 
 
-def _pil_taps(n_in, n_out):
-    """Resample.c precompute_coeffs + normalize_coeffs_8bpc (bilinear, support 1): per output index the first tap, the
-    number of taps and the 22-bit fixed-point weights [n_out, ksize] (zero past the tap count)."""
-    scale = float(n_in) / n_out
-    fs = max(scale, 1.0)
-    ss = 1.0 / fs
+def _pil_bounds(n_in, n_out):
+    """The tap bounds of Resample.c precompute_coeffs (bilinear, support 1): per output index the first tap and the number
+    of taps [..., n_out], with the scale, support and centers they come from.  n_in may be an int64 array of shape [k, 1]:
+    then the bounds of k axes n_in[i] -> n_out at once."""
+    scale = np.asarray(n_in, np.float64) / float(n_out)
+    fs = np.maximum(scale, 1.0)
     center = (np.arange(n_out, dtype=np.float64) + 0.5) * scale
     xmin = np.maximum(np.trunc(center - fs + 0.5).astype(np.int64), 0)
     cnt = np.minimum(np.trunc(center + fs + 0.5).astype(np.int64), n_in) - xmin
+    return xmin, cnt, float(scale) if scale.ndim == 0 else scale, fs, center
+
+
+def _pil_taps(n_in, n_out):
+    """Resample.c precompute_coeffs + normalize_coeffs_8bpc (bilinear, support 1): per output index the first tap, the
+    number of taps and the 22-bit fixed-point weights [n_out, ksize] (zero past the tap count)."""
+    xmin, cnt, scale, fs, center = _pil_bounds(n_in, n_out)
+    fs = float(fs)
+    ss = 1.0 / fs
     ksize = int(np.ceil(fs)) * 2 + 1
     ws, ww = [], np.zeros(n_out)
     for x in range(ksize):                             # summed in tap order, as the C loop does
@@ -66,11 +76,17 @@ def resize_pil_bilinear_u8(src, dh, dw):
     if (sh, sw) == (dh, dw):
         return src.copy()
     a = src.astype(np.int64)
-    if sw != dw:                                        # Pillow skips a pass whose axis keeps its size
-        a = _pil_pass(a, dw, 1)
-    if sh != dh:
-        a = _pil_pass(a, dh, 0)
+    # Pillow skips a pass whose axis keeps its size, and runs the vertical pass first for an image more than 100 times
+    # taller than wide whose height shrinks (PIL/Image.py, Image.resize)
+    for axis in ((0, 1) if pil_height_first(sh, sw, dh) else (1, 0)):
+        if a.shape[axis] != (dh, dw)[axis]:
+            a = _pil_pass(a, (dh, dw)[axis], axis)
     return a.astype(np.uint8)
+
+
+def pil_height_first(h, w, dh):
+    """Whether Image.resize runs the vertical pass of an h x w image resized to height dh first."""
+    return h > 100 * w and dh < h
 
 
 def bm_preprocess(rgb_u8, min_size=800, max_size=1333, mean=MEAN_BGR, size_divisor=32):

@@ -49,7 +49,12 @@ def _pil_pairs():
              ((480, 640), (800, 1066)), ((1080, 1920), (750, 1333)), ((2048, 1536), (1066, 800)), ((333, 17), (800, 40)),
              ((64, 64), (8, 8)), ((65, 63), (9, 8)), ((800, 96), (100, 12)), ((100, 37), (100, 11)), ((37, 100), (11, 100)),
              ((61, 83), (61, 40)), ((61, 83), (30, 83)), ((17, 23), (340, 460)), ((513, 257), (97, 301)),
-             ((99, 101), (13, 13)), ((56, 1345), (56, 1345)), ((640, 427), (1199, 800)), ((31, 29), (31, 29))]
+             ((99, 101), (13, 13)), ((56, 1345), (56, 1345)), ((640, 427), (1199, 800)), ((31, 29), (31, 29)),
+             # more than 100x taller than wide: Pillow runs the vertical pass first when the height shrinks (h = 100 w
+             # + 1), not at h = 100 w, and not when the height grows
+             ((2001, 20), (1300, 13)), ((1401, 14), (1300, 13)), ((1500, 14), (1285, 12)), ((3000, 20), (1350, 9)),
+             ((2000, 20), (1300, 13)), ((1001, 10), (1000, 9)), ((1000, 10), (999, 9)), ((301, 3), (1304, 13)),
+             ((300, 3), (1300, 13)), ((2001, 20), (2500, 13))]
     rs = np.random.RandomState(7)
     for _ in range(6):
         h, w = rs.randint(1, 300, 2)

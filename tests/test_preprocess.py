@@ -8,7 +8,8 @@ from oracle import preprocess as P
 
 cv2 = pytest.importorskip('cv2')
 
-SHAPES = [(480, 640), (427, 640), (375, 500), (1080, 1920), (333, 500), (800, 1333), (64, 48), (7, 5)]
+SHAPES = [(480, 640), (427, 640), (375, 500), (1080, 1920), (333, 500), (800, 1333), (64, 48), (7, 5),
+          (2048, 9), (9, 2048), (1, 2048), (2048, 1), (1, 1)]                     # extreme aspect ratios
 
 
 def _img(h, w, seed):
