@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "coco_match.cuh"
+#include "cta.cuh"
 
 namespace {
 
@@ -112,34 +113,6 @@ __global__ void __launch_bounds__(kThreads) det_from_record_kernel(
     rows[rj] = r;
   }
 }
-
-// ------------------------------------------------------------------------------------------------ block scans
-template <typename T, typename Op>
-__device__ __forceinline__ T block_inclusive_scan(T v, Op op, T* s_warp, T& total) {
-  const int tid = threadIdx.x, lid = tid & 31, warp = tid >> 5;
-  for (int o = 1; o < 32; o <<= 1) {
-    const T u = __shfl_up_sync(0xffffffffu, v, o);
-    if (lid >= o) v = op(u, v);
-  }
-  if (lid == 31) s_warp[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    T w = lid < kWarps ? s_warp[lid] : s_warp[0];
-    for (int o = 1; o < kWarps; o <<= 1) {
-      const T u = __shfl_up_sync(0xffffffffu, w, o);
-      if (lid >= o) w = op(u, w);
-    }
-    if (lid < kWarps) s_warp[lid] = w;
-  }
-  __syncthreads();
-  if (warp > 0) v = op(s_warp[warp - 1], v);
-  total = s_warp[kWarps - 1];
-  __syncthreads();
-  return v;
-}
-
-struct Add { __device__ int operator()(int a, int b) const { return a + b; } };
-struct Max { __device__ double operator()(double a, double b) const { return a > b ? a : b; } };
 
 // ------------------------------------------------------------------------------------------------ 2b + 2c: IoU, matching
 __device__ __forceinline__ double box_iou(const double* d, const double* g, int crowd) {
@@ -363,7 +336,6 @@ __global__ void __launch_bounds__(kThreads) match2_kernel(
       s_tie[j] = ((uint64_t)(uint32_t)c << 32) | (uint32_t)drow[j].order;
     }
   }
-  __syncthreads();
   auto before = [&](int x, int y) -> bool {        // x ranks before y; padding (-1) after everything
     if (y < 0) return x >= 0;
     if (x < 0) return false;
@@ -372,18 +344,7 @@ __global__ void __launch_bounds__(kThreads) match2_kernel(
     if (s_tie[x] != s_tie[y]) return s_tie[x] < s_tie[y];
     return x < y;
   };
-  for (int k = 2; k <= n_pad; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < n_pad; i += kThreads) {
-        const int l = i ^ j;
-        if (l > i) {
-          const int x = s_idx[i], y = s_idx[l];
-          if ((i & k) == 0 ? before(y, x) : before(x, y)) { s_idx[i] = y; s_idx[l] = x; }
-        }
-      }
-      __syncthreads();
-    }
-  }
+  smb::cta_bitonic_sort(s_idx, n_pad, before);    // synchronises before it reads the rows staged above
   // group g's sorted positions are [s_start[g], s_start[g + 1]): the first position whose group is >= g
   for (int g = tid; g <= n_grp; g += kThreads) {
     int lo = 0, hi = nd;
@@ -615,9 +576,9 @@ __global__ void __launch_bounds__(kThreads) accumulate_kernel(
       fpf = inc && !m && !ig;
     }
     int tot;
-    block_inclusive_scan(inc, Add(), s_wi, tot); nd += tot;
-    block_inclusive_scan(tpf, Add(), s_wi, tot); tp_tot += tot;
-    block_inclusive_scan(fpf, Add(), s_wi, tot); fp_tot += tot;
+    smb::cta_inclusive_scan<kThreads>(inc, smb::Sum(), s_wi, &tot); nd += tot;
+    smb::cta_inclusive_scan<kThreads>(tpf, smb::Sum(), s_wi, &tot); tp_tot += tot;
+    smb::cta_inclusive_scan<kThreads>(fpf, smb::Sum(), s_wi, &tot); fp_tot += tot;
   }
   const double dn = (double)npig;
   if (tid == 0) recall[r_idx] = nd ? __ddiv_rn((double)tp_tot, dn) : 0.0;
@@ -638,14 +599,14 @@ __global__ void __launch_bounds__(kThreads) accumulate_kernel(
       score = o.score;
     }
     int ti, tt, tf;
-    const int si = block_inclusive_scan(inc, Add(), s_wi, ti) + c_inc;
-    const int st = block_inclusive_scan(tpf, Add(), s_wi, tt) + c_tp;
-    const int sf = block_inclusive_scan(fpf, Add(), s_wi, tf) + c_fp;
+    const int si = smb::cta_inclusive_scan<kThreads>(inc, smb::Sum(), s_wi, &ti) + c_inc;
+    const int st = smb::cta_inclusive_scan<kThreads>(tpf, smb::Sum(), s_wi, &tt) + c_tp;
+    const int sf = smb::cta_inclusive_scan<kThreads>(fpf, smb::Sum(), s_wi, &tf) + c_fp;
     const int tp = tp_tot - (st - tpf), fp = fp_tot - (sf - fpf);   // cumulative counts up to and including e
     double pr = -1.0;
     if (inc) pr = __ddiv_rn((double)tp, __dadd_rn((double)(fp + tp), 2.220446049250313e-16));   // + np.spacing(1)
     double tm;
-    double env = block_inclusive_scan(pr, Max(), s_wd, tm);
+    double env = smb::cta_inclusive_scan<kThreads>(pr, smb::Max(), s_wd, &tm);
     env = env > c_max ? env : c_max;
     if (inc) {
       const bool first = (nd - si) == 0;

@@ -10,6 +10,7 @@
 // These paths are integer/compare work on a few thousand boxes: latency-bound, not bandwidth-bound.
 // One CTA per class keeps the sorted boxes and the suppression state in shared memory.
 #include "common.cuh"
+#include "cta.cuh"
 
 namespace smb {
 
@@ -54,96 +55,12 @@ __device__ __forceinline__ float key_score(unsigned long long k) {
   return __uint_as_float(b);
 }
 
-// In-place ascending bitonic sort of P (power of two) keys in shared memory by the whole CTA.
-__device__ void bitonic_sort(unsigned long long* keys, int P) {
-  for (int k = 2; k <= P; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      __syncthreads();
-      for (int t = threadIdx.x; t < (P >> 1); t += blockDim.x) {
-        const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-        const int ixj = i | j;
-        const bool up = (i & k) == 0;
-        const unsigned long long a = keys[i], b = keys[ixj];
-        if ((a > b) == up) { keys[i] = b; keys[ixj] = a; }
-      }
-    }
-  }
-  __syncthreads();
-}
-
-// CTA-wide exclusive scan of one int per thread (blockDim.x == NT); returns exclusive prefix, total in *total.
-__device__ int block_exscan(int v, int* s_warp /* [33] */, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  __syncthreads();
-  if (lane == 31) s_warp[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    int w = (lane < (blockDim.x >> 5)) ? s_warp[lane] : 0;
-    int winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, winc, o);
-      if (lane >= o) winc += t;
-    }
-    s_warp[lane] = winc - w;
-    if (lane == 31) s_warp[32] = winc;
-  }
-  __syncthreads();
-  *total = s_warp[32];
-  return s_warp[wid] + inc - v;
-}
-
-
-// Radix-select helper: given a 256-bin histogram in shared memory and the rank `need` (1-based) still wanted,
-// warp 0 finds the digit d with sum(hist[0..d-1]) < need <= sum(hist[0..d]) and the rank inside that bin.
-// All threads must call it (contains __syncthreads).
-__device__ __forceinline__ void select_digit(const unsigned* s_hist, int* s_k, unsigned long long* s_prefix,
-                                             unsigned long long prefix, int shift) {
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    const int lane = threadIdx.x;
-    int c[8];
-    int sum = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { c[j] = (int)s_hist[lane * 8 + j]; sum += c[j]; }
-    int incl = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += t;
-    }
-    const int excl = incl - sum;
-    const int need = *s_k;
-    if (need > excl && need <= incl) {
-      int r = need - excl, d = lane * 8;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        if (r > c[j]) { r -= c[j]; ++d; } else break;
-      }
-      *s_k = r;
-      *s_prefix = prefix | ((unsigned long long)d << shift);
-    }
-  }
-  __syncthreads();
-}
-
 // Greedy NMS sweep over `m` boxes already sorted by descending score in shared memory.
 // On return bit r of rem[] is set iff sorted row r is suppressed.  `plus_one`/`cmp_ge` select the
 // reference comparator (nms_kernel.cu:61 `>` vs nms_cpu.cpp:56 `>=`).
 __device__ void greedy_sweep_n(const float4* sb, int m, float thr, int cmp_ge, float one,
                                unsigned long long* rem, int rem_words, unsigned long long* diag,
                                unsigned long long* s_keep);
-__device__ __forceinline__ void greedy_sweep(const float4* sb, int m, float thr, int cmp_ge, float one,
-                                             unsigned long long* rem /* [MAXN/64] */, unsigned long long* diag /* [64] */,
-                                             unsigned long long* s_keep) {
-  greedy_sweep_n(sb, m, thr, cmp_ge, one, rem, MAXN / 64, diag, s_keep);
-}
 
 // ---------------------------------------------------------------------------------------------
 // Single-class NMS operator: dets [n,5]; keep ascending original indices.
@@ -154,7 +71,7 @@ struct NmsSmem {
   unsigned long long rem[NMS1 / 64];
   unsigned long long diag[64];
   unsigned long long keepbits;
-  int warp[33];
+  int warp[32];
   unsigned char kept[NMS1];
 };
 
@@ -167,7 +84,7 @@ __global__ void __launch_bounds__(NT) nms_single_kernel(const float* __restrict_
   while (P < n) P <<= 1;
   for (int i = threadIdx.x; i < P; i += NT)
     S.keys[i] = (i < n) ? desc_key(dets[i * 5 + 4], (unsigned)i) : ~0ull;
-  bitonic_sort(S.keys, P);
+  cta_bitonic_sort(S.keys, P, Less());
   for (int r = threadIdx.x; r < n; r += NT) {
     const int i = (int)(S.keys[r] & 0xffffffffu);
     S.sb[r] = make_float4(dets[i * 5], dets[i * 5 + 1], dets[i * 5 + 2], dets[i * 5 + 3]);
@@ -184,10 +101,9 @@ __global__ void __launch_bounds__(NT) nms_single_kernel(const float* __restrict_
     const int i = base + threadIdx.x;
     const int f = (i < n) ? S.kept[i] : 0;
     int tot;
-    const int ex = block_exscan(f, S.warp, &tot);
+    const int ex = cta_exclusive_scan<NT>(f, Sum(), 0, S.warp, &tot);
     if (f) keep_out[running + ex] = i;
     running += tot;
-    __syncthreads();
   }
   if (threadIdx.x == 0) *n_keep_out = running;
 }
@@ -261,7 +177,7 @@ struct McPrepSmem {
   unsigned long long keys[MAXP];
   int cidx[MAXN];
   float cscore[MAXN];
-  int warp[33];
+  int warp[32];
 };
 
 __global__ void __launch_bounds__(NT) mc_prepare_kernel(const float* __restrict__ boxes, const float* __restrict__ scores,
@@ -280,7 +196,7 @@ __global__ void __launch_bounds__(NT) mc_prepare_kernel(const float* __restrict_
     int f = 0;
     if (i < n) { s = scores[(size_t)i * C + c]; f = s > score_thr; }       // bbox_nms.py:111
     int tot;
-    const int ex = block_exscan(f, S.warp, &tot);
+    const int ex = cta_exclusive_scan<NT>(f, Sum(), 0, S.warp, &tot);
     if (f) { S.cidx[m + ex] = i; S.cscore[m + ex] = __fmul_rn(s, ctr[i]); }  // bbox_nms.py:122
     m += tot;
     __syncthreads();
@@ -290,7 +206,7 @@ __global__ void __launch_bounds__(NT) mc_prepare_kernel(const float* __restrict_
   int P = 1;
   while (P < m) P <<= 1;
   for (int i = threadIdx.x; i < P; i += NT) S.keys[i] = (i < m) ? desc_key(S.cscore[i], (unsigned)i) : ~0ull;
-  bitonic_sort(S.keys, P);
+  cta_bitonic_sort(S.keys, P, Less());
   for (int r = threadIdx.x; r < m; r += NT) {
     const unsigned long long k = S.keys[r];
     const int pos = (int)(k & 0xffffffffu);
@@ -361,7 +277,7 @@ struct McSweepSmem {
   unsigned long long rem[MAXN / 64];
   unsigned long long diag[64];
   unsigned long long keepbits;
-  int warp[33];
+  int warp[32];
   unsigned char kept[MAXN];
 };
 
@@ -420,13 +336,12 @@ __global__ void __launch_bounds__(NT) mc_sweep_kernel(const unsigned long long* 
     const int p = base + threadIdx.x;
     const int f = (p < m) ? S.kept[p] : 0;
     int tot;
-    const int ex = block_exscan(f, S.warp, &tot);
+    const int ex = cta_exclusive_scan<NT>(f, Sum(), 0, S.warp, &tot);
     if (f) {
       ws_idx[(size_t)c * n + running + ex] = w_cidx[(size_t)c * n + p];
       ws_score[(size_t)c * n + running + ex] = w_cscore[(size_t)c * n + p];
     }
     running += tot;
-    __syncthreads();
   }
   if (threadIdx.x == 0) ws_count[c] = running;
 }
@@ -445,17 +360,14 @@ __global__ void __launch_bounds__(NT) finalize_kernel(const float* __restrict__ 
                                                       long long* __restrict__ idx_out, int* __restrict__ count_out) {
   pdl_wait();
   __shared__ int s_off[1025];
-  __shared__ int s_warp[33];
-  __shared__ unsigned s_hist[256];
+  __shared__ int s_warp[32];
   __shared__ unsigned long long s_sel[1024];
-  __shared__ int s_nsel;
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_k;
+  __shared__ SelectSmem s_select;
   // class offsets
   {
     const int v = (threadIdx.x < C) ? ws_count[threadIdx.x] : 0;
     int tot;
-    const int ex = block_exscan(v, s_warp, &tot);
+    const int ex = cta_exclusive_scan<NT>(v, Sum(), 0, s_warp, &tot);
     if (threadIdx.x < C) s_off[threadIdx.x] = ex;
     if (threadIdx.x == 0) s_off[C] = tot;
   }
@@ -496,38 +408,8 @@ __global__ void __launch_bounds__(NT) finalize_kernel(const float* __restrict__ 
       gval[g] = (c << 16) | ws_idx[(size_t)c * list_pitch + k];
     }
   }
-  __syncthreads();
-  // radix-select the kout-th smallest key (keys are unique)
-  if (threadIdx.x == 0) { s_prefix = 0ull; s_k = kout; }
-  __syncthreads();
-  if (K > kout) {
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      for (int i = threadIdx.x; i < 256; i += NT) s_hist[i] = 0u;
-      __syncthreads();
-      const unsigned long long prefix = s_prefix;
-      const unsigned long long himask = (shift == 56) ? 0ull : (~0ull << (shift + 8));
-      for (int g = threadIdx.x; g < K; g += NT) {
-        const unsigned long long k = gkey[g];
-        if ((k & himask) == prefix) atomicAdd(&s_hist[(unsigned)(k >> shift) & 255u], 1u);
-      }
-      select_digit(s_hist, &s_k, &s_prefix, prefix, shift);
-    }
-  } else {
-    if (threadIdx.x == 0) s_prefix = ~0ull;
-    __syncthreads();
-  }
-  const unsigned long long kth = s_prefix;
-  if (threadIdx.x == 0) s_nsel = 0;
-  for (int i = threadIdx.x; i < 1024; i += NT) s_sel[i] = ~0ull;
-  __syncthreads();
-  for (int g = threadIdx.x; g < K; g += NT) {
-    const unsigned long long k = gkey[g];
-    if (k <= kth) { const int p = atomicAdd(&s_nsel, 1); if (p < 1024) s_sel[p] = k; }
-  }
-  __syncthreads();
-  int P = 1;
-  while (P < kout) P <<= 1;
-  bitonic_sort(s_sel, P);
+  // the kout smallest keys in order (keys are unique); the select synchronises before it reads gkey
+  cta_smallest_sorted<NT>(K, kout, [&](int g) { return gkey[g]; }, s_sel, 1024, s_select);
   for (int r = threadIdx.x; r < kout; r += NT) {
     const unsigned long long k = s_sel[r];
     const int g = (int)(k & 0xffffffffu);
@@ -549,7 +431,7 @@ struct FastSmem {
   float4 sb[256];
   float sscore[256];
   unsigned char kept[256];
-  int warp[33];
+  int warp[32];
 };
 
 __global__ void __launch_bounds__(NT) fast_nms_class_kernel(const float* __restrict__ boxes, const float* __restrict__ scores,
@@ -563,7 +445,7 @@ __global__ void __launch_bounds__(NT) fast_nms_class_kernel(const float* __restr
   while (P < n) P <<= 1;
   for (int i = threadIdx.x; i < P; i += NT)
     S.keys[i] = (i < n) ? desc_key(__fmul_rn(scores[(size_t)i * C + c], ctr[i]), (unsigned)i) : ~0ull;
-  bitonic_sort(S.keys, P);
+  cta_bitonic_sort(S.keys, P, Less());
   const int m = min(n, top_k);
   for (int r = threadIdx.x; r < m; r += NT) {
     const unsigned long long k = S.keys[r];
@@ -590,13 +472,12 @@ __global__ void __launch_bounds__(NT) fast_nms_class_kernel(const float* __restr
     const int p = base + threadIdx.x;
     const int f = (p < m) ? S.kept[p] : 0;
     int tot;
-    const int ex = block_exscan(f, S.warp, &tot);
+    const int ex = cta_exclusive_scan<NT>(f, Sum(), 0, S.warp, &tot);
     if (f) {
       ws_idx[(size_t)c * top_k + running + ex] = (int)(S.keys[p] & 0xffffffffu);
       ws_score[(size_t)c * top_k + running + ex] = S.sscore[p];
     }
     running += tot;
-    __syncthreads();
   }
   if (threadIdx.x == 0) ws_count[c] = running;
 }
@@ -638,11 +519,8 @@ __global__ void level_score_kernel(Levels L, int C, float* __restrict__ s) {
 __global__ void __launch_bounds__(NT) level_topk_kernel(Levels L, int nms_pre, const float* __restrict__ s,
                                                         int* __restrict__ sel) {
   pdl_wait();
-  __shared__ unsigned s_hist[256];
   __shared__ unsigned long long s_sel[1024];
-  __shared__ int s_nsel;
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_k;
+  __shared__ SelectSmem s_select;
   const int l = blockIdx.x;
   const int hw = L.loc_off[l + 1] - L.loc_off[l];
   const float* sl = s + L.loc_off[l];
@@ -651,31 +529,7 @@ __global__ void __launch_bounds__(NT) level_topk_kernel(Levels L, int nms_pre, c
     for (int i = threadIdx.x; i < hw; i += NT) out[i] = i;
     return;
   }
-  if (threadIdx.x == 0) { s_prefix = 0ull; s_k = nms_pre; }
-  __syncthreads();
-  for (int shift = 56; shift >= 0; shift -= 8) {
-    for (int i = threadIdx.x; i < 256; i += NT) s_hist[i] = 0u;
-    __syncthreads();
-    const unsigned long long prefix = s_prefix;
-    const unsigned long long himask = (shift == 56) ? 0ull : (~0ull << (shift + 8));
-    for (int i = threadIdx.x; i < hw; i += NT) {
-      const unsigned long long k = desc_key(sl[i], (unsigned)i);
-      if ((k & himask) == prefix) atomicAdd(&s_hist[(unsigned)(k >> shift) & 255u], 1u);
-    }
-    select_digit(s_hist, &s_k, &s_prefix, prefix, shift);
-  }
-  const unsigned long long kth = s_prefix;
-  if (threadIdx.x == 0) s_nsel = 0;
-  for (int i = threadIdx.x; i < 1024; i += NT) s_sel[i] = ~0ull;
-  __syncthreads();
-  for (int i = threadIdx.x; i < hw; i += NT) {
-    const unsigned long long k = desc_key(sl[i], (unsigned)i);
-    if (k <= kth) { const int p = atomicAdd(&s_nsel, 1); if (p < 1024) s_sel[p] = k; }
-  }
-  __syncthreads();
-  int P = 1;
-  while (P < nms_pre) P <<= 1;
-  bitonic_sort(s_sel, P);
+  cta_smallest_sorted<NT>(hw, nms_pre, [&](int i) { return desc_key(sl[i], (unsigned)i); }, s_sel, 1024, s_select);
   for (int r = threadIdx.x; r < nms_pre; r += NT) out[r] = (int)(s_sel[r] & 0xffffffffu);
 }
 
@@ -843,10 +697,8 @@ constexpr int PAIR_RUN = 16;       // consecutive pairs per thread in the ordere
 __global__ void __launch_bounds__(NT) pair_select_kernel(PairLevels L, int nms_pre, const unsigned* __restrict__ keys,
                                                          int* __restrict__ sel, int* __restrict__ sel_count) {
   pdl_wait();
-  __shared__ unsigned s_hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_k;
-  __shared__ int s_warp[33];
+  __shared__ SelectSmem s_select;
+  __shared__ int s_warp[32];
   const int l = blockIdx.x;
   const int n = (int)(L.pair_off[l + 1] - L.pair_off[l]);
   const unsigned* kl = keys + L.pair_off[l];
@@ -856,27 +708,15 @@ __global__ void __launch_bounds__(NT) pair_select_kernel(PairLevels L, int nms_p
   int mine = 0;
   for (int i = threadIdx.x; i < n; i += NT) mine += kl[i] != 0u;
   int n_pass;
-  block_exscan(mine, s_warp, &n_pass);
+  cta_inclusive_scan<NT>(mine, Sum(), s_warp, &n_pass);
   // threshold key T and the number of pairs equal to T that may still be taken (lowest indices first)
   unsigned T = 1u;
   int budget = 0x7fffffff;
   if (n_pass > cap) {
-    // radix-select the cap-th smallest of ~key (= the cap-th largest key) over 4 bytes
-    if (threadIdx.x == 0) { s_prefix = 0ull; s_k = cap; }
-    __syncthreads();
-    for (int shift = 24; shift >= 0; shift -= 8) {
-      for (int i = threadIdx.x; i < 256; i += NT) s_hist[i] = 0u;
-      __syncthreads();
-      const unsigned long long prefix = s_prefix;
-      const unsigned himask = (shift == 24) ? 0u : (0xffffffffu << (shift + 8));
-      for (int i = threadIdx.x; i < n; i += NT) {
-        const unsigned k = ~kl[i];
-        if ((k & himask) == (unsigned)prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1u);
-      }
-      select_digit(s_hist, &s_k, &s_prefix, prefix, shift);
-    }
-    T = ~(unsigned)s_prefix;
-    budget = s_k;                       // rank of the cap-th key among the keys equal to T
+    // the cap-th smallest of ~key (= the cap-th largest key), and its rank among the keys equal to it
+    const RadixKth<unsigned> kth = cta_radix_select<NT, unsigned>(n, cap, [&](int i) { return ~kl[i]; }, s_select);
+    T = ~kth.key;
+    budget = kth.rank;
   }
   // ordered compaction: thread t owns PAIR_RUN consecutive pairs of each chunk
   int running = 0, tie_running = 0;
@@ -890,7 +730,7 @@ __global__ void __launch_bounds__(NT) pair_select_kernel(PairLevels L, int nms_p
       ties += k[j] == T;
     }
     int tie_tot;
-    int tie_rank = tie_running + block_exscan(ties, s_warp, &tie_tot);
+    int tie_rank = tie_running + cta_exclusive_scan<NT>(ties, Sum(), 0, s_warp, &tie_tot);
     unsigned take = 0u;
     int cnt = 0;
 #pragma unroll
@@ -900,7 +740,7 @@ __global__ void __launch_bounds__(NT) pair_select_kernel(PairLevels L, int nms_p
       if (f) { take |= 1u << j; ++cnt; }
     }
     int tot;
-    int pos = running + block_exscan(cnt, s_warp, &tot);
+    int pos = running + cta_exclusive_scan<NT>(cnt, Sum(), 0, s_warp, &tot);
 #pragma unroll
     for (int j = 0; j < PAIR_RUN; ++j)
       if ((take >> j) & 1u) {
@@ -973,7 +813,7 @@ __global__ void __launch_bounds__(NT) ml_prepare_kernel(const float* __restrict_
   int P = 1;
   while (P < n) P <<= 1;
   for (int i = threadIdx.x; i < P; i += NT) keys[i] = (i < n) ? desc_key(scores[i], (unsigned)i) : ~0ull;
-  bitonic_sort(keys, P);
+  cta_bitonic_sort(keys, P, Less());
   for (int r = threadIdx.x; r < n; r += NT) {
     const unsigned long long k = keys[r];
     const int i = (int)(k & 0xffffffffu);
@@ -1030,27 +870,14 @@ __global__ void __launch_bounds__(NT) ml_finalize_kernel(const float* __restrict
                                                          long long* __restrict__ label_out, long long* __restrict__ idx_out,
                                                          int* __restrict__ count_out, int* __restrict__ kept_total_out) {
   pdl_wait();
-  __shared__ unsigned s_hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_k;
-  __shared__ int s_warp[33];
+  __shared__ SelectSmem s_select;
+  __shared__ int s_warp[32];
   const int K = min(max(*ws_count, 0), cap);
   float thr = -INFINITY;
   if (max_per_img > 0 && K > max_per_img) {
-    if (threadIdx.x == 0) { s_prefix = 0ull; s_k = max_per_img; }
-    __syncthreads();
-    for (int shift = 56; shift >= 32; shift -= 8) {
-      for (int i = threadIdx.x; i < 256; i += NT) s_hist[i] = 0u;
-      __syncthreads();
-      const unsigned long long prefix = s_prefix;
-      const unsigned long long himask = (shift == 56) ? 0ull : (~0ull << (shift + 8));
-      for (int g = threadIdx.x; g < K; g += NT) {
-        const unsigned long long k = desc_key(ws_score[g], 0u);
-        if ((k & himask) == prefix) atomicAdd(&s_hist[(unsigned)(k >> shift) & 255u], 1u);
-      }
-      select_digit(s_hist, &s_k, &s_prefix, prefix, shift);
-    }
-    thr = key_score(s_prefix);
+    // the max_per_img-th largest score: the max_per_img-th smallest key, resolved in its top 32 bits (the score)
+    const auto key_at = [&](int g) { return desc_key(ws_score[g], 0u); };
+    thr = key_score(cta_radix_select<NT, unsigned long long, 4>(K, max_per_img, key_at, s_select).key);
   }
   int running = 0;
   for (int base = 0; base < K; base += NT) {
@@ -1058,7 +885,7 @@ __global__ void __launch_bounds__(NT) ml_finalize_kernel(const float* __restrict
     const float s = (g < K) ? ws_score[g] : 0.f;
     const int f = (g < K) && (s >= thr);
     int tot;
-    const int pos = running + block_exscan(f, s_warp, &tot);
+    const int pos = running + cta_exclusive_scan<NT>(f, Sum(), 0, s_warp, &tot);
     if (f && pos < out_cap) {
       const int i = ws_idx[g];
       const float4 b = *reinterpret_cast<const float4*>(boxes + (size_t)i * 4);
@@ -1099,7 +926,7 @@ struct SoftSmem {
   unsigned long long tab[32];
   float best_v[SNT / 32];
   int best_p[SNT / 32];
-  int warp[33];
+  int warp[SNT / 32];
   int sel;
 };
 
@@ -1220,7 +1047,7 @@ __device__ __forceinline__ int soft_nms_run(SoftSmem& S, int m, float thr, int m
       }
     }
     int S_tot;
-    block_exscan(surv, S.warp, &S_tot);
+    cta_inclusive_scan<SNT>(surv, Sum(), S.warp, &S_tot);
     const int fend = i + 1 + S_tot;
     if (S_tot < len) {
       int holes = 0, backs = 0;
@@ -1230,7 +1057,7 @@ __device__ __forceinline__ int soft_nms_run(SoftSmem& S, int m, float thr, int m
         backs += (!r && j >= fend);
       }
       int tot;
-      const int ex = block_exscan((holes << 16) | backs, S.warp, &tot);
+      const int ex = cta_exclusive_scan<SNT>((holes << 16) | backs, Sum(), 0, S.warp, &tot);
       int hr = ex >> 16, br = ex & 0xffff;
       const int nback = tot & 0xffff;
       for (int j = j0; j < j1; ++j)
@@ -1298,7 +1125,7 @@ __global__ void __launch_bounds__(SNT, 1) mc_soft_nms_kernel(const float* __rest
     int f = 0;
     if (i < nn) { s = scores[(size_t)i * C + c]; f = s > score_thr; }
     int tot;
-    const int ex = block_exscan(f, S.warp, &tot);
+    const int ex = cta_exclusive_scan<SNT>(f, Sum(), 0, S.warp, &tot);
     if (f) {
       S.id[m + ex] = i;
       S.score[m + ex] = __fmul_rn(s, ctr[i]);

@@ -19,6 +19,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "cta.cuh"
 
 namespace smb {
 
@@ -40,33 +41,6 @@ __device__ __forceinline__ uint32_t transpose32(uint32_t w, int lane) {
 
 __device__ __forceinline__ uint32_t pixel_bit(const uint32_t* m, int words, int x, int y) {
   return (m[(size_t)y * words + (x >> 5)] >> (x & 31)) & 1u;
-}
-
-// Exclusive prefix sum over the RLE_THREADS threads of the block (all of them call it); *total = the sum.
-__device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp, int* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += u;
-  }
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    int wv = s_warp[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, wv, o);
-      if (lane >= o) wv += u;
-    }
-    s_warp[lane] = wv;
-  }
-  __syncthreads();
-  const int r = (warp ? s_warp[warp - 1] : 0) + inc - v;
-  *total = s_warp[31];
-  __syncthreads();                                 // s_warp is free for the next scan
-  return r;
 }
 
 // The column-major run boundaries of column x = 32*wq + lane (the whole warp calls it): f(yc, t) receives, chunk by
@@ -110,7 +84,7 @@ __device__ int boundary_positions(const uint32_t* m, int words, int H, int W, ui
     const int i0 = 2 * threadIdx.x, i1 = i0 + 1;
     const int a0 = i0 < ncol ? s_cnt[i0] : 0, a1 = i1 < ncol ? s_cnt[i1] : 0;
     int total;
-    const int base = carry + block_exclusive_scan(a0 + a1, s_warp, &total);
+    const int base = carry + cta_exclusive_scan<RLE_THREADS>(a0 + a1, Sum(), 0, s_warp, &total);
     if (i0 < ncol) s_cnt[i0] = base;
     if (i1 < ncol) s_cnt[i1] = base + a0;
     __syncthreads();
@@ -227,7 +201,7 @@ __global__ void __launch_bounds__(RLE_THREADS) rle_encode_kernel(const uint32_t*
       nch = rle_count_chars(x, nullptr, 0);
     }
     int stripe;
-    const int o = carry + block_exclusive_scan(nch, s_warp, &stripe);
+    const int o = carry + cta_exclusive_scan<RLE_THREADS>(nch, Sum(), 0, s_warp, &stripe);
     if (k <= T && o < str_cap) rle_count_chars(x, str + o, str_cap - o);
     carry += stripe;
   }
@@ -259,7 +233,7 @@ __global__ void __launch_bounds__(RLE_THREADS) rle_pack_kernel(const int* __rest
     }
   }
   int total;
-  const int off = block_exclusive_scan(len, s_warp, &total);
+  const int off = cta_exclusive_scan<RLE_THREADS>(len, Sum(), 0, s_warp, &total);
   if ((int)threadIdx.x < max_num) s_off[threadIdx.x] = off;
   if (threadIdx.x == 0) s_off[max_num] = total;
   const int hdr_words = max_num + 3;

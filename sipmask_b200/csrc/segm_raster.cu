@@ -20,6 +20,7 @@
 #include <limits.h>
 
 #include "common.cuh"
+#include "cta.cuh"
 
 namespace {
 
@@ -158,22 +159,11 @@ __global__ void __launch_bounds__(kThreads) segm_toggle_kernel(Launch L, int* __
     uint64_t carry = 0;
     for (int64_t base = 0; base < it.n; base += kThreads) {
       const int64_t e = base + tid;
-      uint64_t v = e < it.n ? cnts[e] : 0;
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint64_t u = __shfl_up_sync(0xffffffffu, v, o);
-        if (lid >= o) v += u;
-      }
-      if (lid == 31) s_warp[warp] = v;
-      __syncthreads();
-      uint64_t before = carry, total = carry;
-      for (int q = 0; q < kWarps; ++q) {
-        if (q < warp) before += s_warp[q];
-        total += s_warp[q];
-      }
-      __syncthreads();
-      const uint64_t pos = before + v;
+      const uint64_t v = e < it.n ? cnts[e] : 0;
+      uint64_t total;
+      const uint64_t pos = carry + smb::cta_inclusive_scan<kThreads>(v, smb::Sum(), s_warp, &total);
       if (e < it.n && pos < (uint64_t)hw) toggle(scratch, colpar, (int64_t)pos, (int)(pos / (uint64_t)h));
-      carry = total;
+      carry += total;
     }
   }
 }
@@ -212,11 +202,7 @@ __global__ void __launch_bounds__(kThreads) segm_fill_kernel(Launch L) {
       v ^= v << 1; v ^= v << 2; v ^= v << 4; v ^= v << 8; v ^= v << 16;      // bit r = parity of the toggles <= r
       v &= valid;
       const uint32_t par = valid ? (v >> (31 - __clz(valid))) & 1u : 0u;     // parity of the whole word
-      uint32_t incl = par;
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lid >= o) incl ^= u;
-      }
+      const uint32_t incl = smb::warp_inclusive_scan(par, smb::Xor());
       if (carry[k] ^ incl ^ par) v ^= valid;
       carry[k] ^= __shfl_sync(0xffffffffu, incl, 31);
       s_tile[c][lid] = v;
