@@ -64,12 +64,16 @@ static_assert(4 * kEpiSlots * 8 <= 256, "epilogue barriers exceed their reserve"
 // Timing build only (tools/conv_tile_phases.py compiles it; the library never does).  clock64 stamps per CTA:
 //   [0, 4): globaltimer / clock64 at the first and last stamp (cycles -> ns);
 //   [4, 8): warp 9: cycles blocked in bulk_wait_read, cycles blocked on epi_ready, stores committed, fills;  [8]: tiles;
+//   [9, 11): warp 9: cycles from a store step's first epi_ready wait to its commit (waits included), cycles issuing fills
+//   (residual TMA load or release arrival);
 //   [16 + (sample * 2 + wg) * kPhaseTile, + kPhaseTile): the sample-th recorded tile of consumer warpgroup wg (every
 //   phase_every-th tile of the CTA): mainloop start, last wgmma_wait<0> returned, epilogue end, cycles blocked in epi_full
 //   waits, cycles in the GroupNorm statistics' shuffle reductions, cycles handing the tile's statistics to warp 10 (the
-//   wait for the previous tile's flush and the arrival).
+//   wait for the previous tile's flush and the arrival), and per link of the chunk chain summed over the tile's chunks:
+//   slot ready -> results in registers (ldmatrix, arithmetic, GroupNorm partials), stmatrix, proxy fence, slot arrival;
+//   last, the cycles staging the tile's bias before its first chunk.
 constexpr int kPhaseSamples = 64;
-constexpr int kPhaseTile = 6;
+constexpr int kPhaseTile = 11;
 constexpr int kPhaseWords = 16 + kPhaseSamples * 2 * kPhaseTile;
 __device__ __forceinline__ unsigned long long globaltimer() {
   unsigned long long t;
@@ -195,6 +199,10 @@ __device__ __forceinline__ void wgmma_f16<256>(float* d, uint64_t a, uint64_t b,
 }
 
 // ------------------------------------------------------------------------------------------------ kernel
+// a compile-time value carried by a function argument's type (selects a template specialisation from a run-time flag)
+template <typename T, T V>
+struct Const { static constexpr T value = V; };
+
 // work unit -> tile.  Units of the same M-tile with different N-tiles are adjacent, so concurrently running CTAs share the
 // activation patch in L2.
 struct TileCoord {
@@ -273,9 +281,10 @@ __device__ __forceinline__ void gn_reduce_chunk(float* v, int lane, unsigned lon
 
 // Collects one 8-channel block's statistics (s, q: the lane's sum and sum of squares over its valid rows) into the
 // chunk's v[] of gn_reduce_chunk; after the chunk's last block (jj = 3) reduces them into the warp's partials of chunk c.
-__device__ __forceinline__ void gn_block(const ConvParams& p, float* v, int jj, float s, float q, int lane,
+// group: channels per GroupNorm group, 8 or 16 (a constant where the caller is specialised on it).
+__device__ __forceinline__ void gn_block(int group, float* v, int jj, float s, float q, int lane,
                                          unsigned long long (*part)[2], int c PHASE(, unsigned& shfl)) {
-  if (p.gn_group == 8) {
+  if (group == 8) {
     v[2 * jj] = s; v[2 * jj + 1] = q;
   } else {                                           // 16-channel groups: blocks 2g and 2g + 1 summed in that order
     const int g = jj >> 1;
@@ -284,7 +293,7 @@ __device__ __forceinline__ void gn_block(const ConvParams& p, float* v, int jj, 
   }
   if (jj == 3) {
     PHASE(const unsigned w0 = clock();)
-    if (p.gn_group == 8) gn_reduce_chunk<8>(v, lane, part + 4 * c);
+    if (group == 8) gn_reduce_chunk<8>(v, lane, part + 4 * c);
     else gn_reduce_chunk<4>(v, lane, part + 2 * c);
     PHASE(shfl += clock() - w0;)
   }
@@ -365,7 +374,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
       // per-(image, group) sum / sum of squares of the conv output (pre-activation): fp32 over the warp's 16 rows, then
       // 64-bit fixed point, summed over the tile by warp 10 (integer sums: bit-reproducible whatever the tile order).
       // GroupNorm plans have Cout 256 or 512, so every 32-channel chunk is whole.
-      if (p.gn_group) gn_block(p, gv, j & 3, s, q, lane, gn_part[warp], j >> 2 PHASE(, shfl));
+      if (p.gn_group) gn_block(p.gn_group, gv, j & 3, s, q, lane, gn_part[warp], j >> 2 PHASE(, shfl));
     }
   }
 }
@@ -375,11 +384,14 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, const TileCoord& t
 // (residual) or freed it, ldmatrix the residual, stmatrix the fp16 results over it, hand the slot to warp 9's TMA store.
 // Slot layout: pixel row r (0..63, accumulator row order) at r * 64 bytes, its 16-byte channel quad q at
 // ((q ^ (r >> 1) & 3) * 16): the TMA 64-byte swizzle (address bits [4,6) ^= bits [7,9)).
-template <int N>
+// Specialised on the plan's residual (RES), GroupNorm group size (GN: 0 = no statistics, 8, 16) and ReLU: the epilogue is
+// bound by the consumers' instruction issue (two warps per scheduler, about 0.2 µs per chunk), and with these as run-time
+// flags every chunk issued the predicated residual conversions, statistics arithmetic and ReLU of every plan.
+template <int N, bool RES, int GN, bool RELU>
 __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoord& tc, const float* acc, int wg, int warp,
-                                             int lane, GnPart& gn_part, uint32_t slots, uint64_t* epi_full,
-                                             uint64_t* epi_ready, int& es, uint32_t& eph
-                                             PHASE(, long long& blocked, unsigned& shfl)) {
+                                             int lane, GnPart& gn_part, const float* tile_bias, uint32_t slots,
+                                             uint64_t* epi_full, uint64_t* epi_ready, int& es, uint32_t& eph
+                                             PHASE(, long long* link, unsigned& shfl)) {
   const LevelDesc& L = p.lv[tc.lvl];
   const int bw_shift = 31 - __clz(L.BW);
   bool valid[2];
@@ -396,15 +408,13 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
   const uint32_t q1 = (uint32_t)((2 + (lane >> 4)) ^ ((mrow >> 1) & 3)) << 4;
   const int cq = 2 * (lane & 3);
   const int nchunks = (min(N, p.Cout - tc.n0) + 31) >> 5;
-  // bias of 8-channel block jj of chunk cc (zero past Cout).  The slot wait's memory clobber keeps every load after it, so
-  // a chunk's bias is loaded one chunk ahead, before that wait: one global round trip per tile instead of one per chunk.
+  // bias of 8-channel block jj of chunk cc, from the tile's copy in shared memory (tile_bias: zero past Cout): four
+  // shared loads at fixed offsets per chunk, where eight predicated global loads with their bounds tests cost 0.6-0.7 µs
+  // per N = 256 tile (DESIGN.md §6).  The slot wait's memory clobber keeps every load after it, so a chunk's bias is
+  // read one chunk ahead, before that wait.
   auto chunk_bias = [&](int cc, float2* b) {
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-      const int ch0 = tc.n0 + 8 * (4 * cc + jj);
-      b[jj] = make_float2(0.f, 0.f);
-      if (p.bias && ch0 < p.Cout) b[jj] = make_float2(__ldg(p.bias + ch0 + cq), __ldg(p.bias + ch0 + cq + 1));
-    }
+    for (int jj = 0; jj < 4; ++jj) b[jj] = *reinterpret_cast<const float2*>(tile_bias + 8 * (4 * cc + jj) + cq);
   };
   float2 bnext[4];
   chunk_bias(0, bnext);
@@ -418,10 +428,10 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
     if (c + 1 < nchunks) chunk_bias(c + 1, bnext);
     PHASE(const long long w0 = clock64();)
     mbar_wait(&epi_full[wg * kEpiSlots + es], eph);
-    PHASE(blocked += clock64() - w0;)
+    PHASE(long long w1 = clock64(); link[0] += w1 - w0;)
     const uint32_t sa = row_addr + (uint32_t)es * kEpiSlotBytes;
     uint32_t rh[8], oh[8];                           // residual / output: block jj, row half i in register 2 jj + i
-    if (p.res_mode) { ldmatrix_x4(sa + q0, rh); ldmatrix_x4(sa + q1, rh + 4); }
+    if (RES) { ldmatrix_x4(sa + q0, rh); ldmatrix_x4(sa + q1, rh + 4); }
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       const int j = 4 * c + jj;
@@ -431,21 +441,27 @@ __device__ __forceinline__ void epilogue_tma(const ConvParams& p, const TileCoor
       for (int i = 0; i < 2; ++i) {
         float f0 = acc[4 * j + 2 * i] + bb.x, f1 = acc[4 * j + 2 * i + 1] + bb.y;
         if (p.alpha != 1.0f) { f0 *= p.alpha; f1 *= p.alpha; }
-        if (p.res_mode) {
+        if (RES) {
           const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rh[2 * jj + i]));
           f0 += r.x; f1 += r.y;
         }
-        if (valid[i]) { s += f0 + f1; q += f0 * f0 + f1 * f1; }
-        if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+        if (GN && valid[i]) { s += f0 + f1; q += f0 * f0 + f1 * f1; }
+        if (RELU) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
         const __half2 h = __floats2half2_rn(f0, f1);
         oh[2 * jj + i] = *reinterpret_cast<const uint32_t*>(&h);
       }
-      if (p.gn_group) gn_block(p, gv, jj, s, q, lane, gn_part[warp], c PHASE(, shfl));   // whole chunks (Cout 256 / 512)
+      if (GN) gn_block(GN, gv, jj, s, q, lane, gn_part[warp], c PHASE(, shfl));   // whole chunks (Cout 256 / 512)
     }
+    // timing build: the results are pinned before the stamp so that the arithmetic is counted before stmatrix
+    PHASE(asm volatile("" ::"r"(oh[0]), "r"(oh[1]), "r"(oh[2]), "r"(oh[3]), "r"(oh[4]), "r"(oh[5]), "r"(oh[6]), "r"(oh[7]));
+          long long w2 = clock64(); link[1] += w2 - w1;)
     stmatrix_x4(sa + q0, oh);
     stmatrix_x4(sa + q1, oh + 4);
+    PHASE(w1 = clock64(); link[2] += w1 - w2;)
     fence_proxy_async_smem();
+    PHASE(w2 = clock64(); link[3] += w2 - w1;)
     mbar_arrive(&epi_ready[wg * kEpiSlots + es]);
+    PHASE(link[4] += clock64() - w2;)
     if (++es == kEpiSlots) { es = 0; eph ^= 1; }
   }
 }
@@ -463,6 +479,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   // GroupNorm plans: gn_bar[0] = a tile's partials written (every consumer thread), gn_bar[1] = summed by warp 10 (its 32
   // lanes), so the consumers may overwrite them with the next tile's
   __shared__ uint64_t gn_bar[2];
+  // epi_tma plans: the bias of a tile's N channels (zero past Cout), by tile parity.  Consumer thread t loads channel t at
+  // the tile's start and writes it after the mainloop; a named barrier of the 256 consumer threads publishes the tile's
+  // copy, and the parity keeps it apart from the previous tile's, which a warp may still be reading.
+  __shared__ float bias_s[2][256];
   // the 128-byte swizzle atoms (8 rows x 128 B) must start on 1024-byte boundaries
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -529,7 +549,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       if (p.res_mode) tma_prefetch_desc(&p.rmap);
       int s = 0, c = 0, nchunks = 0, filled = 0;
       uint32_t ph = 0;
-      PHASE(long long read_wait = 0, ready_wait = 0, stores = 0;)
+      PHASE(long long read_wait = 0, ready_wait = 0, stores = 0, store_cyc = 0, fill_cyc = 0;)
       int unit = blockIdx.x;
       TileCoord tc = {};
       for (int step = 0;; ++step) {
@@ -538,6 +558,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (step >= kEpiSlots && step - kEpiSlots < filled) {
           const int4 q = pend[s];
           const LevelDesc& L = p.lv[q.w & 7];
+          PHASE(const long long s0 = clock64();)
 #pragma unroll
           for (int wg = 0; wg < 2; ++wg) {
             int x, y;
@@ -548,7 +569,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             tma_store_4d(&p.omap[q.w & 7], epi_slots + (wg * kEpiSlots + s) * kEpiSlotBytes, q.x, x, y, q.w >> 3);
           }
           bulk_commit();
-          PHASE(++stores;)
+          PHASE(++stores; store_cyc += clock64() - s0;)
         }
         if (fill) {
           if (c == 0) {
@@ -557,7 +578,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           }
           PHASE(const long long w0 = clock64();)
           bulk_wait_read_all();                        // the store above has read the slot
-          PHASE(read_wait += clock64() - w0;)
+          PHASE(const long long f0 = clock64(); read_wait += f0 - w0;)
 #pragma unroll
           for (int wg = 0; wg < 2; ++wg) {
             uint64_t* bar = &epi_full[wg * kEpiSlots + s];
@@ -570,6 +591,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
               mbar_arrive(bar);
             }
           }
+          PHASE(fill_cyc += clock64() - f0;)
           pend[s] = make_int4(tc.n0 + 32 * c, tc.x0, tc.y0, tc.img * 8 + tc.lvl);
           ++filled;
           if (++c == nchunks) { c = 0; unit += gridDim.x; }
@@ -579,7 +601,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       bulk_wait_read_all();                          // the slots stay allocated until the last store has read them
       PHASE(if (p.phases) {
               unsigned long long* r = p.phases + (size_t)blockIdx.x * kPhaseWords;
-              r[4] = read_wait; r[5] = ready_wait; r[6] = stores; r[7] = filled;
+              r[4] = read_wait; r[5] = ready_wait; r[6] = stores; r[7] = filled; r[9] = store_cyc; r[10] = fill_cyc;
             })
     } else if (warp == kGnWarp && p.gn_group) {
       // ===================== GroupNorm statistics (whole warp): the consumers' tile sequence =====================
@@ -612,7 +634,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     float acc[N / 2];
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-    int s = 0, es = 0;
+    int s = 0, es = 0, tpar = 0;
     uint32_t ph = 0, eph = 0, gph = 0;
     PHASE(unsigned long long* const rec = p.phases + (size_t)blockIdx.x * kPhaseWords;
           const bool stamp = p.phases && (threadIdx.x & 127) == 0;
@@ -621,7 +643,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
       const TileCoord tc = decode_tile(p, unit);
       PHASE(const int sample = tile_i % p.phase_every == 0 ? tile_i / p.phase_every : kPhaseSamples;
-            const long long t_main = clock64(); long long blocked = 0; unsigned shfl = 0, hand = 0; ++tile_i;)
+            const long long t_main = clock64(); long long link[5] = {0, 0, 0, 0, 0}, bias_cyc = 0;
+            unsigned shfl = 0, hand = 0; ++tile_i;)
+      // this thread's channel of the tile's bias (bias_s): loaded here, so that the load is long done when it is written
+      float bias_t = 0.f;
+      if (p.epi_tma && p.bias && threadIdx.x < N && tc.n0 + (int)threadIdx.x < p.Cout) bias_t = __ldg(p.bias + tc.n0 + threadIdx.x);
       int prev = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(&full_bar[s], ph);
@@ -645,17 +671,36 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       PHASE(unsigned t_hand = clock();)
       if (p.gn_group) mbar_wait(&gn_bar[1], gph ^ 1);    // warp 10 has summed the previous tile's partials
       PHASE(hand = clock() - t_hand;)
-      if (p.epi_tma)
-        epilogue_tma<N>(p, tc, acc, wg, warp, lane, gn_part, smem_u32(epi_slots), epi_full, epi_ready, es,
-                        eph PHASE(, blocked, shfl));
-      else
+      if (p.epi_tma) {
+        PHASE(const long long b0 = clock64();)
+        if (threadIdx.x < N) bias_s[tpar][threadIdx.x] = bias_t;
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory");
+        PHASE(bias_cyc = clock64() - b0;)
+        // the plan's specialisation of epilogue_tma (RES, GN, RELU), chosen from the parameters of the launch
+        auto run = [&](auto res, auto gn, auto relu) {
+          epilogue_tma<N, decltype(res)::value, decltype(gn)::value, decltype(relu)::value>(
+              p, tc, acc, wg, warp, lane, gn_part, bias_s[tpar], smem_u32(epi_slots), epi_full, epi_ready, es,
+              eph PHASE(, link, shfl));
+        };
+        auto with_relu = [&](auto res, auto gn) {
+          if (p.relu) run(res, gn, Const<bool, true>()); else run(res, gn, Const<bool, false>());
+        };
+        auto with_gn = [&](auto res) {
+          if (p.gn_group == 8) with_relu(res, Const<int, 8>());
+          else if (p.gn_group == 16) with_relu(res, Const<int, 16>());
+          else with_relu(res, Const<int, 0>());
+        };
+        if (p.res_mode) with_gn(Const<bool, true>()); else with_gn(Const<bool, false>());
+        tpar ^= 1;
+      } else
         epilogue<N>(p, tc, acc, wg, warp, lane, gn_part PHASE(, shfl));
       PHASE(t_hand = clock();)
       if (p.gn_group) { mbar_arrive(&gn_bar[0]); gph ^= 1; }
       PHASE(hand += clock() - t_hand;
             if (stamp && sample < kPhaseSamples) {
               unsigned long long* r = rec + 16 + (sample * 2 + wg) * kPhaseTile;
-              r[0] = t_main; r[1] = t_mma; r[2] = clock64(); r[3] = blocked; r[4] = shfl; r[5] = hand;
+              r[0] = t_main; r[1] = t_mma; r[2] = clock64(); r[3] = link[0]; r[4] = shfl; r[5] = hand;
+              r[6] = link[1]; r[7] = link[2]; r[8] = link[3]; r[9] = link[4]; r[10] = bias_cyc;
             })
     }
     PHASE(if (threadIdx.x == 0 && p.phases) { rec[2] = globaltimer(); rec[3] = clock64(); rec[8] = tile_i; })

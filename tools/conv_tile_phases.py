@@ -9,6 +9,10 @@ at 16 CTAs (`--caps`).  Per plan and grid: mean µs per recorded tile of a consu
 MMA-idle fraction epi / (main + epi), chunks per tile, and warp 9's µs per tile blocked in `wait_group.read` and on
 `epi_ready`.  GroupNorm plans also report the part of epi spent in the statistics' shuffle reductions (gn_shfl) and in
 handing the tile's statistics over (gn_hand: the statistics barriers, or the wait for the previous tile's flush).
+Each link of the chunk chain is reported per tile, summed over its chunks: from the slot being ready to the results in
+registers (cmp: ldmatrix, arithmetic and gn_shfl), stmatrix (stsm), the proxy fence (fence), the slot arrival (arr), and
+the staging of the tile's bias before its first chunk (bias); and on warp 9's side per tile, the store steps' issue and
+commit time outside the epi_ready waits (w9st) and the fills' issue time (w9fill).
 `--src` times another version of conv_wgmma.cu (e.g. a parent commit's, with the same stamps).  Cycles are converted with the ratio of globaltimer to clock64 over all CTAs of the launch (sm_mhz)."""
 import argparse
 import ctypes
@@ -20,6 +24,7 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PHASE_TILE = 11                                                # kPhaseTile of the kernel's timing build
 sys.path.insert(0, ROOT)
 from sipmask_b200 import build as B  # noqa: E402
 from sipmask_b200 import _lib  # noqa: E402
@@ -47,7 +52,7 @@ def stamp(plan, buf, words, torch):
     r = buf.view(-1, words).cpu().numpy().astype('int64')
     ctas = r[r[:, 1] != 0]
     ns_per_cyc = (ctas[:, 2] - ctas[:, 0]).sum() / (ctas[:, 3] - ctas[:, 1]).sum()
-    tiles = ctas[:, 16:].reshape(len(ctas), -1, 6)             # [cta, sample * 2 + wg, 6]
+    tiles = ctas[:, 16:].reshape(len(ctas), -1, PHASE_TILE)    # [cta, sample * 2 + wg, PHASE_TILE]
     k = ns_per_cyc
     have = tiles[:, :, 0] != 0
     main = ((tiles[:, :, 1] - tiles[:, :, 0]) * k)[have] / 1e3
@@ -55,13 +60,17 @@ def stamp(plan, buf, words, torch):
     blk = (tiles[:, :, 3] * k)[have] / 1e3
     shfl = (tiles[:, :, 4] * k)[have] / 1e3
     hand = (tiles[:, :, 5] * k)[have] / 1e3
+    links = [float(((tiles[:, :, i] * k)[have] / 1e3).mean()) for i in (6, 7, 8, 9, 10)]
     ntiles = ctas[:, 8].sum()                                 # all tiles; the first kPhaseSamples per CTA are recorded
     stores = ctas[:, 6].sum()
     return dict(ctas=int(len(ctas)), tiles=int(ntiles), sm_mhz=float(1e3 / ns_per_cyc), main_us=float(main.mean()), epi_us=float(epi.mean()),
                 blocked_us=float(blk.mean()), gn_shfl_us=float(shfl.mean()), gn_hand_us=float(hand.mean()), idle=float(epi.mean() / (main.mean() + epi.mean())),
                 chunks=float(stores / ntiles) if stores else 0.0,
                 w9_read_us=float((ctas[:, 4] * ns_per_cyc).sum() / 1e3 / ntiles),
-                w9_ready_us=float((ctas[:, 5] * ns_per_cyc).sum() / 1e3 / ntiles))
+                w9_ready_us=float((ctas[:, 5] * ns_per_cyc).sum() / 1e3 / ntiles),
+                cmp_us=links[0], stsm_us=links[1], fence_us=links[2], arrive_us=links[3], bias_us=links[4],
+                w9_store_us=float(((ctas[:, 9] - ctas[:, 5]) * ns_per_cyc).sum() / 1e3 / ntiles),
+                w9_fill_us=float((ctas[:, 10] * ns_per_cyc).sum() / 1e3 / ntiles))
 
 
 def main():
@@ -93,9 +102,9 @@ def main():
     caps = [int(c) for c in args.caps.split(',') if c]
     out = []
     only = [o for o in (args.only or '').split(',') if o]
-    print('%-40s %5s %5s %5s | %4s %5s %8s %8s %8s %8s %8s %6s %8s %8s %6s' % (
+    print('%-40s %5s %5s %5s | %4s %5s %8s %8s %8s %8s %8s %6s %8s %8s %6s | %7s %7s %7s %7s %7s %7s %7s' % (
         'conv', 'Cout', 'K', 'chunk', 'ctas', 'tiles', 'main_us', 'epi_us', 'blk_us', 'gnshf_us', 'gnhnd_us', 'idle',
-        'w9rd_us', 'w9rdy_us', 'MHz'))
+        'w9rd_us', 'w9rdy_us', 'MHz', 'bias', 'cmp', 'stsm', 'fence', 'arr', 'w9st', 'w9fill'))
     for plan, m in zip(eng.conv_plans, eng.conv_meta):
         if only and not any(o in m['name'] or (o == 'gn' and m['gn']) for o in only):
             continue
@@ -107,9 +116,12 @@ def main():
             plan.set_max_ctas(c)
             rows.append(stamp(plan, buf, words, torch))
         for r in rows:
-            print('%-40s %5d %5d %5.1f | %4d %5d %8.2f %8.2f %8.2f %8.2f %8.2f %6.3f %8.2f %8.2f %6.0f' % (
-                name[-40:], m['N'], m['K'], r['chunks'], r['ctas'], r['tiles'], r['main_us'], r['epi_us'],
-                r['blocked_us'], r['gn_shfl_us'], r['gn_hand_us'], r['idle'], r['w9_read_us'], r['w9_ready_us'], r['sm_mhz']))
+            print('%-40s %5d %5d %5.1f | %4d %5d %8.2f %8.2f %8.2f %8.2f %8.2f %6.3f %8.2f %8.2f %6.0f | %7.2f %7.2f %7.2f %7.2f '
+                  '%7.2f %7.2f %7.2f' % (
+                      name[-40:], m['N'], m['K'], r['chunks'], r['ctas'], r['tiles'], r['main_us'], r['epi_us'],
+                      r['blocked_us'], r['gn_shfl_us'], r['gn_hand_us'], r['idle'], r['w9_read_us'], r['w9_ready_us'],
+                      r['sm_mhz'], r['bias_us'], r['cmp_us'], r['stsm_us'], r['fence_us'], r['arrive_us'], r['w9_store_us'],
+                      r['w9_fill_us']))
         out.append(dict(name=name, Cout=m['N'], K=m['K'], flops=m['flops'], grids=rows))
     print('card: %s' % torch.cuda.get_device_name(0))
     if args.json:
