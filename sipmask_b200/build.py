@@ -54,5 +54,28 @@ def build(verbose=False, force=False):
     return LIB
 
 
+# The test harness of csrc/cta.cuh's primitives (tests/csrc/cta_harness.cu): a library of its own, so the product
+# library exports and contains only product code.
+CTA_HARNESS_SRC = os.path.join(HERE, '..', 'tests', 'csrc', 'cta_harness.cu')
+CTA_HARNESS_LIB = os.path.join(HERE, 'lib', 'libsmb_cta_harness.so')
+
+
+def build_cta_harness(out=CTA_HARNESS_LIB, force=False):
+    deps = [CTA_HARNESS_SRC, os.path.join(CSRC, 'cta.cuh')]
+    if not force and os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in deps):
+        return out
+    logdir = os.path.join(os.path.dirname(out), 'obj')
+    os.makedirs(logdir, exist_ok=True)
+    tmp, log_path = out + '.tmp.so', os.path.join(logdir, 'cta_harness.log')
+    with open(log_path, 'w') as log:
+        rc = subprocess.call([NVCC] + FLAGS + ['-shared', '-I', CSRC, CTA_HARNESS_SRC, '-o', tmp],
+                             stdout=log, stderr=subprocess.STDOUT)
+    if rc != 0:
+        sys.stderr.write(open(log_path).read())
+        raise RuntimeError('nvcc failed on %s' % CTA_HARNESS_SRC)
+    os.replace(tmp, out)
+    return out
+
+
 if __name__ == '__main__':
     print(build(verbose='-v' in sys.argv, force='-f' in sys.argv))

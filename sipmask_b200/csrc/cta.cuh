@@ -3,10 +3,12 @@
 //
 // Sync contract, the same for every helper here: every thread of the CTA calls it (it contains __syncthreads()), and
 // when it returns, its shared scratch is free for the next call.  The scans read no shared memory of the caller.  The
-// sort and the selects synchronise before they read the caller's keys and after they write, so a caller may write the
-// keys right before the call and read the result right after it.  A helper with a kThreads template argument runs in
-// CTAs of exactly kThreads threads (blockDim.x, a multiple of 32 up to 1024): its strides and warp count are then
-// compile-time constants, which the select loops need to keep the speed of the code they replace.
+// sort and the selects synchronise before they first read or write the caller's memory (its keys, and the sel buffer
+// of cta_smallest_sorted) and after their last write, so a caller may write the keys right before the call and read the
+// result right after it, also when it calls again while other threads still read the previous result.  A helper with a
+// kThreads template argument runs in CTAs of exactly kThreads threads (blockDim.x, a multiple of 32 up to 1024): its
+// strides and warp count are then compile-time constants, which the select loops need to keep the speed of the code
+// they replace.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -152,10 +154,14 @@ __device__ __forceinline__ RadixKth<K> cta_radix_select(int n, int k, KeyAt key_
 }
 
 // The k smallest of the n distinct 64-bit keys key_at(0 .. n - 1), ascending, into sel[0 .. k).  sel holds cap keys and
-// is padded with ~0 up to the next power of two of k, which must not exceed cap.
+// is padded with ~0 up to the next power of two of k, which must not exceed cap.  When n < k, sel[0 .. n) holds all n
+// keys and the rest is padding.
 template <int kThreads, typename KeyAt>
 __device__ __forceinline__ void cta_smallest_sorted(int n, int k, KeyAt key_at, unsigned long long* sel, int cap,
                                                     SelectSmem& s) {
+  // With n <= k no select runs, and the fill of sel below would otherwise be the first thing a thread does: wait for
+  // every thread, so no thread overwrites sel (or s.count) while another still reads what a previous call left there.
+  __syncthreads();
   const unsigned long long kth = (n > k) ? cta_radix_select<kThreads, unsigned long long>(n, k, key_at, s).key : ~0ull;
   if (threadIdx.x == 0) s.count = 0;
   for (int i = threadIdx.x; i < cap; i += kThreads) sel[i] = ~0ull;
